@@ -579,7 +579,7 @@ static int render_collect(rtb200_scene_handle h, rt_stats* stats) {
     if (h->tp.npix_local == 0 || h->last_batches == 0 || h->pending_frames == 0) { h->pending_frames = 0; h->n_streams = 0; return RT_OK; }
     cudaStream_t st = h->last_stream;
     DeviceCtx::WorkSet& W = ctx->ws[h->last_set];
-    unsigned long long hstat[16] = {0}, herr[2] = {0, 0};
+    unsigned long long hstat[32] = {0}, herr[2] = {0, 0};   // the whole 256-byte stat block
     for (int i = 0; i < h->n_streams; ++i) if (h->streams[i] != st) CU(cudaStreamSynchronize(h->streams[i]));
     h->n_streams = 0;
     // error counters accumulate over every frame since the last wait (each frame adds to them; nothing clears them in between)
@@ -608,9 +608,17 @@ static int render_collect(rtb200_scene_handle h, rt_stats* stats) {
             fprintf(stderr, "[rtb200] trace kernel: first CTA start -> last CTA exit %.3f ms; queue dry -> last CTA exit (tail) %.3f ms; iterations after the queue ran dry: max %llu, mean %.1f per CTA\n",
                     total, tail, hstat[11], (double)hstat[12] / std::max(1, h->grid));
         }
-        if (getenv("RTB200_PRINT_PHASES")) {
-            fprintf(stderr, "[rtb200] fallbacks=%llu phases(warp-cycles): traverse=%llu exact=%llu waitA=%llu sort=%llu shade=%llu waitC=%llu warp_iters=%llu\n",
-                    hstat[2], hstat[8], hstat[9], hstat[10], hstat[11], hstat[12], hstat[13], hstat[14]);
+        if (getenv("RTB200_PRINT_PHASES")) {   // last batch of the last frame
+            const unsigned long long* ph = hstat + kPhaseStat;
+            if (ph[PH_ITERS] == 0) {
+                fprintf(stderr, "[rtb200] fallbacks=%llu; no phase clocks: this library was built without RT_PHASE_CLOCKS (make -C rust-raytracer_b200 phase)\n", hstat[2]);
+            } else {
+                const double it = (double)ph[PH_ITERS];
+                fprintf(stderr, "[rtb200] fallbacks=%llu phases (clock64 cycles per warp iteration): closest_hit=%.0f sort+waitA=%.0f shade=%.0f regen=%.0f waitC=%.0f; "
+                        "warp_iters=%llu scatters=%llu deferred=%llu (%.4f of scatters)\n",
+                        hstat[2], ph[PH_HIT] / it, ph[PH_SORT_WAIT_A] / it, ph[PH_SHADE] / it, ph[PH_REGEN] / it, ph[PH_WAIT_C] / it,
+                        ph[PH_ITERS], ph[PH_SCATTERS], ph[PH_DEFERRED], (double)ph[PH_DEFERRED] / (double)std::max(1ull, ph[PH_SCATTERS]));
+            }
         }
         if (h->tp.max_depth == 0) stats->samples = (uint64_t)h->tp.npix_local * h->tp.spp;   // no kernel ran: every sample is black
         stats->kernel_launches = h->last_launches * frames; stats->batches = h->last_batches;

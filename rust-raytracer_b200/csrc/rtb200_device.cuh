@@ -79,15 +79,20 @@ RT_DEV double rng_m1_1(Rng& g, uint32_t k0, uint32_t k1) {
     double v01 = __dsub_rn(__longlong_as_double((long long)bits), 1.0);
     return __dadd_rn(__dmul_rn(v01, 2.0), -1.0);
 }
-// Same stream, same draws, but two rejection trials per loop trip and their three Philox blocks computed together
-// (instruction-level parallelism: the shade stage is bound by the latency of this dependent chain, not by throughput).
 RT_DEV double u64_to_m1_1(uint32_t lo, uint32_t hi) {
     unsigned long long bits = ((((unsigned long long)hi << 32) | lo) >> 12) | 0x3FF0000000000000ull;
     double v01 = __dsub_rn(__longlong_as_double((long long)bits), 1.0);
     return __dadd_rn(__dmul_rn(v01, 2.0), -1.0);
 }
-RT_DEV D3 random_in_unit_sphere_ilp(Rng& g, uint32_t k0, uint32_t k1) {                                       // point3d.rs:22-38
-    for (;;) {
+// random_in_unit_sphere (point3d.rs:22-38) on the same stream with the same draws, but two rejection trials per loop trip
+// and their three Philox blocks computed together (instruction-level parallelism: the shade stage is bound by the latency
+// of this dependent chain, not by throughput). At most TRIPS trips: returns true with the accepted point in `out`, or
+// false with the stream position (blk, has, cached half-block) exactly where the unbounded loop stands after the same
+// trips, so that a later call continues the same rejection sequence and accepts the same point.
+template <int TRIPS>
+RT_DEV bool random_in_unit_sphere_ilp(Rng& g, uint32_t k0, uint32_t k1, D3& out) {
+#pragma unroll 1
+    for (int trip = 0; trip < TRIPS; ++trip) {
         uint32_t A[4], B[4], Cc[4];
         philox4x32_10(g.blk, g.sample, g.pixel, 0u, k0, k1, A);
         philox4x32_10(g.blk + 1u, g.sample, g.pixel, 0u, k0, k1, B);
@@ -105,16 +110,10 @@ RT_DEV D3 random_in_unit_sphere_ilp(Rng& g, uint32_t k0, uint32_t k1) {         
         g.blk = (pos + 1u) >> 1;
         g.has = pos & 1u;
         g.c_lo = a1 ? lo[3] : lo[6]; g.c_hi = a1 ? hi[3] : hi[6];   // the next unread draw; it is a block's second half exactly when pos is odd
-        if (a1) return p1;
-        if (a2) return p2;
+        if (a1) { out = p1; return true; }
+        if (a2) { out = p2; return true; }
     }
-}
-RT_DEV D3 random_in_unit_sphere(Rng& g, uint32_t k0, uint32_t k1) {                                           // point3d.rs:22-38
-    for (;;) {
-        double x = rng_m1_1(g, k0, k1), y = rng_m1_1(g, k0, k1), z = rng_m1_1(g, k0, k1);
-        D3 p = mk(x, y, z);
-        if (length_squared(p) < 1.0) return p;
-    }
+    return false;
 }
 
 // ---- Camera::get_ray (camera.rs:79-84) -------------------------------------------------------------

@@ -12,6 +12,13 @@ namespace rtk {
 #define RT_BLOCK 256
 #endif
 constexpr int kBlock = RT_BLOCK;   // threads (= ray slots) per CTA of the trace kernel
+#ifndef RT_PHASE_CLOCKS
+#define RT_PHASE_CLOCKS 0          // 1: the trace kernel accounts its stages per warp (Makefile target `phase`, RTB200_PRINT_PHASES)
+#endif
+// stat[kPhaseStat + k] of an RT_PHASE_CLOCKS build: clock64() cycles of each stage summed over warps (k < PH_ITERS), warp
+// iterations, diffuse / metal vertices shaded (scatter attempts), and those of them whose scatter sample was deferred
+enum : uint32_t { PH_HIT, PH_SORT_WAIT_A, PH_SHADE, PH_REGEN, PH_WAIT_C, PH_ITERS, PH_SCATTERS, PH_DEFERRED, kPhaseN };
+constexpr uint32_t kPhaseStat = 13;
 #ifndef RT_LEAF_K
 #define RT_LEAF_K 8
 #endif
@@ -81,8 +88,7 @@ struct TraceParams {
     ShadowFrame* frames;         // [max_shadow][stack_stride], only when n_lights > 0
     uint32_t max_shadow;         // nested light-test frames per path (a level nests with probability <= n_lights*0.1)
     float* lterm;                // [2 levels][3][stack_stride] light terms of the first two path levels
-    unsigned long long* stat;    // per frame: [0]=rays [1]=f64 tests [2]=all-spheres fallbacks [3]=samples [4]=leaf visits [6]=node visits
-                                 // [8..15] phase clocks (RT_PROFILE_PHASES)
+    unsigned long long* stat;    // per frame: [0]=rays [1]=f64 tests [2]=all-spheres fallbacks [3]=samples [4]=leaf visits [6]=node visits, [8..12] frame tail, [kPhaseStat..] phase clocks
     unsigned long long* err;     // per scene handle, accumulated over frames: [0]=shadow-frame-stack overflows [1]=traversal guard trips (must stay 0)
 };
 

@@ -18,15 +18,23 @@ namespace rtk {
 
 using namespace rtd;
 
-#ifndef RT_SAMPLE_ILP
-#define RT_SAMPLE_ILP 1   // two rejection trials per trip with their Philox blocks computed together (bit-identical stream)
+#ifndef RT_SCATTER_TRIPS
+// Rejection-loop trips (two trials each) of the unit-sphere sampler per shade stage; a scatter still unresolved after them
+// carries over to the next iteration. On C2 on an H100, 2 trips beat 1 (16 % more iterations) and 3 (DESIGN.md §4.3).
+#define RT_SCATTER_TRIPS 2
 #endif
 #ifndef RT_SMEM_STACK
-#define RT_SMEM_STACK 3   // albedo-stack levels kept in shared memory per slot (deeper levels live in global memory)
+// Albedo-stack levels kept in shared memory per slot; deeper levels live in global memory, and every bounce there costs a
+// global store and, when the path is unwound, a dependent global load. 12 levels (65.1 KB per CTA) still leave 3 CTAs per
+// SM; on C2 on an H100 each step from 3 to 5, 8 and 12 levels was faster (DESIGN.md §4.3).
+#define RT_SMEM_STACK 12
 #endif
 
 enum : uint32_t { CLS_MISS = 0, CLS_DIFFUSE = 1, CLS_METAL = 2, CLS_GLASS = 3, CLS_LIGHT = 4, CLS_DEAD = 5, N_CLS = 6 };
 constexpr uint32_t kDeadLevel = 0xffffffffu;
+// Pool.shd bit: the slot's scatter sample is still being drawn; its hit record (bt/bi) and path state are those of the
+// vertex being shaded. The shadow depth in the low bits never exceeds max_shadow (<= 384), so the bit is free.
+constexpr uint32_t kScatterPending = 0x80000000u;
 constexpr uint32_t kLeafBit = 0x80000000u;
 constexpr unsigned long long kNoHitBits = 0x7ff0000000000000ull;   // +inf as the "no root yet" key (roots are > t_min > 0)
 constexpr uint32_t kSlotBytes = 7 * 8 + 9 * 4 + RT_SMEM_STACK * 4;   // shared memory per pool slot
@@ -34,7 +42,7 @@ constexpr uint32_t kSlotBytes = 7 * 8 + 9 * 4 + RT_SMEM_STACK * 4;   // shared m
 // SoA ray pool of a CTA: n_slots slots.
 struct Pool {
     double *ox, *oy, *oz, *dx, *dy, *dz, *bt;                    // ray origin / direction, best root (also updated as u64 bits)
-    uint32_t *bi, *work, *pix, *smp, *blk, *clo, *chi, *lvl, *shd;   // hit index, work id, RNG (pixel, sample, block|has, cached draw), path level, shadow depth
+    uint32_t *bi, *work, *pix, *smp, *blk, *clo, *chi, *lvl, *shd;   // hit index, work id, RNG (pixel, sample, block|has, cached draw), path level, shadow depth | kScatterPending
     uint32_t *stk;                                               // [RT_SMEM_STACK][n_slots] first levels of the albedo stack
     uint32_t n_slots;
     uint32_t stack_col;                                          // this CTA's first column of the global per-slot arrays (stack / frames / lterm)
@@ -120,6 +128,10 @@ RT_DEV float2 fma2_rn(float2 a, float2 b, float2 c) { return make_float2(__fmaf_
         tt = fma2_rn(cx, ox2, tt);                                                                                                   \
         (DV)[q] = fma2_rn(bb, bb, tt);                                                                                               \
     }
+
+RT_DEV uint32_t class_of(uint32_t kind) {
+    return (kind == RT_METAL) ? CLS_METAL : (kind == RT_GLASS) ? CLS_GLASS : (kind == RT_LIGHT) ? CLS_LIGHT : CLS_DIFFUSE;
+}
 
 // =====================================================================================================================
 // closest-hit. Every lane of the warp calls it; lane l owns the ray in pool slot `slot` when `alive`. On return
@@ -362,10 +374,7 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
         }
         const uint32_t fin = P.bi[slot];
         cls = CLS_MISS;
-        if (fin != 0xffffffffu) {
-            uint32_t kind = sc.mat[fin].kind;
-            cls = (kind == RT_METAL) ? CLS_METAL : (kind == RT_GLASS) ? CLS_GLASS : (kind == RT_LIGHT) ? CLS_LIGHT : CLS_DIFFUSE;
-        }
+        if (fin != 0xffffffffu) cls = class_of(sc.mat[fin].kind);
         ++st.rays;
     }
     return cls;
@@ -413,8 +422,8 @@ RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint
     P.work[s] = s_local * p.npix_local + lp; P.pix[s] = rng.pixel; P.smp[s] = rng.sample;   // samplebuf index [sample][pixel]
     P.blk[s] = (rng.blk << 1) | rng.has; P.clo[s] = rng.c_lo; P.chi[s] = rng.c_hi;
     P.lvl[s] = 0u;
+    P.shd[s] = 0u;
     if (LIGHTS) {
-        P.shd[s] = 0u;
         for (int q = 0; q < 6; ++q) p.lterm[(size_t)q * p.stack_stride + P.stack_col + s] = 0.0f;
     }
     ++st.samples;
@@ -424,7 +433,9 @@ RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint
 // =====================================================================================================================
 // One path vertex of slot `s` whose closest-hit result is in the pool; c = the ray's class. Writes the continuation ray
 // (or a shadow ray) back to the pool, or - when the sample is finished - its radiance to samplebuf and marks the slot
-// dead (returns true).
+// dead (returns true). A diffuse or metal vertex whose scatter sample is not accepted within RT_SCATTER_TRIPS trips of
+// the rejection loop saves only its RNG position, is marked kScatterPending and is shaded again in the next iteration
+// (returns false), so that a warp does not loop for its unluckiest lane while the other lanes idle.
 // =====================================================================================================================
 template <bool LIGHTS>
 RT_DEV bool shade_slot(const TraceParams& p, const SceneRefs& sc, const Pool& P, uint32_t s, uint32_t c) {
@@ -438,18 +449,18 @@ RT_DEV bool shade_slot(const TraceParams& p, const SceneRefs& sc, const Pool& P,
     auto stack_get = [&](uint32_t lvl) -> uint32_t {
         return lvl < (uint32_t)RT_SMEM_STACK ? P.stk[lvl * P.n_slots + s] : p.stack[(size_t)lvl * p.stack_stride + col];
     };
+    Rng rng; rng.pixel = P.pix[s]; rng.sample = P.smp[s];
+    { uint32_t bh = P.blk[s]; rng.blk = bh >> 1; rng.has = bh & 1u; }
+    rng.c_lo = P.clo[s]; rng.c_hi = P.chi[s];
     bool done = false;
     D3 o = mk(P.ox[s], P.oy[s], P.oz[s]), d = mk(P.dx[s], P.dy[s], P.dz[s]);
     uint32_t level = P.lvl[s];
-    uint32_t shd = LIGHTS ? P.shd[s] : 0u;       // > 0: this ray is a shadow ray of the light test (raytracer.rs:103-106)
+    uint32_t shd = LIGHTS ? (P.shd[s] & ~kScatterPending) : 0u;   // > 0: this ray is a shadow ray of the light test (raytracer.rs:103-106)
     const uint32_t rays_sample = level + 1u;   // main-path hit_world calls so far, this one included
     float cr = 0.f, cg = 0.f, cb = 0.f;
     bool have_tc = false;                      // a shadow ray's ray_color(.., 2, 1) value is ready
     float tr = 0.f, tg = 0.f, tb = 0.f;
     bool state_dirty = false;                  // o/d/rng/level must be written back to the pool
-    Rng rng; rng.pixel = P.pix[s]; rng.sample = P.smp[s];
-    { uint32_t bh = P.blk[s]; rng.blk = bh >> 1; rng.has = bh & 1u; }
-    rng.c_lo = P.clo[s]; rng.c_hi = P.chi[s];
     if (c == CLS_MISS) {                                                // raytracer.rs:134-163
         float x, y, z;
         sky_color(d, length(d), p.sky_mode, p.sky, x, y, z);
@@ -467,7 +478,19 @@ RT_DEV bool shade_slot(const TraceParams& p, const SceneRefs& sc, const Pool& P,
         bool absorbed = false;
         const bool is_light = (c == CLS_LIGHT);                         // materials.rs:65-69: Some((None, white))
         D3 rs = mk(0, 0, 0);
-        if (c == CLS_DIFFUSE || c == CLS_METAL) rs = RT_SAMPLE_ILP ? random_in_unit_sphere_ilp(rng, k0, k1) : random_in_unit_sphere(rng, k0, k1);   // one rejection loop for a warp that straddles both classes
+        if (c == CLS_DIFFUSE || c == CLS_METAL) {   // one rejection loop for a warp that straddles both classes
+            const unsigned group = __activemask();
+            const bool sampled = random_in_unit_sphere_ilp<RT_SCATTER_TRIPS>(rng, k0, k1, rs);
+            // Reconverge here. The early return below would otherwise put the reconvergence point at the end of the function,
+            // and lanes accepted after different numbers of trips would run the rest of the vertex one group after another.
+            __syncwarp(group);
+            // the scatter draws are the vertex's first draws: a vertex deferred here has changed nothing but its RNG position
+            if (!sampled) {
+                P.blk[s] = (rng.blk << 1) | rng.has; P.clo[s] = rng.c_lo; P.chi[s] = rng.c_hi;
+                P.shd[s] |= kScatterPending;
+                return false;
+            }
+        }
         if (c == CLS_DIFFUSE) {                                         // materials.rs:84-95, 256-267
             D3 sd = add(h.normal, rs);
             if (near_zero(sd)) sd = h.normal;
@@ -570,7 +593,7 @@ RT_DEV bool shade_slot(const TraceParams& p, const SceneRefs& sc, const Pool& P,
         P.ox[s] = o.x; P.oy[s] = o.y; P.oz[s] = o.z; P.dx[s] = d.x; P.dy[s] = d.y; P.dz[s] = d.z;
         P.blk[s] = (rng.blk << 1) | rng.has; P.clo[s] = rng.c_lo; P.chi[s] = rng.c_hi;
         P.lvl[s] = level;
-        if (LIGHTS) P.shd[s] = shd;
+        P.shd[s] = shd;   // also clears kScatterPending
     }
     if (done) {
         // unwind the recursion: c = clamp(light + albedo * c) per level, innermost first (raytracer.rs:117-122)

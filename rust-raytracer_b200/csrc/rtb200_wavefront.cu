@@ -23,6 +23,7 @@ struct WfSmem {
     uint32_t pool;      // kSlotBytes * kBlock
     uint32_t perm;      // uint16[5 classes][kBlock]: every class has its own segment, so a slot's position needs no other class's count
     uint32_t cnt;       // uint32[2][8]
+    uint32_t phase;     // RT_PHASE_CLOCKS: u64[8 warps][kPhaseN]
     uint32_t total;
 };
 
@@ -41,6 +42,7 @@ __host__ __device__ inline WfSmem wf_layout(uint32_t n, uint32_t n_pairs, uint32
     L.pool = off; off += kSlotBytes * (uint32_t)kBlock;
     L.perm = off; off += 5u * kBlock * 2u;
     L.cnt = off; off += 2u * 8u * 4u;
+    L.phase = off; if (RT_PHASE_CLOCKS) off += (uint32_t)(kBlock / 32) * kPhaseN * 8u;
     L.total = off;
     return L;
 }
@@ -103,13 +105,28 @@ __global__ void __launch_bounds__(kBlock, (MINB * 256 / kBlock) > 0 ? (MINB * 25
     regenerate_slot<LIGHTS>(p, P, true, (uint32_t)tid, lane, exhausted, st);   // initial fill of the pool
     __syncthreads();
 
+#if RT_PHASE_CLOCKS
+    // lane 0 of each warp adds the warp's clock64() time of each stage to the warp's own row of ph[]
+    static_assert(kPhaseStat + kPhaseN <= 32, "the per-launch stat block holds 32 counters");
+    unsigned long long* ph = reinterpret_cast<unsigned long long*>(smem_raw + L.phase) + (uint32_t)(tid >> 5) * kPhaseN;
+    if (lane < (int)kPhaseN) ph[lane] = 0ull;
+    unsigned long long t_mark = clock64();
+    auto tick = [&](uint32_t k) { __syncwarp(); const unsigned long long t = clock64(); if (lane == 0) ph[k] += t - t_mark; t_mark = t; };
+#endif
     const uint32_t lt_mask = (1u << lane) - 1u;
     uint32_t it = 0;
     for (;; ++it) {
         uint32_t* cnt = s_cnt + (it & 1u) * 8u;
         // =========================== closest-hit: thread t <-> slot t ===========================
+        // A slot whose scatter sample is pending is not traced: it keeps its hit (and its ray count) and takes the class of
+        // the sphere it hit, so the sort puts it back among the fresh hits of its material.
         const bool alive = P.lvl[tid] != kDeadLevel;
-        const uint32_t cls = closest_hit<MODE>(p, sc, P, W, alive, (uint32_t)tid, lane, st);
+        const bool pending = alive && (P.shd[tid] & kScatterPending) != 0u;
+        uint32_t cls = closest_hit<MODE>(p, sc, P, W, alive && !pending, (uint32_t)tid, lane, st);
+        if (pending) cls = class_of(sc.mat[P.bi[tid]].kind);
+#if RT_PHASE_CLOCKS
+        tick(PH_HIT);
+#endif
 
         // =========================== sort: compact the live slots class by class ===========================
         // warp ballot + one shared-memory atomic per (warp, class) reserve positions in the class's own segment of perm[]
@@ -124,6 +141,9 @@ __global__ void __launch_bounds__(kBlock, (MINB * 256 / kBlock) > 0 ? (MINB * 25
             }
         }
         __syncthreads();   // A: class counts and perm complete (and every warp's closest-hit results are in the pool)
+#if RT_PHASE_CLOCKS
+        tick(PH_SORT_WAIT_A);
+#endif
         uint32_t c0 = cnt[0], c1 = cnt[1], c2 = cnt[2], c3 = cnt[3], c4 = cnt[4];
         const uint32_t e0 = c0, e1 = e0 + c1, e2 = e1 + c2, e3 = e2 + c3, n_live = e3 + c4;   // class end offsets
         if (tid < 8) s_cnt[((it + 1u) & 1u) * 8u + tid] = 0u;   // reset the other counter set for the next iteration
@@ -135,13 +155,32 @@ __global__ void __launch_bounds__(kBlock, (MINB * 256 / kBlock) > 0 ? (MINB * 25
         const uint32_t s = active ? (uint32_t)s_perm[c * (uint32_t)kBlock + ((uint32_t)tid - cstart)] : 0u;
         bool done = false;
         if (active) done = shade_slot<LIGHTS>(p, sc, P, s, c);
+#if RT_PHASE_CLOCKS
+        tick(PH_SHADE);
+        {
+            const bool scatter = active && (c == CLS_DIFFUSE || c == CLS_METAL);
+            const unsigned sm = __ballot_sync(FULL, scatter), dm = __ballot_sync(FULL, scatter && !done && (P.shd[s] & kScatterPending) != 0u);
+            if (lane == 0) { ph[PH_ITERS] += 1ull; ph[PH_SCATTERS] += (unsigned)__popc(sm); ph[PH_DEFERRED] += (unsigned)__popc(dm); }
+        }
+#endif
         regenerate_slot<LIGHTS>(p, P, active && done, s, lane, exhausted, st);
         if (exhausted && !stamped) { stamped = true; if (lane == 0) atomicMin(&p.stat[9], now_ns()); }
         if (stamped) ++dry_iters;
         const bool still_alive = active && (P.lvl[s] != kDeadLevel);
-        if (!__syncthreads_or(still_alive ? 1 : 0)) break;   // C: pool written back; exit when the CTA has no ray left
+#if RT_PHASE_CLOCKS
+        tick(PH_REGEN);
+#endif
+        const int more = __syncthreads_or(still_alive ? 1 : 0);   // C: pool written back; exit when the CTA has no ray left
+#if RT_PHASE_CLOCKS
+        tick(PH_WAIT_C);
+#endif
+        if (!more) break;
     }
     flush_stats(p, st, lane);
+#if RT_PHASE_CLOCKS
+    __syncwarp();
+    if (lane < (int)kPhaseN) atomicAdd(&p.stat[kPhaseStat + lane], ph[lane]);
+#endif
     if (tid == 0) { atomicMax(&p.stat[10], now_ns()); atomicMax(&p.stat[11], (unsigned long long)dry_iters); atomicAdd(&p.stat[12], (unsigned long long)dry_iters); }
 }
 

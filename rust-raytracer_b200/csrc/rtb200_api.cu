@@ -70,7 +70,6 @@ struct DeviceCtx {
     bool init = false;
     int device = -1;
     int sm_count = 0;
-    size_t max_smem = 0;
     cudaStream_t stream = nullptr;
     // Two sets of per-frame work buffers: a frame loop that alternates two streams lets frame k+1 start tracing while frame k
     // drains its last paths and resolves (rtb200_render_device_async); blocking calls use set 0 only.
@@ -80,7 +79,7 @@ struct DeviceCtx {
     struct Arena { void* p; size_t cap; };
     std::vector<Arena> arena_cache;
     std::vector<cudaEvent_t> event_pool;  // timing events of released handles (creating four events per one-shot render costs more than the upload)
-    struct OccKey { uint32_t mode; bool lights; int minb; size_t smem; int occ; };
+    struct OccKey { uint32_t mode; bool lights; size_t smem; int occ; };
     std::vector<OccKey> occ_cache;        // cudaOccupancyMaxActiveBlocksPerMultiprocessor answers
     PinnedBuf staging;                    // host image of the arena being uploaded
     cudaEvent_t staging_free = nullptr;   // the last H2D copy out of `staging` has finished
@@ -111,7 +110,6 @@ int get_ctx(int device, DeviceCtx** out) {
         }
         c.device = device;
         c.sm_count = prop.multiProcessorCount;
-        c.max_smem = prop.sharedMemPerBlockOptin;
         CU(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
         CU(cudaEventCreateWithFlags(&c.staging_free, cudaEventDisableTiming));
         c.init = true;
@@ -158,8 +156,6 @@ struct rtb200_scene_t {
     TraceParams tp{};
     rt_options opts{};
     uint32_t mode = MODE_TREE;
-    uint32_t slots_per_cta = kBlock;     // ray slots per CTA (one per thread)
-    int minb = 3;
     int grid = 0;
     int ctas_per_sm = 0;
     size_t smem = 0;
@@ -407,43 +403,21 @@ static int scene_upload_records(const rt_scene* s, const rt_options& opts, uint3
     tp.rows_local = rtb200_shard_rows(s->height, opts.rank, opts.world, opts.band_rows);
     tp.npix_local = tp.rows_local * s->width;
 
-    // ---- launch geometry: persistent grid = SMs x resident CTAs ----
-    // RTB200_WF_SMEM=<mask> (bit0 hierarchy / flat records, bit1 geo, bit2 mat in shared memory) and RTB200_WF_MINB=<2|3|4>
-    // pin the tuning knobs for experiments.
+    // ---- launch geometry: persistent grid = SMs x resident CTAs of the mode's trace kernel ----
+    // Nothing of the scene is staged into shared memory unless RTB200_WF_SMEM=<mask> asks for it (bit0 hierarchy / flat
+    // records, bit1 geo, bit2 mat): for these small, hot arrays a larger L1 beats the staging (DESIGN.md §4.5).
     const char* es = getenv("RTB200_WF_SMEM");
-    {
-        // What could be staged into shared memory next to the ray pool: the hierarchy, exact geometry, materials. Measured in
-        // round 2 (DESIGN.md §4.5): for scenes this small a larger L1 beats the staging, so "nothing staged" is tried first.
-        const char* eb = getenv("RTB200_WF_MINB");
-        const uint32_t masks[] = {0u, 7u, 3u, 1u};   // measured (round 2): a larger L1 beats staging the small scenes' records
-        bool found = false;
-        for (int minb : {4, 3, 2}) {
-            if (minb == 4 && !(eb && atoi(eb) == 4)) continue;   // the 64-register build: only on request
-            if (eb && atoi(eb) != minb) continue;
-            for (int need : {std::max(1, minb * 256 / kBlock), 1}) {   // CTAs per SM this register budget is built for
-                for (uint32_t mask : masks) {
-                    if (found) break;
-                    if (es && (uint32_t)atoi(es) != mask) continue;
-                    if (h->mode == MODE_EXACT && (mask & 1u)) continue;
-                    size_t sm = wavefront_smem_bytes(tp, h->mode, mask);
-                    if (sm > ctx->max_smem) continue;
-                    int occ = -1;
-                    for (auto& k : ctx->occ_cache) if (k.mode == h->mode && k.lights == (n_lights > 0) && k.minb == minb && k.smem == sm) occ = k.occ;
-                    if (occ < 0) {
-                        occ = wavefront_max_ctas_per_sm(h->mode, n_lights > 0, sm, minb);
-                        ctx->occ_cache.push_back(DeviceCtx::OccKey{h->mode, n_lights > 0, minb, sm, occ});
-                    }
-                    if (occ < need || occ <= 0) continue;
-                    h->minb = minb; h->smem = sm; tp.scene_in_smem = mask; h->ctas_per_sm = occ; h->grid = ctx->sm_count * occ;
-                    found = true;
-                }
-                if (found || minb >= 3) break;   // the 80 / 64-register builds are only worth it at full residency
-            }
-            if (found) break;
-        }
-        if (!found) return fail(RT_ERR_UNSUPPORTED, "no launch configuration fits shared memory");
-        h->slots_per_cta = kBlock;
+    tp.scene_in_smem = es ? (uint32_t)atoi(es) : 0u;
+    h->smem = wavefront_smem_bytes(tp, h->mode, tp.scene_in_smem);
+    int occ = -1;
+    for (auto& k : ctx->occ_cache) if (k.mode == h->mode && k.lights == (n_lights > 0) && k.smem == h->smem) occ = k.occ;
+    if (occ < 0) {
+        occ = wavefront_max_ctas_per_sm(h->mode, n_lights > 0, h->smem);
+        ctx->occ_cache.push_back(DeviceCtx::OccKey{h->mode, n_lights > 0, h->smem, occ});
     }
+    if (occ <= 0) return fail(RT_ERR_UNSUPPORTED, "no launch configuration fits shared memory");
+    h->ctas_per_sm = occ;
+    h->grid = ctx->sm_count * occ;
 
     // ---- per-sample staging: samples per batch bounded by the buffer cap ----
     uint64_t cap = opts.sample_buffer_bytes ? opts.sample_buffer_bytes : (1ull << 30);
@@ -482,9 +456,9 @@ int rtb200_scene_kernel_info(rtb200_scene_handle h, rt_kernel_info* out) {
     CU(cudaSetDevice(h->device));
     memset(out, 0, sizeof *out);
     KernelInfo ki{};
-    CU(wavefront_info(h->mode, h->tp.n_lights > 0, h->minb, &ki));
+    CU(wavefront_info(h->mode, h->tp.n_lights > 0, &ki));
     out->registers = ki.registers; out->local_bytes = ki.local_bytes; out->smem_bytes = (uint32_t)h->smem; out->grid = (uint32_t)h->grid;
-    out->block = (uint32_t)kBlock; out->pool_slots = h->slots_per_cta;
+    out->block = (uint32_t)kBlock; out->pool_slots = (uint32_t)kBlock;
     out->ctas_per_sm = (uint32_t)h->ctas_per_sm; out->smem_mask = h->tp.scene_in_smem;
     out->bvh_nodes = h->tp.n_nodes; out->bvh_leaves = h->tp.n_leaves; out->bvh_depth = h->tp.depth;
     snprintf(out->name, sizeof out->name, "%s", ki.name);
@@ -506,7 +480,7 @@ static int render_enqueue(rtb200_scene_handle h, void* dev_rgb8, void* dev_linea
 
     const uint32_t spp = tp.spp, spb = h->spp_batch;
     const uint32_t n_batches = (spp + spb - 1) / spb;
-    const uint32_t threads_total = (uint32_t)h->grid * h->slots_per_cta;   // ray slots of the whole grid: columns of the per-slot global arrays
+    const uint32_t threads_total = (uint32_t)h->grid * (uint32_t)kBlock;   // ray slots of the whole grid: columns of the per-slot global arrays
 
     CU(W.samplebuf.ensure((size_t)spb * tp.npix_local * 16));
     CU(W.accum.ensure((size_t)tp.npix_local * 12));
@@ -554,7 +528,7 @@ static int render_enqueue(rtb200_scene_handle h, void* dev_rgb8, void* dev_linea
         if (tp.max_depth == 0) {
             CU(cudaMemsetAsync(tp.samplebuf, 0, (size_t)tp.total_work * 16, st));   // ray_color(depth 0) = black, no ray (raytracer.rs:80-82)
         } else {
-            CU(launch_wavefront(tp, h->mode, h->grid, h->smem, h->minb, st));
+            CU(launch_wavefront(tp, h->mode, h->grid, h->smem, st));
         }
         CU(cudaEventRecord(fev[3 + 2 * b], st));
         ResolveParams q{};

@@ -105,9 +105,9 @@ struct ResolveParams {
 struct KernelInfo { int registers, max_threads, const_bytes, local_bytes; char name[96]; };
 
 size_t wavefront_smem_bytes(const TraceParams& p, uint32_t mode, uint32_t smem_mask);
-cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, int grid, size_t smem, int minb, cudaStream_t st);
-int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, size_t smem, int minb);
-cudaError_t wavefront_info(uint32_t mode, bool lights, int minb, KernelInfo* out);
+cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, int grid, size_t smem, cudaStream_t st);
+int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, size_t smem);   // 0 when the kernel cannot run on the current device
+cudaError_t wavefront_info(uint32_t mode, bool lights, KernelInfo* out);
 cudaError_t launch_resolve(const ResolveParams& p, cudaStream_t st);
 
 // single-thread probes of the device routines (known-answer tests)

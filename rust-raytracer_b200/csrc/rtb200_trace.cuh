@@ -1,6 +1,6 @@
-// rtb200_trace.cuh — the three stages of the render path as device functions shared by the two trace kernels
-// (rtb200_wavefront.cu; a queue-driven kernel without CTA barriers was built on the same functions in round 2 and lost to
-// instruction-cache misses - DESIGN.md §4.5, tools/experiments/):
+// rtb200_trace.cuh — the three stages of the render path as device functions of the trace kernel (rtb200_wavefront.cu; a
+// queue-driven kernel without CTA barriers was built on the same functions in round 2 and lost to instruction-cache misses -
+// DESIGN.md §4.5, `git show 1f183f9:tools/experiments/rtb200_stream.cu.txt`):
 //
 //   closest_hit<MODE>   hit_world (raytracer.rs:44-59) for the 32 rays a warp holds: WARP-COOPERATIVE traversal of the
 //                       8-wide BVH (node / leaf / exact steps over three per-warp work lists, one pair per lane), or the

@@ -53,8 +53,15 @@ size_t wavefront_smem_bytes(const TraceParams& p, uint32_t mode, uint32_t smem_m
     return wf_layout(p.n, p.n_pairs, p.n_nodes, p.n_leaves, mode, smem_mask).total;
 }
 
-template <int MINB, uint32_t MODE, bool LIGHTS>
-__global__ void __launch_bounds__(kBlock, (MINB * 256 / kBlock) > 0 ? (MINB * 256 / kBlock) : 1) rt_wavefront_kernel(const __grid_constant__ TraceParams p) {
+// CTAs per SM each kernel's register budget is built for: 3 of 256 threads for the BVH path (80 registers), 2 for the
+// validation modes
+constexpr int wf_min_blocks(uint32_t mode) {
+    const int n = (mode == MODE_TREE ? 3 : 2) * 256 / kBlock;
+    return n > 0 ? n : 1;
+}
+
+template <uint32_t MODE, bool LIGHTS>
+__global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kernel(const __grid_constant__ TraceParams p) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const WfSmem L = wf_layout(p.n, p.n_pairs, p.n_nodes, p.n_leaves, MODE, p.scene_in_smem);
     uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw);
@@ -185,17 +192,14 @@ __global__ void __launch_bounds__(kBlock, (MINB * 256 / kBlock) > 0 ? (MINB * 25
 }
 
 template <typename F>
-static auto dispatch(uint32_t mode, bool lights, int minb, F&& f) {
-    // the validation modes exist in one register budget only
-    if (mode == MODE_EXACT) return lights ? f(rt_wavefront_kernel<2, MODE_EXACT, true>) : f(rt_wavefront_kernel<2, MODE_EXACT, false>);
-    if (mode == MODE_BRUTE) return lights ? f(rt_wavefront_kernel<2, MODE_BRUTE, true>) : f(rt_wavefront_kernel<2, MODE_BRUTE, false>);
-    if (minb >= 4) return lights ? f(rt_wavefront_kernel<4, MODE_TREE, true>) : f(rt_wavefront_kernel<4, MODE_TREE, false>);
-    if (minb >= 3) return lights ? f(rt_wavefront_kernel<3, MODE_TREE, true>) : f(rt_wavefront_kernel<3, MODE_TREE, false>);
-    return lights ? f(rt_wavefront_kernel<2, MODE_TREE, true>) : f(rt_wavefront_kernel<2, MODE_TREE, false>);
+static auto dispatch(uint32_t mode, bool lights, F&& f) {
+    if (mode == MODE_EXACT) return lights ? f(rt_wavefront_kernel<MODE_EXACT, true>) : f(rt_wavefront_kernel<MODE_EXACT, false>);
+    if (mode == MODE_BRUTE) return lights ? f(rt_wavefront_kernel<MODE_BRUTE, true>) : f(rt_wavefront_kernel<MODE_BRUTE, false>);
+    return lights ? f(rt_wavefront_kernel<MODE_TREE, true>) : f(rt_wavefront_kernel<MODE_TREE, false>);
 }
 
-cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, int grid, size_t smem, int minb, cudaStream_t st) {
-    return dispatch(mode, p.n_lights > 0, minb, [&](auto kern) -> cudaError_t {
+cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, int grid, size_t smem, cudaStream_t st) {
+    return dispatch(mode, p.n_lights > 0, [&](auto kern) -> cudaError_t {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
         kern<<<grid, kBlock, smem, st>>>(p);
@@ -203,8 +207,8 @@ cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, int grid, size
     });
 }
 
-int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, size_t smem, int minb) {
-    return dispatch(mode, lights, minb, [&](auto kern) -> int {
+int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, size_t smem) {
+    return dispatch(mode, lights, [&](auto kern) -> int {
         int nb = 0;
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return 0; }
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kBlock, smem) != cudaSuccess) { cudaGetLastError(); return 0; }
@@ -212,13 +216,13 @@ int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, size_t smem, int minb)
     });
 }
 
-cudaError_t wavefront_info(uint32_t mode, bool lights, int minb, KernelInfo* out) {
-    return dispatch(mode, lights, minb, [&](auto kern) -> cudaError_t {
+cudaError_t wavefront_info(uint32_t mode, bool lights, KernelInfo* out) {
+    return dispatch(mode, lights, [&](auto kern) -> cudaError_t {
         cudaFuncAttributes a;
         cudaError_t e = cudaFuncGetAttributes(&a, kern);
         if (e != cudaSuccess) return e;
         out->registers = a.numRegs; out->max_threads = a.maxThreadsPerBlock; out->const_bytes = (int)a.constSizeBytes; out->local_bytes = (int)a.localSizeBytes;
-        snprintf(out->name, sizeof out->name, "rt_wavefront_kernel<%d,%s,%s>", mode == MODE_TREE ? (minb >= 4 ? 4 : minb >= 3 ? 3 : 2) : 2,
+        snprintf(out->name, sizeof out->name, "rt_wavefront_kernel<%s,%s>",
                  mode == MODE_TREE ? "MODE_TREE" : mode == MODE_BRUTE ? "MODE_BRUTE" : "MODE_EXACT", lights ? "LIGHTS" : "NO_LIGHTS");
         return cudaSuccess;
     });

@@ -228,6 +228,21 @@ def test_resident_scene_renders_into_device_buffers():
     rs.release()
 
 
+@pytest.mark.parametrize("variant", [R.RT_VARIANT_FILTERED, R.RT_VARIANT_EXACT_F64, R.RT_VARIANT_BRUTE_FORCE])
+def test_resident_scene_launch_shape(variant):
+    """Persistent grid = every SM x the resident CTAs of the variant's kernel; the BVH path runs 3 CTAs of 80 registers."""
+    import torch
+    rs = R.ResidentScene(scenes.cover_scene(32, 24, 1), R.make_options(variant=variant))
+    ki = rs.kernel_info()
+    rs.release()
+    sms = torch.cuda.get_device_properties(torch.cuda.current_device()).multi_processor_count
+    assert ki["grid"] == sms * ki["ctas_per_sm"] and ki["smem_mask"] == 0
+    if variant == R.RT_VARIANT_FILTERED:
+        assert ki["ctas_per_sm"] == 3 and ki["registers"] == 80
+    else:
+        assert ki["ctas_per_sm"] >= 1
+
+
 def test_retired_variant_reports_an_error_not_a_wrong_image():
     cfg = mixed_config(16, 12, 1, 4, seed=1)
     with pytest.raises(R.RtError) as e:

@@ -7,7 +7,7 @@ usage: ncu_stages.py <rep> [kernel-substr] [lib.so]"""
 import collections, csv, os, re, subprocess, sys, tempfile
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 rep = sys.argv[1]
-kname = sys.argv[2] if len(sys.argv) > 2 else "rt_wavefront_kernelILi3ELj0ELb0"
+kname = sys.argv[2] if len(sys.argv) > 2 else "rt_wavefront_kernelILj0ELb0"
 lib = sys.argv[3] if len(sys.argv) > 3 else os.path.join(REPO, "rust-raytracer_b200", "librtb200.so")
 WF = os.path.join(REPO, "rust-raytracer_b200", "csrc", "rtb200_wavefront.cu")
 TR = os.path.join(REPO, "rust-raytracer_b200", "csrc", "rtb200_trace.cuh")

@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Frame-loop timing of ONE GPU's share of an N-GPU run (shard 0 of `world`), pipelined over two streams like
-rtb200/dist.py, without NCCL: what the async grid size does to the step time. usage: pipeline_probe.py [C2] [world] [frames]"""
+rtb200/dist.py, without NCCL. usage: pipeline_probe.py [C2] [world] [frames]"""
 import sys, os
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, os.path.join(REPO, 'rust-raytracer_b200'))
@@ -29,4 +29,4 @@ e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=Tr
 e0.record(); loop(frames); e1.record(); torch.cuda.synchronize()
 st = rs.wait()
 ms = e0.elapsed_time(e1) / frames
-print(f"{name} shard 0 of {world}: {ms:.3f} ms/frame pipelined, {st['rays'] / ms / 1e3:.0f} Mrays/s per GPU (RTB200_ASYNC_CTAS={os.environ.get('RTB200_ASYNC_CTAS', 'default')})", flush=True)
+print(f"{name} shard 0 of {world}: {ms:.3f} ms/frame pipelined, {st['rays'] / ms / 1e3:.0f} Mrays/s per GPU", flush=True)

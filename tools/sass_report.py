@@ -1,6 +1,6 @@
 #!/usr/bin/env python3
 """Static report of the built librtb200.so (no GPU needed): ptxas resource lines of every kernel from the build log and the
-SASS mnemonic mix of one kernel (default: the shipped rt_wavefront_kernel<3,MODE_TREE,no lights>).
+SASS mnemonic mix of one kernel (default: the shipped rt_wavefront_kernel<MODE_TREE,no lights>).
 
     python tools/sass_report.py [substring-of-mangled-name] > sass_static.txt
 """
@@ -8,7 +8,7 @@ import collections, os, re, subprocess, sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PKG = os.path.join(ROOT, "rust-raytracer_b200")
-want = sys.argv[1] if len(sys.argv) > 1 else "rt_wavefront_kernelILi3ELj0ELb0"
+want = sys.argv[1] if len(sys.argv) > 1 else "rt_wavefront_kernelILj0ELb0"
 
 print("== ptxas resource usage (rust-raytracer_b200/build.log, -Xptxas -v) ==")
 log = open(os.path.join(PKG, "build.log")).read().splitlines()

@@ -369,6 +369,7 @@ static int scene_upload_records(const rt_scene* s, const rt_options& opts, uint3
     upload_array(h, R.nodes.data(), R.nodes.size() * 4, (void**)&tp.nodes);
     upload_array(h, R.leaf_rec.data(), R.leaf_rec.size() * 4, (void**)&tp.leaf_rec);
     upload_array(h, R.leaf_id.data(), R.leaf_id.size() * 4, (void**)&tp.leaf_id);
+    upload_array(h, R.skip_pos.data(), R.skip_pos.size() * 4, (void**)&tp.skip_pos);
     upload_array(h, R.always.data(), R.always.size() * 4, (void**)&tp.always);
     if (h->mode == MODE_BRUTE) upload_array(h, R.flat.data(), R.flat.size() * 4, (void**)&tp.filt);
     upload_array(h, R.geo.data(), R.geo.size() * 8, (void**)&tp.geo);
@@ -588,10 +589,11 @@ static int render_collect(rtb200_scene_handle h, rt_stats* stats) {
                 fprintf(stderr, "[rtb200] fallbacks=%llu; no phase clocks: this library was built without RT_PHASE_CLOCKS (make -C rust-raytracer_b200 phase)\n", hstat[2]);
             } else {
                 const double it = (double)ph[PH_ITERS];
-                fprintf(stderr, "[rtb200] fallbacks=%llu phases (clock64 cycles per warp iteration): closest_hit=%.0f sort+waitA=%.0f shade=%.0f regen=%.0f waitC=%.0f; "
-                        "warp_iters=%llu scatters=%llu deferred=%llu (%.4f of scatters)\n",
-                        hstat[2], ph[PH_HIT] / it, ph[PH_SORT_WAIT_A] / it, ph[PH_SHADE] / it, ph[PH_REGEN] / it, ph[PH_WAIT_C] / it,
-                        ph[PH_ITERS], ph[PH_SCATTERS], ph[PH_DEFERRED], (double)ph[PH_DEFERRED] / (double)std::max(1ull, ph[PH_SCATTERS]));
+                fprintf(stderr, "[rtb200] fallbacks=%llu phases (clock64 cycles per warp iteration): closest_hit=%.0f (node steps %.0f, leaf steps %.0f, exact steps %.0f) sort+waitA=%.0f shade=%.0f regen=%.0f waitC=%.0f; "
+                        "warp_iters=%llu scatters=%llu deferred=%llu (%.4f of scatters); exact steps=%llu (%.2f per warp iteration) exact tests=%llu source-sphere skips=%llu rays=%llu\n",
+                        hstat[2], ph[PH_HIT] / it, ph[PH_NODE] / it, ph[PH_LEAF] / it, ph[PH_EXACT] / it, ph[PH_SORT_WAIT_A] / it, ph[PH_SHADE] / it, ph[PH_REGEN] / it, ph[PH_WAIT_C] / it,
+                        ph[PH_ITERS], ph[PH_SCATTERS], ph[PH_DEFERRED], (double)ph[PH_DEFERRED] / (double)std::max(1ull, ph[PH_SCATTERS]),
+                        ph[PH_EXACT_STEPS], ph[PH_EXACT_STEPS] / it, ph[PH_EXACT_TESTS], ph[PH_SRC_SKIPS], hstat[0]);
             }
         }
         if (h->tp.max_depth == 0) stats->samples = (uint64_t)h->tp.npix_local * h->tp.spp;   // no kernel ran: every sample is black

@@ -50,6 +50,10 @@ struct Records {
     std::vector<float> leaf_rec;      // n_leaves * kLeafK * 4
     std::vector<uint32_t> leaf_id;    // n_leaves * kLeafK, 0xffffffff = padding slot
     std::vector<uint32_t> always;     // spheres tested in f64 for every ray
+    // max(n,1): sphere -> where the traversal leaves it out for a ray that starts on it (rtk::kNoSkip etc.):
+    // 0x80000000 | node * kWide + child when it is the only member of that child leaf, else its leaf_id index
+    // leaf * kLeafK + slot, or 0xffffffff when it is in no leaf
+    std::vector<uint32_t> skip_pos;
     uint32_t n_pairs = 0;
     std::vector<float> flat;          // n_pairs * 8: every sphere, list order, pair-packed (padding never hits)
     std::vector<double> geo;          // max(n,1) * 4
@@ -348,6 +352,20 @@ private:
 inline void build_records(const rt_scene* s, bool want_tree, Records& R) {
     Builder b(s, R);
     b.run(want_tree);
+    R.skip_pos.assign(std::max<uint32_t>(R.n, 1), 0xffffffffu);   // every sphere is in one leaf at most
+    for (size_t k = 0; k < R.leaf_id.size(); ++k) if (R.leaf_id[k] < R.n) R.skip_pos[R.leaf_id[k]] = (uint32_t)k;
+    // a leaf with a single member is dropped by its parent node instead: the leaf step is then not run at all
+    for (uint32_t node = 0; node < R.n_nodes; ++node) {
+        for (int c = 0; c < kWide; ++c) {
+            uint32_t ref;
+            std::memcpy(&ref, &R.nodes[(size_t)node * kNodeFloats + 48 + c], 4);
+            if (ref == 0xffffffffu || !(ref & 0x80000000u)) continue;
+            const uint32_t* ids = &R.leaf_id[(size_t)(ref & 0x7fffffffu) * kLeafK];
+            int members = 0;
+            for (int j = 0; j < kLeafK; ++j) members += ids[j] != 0xffffffffu;
+            if (members == 1 && ids[0] < R.n) R.skip_pos[ids[0]] = 0x80000000u | (node * (uint32_t)kWide + (uint32_t)c);
+        }
+    }
 }
 
 }  // namespace rtbvh

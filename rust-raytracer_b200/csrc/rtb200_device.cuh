@@ -140,6 +140,24 @@ RT_DEV bool sphere_root(D3 center, double radius, D3 o, D3 d, double a, double t
     return false;
 }
 
+// Certificate for a ray that starts on the sphere (center, radius), a = length_squared(d): true only when sphere_root(center,
+// radius, o, d, a, 0.001, t_max) provably finds no root, decided with sphere_root's own rounded oc, half_b, c and a but
+// without its square root and divisions (proof in DESIGN.md §4.2). half_b >= 0 (the ray leaves the centre behind) and
+// c >= 0 (the origin rounded onto or outside the sphere): disc <= fl(half_b^2), whose rounded square root is half_b, so
+// both roots are <= 0. c < 0 (rounded just inside): the far root is below fl(a|c|) / (2 half_b a) + 3u half_b / a, and
+// the test bounds it by 0.0009 < t_min with room for every rounding. Inward rays (half_b < 0) are never certified.
+RT_DEV bool leaves_sphere(D3 center, double radius, D3 o, D3 d, double a) {
+    const D3 oc = sub(o, center);
+    const double half_b = dot(oc, d);
+    const double cc = __dsub_rn(length_squared(oc), __dmul_rn(radius, radius));
+    // every product below is a normal finite double; NaNs fail these comparisons
+    if (!(half_b >= 0x1p-300 && half_b <= 0x1p300 && a >= 0x1p-300 && a <= 0x1p300)) return false;
+    if (cc >= 0.0) return true;
+    if (!(cc <= -0x1p-300 && cc >= -0x1p300)) return false;
+    // fl(a |c|) + 2^-48 fl(half_b^2) <= fl(fl(0.0018 a) half_b)
+    return __dadd_rn(__dmul_rn(a, -cc), __dmul_rn(0x1p-48, __dmul_rn(half_b, half_b))) <= __dmul_rn(__dmul_rn(0.0018, a), half_b);
+}
+
 // Two spheres at once: the same operations in the same order per sphere, with the two dependent f64 chains interleaved
 // (the confirmation stage is latency-bound). Root selection as in sphere_root with t_max = +max.
 RT_DEV void sphere_root2(D3 c0, double r0, D3 c1, double r1, D3 o, D3 d, double a, double t_min, bool& h0, double& root0, bool& h1, double& root1) {

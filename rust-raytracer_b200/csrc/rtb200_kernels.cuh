@@ -16,8 +16,11 @@ constexpr int kBlock = RT_BLOCK;   // threads (= ray slots) per CTA of the trace
 #define RT_PHASE_CLOCKS 0          // 1: the trace kernel accounts its stages per warp (Makefile target `phase`, RTB200_PRINT_PHASES)
 #endif
 // stat[kPhaseStat + k] of an RT_PHASE_CLOCKS build: clock64() cycles of each stage summed over warps (k < PH_ITERS), warp
-// iterations, diffuse / metal vertices shaded (scatter attempts), and those of them whose scatter sample was deferred
-enum : uint32_t { PH_HIT, PH_SORT_WAIT_A, PH_SHADE, PH_REGEN, PH_WAIT_C, PH_ITERS, PH_SCATTERS, PH_DEFERRED, kPhaseN };
+// iterations, diffuse / metal vertices shaded (scatter attempts), and those of them whose scatter sample was deferred; then
+// the cycles of closest-hit's node, leaf and exact steps (part of PH_HIT), the exact steps, the (ray, sphere) tests they
+// ran, and the source spheres the node and leaf steps left out because the certificate proved the exact test rejects them
+enum : uint32_t { PH_HIT, PH_SORT_WAIT_A, PH_SHADE, PH_REGEN, PH_WAIT_C, PH_ITERS, PH_SCATTERS, PH_DEFERRED,
+                  PH_NODE, PH_LEAF, PH_EXACT, PH_EXACT_STEPS, PH_EXACT_TESTS, PH_SRC_SKIPS, kPhaseN };
 constexpr uint32_t kPhaseStat = 13;
 #ifndef RT_LEAF_K
 #define RT_LEAF_K 8
@@ -59,6 +62,7 @@ struct TraceParams {
     const float4*   nodes;       // n_nodes * kNodeVec: lo_x[8] lo_y[8] lo_z[8] hi_x[8] hi_y[8] hi_z[8] child[8], f32 boxes rounded outwards
     const float4*   leaf_rec;    // n_leaves * kLeafK float4: kLeafK/2 pair-packed sphere records {cx0,cx1,cy0,cy1},{cz0,cz1,nk0,nk1}
     const uint32_t* leaf_id;     // n_leaves * kLeafK: slot -> ORIGINAL sphere index (0xffffffff = padding)
+    const uint32_t* skip_pos;    // n: where the traversal can leave the sphere out (rtbvh::Records::skip_pos, rtk::kNoSkip)
     const uint32_t* always;      // n_always sphere indices tested in f64 for every ray (not representable in the f32 frame)
     const float4*   filt;        // n_pairs * 2 float4: every sphere in list order, pair-packed (MODE_BRUTE)
     const double4*  geo;         // n: {cx,cy,cz,radius} exact f64

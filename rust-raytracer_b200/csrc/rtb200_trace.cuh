@@ -37,12 +37,19 @@ constexpr uint32_t kDeadLevel = 0xffffffffu;
 constexpr uint32_t kScatterPending = 0x80000000u;
 constexpr uint32_t kLeafBit = 0x80000000u;
 constexpr unsigned long long kNoHitBits = 0x7ff0000000000000ull;   // +inf as the "no root yet" key (roots are > t_min > 0)
-constexpr uint32_t kSlotBytes = 7 * 8 + 9 * 4 + RT_SMEM_STACK * 4;   // shared memory per pool slot
+constexpr uint32_t kNoSphere = 0xffffffffu;     // Pool.src: the ray does not start on a known sphere
+// skip_pos / WarpCtx.skip: where the traversal leaves the certified source sphere out. kSkipNodeBit | node * 8 + child: the
+// node step drops child `child` of `node` (a leaf holding only that sphere); else leaf * kLeafK + slot: the leaf step drops
+// the slot. kNoSkip: nothing (kNoSkip / kLeafK and (kNoSkip & ~kSkipNodeBit) / 8 are no leaf's or node's index, < 2^27).
+constexpr uint32_t kSkipNodeBit = 0x80000000u;
+constexpr uint32_t kNoSkip = 0xffffffffu;
+constexpr uint32_t kSlotBytes = 7 * 8 + 10 * 4 + RT_SMEM_STACK * 4;   // shared memory per pool slot
 
 // SoA ray pool of a CTA: n_slots slots.
 struct Pool {
     double *ox, *oy, *oz, *dx, *dy, *dz, *bt;                    // ray origin / direction, best root (also updated as u64 bits)
     uint32_t *bi, *work, *pix, *smp, *blk, *clo, *chi, *lvl, *shd;   // hit index, work id, RNG (pixel, sample, block|has, cached draw), path level, shadow depth | kScatterPending
+    uint32_t *src;                                               // the sphere the ray starts on (kNoSphere: a primary ray, or not known)
     uint32_t *stk;                                               // [RT_SMEM_STACK][n_slots] first levels of the albedo stack
     uint32_t n_slots;
     uint32_t stack_col;                                          // this CTA's first column of the global per-slot arrays (stack / frames / lterm)
@@ -53,7 +60,7 @@ RT_DEV Pool pool_at(unsigned char* base, uint32_t n_slots, uint32_t stack_col) {
     P.ox = d; P.oy = d + n_slots; P.oz = d + 2 * n_slots; P.dx = d + 3 * n_slots; P.dy = d + 4 * n_slots; P.dz = d + 5 * n_slots; P.bt = d + 6 * n_slots;
     uint32_t* u = reinterpret_cast<uint32_t*>(d + 7 * n_slots);
     P.bi = u; P.work = u + n_slots; P.pix = u + 2 * n_slots; P.smp = u + 3 * n_slots; P.blk = u + 4 * n_slots; P.clo = u + 5 * n_slots;
-    P.chi = u + 6 * n_slots; P.lvl = u + 7 * n_slots; P.shd = u + 8 * n_slots; P.stk = u + 9 * n_slots;
+    P.chi = u + 6 * n_slots; P.lvl = u + 7 * n_slots; P.shd = u + 8 * n_slots; P.src = u + 9 * n_slots; P.stk = u + 10 * n_slots;
     P.n_slots = n_slots; P.stack_col = stack_col;
     return P;
 }
@@ -61,13 +68,15 @@ RT_DEV Pool pool_at(unsigned char* base, uint32_t n_slots, uint32_t stack_col) {
 // per-warp scratch of the closest-hit stage
 struct WarpCtx {
     float4 *cA, *cB, *cC;          // [32] per-ray f32 constants: {o.xyz, slab margin}, {1/d^.xyz, thr}, {d^.xyz, -o.d^}
+    uint32_t *skip;                // [32] per ray: skip_pos of the certified source sphere, or kNoSkip
     uint32_t *l_in, *l_lf, *l_cd;  // work lists: (ray, node), (ray, leaf), (ray, sphere); entries id << 5 | ray
 };
-constexpr uint32_t kWarpCtxBytes = 3 * 32 * 16 + (uint32_t)(kCapIn + kCapLf + kCapCd) * 4;
+constexpr uint32_t kWarpCtxBytes = 3 * 32 * 16 + 32 * 4 + (uint32_t)(kCapIn + kCapLf + kCapCd) * 4;
 RT_DEV WarpCtx warpctx_at(unsigned char* base) {
     WarpCtx W;
     W.cA = reinterpret_cast<float4*>(base); W.cB = W.cA + 32; W.cC = W.cB + 32;
-    W.l_in = reinterpret_cast<uint32_t*>(W.cC + 32); W.l_lf = W.l_in + kCapIn; W.l_cd = W.l_lf + kCapLf;
+    W.skip = reinterpret_cast<uint32_t*>(W.cC + 32);
+    W.l_in = W.skip + 32; W.l_lf = W.l_in + kCapIn; W.l_cd = W.l_lf + kCapLf;
     return W;
 }
 
@@ -76,7 +85,13 @@ struct SceneRefs {
     const double4* geo; const DevMat* mat;
 };
 
-struct Stats { uint32_t rays = 0, cand = 0, ovf = 0, samples = 0, leaves = 0, nodes = 0; };   // per thread and launch: far below 2^32
+struct Stats {   // per thread and launch: far below 2^32
+    uint32_t rays = 0, cand = 0, ovf = 0, samples = 0, leaves = 0, nodes = 0;
+#if RT_PHASE_CLOCKS
+    unsigned long long t_node = 0, t_leaf = 0, t_exact = 0;   // lane 0: clock64() cycles of the warp's node / leaf / exact steps
+    uint32_t exact_steps = 0, exact_tests = 0, src_skips = 0;
+#endif
+};
 
 RT_DEV void bulk_stage(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
     const uint32_t CH = 32768u;
@@ -184,6 +199,17 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
             W.cA[lane] = make_float4(ofx, ofy, ofz, mray);
             W.cB[lane] = make_float4(__frcp_rn(ax), __frcp_rn(ay), __frcp_rn(az), thr);
             W.cC[lane] = make_float4(dnx, dny, dnz, nod);
+            // The sphere the ray starts on is left out of its candidates when a cheap f64 certificate proves that the exact
+            // test rejects it (a ray leaving the surface outwards; DESIGN.md §4.2). The certificate is evaluated on this ray's
+            // own o and d, so even a wrong Pool.src could only cost a missed skip, never a wrong hit.
+            uint32_t skp = kNoSkip;
+            const uint32_t src = alive ? P.src[slot] : kNoSphere;
+            if (src != kNoSphere) {
+                const uint32_t pos = p.skip_pos[src];
+                const double4 gs = sc.geo[src];
+                if (pos != kNoSkip && leaves_sphere(mk(gs.x, gs.y, gs.z), gs.w, o, d, a)) skp = pos;
+            }
+            W.skip[lane] = skp;
             // LIFO reserve: single-entry descents grow the node stack by at most 7 per level, so multi-entry steps may fill it
             // only up to fat_in; above that the stack is popped one entry at a time and can never overflow (DESIGN.md §4.1).
             const uint32_t fat_in = (uint32_t)kCapIn - 7u * p.depth - 8u;
@@ -195,6 +221,9 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
             __syncwarp();
             uint32_t guard = 0;
             for (;;) {
+#if RT_PHASE_CLOCKS
+                const unsigned long long t_step = clock64();
+#endif
                 if (n_in != 0u && n_lf <= (uint32_t)(kCapLf - 64)) {
                     // ---------------- node step: lane <-> one (ray, node) pair from the top of the stack ----------------
                     const uint32_t m = n_in < 32u ? n_in : 32u;
@@ -236,6 +265,15 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                         leafbits = (R0.x >> 31) | ((R0.y >> 31) << 1) | ((R0.z >> 31) << 2) | ((R0.w >> 31) << 3) |
                                    ((R1.x >> 31) << 4) | ((R1.y >> 31) << 5) | ((R1.z >> 31) << 6) | ((R1.w >> 31) << 7);
                     }
+                    {   // a leaf that holds nothing but the certified source sphere is not visited at all
+                        const uint32_t sk = W.skip[ray] ^ (kSkipNodeBit | node << 3);   // < 8: the child to drop
+                        if (sk < 8u) {
+#if RT_PHASE_CLOCKS
+                            st.src_skips += (hit >> sk) & 1u;
+#endif
+                            hit &= ~(1u << sk);
+                        }
+                    }
                     const uint32_t packed = (uint32_t)__popc(hit & ~leafbits) | ((uint32_t)__popc(hit & leafbits) << 16);
                     const uint32_t inc = warp_scan_incl(packed, lane);
                     // commit the longest prefix of lanes (top of the stack first) whose pushes fit
@@ -264,6 +302,9 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                     n_in = n_in - k + (tot & 0xffffu);
                     n_lf += tot >> 16;
                     __syncwarp();
+#if RT_PHASE_CLOCKS
+                    if (lane == 0) st.t_node += clock64() - t_step;
+#endif
                 } else if (n_lf != 0u && n_cd <= (uint32_t)(kCapCd - 32)) {
                     // ---------------- leaf step: lane <-> one (ray, leaf) pair: conservative sphere test on its spheres ----------------
                     const uint32_t m = n_lf < 32u ? n_lf : 32u;
@@ -282,6 +323,14 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                         RT_FILTER_PAIRS(rec, Dv, kLeafK / 2)
 #pragma unroll
                         for (int q = 0; q < kLeafK / 2; ++q) hit |= (Dv[q].x >= th ? 1u : 0u) << (2 * q) | (Dv[q].y >= th ? 1u : 0u) << (2 * q + 1);
+                        // the sphere the ray starts on, when its certificate proved that the exact test rejects it
+                        const uint32_t sk = W.skip[ray];
+                        if (sk / (uint32_t)kLeafK == leaf) {
+#if RT_PHASE_CLOCKS
+                            st.src_skips += (hit >> (sk % (uint32_t)kLeafK)) & 1u;
+#endif
+                            hit &= ~(1u << (sk % (uint32_t)kLeafK));
+                        }
                     }
                     const uint32_t cntc = (uint32_t)__popc(hit);
                     const uint32_t inc = warp_scan_incl(cntc, lane);
@@ -305,6 +354,9 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                     n_lf -= k;
                     n_cd += tot;
                     __syncwarp();
+#if RT_PHASE_CLOCKS
+                    if (lane == 0) st.t_leaf += clock64() - t_step;
+#endif
                 } else if (n_cd != 0u) {
                     // ---------------- exact step: lane <-> one (ray, sphere) candidate, reference-exact f64 Sphere::hit ----------------
                     const uint32_t m = n_cd < 32u ? n_cd : 32u;
@@ -318,6 +370,9 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                         double root;
                         if (sphere_root(mk(gq.x, gq.y, gq.z), gq.w, ro, rd, length_squared(rd), 0.001, DBL_MAX, root)) key = (unsigned long long)__double_as_longlong(root);
                         ++st.cand;
+#if RT_PHASE_CLOCKS
+                        ++st.exact_tests;
+#endif
                     }
                     // per-ray lexicographic minimum of (root, sphere index): roots are positive, so their bit patterns order like the values
                     const bool h = key != ~0ull;
@@ -331,6 +386,9 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                     if (mine) atomicMin(&P.bi[rs], sph);
                     n_cd -= m;
                     __syncwarp();
+#if RT_PHASE_CLOCKS
+                    if (lane == 0) { st.t_exact += clock64() - t_step; ++st.exact_steps; }
+#endif
                 } else {
                     break;
                 }
@@ -423,6 +481,7 @@ RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint
     P.blk[s] = (rng.blk << 1) | rng.has; P.clo[s] = rng.c_lo; P.chi[s] = rng.c_hi;
     P.lvl[s] = 0u;
     P.shd[s] = 0u;
+    P.src[s] = kNoSphere;
     if (LIGHTS) {
         for (int q = 0; q < 6; ++q) p.lterm[(size_t)q * p.stack_stride + P.stack_col + s] = 0.0f;
     }
@@ -539,12 +598,13 @@ RT_DEV bool shade_slot(const TraceParams& p, const SceneRefs& sc, const Pool& P,
                 ++shd;
                 double4 lq = geo[p.lights[0]];
                 o = h.point; d = sub(mk(lq.x, lq.y, lq.z), h.point);   // Ray::new(point, light.center - point)
+                P.src[s] = best;
             } else if (shd == 0u) {
                 if (is_light) { cr = 1.f; cg = 1.f; cb = 1.f; done = true; }   // `None => albedo` (raytracer.rs:124)
                 else {
                     stack_push(level, code);
                     ++level;
-                    o = h.point; d = nd;
+                    o = h.point; d = nd; P.src[s] = best;
                     if (level == p.max_depth) done = true;   // the next ray_color call returns black (raytracer.rs:80-82)
                 }
             } else {
@@ -565,6 +625,7 @@ RT_DEV bool shade_slot(const TraceParams& p, const SceneRefs& sc, const Pool& P,
                 p.frames[(size_t)(shd - 1u) * p.stack_stride + col] = f;
                 double4 lq = geo[p.lights[f.li]];
                 o = mk(f.px, f.py, f.pz); d = sub(mk(lq.x, lq.y, lq.z), o);
+                P.src[s] = kNoSphere;   // reading the frame's sphere here made the LIGHTS kernel spill 116 B instead of 76 B
                 have_tc = false;
             } else {
                 const float nl = (float)p.n_lights;
@@ -580,6 +641,7 @@ RT_DEV bool shade_slot(const TraceParams& p, const SceneRefs& sc, const Pool& P,
                         stack_push(level, f.code);
                         ++level;
                         o = mk(f.px, f.py, f.pz); d = mk(f.ndx, f.ndy, f.ndz);
+                        P.src[s] = kNoSphere;
                         if (level == p.max_depth) done = true;
                     }
                 } else if (f.is_light) { tr = tg = tb = 1.f; }
@@ -633,6 +695,18 @@ RT_DEV void flush_stats(const TraceParams& p, const Stats& st, int lane) {
         atomicAdd(&p.stat[4], v[4]);
         atomicAdd(&p.stat[6], v[5]);
     }
+#if RT_PHASE_CLOCKS
+    unsigned long long w[6] = {st.t_node, st.t_leaf, st.t_exact, st.exact_steps, st.exact_tests, st.src_skips};
+#pragma unroll
+    for (int k = 0; k < 6; ++k) {
+#pragma unroll
+        for (int off = 16; off > 0; off >>= 1) w[k] += __shfl_down_sync(0xffffffffu, w[k], off);
+    }
+    if (lane == 0) {
+#pragma unroll
+        for (int k = 0; k < 6; ++k) atomicAdd(&p.stat[kPhaseStat + PH_NODE + k], w[k]);
+    }
+#endif
 }
 
 }  // namespace rtk

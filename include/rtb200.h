@@ -190,6 +190,36 @@ int rtb200_render_device_wait(rtb200_scene_handle h, rt_stats* stats);
 int rtb200_scene_release(rtb200_scene_handle h);
 int rtb200_scene_kernel_info(rtb200_scene_handle h, rt_kernel_info* out);
 
+/* ---- animations: many frames of one scene ------------------------------------------------------------------------------
+ * One frame of an animation over a resident scene: the view, the RNG key and the depth that replace the scene's own. */
+typedef struct {
+    rt_camera camera;     /* Camera::new of this frame's CameraParams (rtb200_camera_from_params) */
+    uint64_t  seed;       /* Philox key of this frame, as rt_scene.seed */
+    uint32_t  max_depth;  /* as rt_scene.max_depth (0 = black frame, no ray) */
+    uint32_t  reserved;   /* must be 0 */
+} rt_frame;               /* 112 bytes */
+
+/* Render n_frames frames of one scene. Frame i is bit-identical, in linear f32 and RGB8, to rtb200_render_rgb8 /
+ * rtb200_render_linear_f32 of the scene with camera, seed and max_depth taken from frames[i]; the scene's own camera, seed
+ * and max_depth are ignored, its size, samples_per_pixel, sky, spheres and textures are shared by all frames. Shards
+ * (opts->rank/world/band_rows) and every variant work as for one frame.
+ * Outputs are frame-major and contiguous: n_frames * rows * width * 3 (rows = rtb200_shard_rows(...) for a shard); either may
+ * be NULL, not both. Consecutive frames with equal max_depth whose samples fit the sample-buffer cap together
+ * (F * samples_per_pixel * rows * width * 16 bytes <= opts->sample_buffer_bytes) are traced by ONE persistent launch whose work
+ * queue spans all of them, so that only the last frame of a launch waits for its slowest paths; frames of more than 2^24
+ * samples (samples_per_pixel * rows * width) are long enough to hide their own tail and are traced one launch each.
+ * stats: rays and samples are sums over the frames; frames = n_frames; batches = trace launches (or black max_depth 0 batches);
+ * kernel_launches = trace + resolve launches. RT_ERR_INVALID, before any device is touched, for n_frames == 0, a NULL frames,
+ * a nonzero rt_frame.reserved or n_frames * rows * width * 3 overflowing 64 bits.
+ * rtb200_render_frames uploads the scene, renders, copies back and releases, like rtb200_render_rgb8. */
+int rtb200_render_frames(const rt_scene* scene, const rt_options* opts, const rt_frame* frames, uint32_t n_frames,
+                         uint8_t* out_rgb8, float* out_linear_f32, rt_stats* stats);
+/* The same on a resident scene into DEVICE buffers. Blocking: drains the handle's asynchronous frames first, uploads the frame
+ * table on `stream` (NULL: the library's stream) and returns when the frames are done. The handle's own view is unchanged:
+ * a later rtb200_render_device renders the camera it was uploaded with. */
+int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, uint32_t n_frames,
+                                void* dev_rgb8, void* dev_linear_f32, void* stream, rt_stats* stats);
+
 /* load_texture_image — materials.rs:213-219, config.rs:36-47: decode a baseline JPEG file to RGB8 (host-side scene staging
  * helper for hosts without their own decoder; the reference uses the jpeg-decoder crate). *out_rgb8 is released with rtb200_free(). */
 int  rtb200_decode_jpeg_file(const char* path, uint8_t** out_rgb8, uint64_t* width, uint64_t* height);

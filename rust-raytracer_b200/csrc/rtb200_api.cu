@@ -73,13 +73,13 @@ struct DeviceCtx {
     cudaStream_t stream = nullptr;
     // Two sets of per-frame work buffers: a frame loop that alternates two streams lets frame k+1 start tracing while frame k
     // drains its last paths and resolves (rtb200_render_device_async); blocking calls use set 0 only.
-    struct WorkSet { GrowBuf samplebuf, accum, stack, small, frames, lterm; } ws[2];
+    struct WorkSet { GrowBuf samplebuf, accum, stack, small, frames, lterm, ftab; } ws[2];   // ftab: rtb200_render_frames_device's frame table
     GrowBuf out_rgb8, out_lin, probe, frame;
     // scene arenas of released handles, kept for the next upload (a per-frame upload costs no cudaMalloc / cudaFree)
     struct Arena { void* p; size_t cap; };
     std::vector<Arena> arena_cache;
     std::vector<cudaEvent_t> event_pool;  // timing events of released handles (creating four events per one-shot render costs more than the upload)
-    struct OccKey { uint32_t mode; bool lights; size_t smem; int occ; };
+    struct OccKey { uint32_t mode; bool lights, frames; size_t smem; int occ; };
     std::vector<OccKey> occ_cache;        // cudaOccupancyMaxActiveBlocksPerMultiprocessor answers
     PinnedBuf staging;                    // host image of the arena being uploaded
     cudaEvent_t staging_free = nullptr;   // the last H2D copy out of `staging` has finished
@@ -146,6 +146,14 @@ int guarded(F&& f) {
 
 uint32_t mode_of(uint32_t variant) {
     return variant == RT_VARIANT_EXACT_F64 ? MODE_EXACT : (variant == RT_VARIANT_BRUTE_FORCE ? MODE_BRUTE : MODE_TREE);
+}
+
+// resident CTAs per SM of one trace kernel with `smem` bytes of dynamic shared memory (cached per context)
+int occupancy(DeviceCtx* ctx, uint32_t mode, bool lights, bool frames, size_t smem) {
+    for (auto& k : ctx->occ_cache) if (k.mode == mode && k.lights == lights && k.frames == frames && k.smem == smem) return k.occ;
+    const int occ = wavefront_max_ctas_per_sm(mode, lights, frames, smem);
+    ctx->occ_cache.push_back(DeviceCtx::OccKey{mode, lights, frames, smem, occ});
+    return occ;
 }
 
 }  // namespace
@@ -409,13 +417,8 @@ static int scene_upload_records(const rt_scene* s, const rt_options& opts, uint3
     // records, bit1 geo, bit2 mat): for these small, hot arrays a larger L1 beats the staging (DESIGN.md §4.5).
     const char* es = getenv("RTB200_WF_SMEM");
     tp.scene_in_smem = es ? (uint32_t)atoi(es) : 0u;
-    h->smem = wavefront_smem_bytes(tp, h->mode, tp.scene_in_smem);
-    int occ = -1;
-    for (auto& k : ctx->occ_cache) if (k.mode == h->mode && k.lights == (n_lights > 0) && k.smem == h->smem) occ = k.occ;
-    if (occ < 0) {
-        occ = wavefront_max_ctas_per_sm(h->mode, n_lights > 0, h->smem);
-        ctx->occ_cache.push_back(DeviceCtx::OccKey{h->mode, n_lights > 0, h->smem, occ});
-    }
+    h->smem = wavefront_smem_bytes(tp, h->mode, tp.scene_in_smem, false);
+    const int occ = occupancy(ctx, h->mode, n_lights > 0, false, h->smem);
     if (occ <= 0) return fail(RT_ERR_UNSUPPORTED, "no launch configuration fits shared memory");
     h->ctas_per_sm = occ;
     h->grid = ctx->sm_count * occ;
@@ -457,12 +460,72 @@ int rtb200_scene_kernel_info(rtb200_scene_handle h, rt_kernel_info* out) {
     CU(cudaSetDevice(h->device));
     memset(out, 0, sizeof *out);
     KernelInfo ki{};
-    CU(wavefront_info(h->mode, h->tp.n_lights > 0, &ki));
+    CU(wavefront_info(h->mode, h->tp.n_lights > 0, false, &ki));
     out->registers = ki.registers; out->local_bytes = ki.local_bytes; out->smem_bytes = (uint32_t)h->smem; out->grid = (uint32_t)h->grid;
     out->block = (uint32_t)kBlock; out->pool_slots = (uint32_t)kBlock;
     out->ctas_per_sm = (uint32_t)h->ctas_per_sm; out->smem_mask = h->tp.scene_in_smem;
     out->bvh_nodes = h->tp.n_nodes; out->bvh_leaves = h->tp.n_leaves; out->bvh_depth = h->tp.depth;
     snprintf(out->name, sizeof out->name, "%s", ki.name);
+    return RT_OK;
+}
+
+// Work buffers of W for launches of up to `threads_total` threads that trace paths up to `max_depth` deep, stage up to
+// `samplebuf_bytes` of per-sample radiance and take `n_counters` queue counters; points tp at them (stack_stride excepted).
+static int prepare_work(DeviceCtx::WorkSet& W, TraceParams& tp, uint32_t threads_total, uint32_t max_depth,
+                        size_t samplebuf_bytes, uint32_t n_counters) {
+    CU(W.samplebuf.ensure(samplebuf_bytes));
+    CU(W.accum.ensure((size_t)tp.npix_local * 12));
+    CU(W.stack.ensure((size_t)std::max<uint32_t>(max_depth, 1) * threads_total * 4));
+    CU(W.small.ensure(256 + (size_t)n_counters * 4));
+    if (tp.n_lights > 0) {
+        // Nested light tests form a branching process: a vertex nests with probability 0.1 n and then spawns n shadow rays, so
+        // depth d is reached with probability ~(0.1 n^2 P_hit)^d: harmless for 1-2 lights, near-critical for 3 (the reference
+        // itself recurses hundreds of frames deep there) and super-critical beyond. Size the per-path frame stack accordingly;
+        // an overflow is reported as an error, never rendered wrongly.
+        tp.max_shadow = tp.n_lights == 1 ? 32u : tp.n_lights == 2 ? 96u : 384u;
+        CU(W.frames.ensure((size_t)tp.max_shadow * threads_total * sizeof(ShadowFrame)));
+        CU(W.lterm.ensure((size_t)6 * threads_total * 4));
+    }
+    tp.frames = (ShadowFrame*)W.frames.p;
+    tp.lterm = (float*)W.lterm.p;
+    tp.samplebuf = (float4*)W.samplebuf.p;
+    tp.stack = (uint32_t*)W.stack.p;
+    tp.stat = (unsigned long long*)W.small.p;
+    return RT_OK;
+}
+
+// Zero the stat block and the first n_counters queue counters of W.
+static int clear_stats(DeviceCtx::WorkSet& W, uint32_t n_counters, cudaStream_t st) {
+    CU(cudaMemsetAsync(W.small.p, 0, 256 + (size_t)n_counters * 4, st));
+    CU(cudaMemsetAsync((char*)W.small.p + 64, 0xff, 16, st));   // stat[8], stat[9]: minima (kernel start / first dry-queue time, ns)
+    return RT_OK;
+}
+
+// The sample batches of ONE frame: per batch a launch of the single-frame trace kernel (or, at max_depth 0, a black
+// memset) and a resolve. tp: the frame's parameters with every work buffer set; counters[b]: batch b's queue counter;
+// pair_ev[2b], pair_ev[2b+1] bracket batch b's trace launch.
+static int enqueue_batches(rtb200_scene_handle h, TraceParams tp, DeviceCtx::WorkSet& W, void* dev_rgb8, void* dev_linear_f32,
+                           unsigned int* counters, cudaEvent_t* pair_ev, cudaStream_t st) {
+    const uint32_t spp = tp.spp, spb = h->spp_batch;
+    const uint32_t n_batches = (spp + spb - 1) / spb;
+    for (uint32_t b = 0; b < n_batches; ++b) {
+        tp.s0 = b * spb;
+        tp.s_count = std::min(spb, spp - tp.s0);
+        tp.total_work = tp.s_count * tp.npix_local;
+        tp.work_counter = counters + b;
+        CU(cudaEventRecord(pair_ev[2 * b], st));
+        if (tp.max_depth == 0) {
+            CU(cudaMemsetAsync(tp.samplebuf, 0, (size_t)tp.total_work * 16, st));   // ray_color(depth 0) = black, no ray (raytracer.rs:80-82)
+        } else {
+            CU(launch_wavefront(tp, h->mode, false, h->grid, h->smem, st));
+        }
+        CU(cudaEventRecord(pair_ev[2 * b + 1], st));
+        ResolveParams q{};
+        q.samplebuf = tp.samplebuf; q.accum = (float*)W.accum.p; q.npix_local = tp.npix_local; q.s_count = tp.s_count;
+        q.first = b == 0; q.last = b + 1 == n_batches; q.spp = spp;
+        q.out_linear = (float*)dev_linear_f32; q.out_rgb8 = (uint8_t*)dev_rgb8;
+        CU(launch_resolve(q, st));
+    }
     return RT_OK;
 }
 
@@ -482,22 +545,9 @@ static int render_enqueue(rtb200_scene_handle h, void* dev_rgb8, void* dev_linea
     const uint32_t spp = tp.spp, spb = h->spp_batch;
     const uint32_t n_batches = (spp + spb - 1) / spb;
     const uint32_t threads_total = (uint32_t)h->grid * (uint32_t)kBlock;   // ray slots of the whole grid: columns of the per-slot global arrays
-
-    CU(W.samplebuf.ensure((size_t)spb * tp.npix_local * 16));
-    CU(W.accum.ensure((size_t)tp.npix_local * 12));
-    CU(W.stack.ensure((size_t)std::max<uint32_t>(tp.max_depth, 1) * threads_total * 4));
-    CU(W.small.ensure(256 + (size_t)n_batches * 4));
-    if (tp.n_lights > 0) {
-        // Nested light tests form a branching process: a vertex nests with probability 0.1 n and then spawns n shadow rays, so
-        // depth d is reached with probability ~(0.1 n^2 P_hit)^d: harmless for 1-2 lights, near-critical for 3 (the reference
-        // itself recurses hundreds of frames deep there) and super-critical beyond. Size the per-path frame stack accordingly;
-        // an overflow is reported as an error, never rendered wrongly.
-        tp.max_shadow = tp.n_lights == 1 ? 32u : tp.n_lights == 2 ? 96u : 384u;
-        CU(W.frames.ensure((size_t)tp.max_shadow * threads_total * sizeof(ShadowFrame)));
-        CU(W.lterm.ensure((size_t)6 * threads_total * 4));
-    }
-    tp.frames = (ShadowFrame*)W.frames.p;
-    tp.lterm = (float*)W.lterm.p;
+    int rc = prepare_work(W, tp, threads_total, tp.max_depth, (size_t)spb * tp.npix_local * 16, n_batches);
+    if (rc != RT_OK) return rc;
+    tp.stack_stride = threads_total;
     // event ring: every pending frame owns 2 + 2*n_batches events (begin, end, and a pair around each trace launch)
     const uint32_t kRing = 64, per_frame = 2 + 2 * n_batches;
     if (h->pending_frames >= kRing) return fail(RT_ERR_INVALID, "more than 64 frames enqueued without rtb200_render_device_wait");
@@ -508,41 +558,37 @@ static int render_enqueue(rtb200_scene_handle h, void* dev_rgb8, void* dev_linea
         h->ev.push_back(e);
     }
     cudaEvent_t* fev = h->ev.data() + (size_t)h->pending_frames * per_frame;
-    unsigned long long* stat = (unsigned long long*)W.small.p;
     unsigned int* counters = (unsigned int*)((char*)W.small.p + 256);
-    CU(cudaMemsetAsync(W.small.p, 0, 256 + (size_t)n_batches * 4, st));
-    CU(cudaMemsetAsync((char*)W.small.p + 64, 0xff, 16, st));   // stat[8], stat[9]: minima (kernel start / first dry-queue time, ns)
-
-    tp.samplebuf = (float4*)W.samplebuf.p;
-    tp.stack = (uint32_t*)W.stack.p;
-    tp.stack_stride = threads_total;
-    tp.stat = stat;
+    if ((rc = clear_stats(W, n_batches, st)) != RT_OK) return rc;
 
     CU(cudaEventRecord(fev[0], st));
-    uint32_t launches = 0;
-    for (uint32_t b = 0; b < n_batches; ++b) {
-        tp.s0 = b * spb;
-        tp.s_count = std::min(spb, spp - tp.s0);
-        tp.total_work = tp.s_count * tp.npix_local;
-        tp.work_counter = counters + b;
-        CU(cudaEventRecord(fev[2 + 2 * b], st));
-        if (tp.max_depth == 0) {
-            CU(cudaMemsetAsync(tp.samplebuf, 0, (size_t)tp.total_work * 16, st));   // ray_color(depth 0) = black, no ray (raytracer.rs:80-82)
-        } else {
-            CU(launch_wavefront(tp, h->mode, h->grid, h->smem, st));
-        }
-        CU(cudaEventRecord(fev[3 + 2 * b], st));
-        ResolveParams q{};
-        q.samplebuf = tp.samplebuf; q.accum = (float*)W.accum.p; q.npix_local = tp.npix_local; q.s_count = tp.s_count;
-        q.first = b == 0; q.last = b + 1 == n_batches; q.spp = spp;
-        q.out_linear = (float*)dev_linear_f32; q.out_rgb8 = (uint8_t*)dev_rgb8;
-        CU(launch_resolve(q, st));
-        launches += 2;
-    }
+    if ((rc = enqueue_batches(h, tp, W, dev_rgb8, dev_linear_f32, counters, fev + 2, st)) != RT_OK) return rc;
     CU(cudaEventRecord(fev[1], st));
-    h->last_batches = n_batches; h->last_launches = launches;
+    h->last_batches = n_batches; h->last_launches = 2 * n_batches;
     ++h->pending_frames;
     return RT_OK;
+}
+
+// RTB200_PRINT_TAIL / RTB200_PRINT_PHASES: the frame-tail and phase-clock counters of a stat block (stderr)
+static void print_diagnostics(const unsigned long long* hstat, int grid) {
+    if (getenv("RTB200_PRINT_TAIL") && hstat[8] != ~0ull) {   // when did the global queue run dry, when did the last CTA exit
+        const double total = (double)(hstat[10] - hstat[8]) * 1e-6, tail = hstat[9] != ~0ull ? (double)(hstat[10] - hstat[9]) * 1e-6 : 0.0;
+        fprintf(stderr, "[rtb200] trace kernel: first CTA start -> last CTA exit %.3f ms; queue dry -> last CTA exit (tail) %.3f ms; iterations after the queue ran dry: max %llu, mean %.1f per CTA\n",
+                total, tail, hstat[11], (double)hstat[12] / std::max(1, grid));
+    }
+    if (getenv("RTB200_PRINT_PHASES")) {
+        const unsigned long long* ph = hstat + kPhaseStat;
+        if (ph[PH_ITERS] == 0) {
+            fprintf(stderr, "[rtb200] fallbacks=%llu; no phase clocks: this library was built without RT_PHASE_CLOCKS (make -C rust-raytracer_b200 phase)\n", hstat[2]);
+        } else {
+            const double it = (double)ph[PH_ITERS];
+            fprintf(stderr, "[rtb200] fallbacks=%llu phases (clock64 cycles per warp iteration): closest_hit=%.0f (node steps %.0f, leaf steps %.0f, exact steps %.0f) sort+waitA=%.0f shade=%.0f regen=%.0f waitC=%.0f; "
+                    "warp_iters=%llu scatters=%llu deferred=%llu (%.4f of scatters); exact steps=%llu (%.2f per warp iteration) exact tests=%llu source-sphere skips=%llu rays=%llu\n",
+                    hstat[2], ph[PH_HIT] / it, ph[PH_NODE] / it, ph[PH_LEAF] / it, ph[PH_EXACT] / it, ph[PH_SORT_WAIT_A] / it, ph[PH_SHADE] / it, ph[PH_REGEN] / it, ph[PH_WAIT_C] / it,
+                    ph[PH_ITERS], ph[PH_SCATTERS], ph[PH_DEFERRED], (double)ph[PH_DEFERRED] / (double)std::max(1ull, ph[PH_SCATTERS]),
+                    ph[PH_EXACT_STEPS], ph[PH_EXACT_STEPS] / it, ph[PH_EXACT_TESTS], ph[PH_SRC_SKIPS], hstat[0]);
+        }
+    }
 }
 
 // Wait for the frames of `h` enqueued so far and fetch statistics (counters: the last frame's; times: summed over the frames).
@@ -578,24 +624,7 @@ static int render_collect(rtb200_scene_handle h, rt_stats* stats) {
         stats->device_ms = dv; stats->trace_ms = tr; stats->frames = frames;
         stats->rays = hstat[0]; stats->candidates = hstat[1]; stats->samples = hstat[3]; stats->clusters = hstat[4]; stats->nodes = hstat[6];
         stats->gpus_used = 1;
-        if (getenv("RTB200_PRINT_TAIL") && hstat[8] != ~0ull) {   // last batch of the last frame: when did the global queue run dry, when did the last CTA exit
-            const double total = (double)(hstat[10] - hstat[8]) * 1e-6, tail = hstat[9] != ~0ull ? (double)(hstat[10] - hstat[9]) * 1e-6 : 0.0;
-            fprintf(stderr, "[rtb200] trace kernel: first CTA start -> last CTA exit %.3f ms; queue dry -> last CTA exit (tail) %.3f ms; iterations after the queue ran dry: max %llu, mean %.1f per CTA\n",
-                    total, tail, hstat[11], (double)hstat[12] / std::max(1, h->grid));
-        }
-        if (getenv("RTB200_PRINT_PHASES")) {   // last batch of the last frame
-            const unsigned long long* ph = hstat + kPhaseStat;
-            if (ph[PH_ITERS] == 0) {
-                fprintf(stderr, "[rtb200] fallbacks=%llu; no phase clocks: this library was built without RT_PHASE_CLOCKS (make -C rust-raytracer_b200 phase)\n", hstat[2]);
-            } else {
-                const double it = (double)ph[PH_ITERS];
-                fprintf(stderr, "[rtb200] fallbacks=%llu phases (clock64 cycles per warp iteration): closest_hit=%.0f (node steps %.0f, leaf steps %.0f, exact steps %.0f) sort+waitA=%.0f shade=%.0f regen=%.0f waitC=%.0f; "
-                        "warp_iters=%llu scatters=%llu deferred=%llu (%.4f of scatters); exact steps=%llu (%.2f per warp iteration) exact tests=%llu source-sphere skips=%llu rays=%llu\n",
-                        hstat[2], ph[PH_HIT] / it, ph[PH_NODE] / it, ph[PH_LEAF] / it, ph[PH_EXACT] / it, ph[PH_SORT_WAIT_A] / it, ph[PH_SHADE] / it, ph[PH_REGEN] / it, ph[PH_WAIT_C] / it,
-                        ph[PH_ITERS], ph[PH_SCATTERS], ph[PH_DEFERRED], (double)ph[PH_DEFERRED] / (double)std::max(1ull, ph[PH_SCATTERS]),
-                        ph[PH_EXACT_STEPS], ph[PH_EXACT_STEPS] / it, ph[PH_EXACT_TESTS], ph[PH_SRC_SKIPS], hstat[0]);
-            }
-        }
+        print_diagnostics(hstat, h->grid);   // last batch of the last frame
         if (h->tp.max_depth == 0) stats->samples = (uint64_t)h->tp.npix_local * h->tp.spp;   // no kernel ran: every sample is black
         stats->kernel_launches = h->last_launches * frames; stats->batches = h->last_batches;
     }
@@ -627,6 +656,168 @@ int rtb200_render_device_wait(rtb200_scene_handle h, rt_stats* stats) {
     DeviceRestore restore;
     std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
     return render_collect(h, stats);
+}
+
+// ---- animations: several frames of one resident scene in as few trace launches as the sample buffer allows ----
+// A launch group is a run of consecutive frames with equal max_depth (a launch scalar) whose samples all fit the
+// sample-buffer cap and the u32 work ids. A group of F >= 2 frames is ONE launch of the multi-frame trace kernel - the
+// stragglers of frame i finish while frame i+1's work is handed out, so only the group's last frame pays the frame tail -
+// followed by one resolve per frame; a frame that fits with no other, and every max_depth 0 frame, takes the single-frame
+// path with its sample batches. So does a frame of more than kGroupMaxFrameWork samples: its own tail is a few per cent of
+// its time at most, and the multi-frame kernel, which keeps the Philox key in registers instead of the parameter block,
+// spills more and traced 800x600x128 frames 5 % slower than the single-frame kernel on an H100 (DESIGN.md §4.6).
+struct FrameGroup { uint32_t first, count; };
+constexpr uint64_t kGroupMaxFrameWork = 1ull << 24;   // samples per frame (spp * rows * width): ~8 ms of tracing on an H100
+
+static std::vector<FrameGroup> frame_groups(const rt_frame* frames, uint32_t n, uint64_t frame_work, uint64_t cap) {
+    std::vector<FrameGroup> groups;
+    for (uint32_t i = 0; i < n;) {
+        uint64_t F = 1;
+        if (frames[i].max_depth != 0 && frame_work <= kGroupMaxFrameWork)
+            while (i + F < n && frames[i + F].max_depth == frames[i].max_depth && (F + 1) * frame_work < (1ull << 31) && (F + 1) * frame_work * 16ull <= cap) ++F;
+        groups.push_back(FrameGroup{i, (uint32_t)F});
+        i += (uint32_t)F;
+    }
+    return groups;
+}
+
+// rt_frame checks shared by both entry points (no device is touched)
+static int check_frames(const rt_frame* frames, uint32_t n, uint64_t rows, uint64_t width) {
+    if (n == 0) return fail(RT_ERR_INVALID, "n_frames must be > 0");
+    if (!frames) return fail(RT_ERR_INVALID, "frames is null");
+    const uint64_t per_frame = rows * width * 3ull;   // < 2^33: width * height < 2^31 (validate_scene)
+    if (per_frame != 0 && (uint64_t)n > ~0ull / per_frame) return fail(RT_ERR_INVALID, "n_frames * rows * width * 3 overflows 64 bits");
+    for (uint32_t i = 0; i < n; ++i)
+        if (frames[i].reserved != 0) return fail(RT_ERR_INVALID, "rt_frame.reserved must be 0 (frame " + std::to_string(i) + ")");
+    return RT_OK;
+}
+
+// The frames of rtb200_render_frames_device on work set 0; the handle's lock is held and no frame of it is in flight.
+static int render_frames_run(rtb200_scene_handle h, const rt_frame* frames, uint32_t n, void* dev_rgb8, void* dev_linear_f32,
+                             void* stream_in, rt_stats* stats) {
+    DeviceCtx* ctx = h->ctx;
+    DeviceCtx::WorkSet& W = ctx->ws[0];
+    CU(cudaSetDevice(h->device));
+    cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
+    if (st != ctx->stream) CU(cudaStreamWaitEvent(st, ctx->staging_free, 0));   // the scene upload ran on the context's stream
+    if (stats) { memset(stats, 0, sizeof *stats); stats->frames = n; stats->gpus_used = 1; }
+    TraceParams tp = h->tp;   // the handle's own view stays as uploaded
+    const uint64_t npl = tp.npix_local;
+    if (npl == 0) return RT_OK;
+    const uint32_t spp = tp.spp, spb = h->spp_batch, n_batches = (spp + spb - 1) / spb;
+    const uint64_t frame_work = (uint64_t)spp * npl;
+    const uint64_t cap = h->opts.sample_buffer_bytes ? h->opts.sample_buffer_bytes : (1ull << 30);
+    const std::vector<FrameGroup> groups = frame_groups(frames, n, frame_work, cap);
+
+    // launch geometry of the multi-frame kernel (its pool also holds the slots' frames)
+    size_t smem_f = 0;
+    int grid_f = 0;
+    uint32_t n_batches_total = 0, max_depth = 1;   // trace launches (or black memsets) of the call
+    size_t sbuf = 0;
+    for (const FrameGroup& g : groups) {
+        n_batches_total += g.count > 1 ? 1u : n_batches;
+        sbuf = std::max(sbuf, g.count > 1 ? (size_t)(g.count * frame_work * 16) : (size_t)spb * npl * 16);
+        max_depth = std::max(max_depth, frames[g.first].max_depth);
+        if (g.count > 1 && grid_f == 0) {
+            smem_f = wavefront_smem_bytes(tp, h->mode, tp.scene_in_smem, true);
+            const int occ = occupancy(ctx, h->mode, tp.n_lights > 0, true, smem_f);
+            if (occ <= 0) return fail(RT_ERR_UNSUPPORTED, "no launch configuration of the multi-frame trace kernel fits shared memory");
+            grid_f = ctx->sm_count * occ;
+        }
+    }
+    const uint32_t threads_total = (uint32_t)std::max(h->grid, grid_f) * (uint32_t)kBlock;
+    int rc = prepare_work(W, tp, threads_total, max_depth, sbuf, n_batches_total);
+    if (rc != RT_OK) return rc;
+    CU(W.ftab.ensure((size_t)n * sizeof(FrameRec)));
+    std::vector<FrameRec> tab(n);
+    for (uint32_t i = 0; i < n; ++i) {
+        tab[i].cam = frames[i].camera; tab[i].key0 = (uint32_t)frames[i].seed; tab[i].key1 = (uint32_t)(frames[i].seed >> 32);
+    }
+    // events: begin, end, and a pair around each trace launch
+    while (h->ev.size() < 2 + 2 * (size_t)n_batches_total) {
+        cudaEvent_t e;
+        if (!ctx->event_pool.empty()) { e = ctx->event_pool.back(); ctx->event_pool.pop_back(); }
+        else CU(cudaEventCreate(&e));
+        h->ev.push_back(e);
+    }
+    cudaEvent_t* ev = h->ev.data();
+    unsigned int* counters = (unsigned int*)((char*)W.small.p + 256);
+    const FrameRec* dtab = (const FrameRec*)W.ftab.p;
+    CU(cudaMemcpyAsync(W.ftab.p, tab.data(), (size_t)n * sizeof(FrameRec), cudaMemcpyHostToDevice, st));
+    if ((rc = clear_stats(W, n_batches_total, st)) != RT_OK) return rc;
+
+    CU(cudaEventRecord(ev[0], st));
+    uint32_t b = 0, launches = 0;
+    uint64_t black_samples = 0;   // samples of max_depth 0 frames: black, no kernel counts them
+    for (const FrameGroup& g : groups) {
+        const rt_frame& f0 = frames[g.first];
+        uint8_t* o8 = dev_rgb8 ? (uint8_t*)dev_rgb8 + (size_t)g.first * npl * 3 : nullptr;
+        float* ol = dev_linear_f32 ? (float*)dev_linear_f32 + (size_t)g.first * npl * 3 : nullptr;
+        TraceParams q = tp;
+        q.max_depth = f0.max_depth;
+        if (g.count == 1) {
+            q.cam = tab[g.first].cam; q.key0 = tab[g.first].key0; q.key1 = tab[g.first].key1;
+            q.stack_stride = (uint32_t)h->grid * (uint32_t)kBlock;
+            if ((rc = enqueue_batches(h, q, W, o8, ol, counters + b, ev + 2 + 2 * b, st)) != RT_OK) return rc;
+            b += n_batches; launches += 2 * n_batches;
+            if (f0.max_depth == 0) black_samples += frame_work;
+            continue;
+        }
+        q.ftab = dtab + g.first; q.frame_work = (uint32_t)frame_work;
+        q.s0 = 0; q.s_count = spp; q.total_work = (uint32_t)(g.count * frame_work);
+        q.work_counter = counters + b;
+        q.stack_stride = (uint32_t)grid_f * (uint32_t)kBlock;
+        CU(cudaEventRecord(ev[2 + 2 * b], st));
+        CU(launch_wavefront(q, h->mode, true, grid_f, smem_f, st));
+        CU(cudaEventRecord(ev[3 + 2 * b], st));
+        for (uint32_t k = 0; k < g.count; ++k) {   // samplebuf [frame][sample][pixel]: frame k's samples are one batch
+            ResolveParams r{};
+            r.samplebuf = q.samplebuf + (size_t)k * frame_work; r.accum = (float*)W.accum.p; r.npix_local = (uint32_t)npl; r.s_count = spp;
+            r.first = 1; r.last = 1; r.spp = spp;
+            r.out_linear = ol ? ol + (size_t)k * npl * 3 : nullptr; r.out_rgb8 = o8 ? o8 + (size_t)k * npl * 3 : nullptr;
+            CU(launch_resolve(r, st));
+        }
+        b += 1; launches += 1 + g.count;
+    }
+    CU(cudaEventRecord(ev[1], st));
+
+    unsigned long long hstat[32] = {0}, herr[2] = {0, 0};   // the whole 256-byte stat block, summed over the call's launches
+    CU(cudaMemcpyAsync(hstat, W.small.p, sizeof hstat, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(herr, h->err, sizeof herr, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (herr[0] | herr[1]) CU(cudaMemset(h->err, 0, sizeof herr));
+    if (herr[1] != 0) return fail(RT_ERR_CUDA, "internal error: the traversal guard tripped; the frames are not valid");
+    if (herr[0] != 0) return fail(RT_ERR_UNSUPPORTED, "light-test recursion deeper than the shadow-frame stack occurred in one of the frames; it is not exact (the reference recursion is near-critical for this many lights)");
+    if (stats) {
+        float ms = 0.f;
+        CU(cudaEventElapsedTime(&ms, ev[0], ev[1]));
+        stats->device_ms = ms;
+        double tr = 0.0;
+        for (uint32_t k = 0; k < b; ++k) { CU(cudaEventElapsedTime(&ms, ev[2 + 2 * k], ev[3 + 2 * k])); tr += ms; }
+        stats->trace_ms = tr;
+        stats->rays = hstat[0]; stats->candidates = hstat[1]; stats->samples = hstat[3] + black_samples; stats->clusters = hstat[4]; stats->nodes = hstat[6];
+        stats->kernel_launches = launches; stats->batches = b;
+        stats->h2d_bytes = (uint64_t)n * sizeof(FrameRec);
+        print_diagnostics(hstat, std::max(h->grid, grid_f));   // every launch of the call: the tail is one launch's when the call made one
+    }
+    return RT_OK;
+}
+
+int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, uint32_t n_frames, void* dev_rgb8, void* dev_linear_f32,
+                                void* stream_in, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    int rc = check_frames(frames, n_frames, h->tp.rows_local, h->tp.width);
+    if (rc != RT_OK) return rc;
+    if (!dev_rgb8 && !dev_linear_f32) return fail(RT_ERR_INVALID, "dev_rgb8 and dev_linear_f32 are both null");
+    auto wall0 = std::chrono::steady_clock::now();
+    DeviceRestore restore;
+    std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
+    if (h->pending_frames) { if ((rc = render_collect(h, nullptr)) != RT_OK) return rc; }   // drain frames enqueued earlier
+    rc = render_frames_run(h, frames, n_frames, dev_rgb8, dev_linear_f32, stream_in, stats);
+    if (rc == RT_OK && stats) stats->wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count();
+    return rc;
+  });
 }
 
 static int render_host(const rt_scene* s, const rt_options* opts, uint8_t* out_rgb8, float* out_lin, rt_stats* stats) {
@@ -669,6 +860,44 @@ int rtb200_render_rgb8(const rt_scene* scene, const rt_options* opts, uint8_t* o
 int rtb200_render_linear_f32(const rt_scene* scene, const rt_options* opts, float* out_rgb, rt_stats* stats) {
     if (!scene || !out_rgb) return fail(RT_ERR_INVALID, "null argument");
     return guarded([&]() -> int { return render_host(scene, opts, nullptr, out_rgb, stats); });
+}
+
+int rtb200_render_frames(const rt_scene* s, const rt_options* opts_in, const rt_frame* frames, uint32_t n_frames, uint8_t* out_rgb8,
+                         float* out_lin, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (!s) return fail(RT_ERR_INVALID, "null argument");
+    if (!out_rgb8 && !out_lin) return fail(RT_ERR_INVALID, "out_rgb8 and out_linear_f32 are both null");
+    rt_options opts;
+    int rc = normalise_options(opts_in, &opts);
+    if (rc != RT_OK) return rc;
+    uint32_t n_lights = 0;
+    if ((rc = validate_scene(s, &n_lights)) != RT_OK) return rc;
+    if ((rc = check_frames(frames, n_frames, rtb200_shard_rows(s->height, opts.rank, opts.world, opts.band_rows), s->width)) != RT_OK) return rc;
+    auto wall0 = std::chrono::steady_clock::now();
+    DeviceRestore restore;
+    rtb200_scene_handle h = nullptr;
+    if ((rc = rtb200_scene_upload(s, &opts, &h)) != RT_OK) return rc;
+    struct Rel { rtb200_scene_handle h; ~Rel() { std::string keep = g_last_error; rtb200_scene_release(h); g_last_error = keep; } } rel{h};
+    DeviceCtx* ctx = h->ctx;
+    std::lock_guard<std::recursive_mutex> lk(ctx->mu);
+    CU(cudaSetDevice(h->device));
+    const size_t total = (size_t)n_frames * h->tp.npix_local;   // pixels of all frames
+    void *d8 = nullptr, *dl = nullptr;
+    if (out_rgb8) { CU(ctx->out_rgb8.ensure(total * 3 + 16)); d8 = ctx->out_rgb8.p; }
+    if (out_lin) { CU(ctx->out_lin.ensure(total * 12 + 16)); dl = ctx->out_lin.p; }
+    rt_stats st{};
+    if ((rc = rtb200_render_frames_device(h, frames, n_frames, d8, dl, nullptr, &st)) != RT_OK) return rc;
+    if (total) {
+        if (out_rgb8) CU(cudaMemcpyAsync(out_rgb8, d8, total * 3, cudaMemcpyDeviceToHost, ctx->stream));
+        if (out_lin) CU(cudaMemcpyAsync(out_lin, dl, total * 12, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+    }
+    st.h2d_bytes += h->h2d_bytes;
+    st.d2h_bytes = (out_rgb8 ? total * 3 : 0) + (out_lin ? total * 12 : 0) + 128 + 16;
+    st.wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count();
+    if (stats) *stats = st;
+    return RT_OK;
+  });
 }
 
 // One process, n_gpus devices: the reference's row bands (raytracer.rs:254-262) dealt round-robin to the devices (band b ->

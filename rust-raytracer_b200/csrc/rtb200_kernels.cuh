@@ -57,6 +57,11 @@ static_assert(sizeof(ShadowFrame) == 88, "ShadowFrame layout");
 
 enum TraceMode : uint32_t { MODE_TREE = 0, MODE_BRUTE = 1, MODE_EXACT = 2 };
 
+// One frame of a multi-frame launch (rt_wavefront_kernel<.., FRAMES = true>): the view and the Philox key that replace
+// TraceParams::cam / key0 / key1 for the work ids of that frame.
+struct FrameRec { rt_camera cam; uint32_t key0, key1; };
+static_assert(sizeof(FrameRec) == 104, "FrameRec layout");
+
 struct TraceParams {
     // ---- scene, resident in HBM (built by rtbvh::build_records) ----
     const float4*   nodes;       // n_nodes * kNodeVec: lo_x[8] lo_y[8] lo_z[8] hi_x[8] hi_y[8] hi_z[8] child[8], f32 boxes rounded outwards
@@ -94,6 +99,9 @@ struct TraceParams {
     float* lterm;                // [2 levels][3][stack_stride] light terms of the first two path levels
     unsigned long long* stat;    // per frame: [0]=rays [1]=f64 tests [2]=all-spheres fallbacks [3]=samples [4]=leaf visits [6]=node visits, [8..12] frame tail, [kPhaseStat..] phase clocks
     unsigned long long* err;     // per scene handle, accumulated over frames: [0]=shadow-frame-stack overflows [1]=traversal guard trips (must stay 0)
+    // ---- multi-frame launches only (appended, so that the fields above keep their offsets) ----
+    const FrameRec* ftab;        // [frames of the launch]: work id w belongs to frame w / frame_work
+    uint32_t frame_work;         // work ids per frame = s_count * npix_local; total_work = frames * frame_work
 };
 
 struct ResolveParams {
@@ -108,10 +116,11 @@ struct ResolveParams {
 
 struct KernelInfo { int registers, max_threads, const_bytes, local_bytes; char name[96]; };
 
-size_t wavefront_smem_bytes(const TraceParams& p, uint32_t mode, uint32_t smem_mask);
-cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, int grid, size_t smem, cudaStream_t st);
-int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, size_t smem);   // 0 when the kernel cannot run on the current device
-cudaError_t wavefront_info(uint32_t mode, bool lights, KernelInfo* out);
+// `frames`: the multi-frame kernel (work ids span p.ftab's frames) instead of the single-frame one
+size_t wavefront_smem_bytes(const TraceParams& p, uint32_t mode, uint32_t smem_mask, bool frames);
+cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, bool frames, int grid, size_t smem, cudaStream_t st);
+int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, bool frames, size_t smem);   // 0 when the kernel cannot run on the current device
+cudaError_t wavefront_info(uint32_t mode, bool lights, bool frames, KernelInfo* out);
 cudaError_t launch_resolve(const ResolveParams& p, cudaStream_t st);
 
 // single-thread probes of the device routines (known-answer tests)

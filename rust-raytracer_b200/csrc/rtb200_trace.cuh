@@ -44,6 +44,7 @@ constexpr uint32_t kNoSphere = 0xffffffffu;     // Pool.src: the ray does not st
 constexpr uint32_t kSkipNodeBit = 0x80000000u;
 constexpr uint32_t kNoSkip = 0xffffffffu;
 constexpr uint32_t kSlotBytes = 7 * 8 + 10 * 4 + RT_SMEM_STACK * 4;   // shared memory per pool slot
+constexpr uint32_t kFrameSlotBytes = 4;                               // + Pool.frm per slot in a multi-frame launch
 
 // SoA ray pool of a CTA: n_slots slots.
 struct Pool {
@@ -51,6 +52,7 @@ struct Pool {
     uint32_t *bi, *work, *pix, *smp, *blk, *clo, *chi, *lvl, *shd;   // hit index, work id, RNG (pixel, sample, block|has, cached draw), path level, shadow depth | kScatterPending
     uint32_t *src;                                               // the sphere the ray starts on (kNoSphere: a primary ray, or not known)
     uint32_t *stk;                                               // [RT_SMEM_STACK][n_slots] first levels of the albedo stack
+    uint32_t *frm;                                               // multi-frame launches: the slot's frame (index into TraceParams::ftab), kFrameSlotBytes per slot
     uint32_t n_slots;
     uint32_t stack_col;                                          // this CTA's first column of the global per-slot arrays (stack / frames / lterm)
 };
@@ -61,6 +63,7 @@ RT_DEV Pool pool_at(unsigned char* base, uint32_t n_slots, uint32_t stack_col) {
     uint32_t* u = reinterpret_cast<uint32_t*>(d + 7 * n_slots);
     P.bi = u; P.work = u + n_slots; P.pix = u + 2 * n_slots; P.smp = u + 3 * n_slots; P.blk = u + 4 * n_slots; P.clo = u + 5 * n_slots;
     P.chi = u + 6 * n_slots; P.lvl = u + 7 * n_slots; P.shd = u + 8 * n_slots; P.src = u + 9 * n_slots; P.stk = u + 10 * n_slots;
+    P.frm = u + (10 + RT_SMEM_STACK) * n_slots;   // only multi-frame launches reserve it (and touch it)
     P.n_slots = n_slots; P.stack_col = stack_col;
     return P;
 }
@@ -442,8 +445,10 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
 // Regenerate pool slot `s` from the global (pixel,sample) queue. Warp-synchronous: every lane of the warp calls it,
 // `want` says whether this lane's slot needs a new path; `exhausted` is the warp's (uniform) knowledge that the queue is
 // dry. Returns true when the slot received a new primary ray. raytracer.rs:199-201 + camera.rs:79-84.
+// FRAMES: the queue spans several frames, frame outermost; the frame's camera and key come from p.ftab (read once per
+// sample, off the bounce loop) and the frame is kept in Pool.frm for the shade stage's draws.
 // =====================================================================================================================
-template <bool LIGHTS>
+template <bool LIGHTS, bool FRAMES>
 RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint32_t s, int lane, bool& exhausted, Stats& st) {
     const unsigned FULL = 0xffffffffu;
     want = want && !exhausted;
@@ -457,7 +462,8 @@ RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint
     if (!want) return false;
     unsigned my = base + __popc(need & ((1u << lane) - 1u));
     if (my >= p.total_work) return false;
-    const uint32_t k0 = p.key0, k1 = p.key1;
+    uint32_t f = 0u, k0 = p.key0, k1 = p.key1;
+    if constexpr (FRAMES) { f = my / p.frame_work; my -= f * p.frame_work; k0 = p.ftab[f].key0; k1 = p.ftab[f].key1; }
     // Order of the global queue: image rows from the BOTTOM up, all samples of a row before the next row, x innermost.
     // The long paths of these scenes start at the ground / the spheres; the rows handed out last are the top of the image -
     // sky, one ray per sample - so that the stragglers of the last expensive rows finish under the cover of cheap work
@@ -475,9 +481,13 @@ RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint
     double xi2 = rng_f64(rng, k0, k1);
     double v = __ddiv_rn(__dsub_rn((double)p.height, __dadd_rn((double)y, xi2)), __dsub_rn((double)p.height, 1.0));
     D3 o, d;
-    get_ray(p.cam, u, v, o, d);
+    if constexpr (FRAMES) get_ray(p.ftab[f].cam, u, v, o, d);
+    else get_ray(p.cam, u, v, o, d);
     P.ox[s] = o.x; P.oy[s] = o.y; P.oz[s] = o.z; P.dx[s] = d.x; P.dy[s] = d.y; P.dz[s] = d.z;
-    P.work[s] = s_local * p.npix_local + lp; P.pix[s] = rng.pixel; P.smp[s] = rng.sample;   // samplebuf index [sample][pixel]
+    // samplebuf index [sample][pixel], or [frame][sample][pixel]
+    if constexpr (FRAMES) { P.work[s] = (f * p.s_count + s_local) * p.npix_local + lp; P.frm[s] = f; }
+    else P.work[s] = s_local * p.npix_local + lp;
+    P.pix[s] = rng.pixel; P.smp[s] = rng.sample;
     P.blk[s] = (rng.blk << 1) | rng.has; P.clo[s] = rng.c_lo; P.chi[s] = rng.c_hi;
     P.lvl[s] = 0u;
     P.shd[s] = 0u;
@@ -495,10 +505,12 @@ RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint
 // dead (returns true). A diffuse or metal vertex whose scatter sample is not accepted within RT_SCATTER_TRIPS trips of
 // the rejection loop saves only its RNG position, is marked kScatterPending and is shaded again in the next iteration
 // (returns false), so that a warp does not loop for its unluckiest lane while the other lanes idle.
+// FRAMES: the key is the slot's frame's (Pool.frm, p.ftab).
 // =====================================================================================================================
-template <bool LIGHTS>
+template <bool LIGHTS, bool FRAMES>
 RT_DEV bool shade_slot(const TraceParams& p, const SceneRefs& sc, const Pool& P, uint32_t s, uint32_t c) {
-    const uint32_t k0 = p.key0, k1 = p.key1;
+    uint32_t k0 = p.key0, k1 = p.key1;
+    if constexpr (FRAMES) { const FrameRec& fr = p.ftab[P.frm[s]]; k0 = fr.key0; k1 = fr.key1; }
     const DevMat* mat = sc.mat;
     const double4* geo = sc.geo;
     const size_t col = (size_t)P.stack_col + s;

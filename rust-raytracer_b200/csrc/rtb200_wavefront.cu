@@ -8,7 +8,8 @@
 //
 // The three template modes share everything but the closest-hit stage: MODE_TREE (production: BVH traversal), MODE_BRUTE
 // (RT_VARIANT_BRUTE_FORCE: linear scan with the conservative sphere test) and MODE_EXACT (RT_VARIANT_EXACT_F64: every
-// sphere in f64) - the last two validate the first.
+// sphere in f64) - the last two validate the first. Each mode has a single-frame kernel and a multi-frame one (FRAMES: the
+// queue spans several frames of the scene, each with its own camera and key; rtb200_render_frames, DESIGN.md §4.6).
 #include <cstdio>
 
 #include "rtb200_trace.cuh"
@@ -28,7 +29,8 @@ struct WfSmem {
 };
 
 // mask: bit0 hierarchy (MODE_TREE) / flat records (MODE_BRUTE), bit1 exact geometry, bit2 materials in shared memory
-__host__ __device__ inline WfSmem wf_layout(uint32_t n, uint32_t n_pairs, uint32_t n_nodes, uint32_t n_leaves, uint32_t mode, uint32_t mask) {
+// frames: the multi-frame kernel's pool also holds Pool.frm
+__host__ __device__ inline WfSmem wf_layout(uint32_t n, uint32_t n_pairs, uint32_t n_nodes, uint32_t n_leaves, uint32_t mode, uint32_t mask, bool frames) {
     WfSmem L;
     uint32_t off = 16;   // mbarrier
     L.nodes_off = off;   if (mode == MODE_TREE && (mask & 1u)) off += n_nodes * (uint32_t)(kNodeVec * 16);
@@ -39,7 +41,7 @@ __host__ __device__ inline WfSmem wf_layout(uint32_t n, uint32_t n_pairs, uint32
     L.mat_off = off; if (mask & 4u) off += n * 32u;
     off = (off + 15u) & ~15u;
     L.warpctx = off; if (mode == MODE_TREE) off += (uint32_t)(kBlock / 32) * kWarpCtxBytes;
-    L.pool = off; off += kSlotBytes * (uint32_t)kBlock;
+    L.pool = off; off += (kSlotBytes + (frames ? kFrameSlotBytes : 0u)) * (uint32_t)kBlock;
     L.perm = off; off += 5u * kBlock * 2u;
     L.cnt = off; off += 2u * 8u * 4u;
     L.phase = off; if (RT_PHASE_CLOCKS) off += (uint32_t)(kBlock / 32) * kPhaseN * 8u;
@@ -49,8 +51,8 @@ __host__ __device__ inline WfSmem wf_layout(uint32_t n, uint32_t n_pairs, uint32
 
 }  // namespace
 
-size_t wavefront_smem_bytes(const TraceParams& p, uint32_t mode, uint32_t smem_mask) {
-    return wf_layout(p.n, p.n_pairs, p.n_nodes, p.n_leaves, mode, smem_mask).total;
+size_t wavefront_smem_bytes(const TraceParams& p, uint32_t mode, uint32_t smem_mask, bool frames) {
+    return wf_layout(p.n, p.n_pairs, p.n_nodes, p.n_leaves, mode, smem_mask, frames).total;
 }
 
 // CTAs per SM each kernel's register budget is built for: 3 of 256 threads for the BVH path (80 registers), 2 for the
@@ -60,10 +62,11 @@ constexpr int wf_min_blocks(uint32_t mode) {
     return n > 0 ? n : 1;
 }
 
-template <uint32_t MODE, bool LIGHTS>
+// FRAMES: one launch renders several frames of the scene (TraceParams::ftab / frame_work, rtb200_render_frames)
+template <uint32_t MODE, bool LIGHTS, bool FRAMES>
 __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kernel(const __grid_constant__ TraceParams p) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    const WfSmem L = wf_layout(p.n, p.n_pairs, p.n_nodes, p.n_leaves, MODE, p.scene_in_smem);
+    const WfSmem L = wf_layout(p.n, p.n_pairs, p.n_nodes, p.n_leaves, MODE, p.scene_in_smem, FRAMES);
     uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw);
     const bool tree_smem = (p.scene_in_smem & 1u) != 0u;
     SceneRefs sc;
@@ -109,7 +112,7 @@ __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kern
     bool exhausted = false;   // warp-uniform: this warp has seen the end of the queue
     bool stamped = false;
     uint32_t dry_iters = 0;   // iterations of this CTA after it first found the global queue dry
-    regenerate_slot<LIGHTS>(p, P, true, (uint32_t)tid, lane, exhausted, st);   // initial fill of the pool
+    regenerate_slot<LIGHTS, FRAMES>(p, P, true, (uint32_t)tid, lane, exhausted, st);   // initial fill of the pool
     __syncthreads();
 
 #if RT_PHASE_CLOCKS
@@ -161,7 +164,7 @@ __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kern
         const uint32_t cstart = c == CLS_MISS ? 0u : c == CLS_DIFFUSE ? e0 : c == CLS_METAL ? e1 : c == CLS_GLASS ? e2 : e3;
         const uint32_t s = active ? (uint32_t)s_perm[c * (uint32_t)kBlock + ((uint32_t)tid - cstart)] : 0u;
         bool done = false;
-        if (active) done = shade_slot<LIGHTS>(p, sc, P, s, c);
+        if (active) done = shade_slot<LIGHTS, FRAMES>(p, sc, P, s, c);
 #if RT_PHASE_CLOCKS
         tick(PH_SHADE);
         {
@@ -170,7 +173,7 @@ __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kern
             if (lane == 0) { ph[PH_ITERS] += 1ull; ph[PH_SCATTERS] += (unsigned)__popc(sm); ph[PH_DEFERRED] += (unsigned)__popc(dm); }
         }
 #endif
-        regenerate_slot<LIGHTS>(p, P, active && done, s, lane, exhausted, st);
+        regenerate_slot<LIGHTS, FRAMES>(p, P, active && done, s, lane, exhausted, st);
         if (exhausted && !stamped) { stamped = true; if (lane == 0) atomicMin(&p.stat[9], now_ns()); }
         if (stamped) ++dry_iters;
         const bool still_alive = active && (P.lvl[s] != kDeadLevel);
@@ -191,15 +194,19 @@ __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kern
     if (tid == 0) { atomicMax(&p.stat[10], now_ns()); atomicMax(&p.stat[11], (unsigned long long)dry_iters); atomicAdd(&p.stat[12], (unsigned long long)dry_iters); }
 }
 
+template <bool FRAMES, typename F>
+static auto dispatch_mode(uint32_t mode, bool lights, F&& f) {
+    if (mode == MODE_EXACT) return lights ? f(rt_wavefront_kernel<MODE_EXACT, true, FRAMES>) : f(rt_wavefront_kernel<MODE_EXACT, false, FRAMES>);
+    if (mode == MODE_BRUTE) return lights ? f(rt_wavefront_kernel<MODE_BRUTE, true, FRAMES>) : f(rt_wavefront_kernel<MODE_BRUTE, false, FRAMES>);
+    return lights ? f(rt_wavefront_kernel<MODE_TREE, true, FRAMES>) : f(rt_wavefront_kernel<MODE_TREE, false, FRAMES>);
+}
 template <typename F>
-static auto dispatch(uint32_t mode, bool lights, F&& f) {
-    if (mode == MODE_EXACT) return lights ? f(rt_wavefront_kernel<MODE_EXACT, true>) : f(rt_wavefront_kernel<MODE_EXACT, false>);
-    if (mode == MODE_BRUTE) return lights ? f(rt_wavefront_kernel<MODE_BRUTE, true>) : f(rt_wavefront_kernel<MODE_BRUTE, false>);
-    return lights ? f(rt_wavefront_kernel<MODE_TREE, true>) : f(rt_wavefront_kernel<MODE_TREE, false>);
+static auto dispatch(uint32_t mode, bool lights, bool frames, F&& f) {
+    return frames ? dispatch_mode<true>(mode, lights, f) : dispatch_mode<false>(mode, lights, f);
 }
 
-cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, int grid, size_t smem, cudaStream_t st) {
-    return dispatch(mode, p.n_lights > 0, [&](auto kern) -> cudaError_t {
+cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, bool frames, int grid, size_t smem, cudaStream_t st) {
+    return dispatch(mode, p.n_lights > 0, frames, [&](auto kern) -> cudaError_t {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
         kern<<<grid, kBlock, smem, st>>>(p);
@@ -207,8 +214,8 @@ cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, int grid, size
     });
 }
 
-int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, size_t smem) {
-    return dispatch(mode, lights, [&](auto kern) -> int {
+int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, bool frames, size_t smem) {
+    return dispatch(mode, lights, frames, [&](auto kern) -> int {
         int nb = 0;
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return 0; }
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kBlock, smem) != cudaSuccess) { cudaGetLastError(); return 0; }
@@ -216,14 +223,14 @@ int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, size_t smem) {
     });
 }
 
-cudaError_t wavefront_info(uint32_t mode, bool lights, KernelInfo* out) {
-    return dispatch(mode, lights, [&](auto kern) -> cudaError_t {
+cudaError_t wavefront_info(uint32_t mode, bool lights, bool frames, KernelInfo* out) {
+    return dispatch(mode, lights, frames, [&](auto kern) -> cudaError_t {
         cudaFuncAttributes a;
         cudaError_t e = cudaFuncGetAttributes(&a, kern);
         if (e != cudaSuccess) return e;
         out->registers = a.numRegs; out->max_threads = a.maxThreadsPerBlock; out->const_bytes = (int)a.constSizeBytes; out->local_bytes = (int)a.localSizeBytes;
-        snprintf(out->name, sizeof out->name, "rt_wavefront_kernel<%s,%s>",
-                 mode == MODE_TREE ? "MODE_TREE" : mode == MODE_BRUTE ? "MODE_BRUTE" : "MODE_EXACT", lights ? "LIGHTS" : "NO_LIGHTS");
+        snprintf(out->name, sizeof out->name, "rt_wavefront_kernel<%s,%s%s>",
+                 mode == MODE_TREE ? "MODE_TREE" : mode == MODE_BRUTE ? "MODE_BRUTE" : "MODE_EXACT", lights ? "LIGHTS" : "NO_LIGHTS", frames ? ",FRAMES" : "");
         return cudaSuccess;
     });
 }

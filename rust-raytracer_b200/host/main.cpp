@@ -3,17 +3,59 @@
 // reference panic print a message to stderr and exit with status 101 (Rust's panic exit code).
 // Extra knobs, so the CLI stays identical: RTB200_SEED, RTB200_DEVICE, RTB200_GPUS=<n|0=all> (row bands dealt over n GPUs of
 // this process, rtb200_render_rgb8_multi), RTB200_STATS=1 (prints rays / Mrays/s to stderr).
+// RTB200_FRAMES=<frames.json> renders an animation over the scene (rtb200_render_frames): the file is a JSON array of
+// {"camera": {<the config's camera schema>}, "seed"?: n, "max_depth"?: n}, omitted fields are the scene's, and <output_file> is a
+// prefix: frame i is written to <prefix>_{i:03}.png (the reference's commented-out per-frame name, main.rs:17). Stdout gets
+// "\nRendering <file>" per frame and one "Frames time: <ms>ms for <n> frames" line.
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
 #include <fstream>
 #include <iostream>
 #include <sstream>
+#include <string>
 #include <vector>
 
 #include "../../include/rtb200.h"
 #include "png_writer.hpp"
 #include "scene_json.hpp"
+
+// RTB200_FRAMES: every frame of frames_path over `s`, written to <prefix>_000.png, <prefix>_001.png, ...
+static int render_animation(const rt_scene& s, const char* frames_path, const std::string& prefix) {
+    if (getenv("RTB200_GPUS")) { fprintf(stderr, "RTB200_FRAMES with RTB200_GPUS is not supported: animations render on one GPU\n"); return 101; }
+    std::ifstream f(frames_path, std::ios::binary);
+    if (!f) { fprintf(stderr, "Unable to read frames file.: %s\n", frames_path); return 101; }
+    std::stringstream ss; ss << f.rdbuf();
+    std::vector<rt_frame> frames;
+    try { frames = rthost::load_frames_json(ss.str(), s); }
+    catch (const std::exception& e) { fprintf(stderr, "Unable to parse frames json: %s\n", e.what()); return 101; }
+    std::vector<std::string> files(frames.size());
+    for (size_t i = 0; i < frames.size(); ++i) {
+        char num[32];
+        snprintf(num, sizeof num, "%03zu", i);   // Rust's {:0>3}: at least three digits
+        files[i] = prefix + "_" + num + ".png";
+        printf("\nRendering %s\n", files[i].c_str());
+    }
+    fflush(stdout);
+    const size_t frame_bytes = (size_t)s.width * s.height * 3;
+    std::vector<uint8_t> pixels(frame_bytes * frames.size());
+    rt_options opts{};
+    opts.device = getenv("RTB200_DEVICE") ? atoi(getenv("RTB200_DEVICE")) : -1; opts.rank = 0; opts.world = 1; opts.band_rows = 1;
+    rt_stats st{};
+    auto t0 = std::chrono::steady_clock::now();
+    int rc = rtb200_render_frames(&s, &opts, frames.data(), (uint32_t)frames.size(), pixels.data(), nullptr, &st);
+    if (rc != 0) { fprintf(stderr, "render failed (%d): %s\n", rc, rtb200_last_error()); return 101; }
+    long long ms = std::chrono::duration_cast<std::chrono::milliseconds>(std::chrono::steady_clock::now() - t0).count();
+    printf("Frames time: %lldms for %zu frames\n", ms, frames.size());
+    if (getenv("RTB200_STATS"))
+        fprintf(stderr, "rays=%llu samples=%llu device_ms=%.3f Mrays/s=%.1f launches=%u\n", (unsigned long long)st.rays, (unsigned long long)st.samples, st.device_ms,
+                st.device_ms > 0 ? st.rays / st.device_ms / 1e3 : 0.0, st.kernel_launches);
+    for (size_t i = 0; i < frames.size(); ++i) {
+        std::string err;
+        if (!rthost::write_png_rgb8(files[i].c_str(), pixels.data() + i * frame_bytes, s.width, s.height, &err)) { fprintf(stderr, "error writing image: %s\n", err.c_str()); return 101; }
+    }
+    return 0;
+}
 
 int main(int argc, char** argv) {
     if (argc != 3) {                                                       // main.rs:9-12
@@ -30,6 +72,7 @@ int main(int argc, char** argv) {
         rthost::load_scene_json(ss.str(), slash == std::string::npos ? std::string(".") : path.substr(0, slash), &holder);
     } catch (const std::exception& e) { fprintf(stderr, "Unable to parse config json: %s\n", e.what()); return 101; }   // main.rs:15
     if (const char* sd = getenv("RTB200_SEED")) holder.scene.seed = strtoull(sd, nullptr, 0);
+    if (const char* fp = getenv("RTB200_FRAMES")) return render_animation(holder.scene, fp, argv[2]);
     printf("\nRendering %s\n", argv[2]);                                  // main.rs:18
     fflush(stdout);
     const rt_scene& s = holder.scene;

@@ -85,4 +85,26 @@ void load_scene_json(const std::string& text, const std::string& base_dir, Scene
     s.spheres = out->spheres.data(); s.n_spheres = out->spheres.size();
     s.textures = out->textures.data(); s.n_textures = out->textures.size();
 }
+
+std::vector<rt_frame> load_frames_json(const std::string& text, const rt_scene& scene) {
+    Json root = JsonParser::parse(text);
+    if (root.kind != Json::Arr) throw std::runtime_error("frames: array expected");
+    if (root.arr.empty()) throw std::runtime_error("frames: at least one frame expected");
+    if (root.arr.size() > 0xffffffffull) throw std::runtime_error("frames: too many frames");
+    std::vector<rt_frame> frames(root.arr.size());
+    for (size_t i = 0; i < root.arr.size(); ++i) {
+        const Json& f = root.arr[i];
+        if (f.kind != Json::Obj) throw std::runtime_error("frame " + std::to_string(i) + ": object expected");
+        rt_frame& fr = frames[i];
+        fr = rt_frame{};
+        const Json& cam = f.at("camera");   // the config's camera schema (camera.rs:29-36)
+        rt_camera_params cp{vec3(cam.at("look_from")), vec3(cam.at("look_at")), vec3(cam.at("vup")), cam.at("vfov").number(), cam.at("aspect").number()};
+        if (rtb200_camera_from_params(&cp, &fr.camera) != 0) throw std::runtime_error("frame " + std::to_string(i) + ": invalid camera");
+        const Json* seed = f.find("seed");
+        fr.seed = seed ? uint_field(*seed, "seed", 9007199254740992.0) : scene.seed;
+        const Json* depth = f.find("max_depth");
+        fr.max_depth = depth ? (uint32_t)uint_field(*depth, "max_depth", 4294967295.0) : scene.max_depth;
+    }
+    return frames;
+}
 }  // namespace rthost

@@ -96,7 +96,12 @@ class rt_kernel_info(C.Structure):
         return d
 
 
-assert C.sizeof(rt_sphere) == 64
+class rt_frame(C.Structure):
+    """One frame of an animation over one scene: the view, the RNG key and the depth that replace the scene's own."""
+    _fields_ = [("camera", rt_camera), ("seed", C.c_uint64), ("max_depth", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+assert C.sizeof(rt_sphere) == 64 and C.sizeof(rt_frame) == 112
 
 # every symbol include/rtb200.h declares (tests check that the library exports all of them)
 ABI_SYMBOLS = [
@@ -106,6 +111,7 @@ ABI_SYMBOLS = [
     "rtb200_probe_sky", "rtb200_probe_get_ray", "rtb200_probe_rng", "rtb200_probe_quantise",
     "rtb200_decode_jpeg_file", "rtb200_free", "rtb200_render_device_async", "rtb200_render_device_wait",
     "rtb200_debug_bvh", "rtb200_probe_sphere_uv", "rtb200_device_count", "rtb200_render_rgb8_multi", "rtb200_scene_kernel_info",
+    "rtb200_render_frames", "rtb200_render_frames_device",
 ]
 
 _lib = None
@@ -149,6 +155,10 @@ def lib() -> C.CDLL:
     L.rtb200_device_count.restype = C.c_int
     L.rtb200_render_rgb8_multi.argtypes = [C.POINTER(rt_scene), C.POINTER(rt_options), C.c_int32, C.c_void_p, C.POINTER(rt_stats)]
     L.rtb200_scene_kernel_info.argtypes = [C.c_void_p, C.POINTER(rt_kernel_info)]
+    L.rtb200_render_frames.argtypes = [C.POINTER(rt_scene), C.POINTER(rt_options), C.POINTER(rt_frame), C.c_uint32, C.c_void_p, C.c_void_p,
+                                       C.POINTER(rt_stats)]
+    L.rtb200_render_frames_device.argtypes = [C.c_void_p, C.POINTER(rt_frame), C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.POINTER(rt_stats)]
     _lib = L
     return L
 
@@ -389,6 +399,35 @@ def render_rgb8_multi(scene: Scene, n_gpus: int = 0, opts: Optional[rt_options] 
     return out, st.as_dict()
 
 
+def make_frame(scene: Scene, look_from=None, look_at=None, vup=None, vfov: Optional[float] = None, aspect: Optional[float] = None,
+               seed: Optional[int] = None, max_depth: Optional[int] = None) -> rt_frame:
+    """One frame of an animation over `scene`: camera fields, seed and max_depth that are not given are the scene's own."""
+    p = dict(scene.camera_params)
+    for k, v in (("look_from", look_from), ("look_at", look_at), ("vup", vup), ("vfov", vfov), ("aspect", aspect)):
+        if v is not None:
+            p[k] = v
+    cam = camera_from_params(p["look_from"], p["look_at"], p["vup"], p["vfov"], p["aspect"])
+    return rt_frame(cam, scene.seed if seed is None else int(seed), scene.c.max_depth if max_depth is None else int(max_depth), 0)
+
+
+def _frame_array(frames: Sequence[rt_frame]):
+    arr = (rt_frame * max(len(frames), 1))(*frames)
+    return arr, len(frames)
+
+
+def render_frames(scene: Scene, frames: Sequence[rt_frame], opts: Optional[rt_options] = None, linear: bool = False):
+    """Render len(frames) frames of one scene in as few trace launches as the sample buffer allows (rtb200_render_frames).
+    Frame i equals render_rgb8 / render_linear of the scene with frames[i]'s camera, seed and max_depth. Returns
+    (uint8 [n,rows,w,3], or float32 with linear=True, stats dict)."""
+    rows = scene.c.height if (opts is None or opts.world <= 1) else shard_rows(scene.c.height, opts.rank, opts.world, opts.band_rows)
+    arr, n = _frame_array(frames)
+    out = np.empty((n, rows, scene.c.width, 3), dtype=np.float32 if linear else np.uint8)
+    st = rt_stats()
+    _check(lib().rtb200_render_frames(C.byref(scene.c), C.byref(opts) if opts is not None else None, arr, n,
+                                      None if linear else out.ctypes.data, out.ctypes.data if linear else None, C.byref(st)))
+    return out, st.as_dict()
+
+
 class ResidentScene:
     """Scene kept in HBM between frames (rtb200_scene_upload / rtb200_render_device)."""
 
@@ -412,6 +451,15 @@ class ResidentScene:
     def wait(self) -> dict:
         st = rt_stats()
         _check(lib().rtb200_render_device_wait(self.h, C.byref(st)))
+        return st.as_dict()
+
+    def render_frames(self, frames: Sequence[rt_frame], dev_rgb8_ptr: int = 0, dev_linear_ptr: int = 0, stream: int = 0) -> dict:
+        """Render len(frames) frames into device buffers of n * rows * w * 3 elements (blocking; the handle's own camera,
+        seed and max_depth stay as uploaded)."""
+        arr, n = _frame_array(frames)
+        st = rt_stats()
+        _check(lib().rtb200_render_frames_device(self.h, arr, n, C.c_void_p(dev_rgb8_ptr or None), C.c_void_p(dev_linear_ptr or None),
+                                                 C.c_void_p(stream or None), C.byref(st)))
         return st.as_dict()
 
     def kernel_info(self) -> dict:

@@ -122,9 +122,10 @@ typedef struct {
     uint32_t batches;
     uint64_t h2d_bytes, d2h_bytes;
     uint64_t clusters;      /* BVH leaves visited (diagnostic) */
-    uint64_t frames;        /* frames covered by device_ms / trace_ms / kernel_launches (1 for the blocking calls) */
+    uint64_t frames;        /* frames covered by device_ms / trace_ms / kernel_launches (1 for the blocking one-frame calls,
+                               n_frames for the frames calls, also on a shard with no rows) */
     uint64_t nodes;         /* BVH nodes visited (diagnostic) */
-    int32_t  gpus_used;     /* devices that rendered this frame */
+    int32_t  gpus_used;     /* devices that rendered this frame (1 on a shard with no rows) */
     int32_t  reserved;
 } rt_stats;
 
@@ -215,7 +216,8 @@ typedef struct {
 int rtb200_render_frames(const rt_scene* scene, const rt_options* opts, const rt_frame* frames, uint32_t n_frames,
                          uint8_t* out_rgb8, float* out_linear_f32, rt_stats* stats);
 /* The same on a resident scene into DEVICE buffers. Blocking: drains the handle's asynchronous frames first, uploads the frame
- * table on `stream` (NULL: the library's stream) and returns when the frames are done. The handle's own view is unchanged:
+ * table of the frames that share a launch (counted in h2d_bytes) on `stream` (NULL: the library's stream) and returns when
+ * the frames are done. The handle's own view is unchanged:
  * a later rtb200_render_device renders the camera it was uploaded with. */
 int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, uint32_t n_frames,
                                 void* dev_rgb8, void* dev_linear_f32, void* stream, rt_stats* stats);

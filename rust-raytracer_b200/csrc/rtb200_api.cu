@@ -1,5 +1,6 @@
-// rtb200_api.cu — the C ABI of include/rtb200.h: scene staging into HBM, batch scheduling of the trace /
-// resolve kernels, single- and multi-GPU frames, device<->host copies and error reporting. No CPU render path exists here.
+// rtb200_api.cu — the C ABI of include/rtb200.h: scene staging into HBM, scheduling of the trace / resolve kernels, multi-GPU
+// frames, device<->host copies and error reporting. Every render entry point, one frame or many, blocking or asynchronous,
+// enqueues its frames through render_enqueue and reports them through render_collect. No CPU render path exists here.
 #include <algorithm>
 #include <chrono>
 #include <cmath>
@@ -73,7 +74,7 @@ struct DeviceCtx {
     cudaStream_t stream = nullptr;
     // Two sets of per-frame work buffers: a frame loop that alternates two streams lets frame k+1 start tracing while frame k
     // drains its last paths and resolves (rtb200_render_device_async); blocking calls use set 0 only.
-    struct WorkSet { GrowBuf samplebuf, accum, stack, small, frames, lterm, ftab; } ws[2];   // ftab: rtb200_render_frames_device's frame table
+    struct WorkSet { GrowBuf samplebuf, accum, stack, small, frames, lterm, ftab; } ws[2];   // ftab: the multi-frame kernel's frame table
     GrowBuf out_rgb8, out_lin, probe, frame;
     // scene arenas of released handles, kept for the next upload (a per-frame upload costs no cudaMalloc / cudaFree)
     struct Arena { void* p; size_t cap; };
@@ -173,15 +174,26 @@ struct rtb200_scene_t {
     unsigned long long* err = nullptr;   // device: [0] shadow-frame-stack overflows, [1] traversal guard trips; accumulated over frames, cleared by wait
     struct Upload { const void* src; size_t bytes; void** field; };
     std::vector<Upload> uploads;         // pending scene arrays (commit_uploads)
-    std::vector<cudaEvent_t> ev;         // event ring of the frames in flight (per handle)
-    cudaStream_t last_stream = nullptr;  // stream, work set, batch and launch count of the most recently enqueued frame
-    int last_set = 0;
-    cudaStream_t streams[2] = {nullptr, nullptr};   // distinct streams used by the pending frames
-    int n_streams = 0;
+    std::vector<cudaEvent_t> ev;         // timing events of the pending submissions, each one's ev[ev0, ev0 + n_ev)
+    // What one render_enqueue put on a stream. Events: begin, end, and a pair around each trace launch (or black memset).
+    struct Submission {
+        cudaStream_t stream;
+        int set;                         // work set: its stat block holds the submission's counters
+        uint32_t ev0, n_ev;              // n_ev = 0: a shard with no rows, nothing was enqueued
+        uint32_t frames, batches, launches;
+        int grid;                        // of the widest launch (print_diagnostics)
+        uint64_t black_samples;          // samples of max_depth 0 frames: black, no kernel counts them
+        uint64_t ftab_bytes;             // frame table uploaded
+    };
+    std::vector<Submission> pending;     // enqueued since the last render_collect, oldest first
     uint32_t frame_counter = 0;
-    uint32_t last_batches = 0, last_launches = 0;
-    uint32_t pending_frames = 0;
     uint64_t h2d_bytes = 0;
+};
+
+// Releases a scene handle on scope exit; the error that made the scope return early survives the release.
+struct ReleaseGuard {
+    rtb200_scene_handle h;
+    ~ReleaseGuard() { std::string keep = g_last_error; rtb200_scene_release(h); g_last_error = keep; }
 };
 
 extern "C" {
@@ -258,7 +270,7 @@ int rtb200_scene_release(rtb200_scene_handle h) {
     if (h->ctx) {
         std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
         cudaSetDevice(h->device);
-        if (h->pending_frames) render_collect(h, nullptr);   // frames still in flight read the scene arrays
+        if (!h->pending.empty()) render_collect(h, nullptr);   // frames still in flight read the scene arrays
         else if (h->ctx->stream) cudaStreamSynchronize(h->ctx->stream);
         for (cudaEvent_t e : h->ev) h->ctx->event_pool.push_back(e);
         if (h->arena) {
@@ -501,71 +513,156 @@ static int clear_stats(DeviceCtx::WorkSet& W, uint32_t n_counters, cudaStream_t 
     return RT_OK;
 }
 
-// The sample batches of ONE frame: per batch a launch of the single-frame trace kernel (or, at max_depth 0, a black
-// memset) and a resolve. tp: the frame's parameters with every work buffer set; counters[b]: batch b's queue counter;
-// pair_ev[2b], pair_ev[2b+1] bracket batch b's trace launch.
-static int enqueue_batches(rtb200_scene_handle h, TraceParams tp, DeviceCtx::WorkSet& W, void* dev_rgb8, void* dev_linear_f32,
-                           unsigned int* counters, cudaEvent_t* pair_ev, cudaStream_t st) {
-    const uint32_t spp = tp.spp, spb = h->spp_batch;
-    const uint32_t n_batches = (spp + spb - 1) / spb;
-    for (uint32_t b = 0; b < n_batches; ++b) {
-        tp.s0 = b * spb;
-        tp.s_count = std::min(spb, spp - tp.s0);
-        tp.total_work = tp.s_count * tp.npix_local;
-        tp.work_counter = counters + b;
-        CU(cudaEventRecord(pair_ev[2 * b], st));
-        if (tp.max_depth == 0) {
-            CU(cudaMemsetAsync(tp.samplebuf, 0, (size_t)tp.total_work * 16, st));   // ray_color(depth 0) = black, no ray (raytracer.rs:80-82)
-        } else {
-            CU(launch_wavefront(tp, h->mode, false, h->grid, h->smem, st));
-        }
-        CU(cudaEventRecord(pair_ev[2 * b + 1], st));
-        ResolveParams q{};
-        q.samplebuf = tp.samplebuf; q.accum = (float*)W.accum.p; q.npix_local = tp.npix_local; q.s_count = tp.s_count;
-        q.first = b == 0; q.last = b + 1 == n_batches; q.spp = spp;
-        q.out_linear = (float*)dev_linear_f32; q.out_rgb8 = (uint8_t*)dev_rgb8;
-        CU(launch_resolve(q, st));
+// ---- scheduling: frames of one resident scene in as few trace launches as the sample buffer allows ----
+// A launch group is a run of consecutive frames with equal max_depth (a launch scalar) whose samples all fit the
+// sample-buffer cap and the u32 work ids. A group of F >= 2 frames is ONE launch of the multi-frame trace kernel - the
+// stragglers of frame i finish while frame i+1's work is handed out, so only the group's last frame pays the frame tail -
+// followed by one resolve per frame. A frame that fits with no other, and every max_depth 0 frame, runs alone: per sample
+// batch one launch of the single-frame trace kernel (a black memset at max_depth 0) and a resolve. So does a frame of more
+// than kGroupMaxFrameWork samples: its own tail is a few per cent of its time at most, and the multi-frame kernel, which
+// keeps the Philox key in registers instead of the parameter block, spills more and traced 800x600x128 frames 5 % slower
+// than the single-frame kernel on an H100 (DESIGN.md §4.6).
+struct FrameGroup { uint32_t first, count; };
+constexpr uint64_t kGroupMaxFrameWork = 1ull << 24;   // samples per frame (spp * rows * width): ~8 ms of tracing on an H100
+
+static std::vector<FrameGroup> frame_groups(const rt_frame* frames, uint32_t n, uint64_t frame_work, uint64_t cap) {
+    std::vector<FrameGroup> groups;
+    for (uint32_t i = 0; i < n;) {
+        uint64_t F = 1;
+        if (frames[i].max_depth != 0 && frame_work <= kGroupMaxFrameWork)
+            while (i + F < n && frames[i + F].max_depth == frames[i].max_depth && (F + 1) * frame_work < (1ull << 31) && (F + 1) * frame_work * 16ull <= cap) ++F;
+        groups.push_back(FrameGroup{i, (uint32_t)F});
+        i += (uint32_t)F;
     }
+    return groups;
+}
+
+// rt_frame checks shared by both frames entry points (no device is touched)
+static int check_frames(const rt_frame* frames, uint32_t n, uint64_t rows, uint64_t width) {
+    if (n == 0) return fail(RT_ERR_INVALID, "n_frames must be > 0");
+    if (!frames) return fail(RT_ERR_INVALID, "frames is null");
+    const uint64_t per_frame = rows * width * 3ull;   // < 2^33: width * height < 2^31 (validate_scene)
+    if (per_frame != 0 && (uint64_t)n > ~0ull / per_frame) return fail(RT_ERR_INVALID, "n_frames * rows * width * 3 overflows 64 bits");
+    for (uint32_t i = 0; i < n; ++i)
+        if (frames[i].reserved != 0) return fail(RT_ERR_INVALID, "rt_frame.reserved must be 0 (frame " + std::to_string(i) + ")");
     return RT_OK;
 }
 
-// Enqueue one frame on `stream_in` (or the context's stream) without waiting for it.
-static int render_enqueue(rtb200_scene_handle h, void* dev_rgb8, void* dev_linear_f32, void* stream_in, int set) {
-    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+// The handle's own view (the camera, seed and depth it was uploaded with) as a frame.
+static rt_frame own_frame(rtb200_scene_handle h) { return rt_frame{h->tp.cam, h->tp.key0 | (uint64_t)h->tp.key1 << 32, h->tp.max_depth, 0}; }
+
+// Enqueue frames[0, n) of h on `stream_in` (NULL: the context's stream) with work set `set`, without waiting, and append the
+// submission to h->pending; the caller holds the context's lock. Frame i goes to output slice i (rows * width * 3 elements).
+// A submission that fails part-way is not recorded.
+static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_t n, void* dev_rgb8, void* dev_linear_f32,
+                          void* stream_in, int set) {
+    if (h->pending.size() >= 64) return fail(RT_ERR_INVALID, "more than 64 frames enqueued without rtb200_render_device_wait");
     DeviceCtx* ctx = h->ctx;
-    DeviceCtx::WorkSet& W = ctx->ws[set & 1];
+    DeviceCtx::WorkSet& W = ctx->ws[set];
     CU(cudaSetDevice(h->device));
     cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
     if (st != ctx->stream) CU(cudaStreamWaitEvent(st, ctx->staging_free, 0));   // the scene upload ran on the context's stream
-    TraceParams tp = h->tp;
-    h->last_stream = st; h->last_set = set & 1; h->last_batches = 0; h->last_launches = 0;
-    if (h->n_streams < 2 && (h->n_streams == 0 || h->streams[0] != st)) h->streams[h->n_streams++] = st;
-    if (tp.npix_local == 0) return RT_OK;
+    const rtb200_scene_t::Submission* prev = h->pending.empty() ? nullptr : &h->pending.back();
+    rtb200_scene_t::Submission sub{st, set, prev ? prev->ev0 + prev->n_ev : 0u, 0, n, 0, 0, h->grid, 0, 0};
+    TraceParams tp = h->tp;   // the handle's own view stays as uploaded
+    const uint64_t npl = tp.npix_local;
+    if (npl == 0) { h->pending.push_back(sub); return RT_OK; }   // a shard with no rows: nothing to trace
+    const uint32_t spp = tp.spp, spb = h->spp_batch, n_batches = (spp + spb - 1) / spb;
+    const uint64_t frame_work = (uint64_t)spp * npl;
+    const uint64_t cap = h->opts.sample_buffer_bytes ? h->opts.sample_buffer_bytes : (1ull << 30);
+    const std::vector<FrameGroup> groups = frame_groups(frames, n, frame_work, cap);
 
-    const uint32_t spp = tp.spp, spb = h->spp_batch;
-    const uint32_t n_batches = (spp + spb - 1) / spb;
-    const uint32_t threads_total = (uint32_t)h->grid * (uint32_t)kBlock;   // ray slots of the whole grid: columns of the per-slot global arrays
-    int rc = prepare_work(W, tp, threads_total, tp.max_depth, (size_t)spb * tp.npix_local * 16, n_batches);
+    // trace launches, work buffer sizes and the launch geometry of the multi-frame kernel (its pool also holds the slots' frames)
+    size_t smem_f = 0;
+    int grid_f = 0;
+    uint32_t max_depth = 1;
+    size_t sbuf = 0;
+    for (const FrameGroup& g : groups) {
+        sub.batches += g.count > 1 ? 1u : n_batches;   // trace launches (or black memsets)
+        sbuf = std::max(sbuf, g.count > 1 ? (size_t)(g.count * frame_work * 16) : (size_t)spb * npl * 16);
+        max_depth = std::max(max_depth, frames[g.first].max_depth);
+        if (g.count > 1 && grid_f == 0) {
+            smem_f = wavefront_smem_bytes(tp, h->mode, tp.scene_in_smem, true);
+            const int occ = occupancy(ctx, h->mode, tp.n_lights > 0, true, smem_f);
+            if (occ <= 0) return fail(RT_ERR_UNSUPPORTED, "no launch configuration of the multi-frame trace kernel fits shared memory");
+            grid_f = ctx->sm_count * occ;
+        }
+    }
+    sub.grid = std::max(h->grid, grid_f);
+    const uint32_t threads_total = (uint32_t)sub.grid * (uint32_t)kBlock;   // ray slots of the widest grid: columns of the per-slot global arrays
+    int rc = prepare_work(W, tp, threads_total, max_depth, sbuf, sub.batches);
     if (rc != RT_OK) return rc;
-    tp.stack_stride = threads_total;
-    // event ring: every pending frame owns 2 + 2*n_batches events (begin, end, and a pair around each trace launch)
-    const uint32_t kRing = 64, per_frame = 2 + 2 * n_batches;
-    if (h->pending_frames >= kRing) return fail(RT_ERR_INVALID, "more than 64 frames enqueued without rtb200_render_device_wait");
-    while (h->ev.size() < (size_t)(h->pending_frames + 1) * per_frame) {
+    if (grid_f) {   // the multi-frame kernel reads each frame's camera and key from this table
+        std::vector<FrameRec> tab(n);
+        for (uint32_t i = 0; i < n; ++i) {
+            tab[i].cam = frames[i].camera; tab[i].key0 = (uint32_t)frames[i].seed; tab[i].key1 = (uint32_t)(frames[i].seed >> 32);
+        }
+        sub.ftab_bytes = (uint64_t)n * sizeof(FrameRec);
+        CU(W.ftab.ensure(sub.ftab_bytes));
+        CU(cudaMemcpyAsync(W.ftab.p, tab.data(), sub.ftab_bytes, cudaMemcpyHostToDevice, st));
+    }
+    sub.n_ev = 2 + 2 * sub.batches;
+    while (h->ev.size() < (size_t)sub.ev0 + sub.n_ev) {
         cudaEvent_t e;
         if (!ctx->event_pool.empty()) { e = ctx->event_pool.back(); ctx->event_pool.pop_back(); }
         else CU(cudaEventCreate(&e));
         h->ev.push_back(e);
     }
-    cudaEvent_t* fev = h->ev.data() + (size_t)h->pending_frames * per_frame;
+    cudaEvent_t* ev = h->ev.data() + sub.ev0;
     unsigned int* counters = (unsigned int*)((char*)W.small.p + 256);
-    if ((rc = clear_stats(W, n_batches, st)) != RT_OK) return rc;
+    if ((rc = clear_stats(W, sub.batches, st)) != RT_OK) return rc;
 
-    CU(cudaEventRecord(fev[0], st));
-    if ((rc = enqueue_batches(h, tp, W, dev_rgb8, dev_linear_f32, counters, fev + 2, st)) != RT_OK) return rc;
-    CU(cudaEventRecord(fev[1], st));
-    h->last_batches = n_batches; h->last_launches = 2 * n_batches;
-    ++h->pending_frames;
+    CU(cudaEventRecord(ev[0], st));
+    uint32_t b = 0;   // trace launch (or black memset) index: its queue counter and its event pair
+    for (const FrameGroup& g : groups) {
+        const rt_frame& f0 = frames[g.first];
+        uint8_t* o8 = dev_rgb8 ? (uint8_t*)dev_rgb8 + (size_t)g.first * npl * 3 : nullptr;
+        float* ol = dev_linear_f32 ? (float*)dev_linear_f32 + (size_t)g.first * npl * 3 : nullptr;
+        TraceParams q = tp;
+        q.max_depth = f0.max_depth;
+        if (g.count == 1) {
+            q.cam = f0.camera; q.key0 = (uint32_t)f0.seed; q.key1 = (uint32_t)(f0.seed >> 32);
+            q.stack_stride = (uint32_t)h->grid * (uint32_t)kBlock;
+            for (uint32_t k = 0; k < n_batches; ++k, ++b) {
+                q.s0 = k * spb;
+                q.s_count = std::min(spb, spp - q.s0);
+                q.total_work = q.s_count * q.npix_local;
+                q.work_counter = counters + b;
+                CU(cudaEventRecord(ev[2 + 2 * b], st));
+                if (q.max_depth == 0) {
+                    CU(cudaMemsetAsync(q.samplebuf, 0, (size_t)q.total_work * 16, st));   // ray_color(depth 0) = black, no ray (raytracer.rs:80-82)
+                } else {
+                    CU(launch_wavefront(q, h->mode, false, h->grid, h->smem, st));
+                }
+                CU(cudaEventRecord(ev[3 + 2 * b], st));
+                ResolveParams r{};
+                r.samplebuf = q.samplebuf; r.accum = (float*)W.accum.p; r.npix_local = q.npix_local; r.s_count = q.s_count;
+                r.first = k == 0; r.last = k + 1 == n_batches; r.spp = spp;
+                r.out_linear = ol; r.out_rgb8 = o8;
+                CU(launch_resolve(r, st));
+            }
+            sub.launches += 2 * n_batches;
+            if (f0.max_depth == 0) sub.black_samples += frame_work;
+            continue;
+        }
+        q.ftab = (const FrameRec*)W.ftab.p + g.first; q.frame_work = (uint32_t)frame_work;
+        q.s0 = 0; q.s_count = spp; q.total_work = (uint32_t)(g.count * frame_work);
+        q.work_counter = counters + b;
+        q.stack_stride = (uint32_t)grid_f * (uint32_t)kBlock;
+        CU(cudaEventRecord(ev[2 + 2 * b], st));
+        CU(launch_wavefront(q, h->mode, true, grid_f, smem_f, st));
+        CU(cudaEventRecord(ev[3 + 2 * b], st));
+        for (uint32_t k = 0; k < g.count; ++k) {   // samplebuf [frame][sample][pixel]: frame k's samples are one batch
+            ResolveParams r{};
+            r.samplebuf = q.samplebuf + (size_t)k * frame_work; r.accum = (float*)W.accum.p; r.npix_local = (uint32_t)npl; r.s_count = spp;
+            r.first = 1; r.last = 1; r.spp = spp;
+            r.out_linear = ol ? ol + (size_t)k * npl * 3 : nullptr; r.out_rgb8 = o8 ? o8 + (size_t)k * npl * 3 : nullptr;
+            CU(launch_resolve(r, st));
+        }
+        b += 1; sub.launches += 1 + g.count;
+    }
+    CU(cudaEventRecord(ev[1], st));
+    h->pending.push_back(sub);
     return RT_OK;
 }
 
@@ -591,64 +688,69 @@ static void print_diagnostics(const unsigned long long* hstat, int grid) {
     }
 }
 
-// Wait for the frames of `h` enqueued so far and fetch statistics (counters: the last frame's; times: summed over the frames).
+// Wait for the pending submissions of h and report them (stats may be NULL). Counters, batches and the diagnostics are the
+// last submission's; times, frames, kernel launches and frame-table bytes are summed over the submissions.
 static int render_collect(rtb200_scene_handle h, rt_stats* stats) {
-    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
-    DeviceCtx* ctx = h->ctx;
-    CU(cudaSetDevice(h->device));
     if (stats) memset(stats, 0, sizeof *stats);
-    if (h->tp.npix_local == 0 || h->last_batches == 0 || h->pending_frames == 0) { h->pending_frames = 0; h->n_streams = 0; return RT_OK; }
-    cudaStream_t st = h->last_stream;
-    DeviceCtx::WorkSet& W = ctx->ws[h->last_set];
+    if (h->pending.empty()) return RT_OK;
+    CU(cudaSetDevice(h->device));
+    const rtb200_scene_t::Submission last = h->pending.back();
+    for (const auto& p : h->pending) if (p.stream != last.stream) CU(cudaStreamSynchronize(p.stream));
     unsigned long long hstat[32] = {0}, herr[2] = {0, 0};   // the whole 256-byte stat block
-    for (int i = 0; i < h->n_streams; ++i) if (h->streams[i] != st) CU(cudaStreamSynchronize(h->streams[i]));
-    h->n_streams = 0;
-    // error counters accumulate over every frame since the last wait (each frame adds to them; nothing clears them in between)
-    CU(cudaMemcpyAsync(hstat, W.small.p, sizeof hstat, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(herr, h->err, sizeof herr, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    if (herr[0] | herr[1]) CU(cudaMemset(h->err, 0, sizeof herr));
-    const uint32_t frames = h->pending_frames;
-    h->pending_frames = 0;
-    if (herr[1] != 0) return fail(RT_ERR_CUDA, "internal error: the traversal guard tripped; the frame is not valid");
-    if (herr[0] != 0) return fail(RT_ERR_UNSUPPORTED, "light-test recursion deeper than the shadow-frame stack occurred in one of the frames; it is not exact (the reference recursion is near-critical for this many lights)");
-    if (stats) {
-        float ms = 0.f;
-        double dv = 0.0, tr = 0.0;
-        const uint32_t per_frame = 2 + 2 * h->last_batches;
-        for (uint32_t f = 0; f < frames; ++f) {
-            cudaEvent_t* fev = h->ev.data() + (size_t)f * per_frame;
-            CU(cudaEventElapsedTime(&ms, fev[0], fev[1])); dv += ms;
-            for (uint32_t b = 0; b < h->last_batches; ++b) { CU(cudaEventElapsedTime(&ms, fev[2 + 2 * b], fev[3 + 2 * b])); tr += ms; }
-        }
-        stats->device_ms = dv; stats->trace_ms = tr; stats->frames = frames;
-        stats->rays = hstat[0]; stats->candidates = hstat[1]; stats->samples = hstat[3]; stats->clusters = hstat[4]; stats->nodes = hstat[6];
-        stats->gpus_used = 1;
-        print_diagnostics(hstat, h->grid);   // last batch of the last frame
-        if (h->tp.max_depth == 0) stats->samples = (uint64_t)h->tp.npix_local * h->tp.spp;   // no kernel ran: every sample is black
-        stats->kernel_launches = h->last_launches * frames; stats->batches = h->last_batches;
+    if (last.n_ev) {
+        // error counters accumulate over every frame since the last collect (each frame adds to them; nothing clears them in between)
+        CU(cudaMemcpyAsync(hstat, h->ctx->ws[last.set].small.p, sizeof hstat, cudaMemcpyDeviceToHost, last.stream));
+        CU(cudaMemcpyAsync(herr, h->err, sizeof herr, cudaMemcpyDeviceToHost, last.stream));
     }
+    CU(cudaStreamSynchronize(last.stream));
+    if (herr[0] | herr[1]) CU(cudaMemset(h->err, 0, sizeof herr));
+    std::vector<rtb200_scene_t::Submission> subs;
+    subs.swap(h->pending);
+    if (herr[1] != 0) return fail(RT_ERR_CUDA, "internal error: the traversal guard tripped; the frames are not valid");
+    if (herr[0] != 0) return fail(RT_ERR_UNSUPPORTED, "light-test recursion deeper than the shadow-frame stack occurred in one of the frames; it is not exact (the reference recursion is near-critical for this many lights)");
+    if (!stats) return RT_OK;
+    float ms = 0.f;
+    for (const auto& p : subs) {
+        const cudaEvent_t* ev = h->ev.data() + p.ev0;
+        if (p.n_ev) { CU(cudaEventElapsedTime(&ms, ev[0], ev[1])); stats->device_ms += ms; }
+        for (uint32_t b = 0; b < p.batches; ++b) { CU(cudaEventElapsedTime(&ms, ev[2 + 2 * b], ev[3 + 2 * b])); stats->trace_ms += ms; }
+        stats->frames += p.frames; stats->kernel_launches += p.launches; stats->h2d_bytes += p.ftab_bytes;
+    }
+    stats->rays = hstat[0]; stats->candidates = hstat[1]; stats->samples = hstat[3] + last.black_samples; stats->clusters = hstat[4]; stats->nodes = hstat[6];
+    stats->batches = last.batches; stats->gpus_used = 1;
+    if (last.n_ev) print_diagnostics(hstat, last.grid);   // every launch of the last submission: the tail is one launch's when it made one
     return RT_OK;
 }
 
-int rtb200_render_device(rtb200_scene_handle h, void* dev_rgb8, void* dev_linear_f32, void* stream_in, rt_stats* stats) {
-    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+// Drain the asynchronous frames of h, render `frames` on work set 0 and wait for them.
+static int render_blocking(rtb200_scene_handle h, const rt_frame* frames, uint32_t n, void* dev_rgb8, void* dev_linear_f32,
+                           void* stream_in, rt_stats* stats) {
     auto wall0 = std::chrono::steady_clock::now();
     DeviceRestore restore;
     std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
-    if (h->pending_frames) { int rcw = render_collect(h, nullptr); if (rcw != RT_OK) return rcw; }   // drain frames enqueued earlier
-    int rc = render_enqueue(h, dev_rgb8, dev_linear_f32, stream_in, 0);
-    if (rc != RT_OK) return rc;
-    rc = render_collect(h, stats);
+    int rc = render_collect(h, nullptr);
+    if (rc == RT_OK) rc = render_enqueue(h, frames, n, dev_rgb8, dev_linear_f32, stream_in, 0);
+    if (rc == RT_OK) rc = render_collect(h, stats);
     if (rc == RT_OK && stats) stats->wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count();
     return rc;
 }
 
+int rtb200_render_device(rtb200_scene_handle h, void* dev_rgb8, void* dev_linear_f32, void* stream_in, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    const rt_frame f = own_frame(h);
+    return render_blocking(h, &f, 1, dev_rgb8, dev_linear_f32, stream_in, stats);
+  });
+}
+
 int rtb200_render_device_async(rtb200_scene_handle h, void* dev_rgb8, void* dev_linear_f32, void* stream_in) {
+  return guarded([&]() -> int {
     if (!h) return fail(RT_ERR_INVALID, "null scene handle");
     DeviceRestore restore;
     std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
-    return render_enqueue(h, dev_rgb8, dev_linear_f32, stream_in, (int)(h->frame_counter++ & 1u));
+    const rt_frame f = own_frame(h);
+    return render_enqueue(h, &f, 1, dev_rgb8, dev_linear_f32, stream_in, (int)(h->frame_counter++ & 1u));
+  });
 }
 
 int rtb200_render_device_wait(rtb200_scene_handle h, rt_stats* stats) {
@@ -658,151 +760,6 @@ int rtb200_render_device_wait(rtb200_scene_handle h, rt_stats* stats) {
     return render_collect(h, stats);
 }
 
-// ---- animations: several frames of one resident scene in as few trace launches as the sample buffer allows ----
-// A launch group is a run of consecutive frames with equal max_depth (a launch scalar) whose samples all fit the
-// sample-buffer cap and the u32 work ids. A group of F >= 2 frames is ONE launch of the multi-frame trace kernel - the
-// stragglers of frame i finish while frame i+1's work is handed out, so only the group's last frame pays the frame tail -
-// followed by one resolve per frame; a frame that fits with no other, and every max_depth 0 frame, takes the single-frame
-// path with its sample batches. So does a frame of more than kGroupMaxFrameWork samples: its own tail is a few per cent of
-// its time at most, and the multi-frame kernel, which keeps the Philox key in registers instead of the parameter block,
-// spills more and traced 800x600x128 frames 5 % slower than the single-frame kernel on an H100 (DESIGN.md §4.6).
-struct FrameGroup { uint32_t first, count; };
-constexpr uint64_t kGroupMaxFrameWork = 1ull << 24;   // samples per frame (spp * rows * width): ~8 ms of tracing on an H100
-
-static std::vector<FrameGroup> frame_groups(const rt_frame* frames, uint32_t n, uint64_t frame_work, uint64_t cap) {
-    std::vector<FrameGroup> groups;
-    for (uint32_t i = 0; i < n;) {
-        uint64_t F = 1;
-        if (frames[i].max_depth != 0 && frame_work <= kGroupMaxFrameWork)
-            while (i + F < n && frames[i + F].max_depth == frames[i].max_depth && (F + 1) * frame_work < (1ull << 31) && (F + 1) * frame_work * 16ull <= cap) ++F;
-        groups.push_back(FrameGroup{i, (uint32_t)F});
-        i += (uint32_t)F;
-    }
-    return groups;
-}
-
-// rt_frame checks shared by both entry points (no device is touched)
-static int check_frames(const rt_frame* frames, uint32_t n, uint64_t rows, uint64_t width) {
-    if (n == 0) return fail(RT_ERR_INVALID, "n_frames must be > 0");
-    if (!frames) return fail(RT_ERR_INVALID, "frames is null");
-    const uint64_t per_frame = rows * width * 3ull;   // < 2^33: width * height < 2^31 (validate_scene)
-    if (per_frame != 0 && (uint64_t)n > ~0ull / per_frame) return fail(RT_ERR_INVALID, "n_frames * rows * width * 3 overflows 64 bits");
-    for (uint32_t i = 0; i < n; ++i)
-        if (frames[i].reserved != 0) return fail(RT_ERR_INVALID, "rt_frame.reserved must be 0 (frame " + std::to_string(i) + ")");
-    return RT_OK;
-}
-
-// The frames of rtb200_render_frames_device on work set 0; the handle's lock is held and no frame of it is in flight.
-static int render_frames_run(rtb200_scene_handle h, const rt_frame* frames, uint32_t n, void* dev_rgb8, void* dev_linear_f32,
-                             void* stream_in, rt_stats* stats) {
-    DeviceCtx* ctx = h->ctx;
-    DeviceCtx::WorkSet& W = ctx->ws[0];
-    CU(cudaSetDevice(h->device));
-    cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
-    if (st != ctx->stream) CU(cudaStreamWaitEvent(st, ctx->staging_free, 0));   // the scene upload ran on the context's stream
-    if (stats) { memset(stats, 0, sizeof *stats); stats->frames = n; stats->gpus_used = 1; }
-    TraceParams tp = h->tp;   // the handle's own view stays as uploaded
-    const uint64_t npl = tp.npix_local;
-    if (npl == 0) return RT_OK;
-    const uint32_t spp = tp.spp, spb = h->spp_batch, n_batches = (spp + spb - 1) / spb;
-    const uint64_t frame_work = (uint64_t)spp * npl;
-    const uint64_t cap = h->opts.sample_buffer_bytes ? h->opts.sample_buffer_bytes : (1ull << 30);
-    const std::vector<FrameGroup> groups = frame_groups(frames, n, frame_work, cap);
-
-    // launch geometry of the multi-frame kernel (its pool also holds the slots' frames)
-    size_t smem_f = 0;
-    int grid_f = 0;
-    uint32_t n_batches_total = 0, max_depth = 1;   // trace launches (or black memsets) of the call
-    size_t sbuf = 0;
-    for (const FrameGroup& g : groups) {
-        n_batches_total += g.count > 1 ? 1u : n_batches;
-        sbuf = std::max(sbuf, g.count > 1 ? (size_t)(g.count * frame_work * 16) : (size_t)spb * npl * 16);
-        max_depth = std::max(max_depth, frames[g.first].max_depth);
-        if (g.count > 1 && grid_f == 0) {
-            smem_f = wavefront_smem_bytes(tp, h->mode, tp.scene_in_smem, true);
-            const int occ = occupancy(ctx, h->mode, tp.n_lights > 0, true, smem_f);
-            if (occ <= 0) return fail(RT_ERR_UNSUPPORTED, "no launch configuration of the multi-frame trace kernel fits shared memory");
-            grid_f = ctx->sm_count * occ;
-        }
-    }
-    const uint32_t threads_total = (uint32_t)std::max(h->grid, grid_f) * (uint32_t)kBlock;
-    int rc = prepare_work(W, tp, threads_total, max_depth, sbuf, n_batches_total);
-    if (rc != RT_OK) return rc;
-    CU(W.ftab.ensure((size_t)n * sizeof(FrameRec)));
-    std::vector<FrameRec> tab(n);
-    for (uint32_t i = 0; i < n; ++i) {
-        tab[i].cam = frames[i].camera; tab[i].key0 = (uint32_t)frames[i].seed; tab[i].key1 = (uint32_t)(frames[i].seed >> 32);
-    }
-    // events: begin, end, and a pair around each trace launch
-    while (h->ev.size() < 2 + 2 * (size_t)n_batches_total) {
-        cudaEvent_t e;
-        if (!ctx->event_pool.empty()) { e = ctx->event_pool.back(); ctx->event_pool.pop_back(); }
-        else CU(cudaEventCreate(&e));
-        h->ev.push_back(e);
-    }
-    cudaEvent_t* ev = h->ev.data();
-    unsigned int* counters = (unsigned int*)((char*)W.small.p + 256);
-    const FrameRec* dtab = (const FrameRec*)W.ftab.p;
-    CU(cudaMemcpyAsync(W.ftab.p, tab.data(), (size_t)n * sizeof(FrameRec), cudaMemcpyHostToDevice, st));
-    if ((rc = clear_stats(W, n_batches_total, st)) != RT_OK) return rc;
-
-    CU(cudaEventRecord(ev[0], st));
-    uint32_t b = 0, launches = 0;
-    uint64_t black_samples = 0;   // samples of max_depth 0 frames: black, no kernel counts them
-    for (const FrameGroup& g : groups) {
-        const rt_frame& f0 = frames[g.first];
-        uint8_t* o8 = dev_rgb8 ? (uint8_t*)dev_rgb8 + (size_t)g.first * npl * 3 : nullptr;
-        float* ol = dev_linear_f32 ? (float*)dev_linear_f32 + (size_t)g.first * npl * 3 : nullptr;
-        TraceParams q = tp;
-        q.max_depth = f0.max_depth;
-        if (g.count == 1) {
-            q.cam = tab[g.first].cam; q.key0 = tab[g.first].key0; q.key1 = tab[g.first].key1;
-            q.stack_stride = (uint32_t)h->grid * (uint32_t)kBlock;
-            if ((rc = enqueue_batches(h, q, W, o8, ol, counters + b, ev + 2 + 2 * b, st)) != RT_OK) return rc;
-            b += n_batches; launches += 2 * n_batches;
-            if (f0.max_depth == 0) black_samples += frame_work;
-            continue;
-        }
-        q.ftab = dtab + g.first; q.frame_work = (uint32_t)frame_work;
-        q.s0 = 0; q.s_count = spp; q.total_work = (uint32_t)(g.count * frame_work);
-        q.work_counter = counters + b;
-        q.stack_stride = (uint32_t)grid_f * (uint32_t)kBlock;
-        CU(cudaEventRecord(ev[2 + 2 * b], st));
-        CU(launch_wavefront(q, h->mode, true, grid_f, smem_f, st));
-        CU(cudaEventRecord(ev[3 + 2 * b], st));
-        for (uint32_t k = 0; k < g.count; ++k) {   // samplebuf [frame][sample][pixel]: frame k's samples are one batch
-            ResolveParams r{};
-            r.samplebuf = q.samplebuf + (size_t)k * frame_work; r.accum = (float*)W.accum.p; r.npix_local = (uint32_t)npl; r.s_count = spp;
-            r.first = 1; r.last = 1; r.spp = spp;
-            r.out_linear = ol ? ol + (size_t)k * npl * 3 : nullptr; r.out_rgb8 = o8 ? o8 + (size_t)k * npl * 3 : nullptr;
-            CU(launch_resolve(r, st));
-        }
-        b += 1; launches += 1 + g.count;
-    }
-    CU(cudaEventRecord(ev[1], st));
-
-    unsigned long long hstat[32] = {0}, herr[2] = {0, 0};   // the whole 256-byte stat block, summed over the call's launches
-    CU(cudaMemcpyAsync(hstat, W.small.p, sizeof hstat, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(herr, h->err, sizeof herr, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    if (herr[0] | herr[1]) CU(cudaMemset(h->err, 0, sizeof herr));
-    if (herr[1] != 0) return fail(RT_ERR_CUDA, "internal error: the traversal guard tripped; the frames are not valid");
-    if (herr[0] != 0) return fail(RT_ERR_UNSUPPORTED, "light-test recursion deeper than the shadow-frame stack occurred in one of the frames; it is not exact (the reference recursion is near-critical for this many lights)");
-    if (stats) {
-        float ms = 0.f;
-        CU(cudaEventElapsedTime(&ms, ev[0], ev[1]));
-        stats->device_ms = ms;
-        double tr = 0.0;
-        for (uint32_t k = 0; k < b; ++k) { CU(cudaEventElapsedTime(&ms, ev[2 + 2 * k], ev[3 + 2 * k])); tr += ms; }
-        stats->trace_ms = tr;
-        stats->rays = hstat[0]; stats->candidates = hstat[1]; stats->samples = hstat[3] + black_samples; stats->clusters = hstat[4]; stats->nodes = hstat[6];
-        stats->kernel_launches = launches; stats->batches = b;
-        stats->h2d_bytes = (uint64_t)n * sizeof(FrameRec);
-        print_diagnostics(hstat, std::max(h->grid, grid_f));   // every launch of the call: the tail is one launch's when the call made one
-    }
-    return RT_OK;
-}
-
 int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, uint32_t n_frames, void* dev_rgb8, void* dev_linear_f32,
                                 void* stream_in, rt_stats* stats) {
   return guarded([&]() -> int {
@@ -810,63 +767,14 @@ int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, u
     int rc = check_frames(frames, n_frames, h->tp.rows_local, h->tp.width);
     if (rc != RT_OK) return rc;
     if (!dev_rgb8 && !dev_linear_f32) return fail(RT_ERR_INVALID, "dev_rgb8 and dev_linear_f32 are both null");
-    auto wall0 = std::chrono::steady_clock::now();
-    DeviceRestore restore;
-    std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
-    if (h->pending_frames) { if ((rc = render_collect(h, nullptr)) != RT_OK) return rc; }   // drain frames enqueued earlier
-    rc = render_frames_run(h, frames, n_frames, dev_rgb8, dev_linear_f32, stream_in, stats);
-    if (rc == RT_OK && stats) stats->wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count();
-    return rc;
+    return render_blocking(h, frames, n_frames, dev_rgb8, dev_linear_f32, stream_in, stats);
   });
 }
 
-static int render_host(const rt_scene* s, const rt_options* opts, uint8_t* out_rgb8, float* out_lin, rt_stats* stats) {
-    auto wall0 = std::chrono::steady_clock::now();
-    DeviceRestore restore;
-    rtb200_scene_handle h = nullptr;
-    int rc = rtb200_scene_upload(s, opts, &h);
-    if (rc != RT_OK) return rc;
-    DeviceCtx* ctx = h->ctx;
-    std::lock_guard<std::recursive_mutex> lk(ctx->mu);
-    cudaSetDevice(h->device);
-    size_t npl = h->tp.npix_local;
-    void *d8 = nullptr, *dl = nullptr;
-    cudaError_t e = cudaSuccess;
-    if (out_rgb8) { e = ctx->out_rgb8.ensure(npl * 3 + 16); d8 = ctx->out_rgb8.p; }
-    if (e == cudaSuccess && out_lin) { e = ctx->out_lin.ensure(npl * 12 + 16); dl = ctx->out_lin.p; }
-    if (e != cudaSuccess) { rtb200_scene_release(h); return fail_cuda(e, "output buffer allocation"); }
-    rt_stats st{};
-    rc = rtb200_render_device(h, d8, dl, nullptr, &st);
-    if (rc == RT_OK && npl) {
-        if (out_rgb8) e = cudaMemcpyAsync(out_rgb8, d8, npl * 3, cudaMemcpyDeviceToHost, ctx->stream);
-        if (e == cudaSuccess && out_lin) e = cudaMemcpyAsync(out_lin, dl, npl * 12, cudaMemcpyDeviceToHost, ctx->stream);
-        if (e == cudaSuccess) e = cudaStreamSynchronize(ctx->stream);
-        if (e != cudaSuccess) rc = fail_cuda(e, "device->host copy of the frame");
-    }
-    st.h2d_bytes = h->h2d_bytes;
-    st.d2h_bytes = (out_rgb8 ? npl * 3 : 0) + (out_lin ? npl * 12 : 0) + 128 + 16;
-    std::string keep = g_last_error;
-    rtb200_scene_release(h);
-    if (rc != RT_OK) g_last_error = keep;
-    st.wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count();
-    if (stats) *stats = st;
-    return rc;
-}
-
-int rtb200_render_rgb8(const rt_scene* scene, const rt_options* opts, uint8_t* out_rgb8, rt_stats* stats) {
-    if (!scene || !out_rgb8) return fail(RT_ERR_INVALID, "null argument");
-    return guarded([&]() -> int { return render_host(scene, opts, out_rgb8, nullptr, stats); });
-}
-int rtb200_render_linear_f32(const rt_scene* scene, const rt_options* opts, float* out_rgb, rt_stats* stats) {
-    if (!scene || !out_rgb) return fail(RT_ERR_INVALID, "null argument");
-    return guarded([&]() -> int { return render_host(scene, opts, nullptr, out_rgb, stats); });
-}
-
-int rtb200_render_frames(const rt_scene* s, const rt_options* opts_in, const rt_frame* frames, uint32_t n_frames, uint8_t* out_rgb8,
-                         float* out_lin, rt_stats* stats) {
-  return guarded([&]() -> int {
-    if (!s) return fail(RT_ERR_INVALID, "null argument");
-    if (!out_rgb8 && !out_lin) return fail(RT_ERR_INVALID, "out_rgb8 and out_linear_f32 are both null");
+// Host buffers: upload the scene, render `frames` into the context's output buffers, copy them to the host and release the
+// scene. The single-frame calls pass the scene's own view as one frame.
+static int render_host(const rt_scene* s, const rt_options* opts_in, const rt_frame* frames, uint32_t n_frames, uint8_t* out_rgb8,
+                       float* out_lin, rt_stats* stats) {
     rt_options opts;
     int rc = normalise_options(opts_in, &opts);
     if (rc != RT_OK) return rc;
@@ -877,7 +785,7 @@ int rtb200_render_frames(const rt_scene* s, const rt_options* opts_in, const rt_
     DeviceRestore restore;
     rtb200_scene_handle h = nullptr;
     if ((rc = rtb200_scene_upload(s, &opts, &h)) != RT_OK) return rc;
-    struct Rel { rtb200_scene_handle h; ~Rel() { std::string keep = g_last_error; rtb200_scene_release(h); g_last_error = keep; } } rel{h};
+    ReleaseGuard rel{h};
     DeviceCtx* ctx = h->ctx;
     std::lock_guard<std::recursive_mutex> lk(ctx->mu);
     CU(cudaSetDevice(h->device));
@@ -886,7 +794,7 @@ int rtb200_render_frames(const rt_scene* s, const rt_options* opts_in, const rt_
     if (out_rgb8) { CU(ctx->out_rgb8.ensure(total * 3 + 16)); d8 = ctx->out_rgb8.p; }
     if (out_lin) { CU(ctx->out_lin.ensure(total * 12 + 16)); dl = ctx->out_lin.p; }
     rt_stats st{};
-    if ((rc = rtb200_render_frames_device(h, frames, n_frames, d8, dl, nullptr, &st)) != RT_OK) return rc;
+    if ((rc = render_blocking(h, frames, n_frames, d8, dl, nullptr, &st)) != RT_OK) return rc;
     if (total) {
         if (out_rgb8) CU(cudaMemcpyAsync(out_rgb8, d8, total * 3, cudaMemcpyDeviceToHost, ctx->stream));
         if (out_lin) CU(cudaMemcpyAsync(out_lin, dl, total * 12, cudaMemcpyDeviceToHost, ctx->stream));
@@ -897,6 +805,25 @@ int rtb200_render_frames(const rt_scene* s, const rt_options* opts_in, const rt_
     st.wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count();
     if (stats) *stats = st;
     return RT_OK;
+}
+
+int rtb200_render_rgb8(const rt_scene* scene, const rt_options* opts, uint8_t* out_rgb8, rt_stats* stats) {
+    if (!scene || !out_rgb8) return fail(RT_ERR_INVALID, "null argument");
+    const rt_frame f{scene->camera, scene->seed, scene->max_depth, 0};
+    return guarded([&]() -> int { return render_host(scene, opts, &f, 1, out_rgb8, nullptr, stats); });
+}
+int rtb200_render_linear_f32(const rt_scene* scene, const rt_options* opts, float* out_rgb, rt_stats* stats) {
+    if (!scene || !out_rgb) return fail(RT_ERR_INVALID, "null argument");
+    const rt_frame f{scene->camera, scene->seed, scene->max_depth, 0};
+    return guarded([&]() -> int { return render_host(scene, opts, &f, 1, nullptr, out_rgb, stats); });
+}
+
+int rtb200_render_frames(const rt_scene* s, const rt_options* opts_in, const rt_frame* frames, uint32_t n_frames, uint8_t* out_rgb8,
+                         float* out_lin, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (!s) return fail(RT_ERR_INVALID, "null argument");
+    if (!out_rgb8 && !out_lin) return fail(RT_ERR_INVALID, "out_rgb8 and out_linear_f32 are both null");
+    return render_host(s, opts_in, frames, n_frames, out_rgb8, out_lin, stats);
   });
 }
 
@@ -926,7 +853,11 @@ int rtb200_render_rgb8_multi(const rt_scene* s, const rt_options* opts_in, int32
     G = std::min(G, 64 - first);   // device contexts exist for ordinals below 64
     const uint32_t bands = (s->height + base.band_rows - 1) / base.band_rows;
     G = (int)std::min<uint32_t>((uint32_t)G, bands);   // a device needs at least one band
-    if (G <= 1) { base.device = first; int r = render_host(s, &base, out_rgb8, nullptr, stats); if (r == RT_OK && stats) stats->gpus_used = 1; return r; }
+    if (G <= 1) {
+        base.device = first;
+        const rt_frame f{s->camera, s->seed, s->max_depth, 0};
+        return render_host(s, &base, &f, 1, out_rgb8, nullptr, stats);
+    }
 
     DeviceRestore restore;
     std::lock_guard<std::mutex> multi_lock(g_multi_mu);
@@ -958,13 +889,14 @@ int rtb200_render_rgb8_multi(const rt_scene* s, const rt_options* opts_in, int32
             rtb200_scene_handle h = nullptr;
             int rcw = scene_upload_records(s, o, n_lights, R, &h);
             if (rcw != RT_OK) return rcw;
-            struct Rel { rtb200_scene_handle h; ~Rel() { std::string keep = g_last_error; rtb200_scene_release(h); g_last_error = keep; } } rel{h};
+            ReleaseGuard rel{h};
             DeviceCtx* c = h->ctx;
             std::lock_guard<std::recursive_mutex> lk(c->mu);
             CU(cudaSetDevice(first + g));
             const size_t rows = h->tp.rows_local;
             CU(c->out_rgb8.ensure(rows * row_bytes + 16));
-            if ((rcw = render_enqueue(h, c->out_rgb8.p, nullptr, nullptr, 0)) != RT_OK) return rcw;
+            const rt_frame f = own_frame(h);
+            if ((rcw = render_enqueue(h, &f, 1, c->out_rgb8.p, nullptr, nullptr, 0)) != RT_OK) return rcw;
             // shard -> frame: full bands as one strided 2-D copy (a "row" of the copy = one band), then the partial last band
             const size_t band_bytes = (size_t)base.band_rows * row_bytes;
             const size_t full = rows / base.band_rows, rem = rows - full * base.band_rows;

@@ -222,6 +222,30 @@ int rtb200_render_frames(const rt_scene* scene, const rt_options* opts, const rt
 int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, uint32_t n_frames,
                                 void* dev_rgb8, void* dev_linear_f32, void* stream, rt_stats* stats);
 
+/* ---- moving spheres of a resident scene ---------------------------------------------------------------------------------
+ * The hierarchy is refitted on the GPU (its topology and recentring stay as uploaded, DESIGN.md §4.7) instead of rebuilt.
+ * Contract: after an update every render of h is bit-identical, in linear f32, RGB8 and ray count, to the same render of a
+ * fresh upload of the edited scene (the diagnostic candidates / clusters / nodes counters may differ: the tree differs).
+ * Stream-ordered, without waiting for the GPU: the update runs on `stream` (NULL: the library's stream) after every frame of
+ * h already enqueued, on any stream, and before every frame enqueued later; rtb200_scene_release waits for it. The first
+ * update of a handle builds the refit's scratch and waits for the library's stream once.
+ * Spheres that no longer fit the f32 frame (non-finite, or max|c - recentre| + |radius| >= 1e15) are tested in f64 by every
+ * ray; the tree gets slower as spheres wander from where they were uploaded: upload again to rebuild it. */
+/* Replace spheres index[k] (k < n) of a resident scene by spheres[k]: centre, radius and material. Everything is checked on
+ * the host before anything is enqueued (on error the scene is unchanged); n == 0 is a no-op. RT_ERR_INVALID: NULL arrays, an
+ * index >= n_spheres, a repeated index, an unknown kind, a texture index outside the uploaded textures (or one whose image was
+ * empty). RT_ERR_UNSUPPORTED: making a sphere a light or a light something else (the light set is fixed at upload; a light may
+ * move). The input is copied into pinned staging memory before the call returns. */
+int rtb200_scene_update_spheres(rtb200_scene_handle h, const uint32_t* index, const rt_sphere* spheres, uint32_t n, void* stream);
+/* Replace the centre and radius of EVERY sphere from device memory: n_spheres x {cx, cy, cz, radius} f64 (the layout of the geo
+ * array); materials stay. Any values are accepted. RT_ERR_INVALID for a NULL pointer or one that is not device memory of h's
+ * device or managed memory. The caller keeps the buffer unchanged until the update has run on `stream`. */
+int rtb200_scene_update_geometry_device(rtb200_scene_handle h, const void* dev_center_radius, void* stream);
+/* Diagnostic: D2H copy of the handle's current nodes / leaf records / flat records (RT_VARIANT_BRUTE_FORCE only) / exact geometry
+ * {cx,cy,cz,radius}, laid out as rtb200_debug_bvh's (same info[]); arrays are filled up to their capacities (elements). */
+int rtb200_scene_debug_records(rtb200_scene_handle h, uint32_t info[8], float* nodes, uint64_t cap_nodes, float* leaf_rec,
+                               uint64_t cap_leaf_rec, float* flat, uint64_t cap_flat, double* geo, uint64_t cap_geo);
+
 /* load_texture_image — materials.rs:213-219, config.rs:36-47: decode a baseline JPEG file to RGB8 (host-side scene staging
  * helper for hosts without their own decoder; the reference uses the jpeg-decoder crate). *out_rgb8 is released with rtb200_free(). */
 int  rtb200_decode_jpeg_file(const char* path, uint8_t** out_rgb8, uint64_t* width, uint64_t* height);

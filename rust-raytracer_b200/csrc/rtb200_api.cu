@@ -188,6 +188,16 @@ struct rtb200_scene_t {
     std::vector<Submission> pending;     // enqueued since the last render_collect, oldest first
     uint32_t frame_counter = 0;
     uint64_t h2d_bytes = 0;
+    // ---- moving spheres (rtb200_scene_update_*): what the upload fixed, and the refit's scratch built at the first update ----
+    std::vector<uint32_t> light_idx;     // the Light spheres, increasing
+    std::vector<uint8_t> tex_ok;         // uploaded textures a Texture sphere may use
+    cudaEvent_t updated = nullptr;       // recorded after the last update; every later frame waits for it
+    void* refit = nullptr;               // node_box, leaf_box, level_nodes
+    double* node_box = nullptr;          // n_nodes exact boxes {lo[3], hi[3]}
+    double* leaf_box = nullptr;          // n_leaves exact boxes
+    uint32_t* level_nodes = nullptr;     // node indices grouped by tree level, deepest level first
+    std::vector<uint32_t> level_off;     // a level's nodes are level_nodes[level_off[k], level_off[k + 1])
+    GrowBuf upd_in;                      // host form's input: geo, materials, indices
 };
 
 // Releases a scene handle on scope exit; the error that made the scope return early survives the release.
@@ -272,6 +282,9 @@ int rtb200_scene_release(rtb200_scene_handle h) {
         cudaSetDevice(h->device);
         if (!h->pending.empty()) render_collect(h, nullptr);   // frames still in flight read the scene arrays
         else if (h->ctx->stream) cudaStreamSynchronize(h->ctx->stream);
+        if (h->updated) { cudaEventSynchronize(h->updated); cudaEventDestroy(h->updated); }   // an update in flight writes them
+        if (h->refit) cudaFree(h->refit);
+        if (h->upd_in.p) cudaFree(h->upd_in.p);
         for (cudaEvent_t e : h->ev) h->ctx->event_pool.push_back(e);
         if (h->arena) {
             auto& cache = h->ctx->arena_cache;
@@ -326,6 +339,12 @@ static int commit_uploads(rtb200_scene_t* h) {
     return RT_OK;
 }
 
+static bool image_ok(const rt_image& im) {
+    if (!im.rgb8 || im.width == 0 || im.height == 0) return false;
+    if (im.width > (1ull << 20) || im.height > (1ull << 20)) return false;
+    return im.width * im.height * 3ull <= im.bytes;   // the callee reads width*height*3 bytes: the buffer must hold them
+}
+
 static int validate_scene(const rt_scene* s, uint32_t* n_lights_out) {
     if (s->width < 2 || s->height < 2) return fail(RT_ERR_INVALID, "width and height must be >= 2 (u,v divide by w-1, h-1: raytracer.rs:199-200)");
     if (s->samples_per_pixel == 0) return fail(RT_ERR_INVALID, "samples_per_pixel must be > 0");
@@ -333,11 +352,6 @@ static int validate_scene(const rt_scene* s, uint32_t* n_lights_out) {
     if (s->n_spheres >= (1ull << 26)) return fail(RT_ERR_UNSUPPORTED, "2^26 or more spheres (list entries carry 27-bit ids)");
     if (s->n_spheres && !s->spheres) return fail(RT_ERR_INVALID, "spheres is null");
     if (s->n_textures && !s->textures) return fail(RT_ERR_INVALID, "textures is null");
-    auto image_ok = [](const rt_image& im) {
-        if (!im.rgb8 || im.width == 0 || im.height == 0) return false;
-        if (im.width > (1ull << 20) || im.height > (1ull << 20)) return false;
-        return im.width * im.height * 3ull <= im.bytes;   // the callee reads width*height*3 bytes: the buffer must hold them
-    };
     uint32_t n_lights = 0;
     for (uint64_t i = 0; i < s->n_spheres; ++i) {
         const rt_sphere& sp = s->spheres[i];
@@ -411,6 +425,8 @@ static int scene_upload_records(const rt_scene* s, const rt_options& opts, uint3
     }
     std::vector<uint32_t> lights;
     for (uint32_t i = 0; i < n; ++i) if (s->spheres[i].kind == RT_LIGHT) lights.push_back(i);
+    h->light_idx = lights;
+    for (uint64_t t = 0; t < s->n_textures; ++t) h->tex_ok.push_back(image_ok(s->textures[t]));
     lights.push_back(0);
     upload_array(h, lights.data(), lights.size() * 4, (void**)&tp.lights);
     upload_array(h, nullptr, 16, (void**)&h->err);   // zero-filled error counters
@@ -562,6 +578,7 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
     CU(cudaSetDevice(h->device));
     cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
     if (st != ctx->stream) CU(cudaStreamWaitEvent(st, ctx->staging_free, 0));   // the scene upload ran on the context's stream
+    if (h->updated) CU(cudaStreamWaitEvent(st, h->updated, 0));                 // and its last update on the update's stream
     const rtb200_scene_t::Submission* prev = h->pending.empty() ? nullptr : &h->pending.back();
     rtb200_scene_t::Submission sub{st, set, prev ? prev->ev0 + prev->n_ev : 0u, 0, n, 0, 0, h->grid, 0, 0};
     TraceParams tp = h->tp;   // the handle's own view stays as uploaded
@@ -768,6 +785,175 @@ int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, u
     if (rc != RT_OK) return rc;
     if (!dev_rgb8 && !dev_linear_f32) return fail(RT_ERR_INVALID, "dev_rgb8 and dev_linear_f32 are both null");
     return render_blocking(h, frames, n_frames, dev_rgb8, dev_linear_f32, stream_in, stats);
+  });
+}
+
+// ---- moving spheres of a resident scene: refit instead of rebuild (DESIGN.md §4.7) ----
+// The refit's scratch, built at the first update of a MODE_TREE handle: exact boxes of the nodes and leaves, and the nodes
+// grouped by tree level from one copy of the child words (an update never changes them). The copies run after the upload's
+// on the context's stream, and this first update waits for them.
+static int refit_prepare(rtb200_scene_handle h) {
+    const uint32_t nn = h->tp.n_nodes, nl = h->tp.n_leaves;
+    if (h->refit || h->mode != MODE_TREE || nn == 0) return RT_OK;
+    cudaStream_t st = h->ctx->stream;
+    std::vector<uint32_t> child((size_t)nn * rtbvh::kWide);
+    CU(cudaMemcpy2DAsync(child.data(), rtbvh::kWide * 4, (const float*)h->tp.nodes + 6 * rtbvh::kWide, rtbvh::kNodeFloats * 4,
+                         rtbvh::kWide * 4, nn, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    std::vector<std::vector<uint32_t>> levels{{0u}};   // the root is node 0
+    for (;;) {
+        std::vector<uint32_t> next;
+        for (uint32_t v : levels.back())
+            for (int c = 0; c < rtbvh::kWide; ++c) {
+                const uint32_t ref = child[(size_t)v * rtbvh::kWide + c];
+                if (ref != rtbvh::kEmptyChild && !(ref & rtbvh::kLeafBit)) next.push_back(ref);
+            }
+        if (next.empty()) break;
+        levels.push_back(std::move(next));
+    }
+    std::vector<uint32_t> order;
+    h->level_off.assign(1, 0u);
+    for (size_t k = levels.size(); k-- > 0;) {
+        order.insert(order.end(), levels[k].begin(), levels[k].end());
+        h->level_off.push_back((uint32_t)order.size());
+    }
+    void* p = nullptr;
+    CU(cudaMalloc(&p, ((size_t)nn + nl) * 6 * sizeof(double) + (size_t)nn * 4));
+    h->refit = p;
+    h->node_box = (double*)p;
+    h->leaf_box = h->node_box + (size_t)nn * 6;
+    h->level_nodes = (uint32_t*)(h->leaf_box + (size_t)nl * 6);
+    CU(cudaMemcpyAsync(h->level_nodes, order.data(), order.size() * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaStreamSynchronize(st));
+    return RT_OK;
+}
+
+// Order `st` after the upload and the previous update (which may still read upd_in).
+static int update_begin(rtb200_scene_handle h, cudaStream_t st) {
+    if (st != h->ctx->stream) CU(cudaStreamWaitEvent(st, h->ctx->staging_free, 0));
+    if (h->updated) CU(cudaStreamWaitEvent(st, h->updated, 0));
+    else CU(cudaEventCreateWithFlags(&h->updated, cudaEventDisableTiming));
+    return RT_OK;
+}
+
+// Order `st` after the frames of h in flight, on any stream: they read the arrays the update writes.
+static int update_after_frames(rtb200_scene_handle h, cudaStream_t st) {
+    for (const auto& p : h->pending) if (p.n_ev) CU(cudaStreamWaitEvent(st, h->ev[p.ev0 + 1], 0));
+    return RT_OK;
+}
+
+// Recompute the arrays of h's mode from its geo and record the end of the update: every frame enqueued later waits for it.
+static int update_finish(rtb200_scene_handle h, cudaStream_t st) {
+    RefitParams p{};
+    p.geo = h->tp.geo; p.n = h->tp.n; p.gx = h->tp.gx; p.gy = h->tp.gy; p.gz = h->tp.gz;
+    if (h->mode == MODE_BRUTE) {
+        p.filt = (float*)h->tp.filt;
+        CU(launch_refit_spheres(p, st));
+    } else if (h->mode == MODE_TREE && h->refit) {
+        p.leaf_id = h->tp.leaf_id; p.leaf_rec = (float*)h->tp.leaf_rec; p.leaf_box = h->leaf_box; p.n_leaves = h->tp.n_leaves;
+        p.nodes = (float*)h->tp.nodes; p.node_box = h->node_box;
+        CU(launch_refit_spheres(p, st));
+        for (size_t k = 0; k + 1 < h->level_off.size(); ++k)
+            CU(launch_refit_nodes(p, h->level_nodes + h->level_off[k], h->level_off[k + 1] - h->level_off[k], st));
+    }
+    CU(cudaEventRecord(h->updated, st));
+    return RT_OK;
+}
+
+int rtb200_scene_update_spheres(rtb200_scene_handle h, const uint32_t* index, const rt_sphere* spheres, uint32_t n, void* stream_in) {
+  return guarded([&]() -> int {
+    if (n && (!index || !spheres)) return fail(RT_ERR_INVALID, "index or spheres is null");
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    if (n == 0) return RT_OK;
+    // everything is checked before anything is enqueued: on error the scene is unchanged
+    std::vector<uint32_t> sorted(index, index + n);
+    std::sort(sorted.begin(), sorted.end());
+    if (sorted.back() >= h->tp.n) return fail(RT_ERR_INVALID, "index " + std::to_string(sorted.back()) + " is not a sphere of the scene (n_spheres = " + std::to_string(h->tp.n) + ")");
+    for (uint32_t k = 1; k < n; ++k)
+        if (sorted[k] == sorted[k - 1]) return fail(RT_ERR_INVALID, "sphere " + std::to_string(sorted[k]) + " is listed twice");
+    for (uint32_t k = 0; k < n; ++k) {
+        const rt_sphere& sp = spheres[k];
+        if (sp.kind > RT_LIGHT) return fail(RT_ERR_INVALID, "unknown material kind (spheres[" + std::to_string(k) + "])");
+        if (sp.kind == RT_TEXTURE && (sp.texture < 0 || (size_t)sp.texture >= h->tex_ok.size() || !h->tex_ok[sp.texture]))
+            return fail(RT_ERR_INVALID, "texture index out of range, or its image was empty at upload (spheres[" + std::to_string(k) + "])");
+        const bool was_light = std::binary_search(h->light_idx.begin(), h->light_idx.end(), index[k]);
+        if (was_light != (sp.kind == RT_LIGHT))
+            return fail(RT_ERR_UNSUPPORTED, "sphere " + std::to_string(index[k]) + ": the set of lights is fixed at upload (upload the scene again to change it)");
+    }
+    DeviceRestore restore;
+    DeviceCtx* ctx = h->ctx;
+    std::lock_guard<std::recursive_mutex> lk(ctx->mu);
+    CU(cudaSetDevice(h->device));
+    int rc = refit_prepare(h);
+    if (rc != RT_OK) return rc;
+    cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
+    if ((rc = update_begin(h, st)) != RT_OK) return rc;
+    // input in the pinned staging buffer (geo, materials, indices), copied before this call returns
+    const size_t geo_b = (size_t)n * 32, mat_b = (size_t)n * sizeof(DevMat), bytes = geo_b + mat_b + (size_t)n * 4;
+    CU(cudaEventSynchronize(ctx->staging_free));   // the previous copy has left the staging buffer
+    CU(ctx->staging.ensure(bytes));
+    char* S = (char*)ctx->staging.p;
+    for (uint32_t k = 0; k < n; ++k) rtbvh::sphere_exact(spheres[k], (double*)S + 4 * (size_t)k, ((rtbvh::Mat32*)(S + geo_b))[k]);
+    memcpy(S + geo_b + mat_b, index, (size_t)n * 4);
+    CU(h->upd_in.ensure(bytes));
+    char* D = (char*)h->upd_in.p;
+    CU(cudaMemcpyAsync(D, S, bytes, cudaMemcpyHostToDevice, st));
+    CU(cudaEventRecord(ctx->staging_free, st));   // before the wait for the frames pending now (DESIGN.md §4.7, Ordering)
+    if ((rc = update_after_frames(h, st)) != RT_OK) return rc;
+    CU(launch_update_scatter((const uint32_t*)(D + geo_b + mat_b), (const double4*)D, (const DevMat*)(D + geo_b), n,
+                             (double4*)h->tp.geo, (DevMat*)h->tp.mat, st));
+    return update_finish(h, st);
+  });
+}
+
+int rtb200_scene_update_geometry_device(rtb200_scene_handle h, const void* dev_center_radius, void* stream_in) {
+  return guarded([&]() -> int {
+    if (!dev_center_radius) return fail(RT_ERR_INVALID, "dev_center_radius is null");
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    DeviceRestore restore;
+    DeviceCtx* ctx = h->ctx;
+    std::lock_guard<std::recursive_mutex> lk(ctx->mu);
+    CU(cudaSetDevice(h->device));
+    cudaPointerAttributes a{};
+    if (cudaPointerGetAttributes(&a, dev_center_radius) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+    if (!((a.type == cudaMemoryTypeDevice && a.device == h->device) || a.type == cudaMemoryTypeManaged))
+        return fail(RT_ERR_INVALID, "dev_center_radius is not device or managed memory of device " + std::to_string(h->device));
+    if (h->tp.n == 0) return RT_OK;
+    int rc = refit_prepare(h);
+    if (rc != RT_OK) return rc;
+    cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
+    if ((rc = update_begin(h, st)) != RT_OK) return rc;
+    if ((rc = update_after_frames(h, st)) != RT_OK) return rc;
+    CU(cudaMemcpyAsync((void*)h->tp.geo, dev_center_radius, (size_t)h->tp.n * 32, cudaMemcpyDeviceToDevice, st));
+    return update_finish(h, st);
+  });
+}
+
+// Diagnostic: the handle's current arrays, laid out as rtb200_debug_bvh's (flat records only in RT_VARIANT_BRUTE_FORCE)
+int rtb200_scene_debug_records(rtb200_scene_handle h, uint32_t info[8], float* nodes, uint64_t cap_nodes, float* leaf_rec,
+                               uint64_t cap_leaf_rec, float* flat, uint64_t cap_flat, double* geo, uint64_t cap_geo) {
+  return guarded([&]() -> int {
+    if (!h || !info) return fail(RT_ERR_INVALID, "null argument");
+    const TraceParams& tp = h->tp;
+    info[0] = tp.n_nodes; info[1] = tp.n_leaves; info[2] = tp.depth; info[3] = (uint32_t)rtbvh::kLeafK; info[4] = tp.n_always;
+    info[5] = (uint32_t)rtbvh::kNodeFloats; info[6] = tp.filt ? tp.n_pairs : 0u; info[7] = 0;
+    DeviceRestore restore;
+    std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
+    CU(cudaSetDevice(h->device));
+    cudaStream_t st = h->ctx->stream;   // after the upload; after the last update:
+    if (h->updated) CU(cudaStreamWaitEvent(st, h->updated, 0));
+    auto get = [&](void* dst, const void* src, uint64_t cap, uint64_t count, size_t elem) -> int {
+        if (dst && src && cap && count) CU(cudaMemcpyAsync(dst, src, std::min(cap, count) * elem, cudaMemcpyDeviceToHost, st));
+        return RT_OK;
+    };
+    int rc = RT_OK;
+    if (rc == RT_OK) rc = get(nodes, tp.nodes, cap_nodes, (uint64_t)tp.n_nodes * rtbvh::kNodeFloats, 4);
+    if (rc == RT_OK) rc = get(leaf_rec, tp.leaf_rec, cap_leaf_rec, (uint64_t)tp.n_leaves * rtbvh::kLeafK * 4, 4);
+    if (rc == RT_OK) rc = get(flat, tp.filt, cap_flat, (uint64_t)info[6] * 8, 4);
+    if (rc == RT_OK) rc = get(geo, tp.geo, cap_geo, (uint64_t)tp.n * 4, 8);
+    if (rc != RT_OK) return rc;
+    CU(cudaStreamSynchronize(st));
+    return RT_OK;
   });
 }
 

@@ -82,6 +82,14 @@ inline bool sphere_record(double x, double y, double z, double r2, float rec[4])
     return std::isfinite(rec[0]) && std::isfinite(rec[1]) && std::isfinite(rec[2]) && std::isfinite(nkd) && c2 < 1e30;
 }
 
+// Exact geometry {cx,cy,cz,radius} and material record of one sphere (the upload and rtb200_scene_update_spheres).
+inline void sphere_exact(const rt_sphere& sp, double G[4], Mat32& m) {
+    G[0] = sp.center.x; G[1] = sp.center.y; G[2] = sp.center.z; G[3] = sp.radius;
+    m.kind = sp.kind; m.param = sp.param; m.tex = sp.texture; m.pad = 0;
+    if (sp.kind == RT_LAMBERTIAN || sp.kind == RT_METAL) { m.r = sp.albedo[0]; m.g = sp.albedo[1]; m.b = sp.albedo[2]; }
+    else { m.r = m.g = m.b = 1.0f; }   // Glass/Light attenuation is (1,1,1) (materials.rs:67,179); Texture uses texels
+}
+
 struct Box {
     double lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
     void grow(const Box& o) { for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], o.lo[a]); hi[a] = std::max(hi[a], o.hi[a]); } }
@@ -178,12 +186,7 @@ private:
                     if (!sphere_record(sp.center.x - R_.g[0], sp.center.y - R_.g[1], sp.center.z - R_.g[2], sp.radius * sp.radius, rec)) {
                         rec[0] = rec[1] = rec[2] = 0.f; rec[3] = INFINITY;   // always a candidate
                     }
-                    double* G = &R_.geo[4 * (size_t)i];
-                    G[0] = sp.center.x; G[1] = sp.center.y; G[2] = sp.center.z; G[3] = sp.radius;
-                    Mat32& m = R_.mat[i];
-                    m.kind = sp.kind; m.param = sp.param; m.tex = sp.texture; m.pad = 0;
-                    if (sp.kind == RT_LAMBERTIAN || sp.kind == RT_METAL) { m.r = sp.albedo[0]; m.g = sp.albedo[1]; m.b = sp.albedo[2]; }
-                    else { m.r = m.g = m.b = 1.0f; }   // Glass/Light attenuation is (1,1,1) (materials.rs:67,179); Texture uses texels
+                    sphere_exact(sp, &R_.geo[4 * (size_t)i], R_.mat[i]);
                 }
                 A[0 + k] = rec[0]; A[2 + k] = rec[1]; A[4 + k] = rec[2]; A[6 + k] = rec[3];
             }

@@ -114,6 +114,21 @@ struct ResolveParams {
     uint8_t* out_rgb8;     // [npix_local][3] or null
 };
 
+// Refit of a resident scene after its spheres moved (rtb200_refit.cu, DESIGN.md §4.7): the records and f32 boxes are
+// recomputed from `geo` on the upload's topology and recentring offset. Exact boxes are {lo[3], hi[3]} f64.
+struct RefitParams {
+    const double4* geo;
+    uint32_t n;
+    double gx, gy, gz;
+    float* filt;                 // MODE_BRUTE: n_pairs * 8 flat records, else null
+    const uint32_t* leaf_id;     // MODE_TREE from here on
+    float* leaf_rec;
+    double* leaf_box;            // n_leaves exact boxes
+    uint32_t n_leaves;
+    float* nodes;
+    double* node_box;            // n_nodes exact boxes (the union of the node's children)
+};
+
 struct KernelInfo { int registers, max_threads, const_bytes, local_bytes; char name[96]; };
 
 // `frames`: the multi-frame kernel (work ids span p.ftab's frames) instead of the single-frame one
@@ -122,6 +137,13 @@ cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, bool frames, i
 int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, bool frames, size_t smem);   // 0 when the kernel cannot run on the current device
 cudaError_t wavefront_info(uint32_t mode, bool lights, bool frames, KernelInfo* out);
 cudaError_t launch_resolve(const ResolveParams& p, cudaStream_t st);
+// geo[idx[k]] = geo_in[k], mat[idx[k]] = mat_in[k] for k < n (idx has no repeats)
+cudaError_t launch_update_scatter(const uint32_t* idx, const double4* geo_in, const DevMat* mat_in, uint32_t n, double4* geo, DevMat* mat,
+                                  cudaStream_t st);
+// flat records (p.filt) or leaf records and leaf boxes (p.leaf_rec), whichever p carries
+cudaError_t launch_refit_spheres(const RefitParams& p, cudaStream_t st);
+// the `count` nodes level_nodes[0, count) of one tree level; their children's exact boxes are final
+cudaError_t launch_refit_nodes(const RefitParams& p, const uint32_t* level_nodes, uint32_t count, cudaStream_t st);
 
 // single-thread probes of the device routines (known-answer tests)
 cudaError_t probe_sphere_hit(const double* in /*12*/, double* out /*9*/, cudaStream_t st);

@@ -24,6 +24,7 @@ RT_SKY_NONE, RT_SKY_GRADIENT, RT_SKY_TEXTURE = 0, 1, 2
 RT_VARIANT_AUTO, RT_VARIANT_FILTERED, RT_VARIANT_EXACT_F64, RT_VARIANT_RETIRED_LANES, RT_VARIANT_BRUTE_FORCE = 0, 1, 2, 3, 4
 
 DEFAULT_SEED = 0x5EED
+CUDA_STREAM_LEGACY = 0x1   # cudaStreamLegacy: torch's default stream has handle 0, which the C ABI reads as "use the library's own stream"
 
 
 class RtError(RuntimeError):
@@ -112,6 +113,7 @@ ABI_SYMBOLS = [
     "rtb200_decode_jpeg_file", "rtb200_free", "rtb200_render_device_async", "rtb200_render_device_wait",
     "rtb200_debug_bvh", "rtb200_probe_sphere_uv", "rtb200_device_count", "rtb200_render_rgb8_multi", "rtb200_scene_kernel_info",
     "rtb200_render_frames", "rtb200_render_frames_device",
+    "rtb200_scene_update_spheres", "rtb200_scene_update_geometry_device", "rtb200_scene_debug_records",
 ]
 
 _lib = None
@@ -159,6 +161,10 @@ def lib() -> C.CDLL:
                                        C.POINTER(rt_stats)]
     L.rtb200_render_frames_device.argtypes = [C.c_void_p, C.POINTER(rt_frame), C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p,
                                               C.POINTER(rt_stats)]
+    L.rtb200_scene_update_spheres.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
+    L.rtb200_scene_update_geometry_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+    L.rtb200_scene_debug_records.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
+                                             C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
     _lib = L
     return L
 
@@ -310,6 +316,39 @@ class Scene:
             self.set_camera(aspect=float(width) / float(height))
         return self
 
+    def set_sphere(self, i: int, center=None, radius: Optional[float] = None, material=None) -> rt_sphere:
+        """Edit sphere i of the host scene in place and return a copy of its record (for ResidentScene.update_spheres, so
+        that a resident handle, a fresh upload and the oracle can render the same edit). `material` is a JSON material
+        ({"Metal": {"albedo": [...], "fuzz": f}}, ...; a Texture names one of the scene's textures by index:
+        {"Texture": {"albedo": [...], "h_offset": f, "texture": k}}) or an rt_sphere whose material is copied."""
+        if not 0 <= i < self.n_spheres:
+            raise IndexError(f"sphere {i} of {self.n_spheres}")
+        s = self._spheres[i]
+        if center is not None:
+            s.center = vec3(center)
+        if radius is not None:
+            s.radius = float(radius)
+        if isinstance(material, rt_sphere):
+            s.kind, s.param, s.texture = material.kind, material.param, material.texture
+            s.albedo[:] = list(material.albedo)
+        elif material is not None:
+            (kind, body), = material.items()
+            s.texture, s.param = -1, 0.0
+            s.albedo[:] = [np.float32(a) for a in body.get("albedo", [0.0, 0.0, 0.0])]
+            if kind == "Lambertian":
+                s.kind = RT_LAMBERTIAN
+            elif kind == "Metal":
+                s.kind = RT_METAL; s.param = float(body["fuzz"])
+            elif kind == "Glass":
+                s.kind = RT_GLASS; s.param = float(body["index_of_refraction"])
+            elif kind == "Texture":
+                s.kind = RT_TEXTURE; s.param = float(body["h_offset"]); s.texture = int(body["texture"])
+            elif kind == "Light":
+                s.kind = RT_LIGHT
+            else:
+                raise ValueError(f"unknown material {kind}")
+        return rt_sphere.from_buffer_copy(s)
+
     @property
     def n_spheres(self):
         return int(self.c.n_spheres)
@@ -428,6 +467,15 @@ def render_frames(scene: Scene, frames: Sequence[rt_frame], opts: Optional[rt_op
     return out, st.as_dict()
 
 
+def _current_device() -> Optional[int]:
+    """The caller's current CUDA device, which an upload without opts.device uses (None when torch is not installed)."""
+    try:
+        import torch
+    except ImportError:
+        return None
+    return torch.cuda.current_device()
+
+
 class ResidentScene:
     """Scene kept in HBM between frames (rtb200_scene_upload / rtb200_render_device)."""
 
@@ -437,6 +485,11 @@ class ResidentScene:
         self.h = C.c_void_p()
         _check(lib().rtb200_scene_upload(C.byref(scene.c), C.byref(opts) if opts is not None else None, C.byref(self.h)))
         self.rows = scene.c.height if (opts is None or opts.world <= 1) else shard_rows(scene.c.height, opts.rank, opts.world, opts.band_rows)
+        self.n = scene.n_spheres
+        self.device = opts.device if opts is not None and opts.device >= 0 else _current_device()   # None: unknown without torch
+        # the uploaded spheres: bvh_records() restates the upload's topology from them
+        self._uploaded = (rt_sphere * max(self.n, 1))()
+        C.memmove(self._uploaded, scene._spheres, self.n * C.sizeof(rt_sphere))
 
     def render(self, dev_rgb8_ptr: int = 0, dev_linear_ptr: int = 0, stream: int = 0) -> dict:
         st = rt_stats()
@@ -461,6 +514,53 @@ class ResidentScene:
         _check(lib().rtb200_render_frames_device(self.h, arr, n, C.c_void_p(dev_rgb8_ptr or None), C.c_void_p(dev_linear_ptr or None),
                                                  C.c_void_p(stream or None), C.byref(st)))
         return st.as_dict()
+
+    def update_spheres(self, indices: Sequence[int], spheres: Sequence[rt_sphere], stream: int = 0):
+        """Replace spheres indices[k] by spheres[k] (centre, radius, material) without rebuilding the hierarchy
+        (rtb200_scene_update_spheres). Stream-ordered: frames enqueued before see the old scene, frames enqueued after the new."""
+        if len(indices) != len(spheres):
+            raise ValueError(f"{len(indices)} indices but {len(spheres)} spheres")
+        idx = np.ascontiguousarray(indices, dtype=np.uint32)
+        arr = (rt_sphere * max(len(spheres), 1))(*spheres)
+        _check(lib().rtb200_scene_update_spheres(self.h, idx.ctypes.data if idx.size else None, arr, len(spheres), C.c_void_p(stream or None)))
+
+    def update_geometry(self, t, stream=None):
+        """Replace the centre and radius of every sphere from a contiguous float64 CUDA tensor [n_spheres, 4] of
+        {cx, cy, cz, radius} on the handle's device (rtb200_scene_update_geometry_device); materials stay. Runs on `stream`
+        (a torch.cuda.Stream, or a cudaStream_t handle where 0 is the library's own stream, as in :meth:`render`), by default
+        torch's current stream, so `t` may be computed on it just before and released just after."""
+        import torch
+        if not isinstance(t, torch.Tensor) or not t.is_cuda:
+            raise ValueError("update_geometry takes a CUDA tensor")
+        if t.dtype != torch.float64 or tuple(t.shape) != (self.n, 4) or not t.is_contiguous():
+            raise ValueError(f"update_geometry takes a contiguous float64 tensor of shape [{self.n}, 4], got {t.dtype} {tuple(t.shape)}")
+        if self.device is not None and t.device.index != self.device:
+            raise ValueError(f"the tensor is on cuda:{t.device.index}, the scene on cuda:{self.device}")
+        if stream is None:
+            stream = torch.cuda.current_stream(t.device)
+        s = (stream.cuda_stream or CUDA_STREAM_LEGACY) if isinstance(stream, torch.cuda.Stream) else int(stream)
+        _check(lib().rtb200_scene_update_geometry_device(self.h, C.c_void_p(t.data_ptr()), C.c_void_p(s or None)))
+
+    def bvh_records(self) -> dict:
+        """The handle's current arrays (rtb200_scene_debug_records) in the layout of :func:`bvh_records`, plus "geo"
+        (float64 [n, 4]). leaf_id, always and recentre are the upload's: an update never changes them."""
+        up = Scene()
+        up.c = rt_scene.from_buffer_copy(self.scene.c)
+        up.c.spheres = C.cast(self._uploaded, C.POINTER(rt_sphere)); up.c.n_spheres = self.n
+        b = bvh_records(up)
+        info = (C.c_uint32 * 8)()
+        _check(lib().rtb200_scene_debug_records(self.h, info, None, 0, None, 0, None, 0, None, 0))
+        n_nodes, n_leaves, depth, k, n_always, fpn, n_pairs, _ = (int(x) for x in info)
+        nodes = np.zeros(max(n_nodes * fpn, 1), np.float32); rec = np.zeros(max(n_leaves * k * 4, 1), np.float32)
+        flat = np.zeros(max(n_pairs * 8, 1), np.float32); geo = np.zeros(max(self.n * 4, 1), np.float64)
+        _check(lib().rtb200_scene_debug_records(self.h, info, nodes.ctypes.data, nodes.size, rec.ctypes.data, rec.size,
+                                                flat.ctypes.data, flat.size, geo.ctypes.data, geo.size))
+        nd = nodes[: n_nodes * fpn].reshape(n_nodes, fpn)
+        b.update({"n_nodes": n_nodes, "n_leaves": n_leaves, "depth": depth,
+                  "lo": nd[:, :24].reshape(n_nodes, 3, 8), "hi": nd[:, 24:48].reshape(n_nodes, 3, 8), "child": nd[:, 48:56].view(np.uint32),
+                  "leaf_rec": rec[: n_leaves * k * 4].reshape(n_leaves, k // 2, 2, 4), "leaf_id": b["leaf_id"][:n_leaves],
+                  "always": b["always"][:n_always], "flat": flat[: n_pairs * 8].reshape(n_pairs, 2, 4), "geo": geo[: self.n * 4].reshape(self.n, 4)})
+        return b
 
     def kernel_info(self) -> dict:
         ki = rt_kernel_info()

@@ -14,9 +14,7 @@ import numpy as np
 import torch
 import torch.distributed as dist
 
-from . import ResidentScene, Scene, make_options, shard_row_indices, shard_rows
-
-CUDA_STREAM_LEGACY = 0x1   # cudaStreamLegacy: torch's default stream has handle 0, which the C ABI reads as "use the library's own stream"
+from . import CUDA_STREAM_LEGACY, ResidentScene, Scene, make_options, shard_row_indices, shard_rows
 
 
 def _torch_stream() -> int:

@@ -17,8 +17,6 @@
 
 using namespace rtk;
 
-static_assert(sizeof(rtbvh::Mat32) == sizeof(DevMat), "host and device material records must agree");
-static_assert(rtbvh::kLeafK == kLeafK && rtbvh::kNodeFloats == kNodeVec * 4, "host and device BVH layouts must agree");
 static_assert(kCapIn >= 32 + 7 * rtbvh::kMaxDepth + 8, "the node stack must hold 32 roots plus a single-entry descent of the deepest tree (LIFO reserve, DESIGN.md 4.1)");
 
 namespace {
@@ -192,11 +190,11 @@ struct rtb200_scene_t {
     std::vector<uint32_t> light_idx;     // the Light spheres, increasing
     std::vector<uint8_t> tex_ok;         // uploaded textures a Texture sphere may use
     cudaEvent_t updated = nullptr;       // recorded after the last update; every later frame waits for it
-    void* refit = nullptr;               // node_box, leaf_box, level_nodes
+    std::vector<uint32_t> level_nodes, level_off;   // MODE_TREE: the builder's level order (rtbvh::Records::level_nodes)
+    void* refit = nullptr;               // node_box, leaf_box, the device copy of level_nodes
     double* node_box = nullptr;          // n_nodes exact boxes {lo[3], hi[3]}
     double* leaf_box = nullptr;          // n_leaves exact boxes
-    uint32_t* level_nodes = nullptr;     // node indices grouped by tree level, deepest level first
-    std::vector<uint32_t> level_off;     // a level's nodes are level_nodes[level_off[k], level_off[k + 1])
+    uint32_t* level_nodes_dev = nullptr;
     GrowBuf upd_in;                      // host form's input: geo, materials, indices
 };
 
@@ -251,6 +249,12 @@ uint32_t rtb200_shard_rows(uint32_t height, int32_t rank, int32_t world, uint32_
 
 static int render_collect(rtb200_scene_handle h, rt_stats* stats);
 
+// info[8] of the diagnostics below
+static void bvh_info(uint32_t info[8], uint32_t n_nodes, uint32_t n_leaves, uint32_t depth, uint32_t n_always, uint32_t n_pairs) {
+    const uint32_t v[8] = {n_nodes, n_leaves, depth, (uint32_t)rtbvh::kLeafK, n_always, (uint32_t)rtbvh::kNodeFloats, n_pairs, 0u};
+    memcpy(info, v, sizeof v);
+}
+
 // Diagnostic (host only, no GPU needed): the hierarchy rtb200_scene_upload would stage for `scene`.
 // info = {n_nodes, n_leaves, depth, leaf_size, n_always, floats_per_node, n_pairs_flat, 0}; arrays are filled up to their capacities (elements).
 int rtb200_debug_bvh(const rt_scene* s, double recentre[3], uint32_t info[8], float* nodes, uint64_t cap_nodes, float* leaf_rec,
@@ -263,8 +267,7 @@ int rtb200_debug_bvh(const rt_scene* s, double recentre[3], uint32_t info[8], fl
     rtbvh::Records R;
     rtbvh::build_records(s, true, R);
     if (recentre) { recentre[0] = R.g[0]; recentre[1] = R.g[1]; recentre[2] = R.g[2]; }
-    info[0] = R.n_nodes; info[1] = R.n_leaves; info[2] = R.depth; info[3] = (uint32_t)rtbvh::kLeafK; info[4] = (uint32_t)R.always.size();
-    info[5] = (uint32_t)rtbvh::kNodeFloats; info[6] = R.n_pairs; info[7] = 0;
+    bvh_info(info, R.n_nodes, R.n_leaves, R.depth, (uint32_t)R.always.size(), R.n_pairs);
     if (nodes) memcpy(nodes, R.nodes.data(), std::min<uint64_t>(cap_nodes, R.nodes.size()) * 4);
     if (leaf_rec) memcpy(leaf_rec, R.leaf_rec.data(), std::min<uint64_t>(cap_leaf_rec, R.leaf_rec.size()) * 4);
     if (leaf_id) memcpy(leaf_id, R.leaf_id.data(), std::min<uint64_t>(cap_leaf_id, R.leaf_id.size()) * 4);
@@ -423,6 +426,7 @@ static int scene_upload_records(const rt_scene* s, const rt_options& opts, uint3
         upload_array(h, s->sky.tex.rgb8, s->sky.tex.width * s->sky.tex.height * 3, (void**)&tp.sky.rgb8);
         tp.sky.width = s->sky.tex.width; tp.sky.height = s->sky.tex.height;
     }
+    if (h->mode == MODE_TREE) { h->level_nodes = R.level_nodes; h->level_off = R.level_off; }
     std::vector<uint32_t> lights;
     for (uint32_t i = 0; i < n; ++i) if (s->spheres[i].kind == RT_LIGHT) lights.push_back(i);
     h->light_idx = lights;
@@ -789,42 +793,18 @@ int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, u
 }
 
 // ---- moving spheres of a resident scene: refit instead of rebuild (DESIGN.md §4.7) ----
-// The refit's scratch, built at the first update of a MODE_TREE handle: exact boxes of the nodes and leaves, and the nodes
-// grouped by tree level from one copy of the child words (an update never changes them). The copies run after the upload's
-// on the context's stream, and this first update waits for them.
-static int refit_prepare(rtb200_scene_handle h) {
+// The refit's scratch, built at the first update of a MODE_TREE handle on the update's stream `st`: exact boxes of the nodes
+// and leaves, and the device copy of the builder's level order (an update never changes the topology).
+static int refit_prepare(rtb200_scene_handle h, cudaStream_t st) {
     const uint32_t nn = h->tp.n_nodes, nl = h->tp.n_leaves;
     if (h->refit || h->mode != MODE_TREE || nn == 0) return RT_OK;
-    cudaStream_t st = h->ctx->stream;
-    std::vector<uint32_t> child((size_t)nn * rtbvh::kWide);
-    CU(cudaMemcpy2DAsync(child.data(), rtbvh::kWide * 4, (const float*)h->tp.nodes + 6 * rtbvh::kWide, rtbvh::kNodeFloats * 4,
-                         rtbvh::kWide * 4, nn, cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    std::vector<std::vector<uint32_t>> levels{{0u}};   // the root is node 0
-    for (;;) {
-        std::vector<uint32_t> next;
-        for (uint32_t v : levels.back())
-            for (int c = 0; c < rtbvh::kWide; ++c) {
-                const uint32_t ref = child[(size_t)v * rtbvh::kWide + c];
-                if (ref != rtbvh::kEmptyChild && !(ref & rtbvh::kLeafBit)) next.push_back(ref);
-            }
-        if (next.empty()) break;
-        levels.push_back(std::move(next));
-    }
-    std::vector<uint32_t> order;
-    h->level_off.assign(1, 0u);
-    for (size_t k = levels.size(); k-- > 0;) {
-        order.insert(order.end(), levels[k].begin(), levels[k].end());
-        h->level_off.push_back((uint32_t)order.size());
-    }
     void* p = nullptr;
     CU(cudaMalloc(&p, ((size_t)nn + nl) * 6 * sizeof(double) + (size_t)nn * 4));
     h->refit = p;
     h->node_box = (double*)p;
     h->leaf_box = h->node_box + (size_t)nn * 6;
-    h->level_nodes = (uint32_t*)(h->leaf_box + (size_t)nl * 6);
-    CU(cudaMemcpyAsync(h->level_nodes, order.data(), order.size() * 4, cudaMemcpyHostToDevice, st));
-    CU(cudaStreamSynchronize(st));
+    h->level_nodes_dev = (uint32_t*)(h->leaf_box + (size_t)nl * 6);
+    CU(cudaMemcpyAsync(h->level_nodes_dev, h->level_nodes.data(), (size_t)nn * 4, cudaMemcpyHostToDevice, st));
     return RT_OK;
 }
 
@@ -845,7 +825,7 @@ static int update_after_frames(rtb200_scene_handle h, cudaStream_t st) {
 // Recompute the arrays of h's mode from its geo and record the end of the update: every frame enqueued later waits for it.
 static int update_finish(rtb200_scene_handle h, cudaStream_t st) {
     RefitParams p{};
-    p.geo = h->tp.geo; p.n = h->tp.n; p.gx = h->tp.gx; p.gy = h->tp.gy; p.gz = h->tp.gz;
+    p.geo = h->tp.geo; p.n = h->tp.n; p.g[0] = h->tp.gx; p.g[1] = h->tp.gy; p.g[2] = h->tp.gz;
     if (h->mode == MODE_BRUTE) {
         p.filt = (float*)h->tp.filt;
         CU(launch_refit_spheres(p, st));
@@ -854,7 +834,7 @@ static int update_finish(rtb200_scene_handle h, cudaStream_t st) {
         p.nodes = (float*)h->tp.nodes; p.node_box = h->node_box;
         CU(launch_refit_spheres(p, st));
         for (size_t k = 0; k + 1 < h->level_off.size(); ++k)
-            CU(launch_refit_nodes(p, h->level_nodes + h->level_off[k], h->level_off[k + 1] - h->level_off[k], st));
+            CU(launch_refit_nodes(p, h->level_nodes_dev + h->level_off[k], h->level_off[k + 1] - h->level_off[k], st));
     }
     CU(cudaEventRecord(h->updated, st));
     return RT_OK;
@@ -884,10 +864,10 @@ int rtb200_scene_update_spheres(rtb200_scene_handle h, const uint32_t* index, co
     DeviceCtx* ctx = h->ctx;
     std::lock_guard<std::recursive_mutex> lk(ctx->mu);
     CU(cudaSetDevice(h->device));
-    int rc = refit_prepare(h);
-    if (rc != RT_OK) return rc;
     cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
-    if ((rc = update_begin(h, st)) != RT_OK) return rc;
+    int rc = update_begin(h, st);
+    if (rc == RT_OK) rc = refit_prepare(h, st);
+    if (rc != RT_OK) return rc;
     // input in the pinned staging buffer (geo, materials, indices), copied before this call returns
     const size_t geo_b = (size_t)n * 32, mat_b = (size_t)n * sizeof(DevMat), bytes = geo_b + mat_b + (size_t)n * 4;
     CU(cudaEventSynchronize(ctx->staging_free));   // the previous copy has left the staging buffer
@@ -919,11 +899,11 @@ int rtb200_scene_update_geometry_device(rtb200_scene_handle h, const void* dev_c
     if (!((a.type == cudaMemoryTypeDevice && a.device == h->device) || a.type == cudaMemoryTypeManaged))
         return fail(RT_ERR_INVALID, "dev_center_radius is not device or managed memory of device " + std::to_string(h->device));
     if (h->tp.n == 0) return RT_OK;
-    int rc = refit_prepare(h);
-    if (rc != RT_OK) return rc;
     cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
-    if ((rc = update_begin(h, st)) != RT_OK) return rc;
-    if ((rc = update_after_frames(h, st)) != RT_OK) return rc;
+    int rc = update_begin(h, st);
+    if (rc == RT_OK) rc = refit_prepare(h, st);
+    if (rc == RT_OK) rc = update_after_frames(h, st);
+    if (rc != RT_OK) return rc;
     CU(cudaMemcpyAsync((void*)h->tp.geo, dev_center_radius, (size_t)h->tp.n * 32, cudaMemcpyDeviceToDevice, st));
     return update_finish(h, st);
   });
@@ -935,8 +915,7 @@ int rtb200_scene_debug_records(rtb200_scene_handle h, uint32_t info[8], float* n
   return guarded([&]() -> int {
     if (!h || !info) return fail(RT_ERR_INVALID, "null argument");
     const TraceParams& tp = h->tp;
-    info[0] = tp.n_nodes; info[1] = tp.n_leaves; info[2] = tp.depth; info[3] = (uint32_t)rtbvh::kLeafK; info[4] = tp.n_always;
-    info[5] = (uint32_t)rtbvh::kNodeFloats; info[6] = tp.filt ? tp.n_pairs : 0u; info[7] = 0;
+    bvh_info(info, tp.n_nodes, tp.n_leaves, tp.depth, tp.n_always, tp.filt ? tp.n_pairs : 0u);
     DeviceRestore restore;
     std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
     CU(cudaSetDevice(h->device));

@@ -16,6 +16,8 @@
 //   * exact geometry {cx,cy,cz,radius} f64 and the material records.
 //
 // Everything is expressed in a frame recentred on the component-wise median of the centres (f32 keeps more bits there).
+// The kernels read these arrays as laid out here. When spheres move, the GPU refit (rtb200_refit.cu) recomputes the
+// position-dependent records with the same RT_HD functions below, compiled for the host and the device.
 #pragma once
 #include <algorithm>
 #include <cmath>
@@ -26,6 +28,12 @@
 
 #include "../../include/rtb200.h"
 
+#ifdef __CUDACC__
+#define RT_HD __host__ __device__
+#else
+#define RT_HD
+#endif
+
 namespace rtbvh {
 
 #ifndef RT_LEAF_K
@@ -33,14 +41,21 @@ namespace rtbvh {
 #endif
 constexpr int kLeafK = RT_LEAF_K; // sphere slots per leaf (RT_LEAF_K/2 pair-packed records); even
 constexpr int kWide = 8;          // children per node
-constexpr int kNodeFloats = 56;   // lo_x[8] lo_y[8] lo_z[8] hi_x[8] hi_y[8] hi_z[8] child[8]  (224 bytes)
-constexpr uint32_t kEmptyChild = 0xffffffffu;
-constexpr uint32_t kLeafBit = 0x80000000u;
+constexpr int kChildOff = 6 * kWide;            // node floats: lo_x[8] lo_y[8] lo_z[8] hi_x[8] hi_y[8] hi_z[8] child[8]
+constexpr int kNodeFloats = kChildOff + kWide;  // (224 bytes)
+constexpr uint32_t kEmptyChild = 0xffffffffu;   // child word of an empty slot
+constexpr uint32_t kLeafBit = 0x80000000u;      // child word of a leaf: kLeafBit | leaf
+constexpr uint32_t kPadId = 0xffffffffu;        // leaf_id of a padding slot
+// skip_pos: kSkipNodeBit | node * kWide + child, or leaf * kLeafK + slot, or kNoSkip (Records::skip_pos)
+constexpr uint32_t kSkipNodeBit = 0x80000000u;
+constexpr uint32_t kNoSkip = 0xffffffffu;
 constexpr int kMaxDepth = 21;     // wide levels the builder can produce; the kernel's node stack needs 32 + 7*depth + 8 entries (rtb200_api.cu asserts it)
 constexpr int kAreaFirstLevels = 15;   // below this wide level children are expanded breadth-first (3 binary levels per wide level)
 constexpr double kU = 5.9604644775390625e-8;   // 2^-24
 
-struct Mat32 { float r, g, b; uint32_t kind; double param; int32_t tex; int32_t pad; };   // = rtk::DevMat
+// 32-byte material record: the material half of rt_sphere as the kernels read it
+struct Mat32 { float r, g, b; uint32_t kind; double param; int32_t tex; int32_t pad; };
+static_assert(sizeof(Mat32) == 32, "Mat32 must be 32 bytes");
 
 struct Records {
     double g[3] = {0, 0, 0};
@@ -48,38 +63,81 @@ struct Records {
     uint32_t n_nodes = 0, n_leaves = 0, depth = 0;
     std::vector<float> nodes;         // n_nodes * kNodeFloats
     std::vector<float> leaf_rec;      // n_leaves * kLeafK * 4
-    std::vector<uint32_t> leaf_id;    // n_leaves * kLeafK, 0xffffffff = padding slot
+    std::vector<uint32_t> leaf_id;    // n_leaves * kLeafK, kPadId = padding slot
     std::vector<uint32_t> always;     // spheres tested in f64 for every ray
-    // max(n,1): sphere -> where the traversal leaves it out for a ray that starts on it (rtk::kNoSkip etc.):
-    // 0x80000000 | node * kWide + child when it is the only member of that child leaf, else its leaf_id index
-    // leaf * kLeafK + slot, or 0xffffffff when it is in no leaf
+    // max(n,1): sphere -> where the traversal leaves it out for a ray that starts on it: kSkipNodeBit | node * kWide + child
+    // when it is the only member of that child leaf, else its leaf_id index leaf * kLeafK + slot, or kNoSkip
     std::vector<uint32_t> skip_pos;
+    std::vector<uint32_t> level_nodes, level_off;   // nodes by wide level, deepest first: level_nodes[level_off[k], level_off[k+1])
     uint32_t n_pairs = 0;
     std::vector<float> flat;          // n_pairs * 8: every sphere, list order, pair-packed (padding never hits)
     std::vector<double> geo;          // max(n,1) * 4
     std::vector<Mat32> mat;           // max(n,1)
 };
 
-inline float f32_up(double x) {     // smallest float >= x
-    float f = (float)x;
-    if ((double)f < x) f = std::nextafterf(f, INFINITY);
-    return f;
-}
-inline float f32_down(double x) {   // largest float <= x
-    float f = (float)x;
-    if ((double)f > x) f = std::nextafterf(f, -INFINITY);
-    return f;
+// ---- rounding primitives: the host's operators (built with -ffp-contract=off) and conversions; on the device, intrinsics
+// that give the same bits (nvcc would otherwise contract a*b+c into an FMA) ----
+#ifdef __CUDA_ARCH__
+RT_HD inline double add_rn(double a, double b) { return __dadd_rn(a, b); }
+RT_HD inline double sub_rn(double a, double b) { return __dsub_rn(a, b); }
+RT_HD inline double mul_rn(double a, double b) { return __dmul_rn(a, b); }
+RT_HD inline float f32_rn(double x) { return __double2float_rn(x); }
+RT_HD inline float f32_up(double x) { return __double2float_ru(x); }
+RT_HD inline float f32_down(double x) { return __double2float_rd(x); }
+#else
+inline double add_rn(double a, double b) { return a + b; }
+inline double sub_rn(double a, double b) { return a - b; }
+inline double mul_rn(double a, double b) { return a * b; }
+inline float f32_rn(double x) { return (float)x; }
+inline float f32_up(double x) { const float f = (float)x; return (double)f < x ? std::nextafterf(f, INFINITY) : f; }      // smallest float >= x
+inline float f32_down(double x) { const float f = (float)x; return (double)f > x ? std::nextafterf(f, -INFINITY) : f; }   // largest float <= x
+#endif
+
+// ---- the position-dependent records of one sphere G = {cx, cy, cz, radius} (Records::geo) in the frame recentred on g ----
+// Record of the conservative sphere test:
+// candidate iff  b^2 + 2c.o + nk >= |o|^2 (1 - 96u),  nk = -(|c|^2 - r^2) + Es rounded up,  Es = 96u|c|^2 + 16u r^2.
+// A sphere the f32 frame cannot hold gets (0, 0, 0, +inf): a candidate for every ray, tested in f64.
+RT_HD inline void sphere_record(const double G[4], const double g[3], float rec[4]) {
+    const double x = sub_rn(G[0], g[0]), y = sub_rn(G[1], g[1]), z = sub_rn(G[2], g[2]), r2 = mul_rn(G[3], G[3]);
+    const double c2 = add_rn(add_rn(mul_rn(x, x), mul_rn(y, y)), mul_rn(z, z));
+    const double Es = add_rn(add_rn(mul_rn(96.0 * kU, c2), mul_rn(16.0 * kU, r2)), 1e-30);
+    const double nkd = add_rn(-sub_rn(c2, r2), Es);
+    rec[0] = f32_rn(x); rec[1] = f32_rn(y); rec[2] = f32_rn(z);
+    rec[3] = std::isfinite(nkd) ? f32_up(nkd) : INFINITY;
+    if (!(std::isfinite(rec[0]) && std::isfinite(rec[1]) && std::isfinite(rec[2]) && std::isfinite(nkd) && c2 < 1e30)) {
+        rec[0] = rec[1] = rec[2] = 0.f; rec[3] = INFINITY;
+    }
 }
 
-// Record of the conservative sphere test for a sphere at recentred (x,y,z) with squared radius r2.
-// candidate iff  b^2 + 2c.o + nk >= |o|^2 (1 - 96u),  nk = -(|c|^2 - r^2) + Es rounded up,  Es = 96u|c|^2 + 16u r^2.
-inline bool sphere_record(double x, double y, double z, double r2, float rec[4]) {
-    const double c2 = x * x + y * y + z * z;
-    const double Es = 96.0 * kU * c2 + 16.0 * kU * r2 + 1e-30;
-    const double nkd = -(c2 - r2) + Es;
-    rec[0] = (float)x; rec[1] = (float)y; rec[2] = (float)z;
-    rec[3] = std::isfinite(nkd) ? f32_up(nkd) : INFINITY;
-    return std::isfinite(rec[0]) && std::isfinite(rec[1]) && std::isfinite(rec[2]) && std::isfinite(nkd) && c2 < 1e30;
+// Exact box (c - g) +- |r|. Returns whether the sphere lives in the f32 frame (finite, max|c - g| + |r| < 1e15; tested for
+// NaN before any max); the builder puts the others on the always-list, and their box is (-inf, +inf) on every axis.
+RT_HD inline bool sphere_box(const double G[4], const double g[3], double lo[3], double hi[3]) {
+    const double c[3] = {sub_rn(G[0], g[0]), sub_rn(G[1], g[1]), sub_rn(G[2], g[2])};
+    const double r = std::fabs(G[3]);
+    const bool fin = std::isfinite(c[0]) && std::isfinite(c[1]) && std::isfinite(c[2]) && std::isfinite(r);
+    const bool inside = fin && add_rn(std::fmax(std::fmax(std::fabs(c[0]), std::fabs(c[1])), std::fabs(c[2])), r) < 1e15;
+    for (int a = 0; a < 3; ++a) { lo[a] = inside ? sub_rn(c[a], r) : -INFINITY; hi[a] = inside ? add_rn(c[a], r) : INFINITY; }
+    return inside;
+}
+
+// Child slot i of `node` gets the exact box {lo, hi}, inflated by m = 32u * max|coordinate| + 1e-30 and rounded outwards
+// (DESIGN.md §4.2: covers the f32 rounding of the slab test on the box's side).
+RT_HD inline void set_child_box(float* node, int i, const double lo[3], const double hi[3]) {
+    double bmax = 0.0;
+    for (int a = 0; a < 3; ++a) bmax = std::fmax(bmax, std::fmax(std::fabs(lo[a]), std::fabs(hi[a])));
+    const double m = add_rn(mul_rn(32.0 * kU, bmax), 1e-30);
+    for (int a = 0; a < 3; ++a) {
+        node[a * kWide + i] = f32_down(sub_rn(lo[a], m));
+        node[3 * kWide + a * kWide + i] = f32_up(add_rn(hi[a], m));
+    }
+}
+
+RT_HD inline uint32_t child_of(const float* node, int i) { uint32_t ref; memcpy(&ref, node + kChildOff + i, 4); return ref; }
+
+// Record `slot` of pair-packed records ({x0,x1,y0,y1},{z0,z1,nk0,nk1} per pair of slots)
+RT_HD inline void put_record(float* pairs, size_t slot, const float rec[4]) {
+    float* A = pairs + slot / 2 * 8 + (slot & 1);
+    A[0] = rec[0]; A[2] = rec[1]; A[4] = rec[2]; A[6] = rec[3];
 }
 
 // Exact geometry {cx,cy,cz,radius} and material record of one sphere (the upload and rtb200_scene_update_spheres).
@@ -115,17 +173,12 @@ public:
         if (!want_tree) return;
         // primitives of the hierarchy: spheres that live in the f32 frame; the rest is tested for every ray
         for (uint32_t i = 0; i < n; ++i) {
-            const rt_sphere& sp = s_->spheres[i];
-            double c[3] = {sp.center.x - R_.g[0], sp.center.y - R_.g[1], sp.center.z - R_.g[2]};
-            const double r = std::fabs(sp.radius);
-            const bool fin = std::isfinite(c[0]) && std::isfinite(c[1]) && std::isfinite(c[2]) && std::isfinite(r);
-            const double ext = fin ? std::max(std::max(std::fabs(c[0]), std::fabs(c[1])), std::fabs(c[2])) + r : INFINITY;
-            if (!fin || !(ext < 1e15)) { R_.always.push_back(i); continue; }
+            const double* G = &R_.geo[4 * (size_t)i];
             Box b;
-            for (int a = 0; a < 3; ++a) { b.lo[a] = c[a] - r; b.hi[a] = c[a] + r; }
+            if (!sphere_box(G, R_.g, b.lo, b.hi)) { R_.always.push_back(i); continue; }
             prim_box_.push_back(b);
             prim_id_.push_back(i);
-            prim_c_.push_back({c[0], c[1], c[2]});
+            prim_c_.push_back({G[0] - R_.g[0], G[1] - R_.g[1], G[2] - R_.g[2]});
         }
         if (prim_id_.empty()) return;
         order_.resize(prim_id_.size());
@@ -138,10 +191,15 @@ public:
         sah_limit_ = std::max(4, 30 - lg - 1);
         if (const char* e = getenv("RTB200_BVH_AREA_LEVELS")) area_levels_ = std::max(1, atoi(e));   // test hook: exercise the breadth-first collapse
         const int root = build(0, (uint32_t)order_.size(), 0);
-        R_.depth = 0;
         emit_wide(root, 1);
+        R_.depth = (uint32_t)levels_.size();
         R_.n_nodes = (uint32_t)(R_.nodes.size() / kNodeFloats);
         R_.n_leaves = (uint32_t)(R_.leaf_id.size() / kLeafK);
+        R_.level_off.assign(1, 0u);
+        for (size_t k = levels_.size(); k-- > 0;) {
+            R_.level_nodes.insert(R_.level_nodes.end(), levels_[k].begin(), levels_[k].end());
+            R_.level_off.push_back((uint32_t)R_.level_nodes.size());
+        }
     }
 
 private:
@@ -153,6 +211,7 @@ private:
     std::vector<P3> prim_c_;
     std::vector<uint32_t> order_;
     std::vector<BinNode> bin_;
+    std::vector<std::vector<uint32_t>> levels_;   // emitted nodes by wide level, root first
     int sah_limit_ = 24;
     int area_levels_ = kAreaFirstLevels;
 
@@ -176,20 +235,13 @@ private:
         R_.geo.assign((size_t)std::max<uint32_t>(n, 1) * 4, 0.0);
         R_.mat.resize(std::max<uint32_t>(n, 1));
         std::memset(R_.mat.data(), 0, R_.mat.size() * sizeof(Mat32));
-        for (uint32_t pp = 0; pp < n_pairs; ++pp) {
-            float* A = &R_.flat[(size_t)pp * 8];
-            for (int k = 0; k < 2; ++k) {
-                const uint32_t i = 2 * pp + k;
-                float rec[4] = {0.f, 0.f, 0.f, -INFINITY};
-                if (i < n) {
-                    const rt_sphere& sp = s_->spheres[i];
-                    if (!sphere_record(sp.center.x - R_.g[0], sp.center.y - R_.g[1], sp.center.z - R_.g[2], sp.radius * sp.radius, rec)) {
-                        rec[0] = rec[1] = rec[2] = 0.f; rec[3] = INFINITY;   // always a candidate
-                    }
-                    sphere_exact(sp, &R_.geo[4 * (size_t)i], R_.mat[i]);
-                }
-                A[0 + k] = rec[0]; A[2 + k] = rec[1]; A[4 + k] = rec[2]; A[6 + k] = rec[3];
+        for (uint32_t i = 0; i < 2 * n_pairs; ++i) {
+            float rec[4] = {0.f, 0.f, 0.f, -INFINITY};   // padding slot: never hit
+            if (i < n) {
+                sphere_exact(s_->spheres[i], &R_.geo[4 * (size_t)i], R_.mat[i]);
+                sphere_record(&R_.geo[4 * (size_t)i], R_.g, rec);
             }
+            put_record(R_.flat.data(), i, rec);
         }
     }
 
@@ -273,7 +325,7 @@ private:
     uint32_t emit_leaf(const BinNode& b) {
         const uint32_t leaf = (uint32_t)(R_.leaf_id.size() / kLeafK);
         R_.leaf_rec.resize(R_.leaf_rec.size() + (size_t)kLeafK * 4, 0.f);
-        R_.leaf_id.resize(R_.leaf_id.size() + kLeafK, 0xffffffffu);
+        R_.leaf_id.resize(R_.leaf_id.size() + kLeafK, kPadId);
         float* rec = &R_.leaf_rec[(size_t)leaf * kLeafK * 4];
         uint32_t* ids = &R_.leaf_id[(size_t)leaf * kLeafK];
         // members in increasing ORIGINAL index (not required for correctness; keeps the layout deterministic)
@@ -284,23 +336,20 @@ private:
         for (int j = 0; j < kLeafK; ++j) {
             float r4[4] = {0.f, 0.f, 0.f, -INFINITY};   // padding slot: never hit
             if (j < n_mem) {
-                const rt_sphere& sp = s_->spheres[mem[j]];
-                if (!sphere_record(sp.center.x - R_.g[0], sp.center.y - R_.g[1], sp.center.z - R_.g[2], sp.radius * sp.radius, r4)) {
-                    r4[0] = r4[1] = r4[2] = 0.f; r4[3] = INFINITY;
-                }
+                sphere_record(&R_.geo[4 * (size_t)mem[j]], R_.g, r4);
                 ids[j] = mem[j];
             }
-            float* A = rec + (size_t)(j / 2) * 8; const int kk = j & 1;
-            A[0 + kk] = r4[0]; A[2 + kk] = r4[1]; A[4 + kk] = r4[2]; A[6 + kk] = r4[3];
+            put_record(rec, j, r4);
         }
         return leaf;
     }
 
     // Collapse the binary tree under `b` into one 8-wide node (largest-area inner child expanded first) and recurse.
     uint32_t emit_wide(int b, uint32_t level) {
-        R_.depth = std::max(R_.depth, level);
         const uint32_t me = (uint32_t)(R_.nodes.size() / kNodeFloats);
         R_.nodes.resize(R_.nodes.size() + kNodeFloats, 0.f);
+        if (levels_.size() < level) levels_.resize(level);
+        levels_[level - 1].push_back(me);
         std::vector<int> kids;
         if (bin_[b].left < 0) kids.push_back(b);   // the whole tree is one leaf
         else { kids.push_back(bin_[b].left); kids.push_back(bin_[b].right); }
@@ -332,20 +381,15 @@ private:
             kids.push_back(bin_[c].right);
         }
         for (int i = 0; i < kWide; ++i) {
-            float lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};   // empty slot: never hit
             uint32_t ref = kEmptyChild;
             if (i < (int)kids.size()) {
                 const BinNode& c = bin_[kids[i]];
-                double bmax = 0.0;
-                for (int a = 0; a < 3; ++a) bmax = std::max(bmax, std::max(std::fabs(c.box.lo[a]), std::fabs(c.box.hi[a])));
-                const double m = 32.0 * kU * bmax + 1e-30;   // DESIGN.md §4.2: covers the f32 rounding of the slab test on the box's side
-                for (int a = 0; a < 3; ++a) { lo[a] = f32_down(c.box.lo[a] - m); hi[a] = f32_up(c.box.hi[a] + m); }
-                if (c.left < 0) ref = kLeafBit | emit_leaf(c);
-                else ref = emit_wide(kids[i], level + 1);
+                ref = c.left < 0 ? kLeafBit | emit_leaf(c) : emit_wide(kids[i], level + 1);
             }
-            float* N = &R_.nodes[(size_t)me * kNodeFloats];   // re-fetch: the vector may have grown
-            for (int a = 0; a < 3; ++a) { N[a * 8 + i] = lo[a]; N[24 + a * 8 + i] = hi[a]; }
-            std::memcpy(&N[48 + i], &ref, 4);
+            float* N = &R_.nodes[(size_t)me * kNodeFloats];   // after the recursion: the vector may have grown
+            if (ref != kEmptyChild) set_child_box(N, i, bin_[kids[i]].box.lo, bin_[kids[i]].box.hi);
+            else for (int a = 0; a < 3; ++a) { N[a * kWide + i] = INFINITY; N[3 * kWide + a * kWide + i] = -INFINITY; }   // never hit
+            std::memcpy(&N[kChildOff + i], &ref, 4);
         }
         return me;
     }
@@ -355,18 +399,17 @@ private:
 inline void build_records(const rt_scene* s, bool want_tree, Records& R) {
     Builder b(s, R);
     b.run(want_tree);
-    R.skip_pos.assign(std::max<uint32_t>(R.n, 1), 0xffffffffu);   // every sphere is in one leaf at most
+    R.skip_pos.assign(std::max<uint32_t>(R.n, 1), kNoSkip);   // every sphere is in one leaf at most
     for (size_t k = 0; k < R.leaf_id.size(); ++k) if (R.leaf_id[k] < R.n) R.skip_pos[R.leaf_id[k]] = (uint32_t)k;
     // a leaf with a single member is dropped by its parent node instead: the leaf step is then not run at all
     for (uint32_t node = 0; node < R.n_nodes; ++node) {
         for (int c = 0; c < kWide; ++c) {
-            uint32_t ref;
-            std::memcpy(&ref, &R.nodes[(size_t)node * kNodeFloats + 48 + c], 4);
-            if (ref == 0xffffffffu || !(ref & 0x80000000u)) continue;
-            const uint32_t* ids = &R.leaf_id[(size_t)(ref & 0x7fffffffu) * kLeafK];
+            const uint32_t ref = child_of(&R.nodes[(size_t)node * kNodeFloats], c);
+            if (ref == kEmptyChild || !(ref & kLeafBit)) continue;
+            const uint32_t* ids = &R.leaf_id[(size_t)(ref & ~kLeafBit) * kLeafK];
             int members = 0;
-            for (int j = 0; j < kLeafK; ++j) members += ids[j] != 0xffffffffu;
-            if (members == 1 && ids[0] < R.n) R.skip_pos[ids[0]] = 0x80000000u | (node * (uint32_t)kWide + (uint32_t)c);
+            for (int j = 0; j < kLeafK; ++j) members += ids[j] != kPadId;
+            if (members == 1 && ids[0] < R.n) R.skip_pos[ids[0]] = kSkipNodeBit | (node * (uint32_t)kWide + (uint32_t)c);
         }
     }
 }

@@ -4,9 +4,16 @@
 #include <stdint.h>
 
 #include "../../include/rtb200.h"
+#include "rtb200_bvh.hpp"
 #include "rtb200_device.cuh"
 
 namespace rtk {
+
+// the scene's layout is rtbvh's (rtb200_bvh.hpp)
+using rtbvh::kLeafK;                                // sphere slots per BVH leaf
+constexpr int kNodeVec = rtbvh::kNodeFloats / 4;    // float4 per 8-wide BVH node
+constexpr int kChildVec = rtbvh::kChildOff / 4;     // float4 offset of a node's child words
+using DevMat = rtbvh::Mat32;                         // 32-byte material record
 
 #ifndef RT_BLOCK
 #define RT_BLOCK 256
@@ -22,11 +29,6 @@ constexpr int kBlock = RT_BLOCK;   // threads (= ray slots) per CTA of the trace
 enum : uint32_t { PH_HIT, PH_SORT_WAIT_A, PH_SHADE, PH_REGEN, PH_WAIT_C, PH_ITERS, PH_SCATTERS, PH_DEFERRED,
                   PH_NODE, PH_LEAF, PH_EXACT, PH_EXACT_STEPS, PH_EXACT_TESTS, PH_SRC_SKIPS, kPhaseN };
 constexpr uint32_t kPhaseStat = 13;
-#ifndef RT_LEAF_K
-#define RT_LEAF_K 8
-#endif
-constexpr int kLeafK = RT_LEAF_K;  // sphere slots per BVH leaf            (= rtbvh::kLeafK)
-constexpr int kNodeVec = 14;       // float4 per 8-wide BVH node (224 B)   (= rtbvh::kNodeFloats / 4)
 // per-warp work lists of the closest-hit stage (entries: id << 5 | ray lane)
 #ifndef RT_CAP_IN
 #define RT_CAP_IN 192
@@ -40,10 +42,6 @@ constexpr int kNodeVec = 14;       // float4 per 8-wide BVH node (224 B)   (= rt
 constexpr int kCapIn = RT_CAP_IN;   // (ray, inner node) pairs: LIFO stack; 7*depth+8 entries are reserved for single-entry descents
 constexpr int kCapLf = RT_CAP_LF;   // (ray, leaf) pairs
 constexpr int kCapCd = RT_CAP_CD;   // (ray, sphere) pairs awaiting the exact f64 test
-
-// 32-byte material record (device copy of the material half of rt_sphere)
-struct DevMat { float r, g, b; uint32_t kind; double param; int32_t tex; int32_t pad; };
-static_assert(sizeof(DevMat) == 32, "DevMat must be 32 bytes");
 
 // One pending light test (raytracer.rs:99-114): the vertex it belongs to and the partial sum over the lights.
 struct ShadowFrame {
@@ -66,8 +64,8 @@ struct TraceParams {
     // ---- scene, resident in HBM (built by rtbvh::build_records) ----
     const float4*   nodes;       // n_nodes * kNodeVec: lo_x[8] lo_y[8] lo_z[8] hi_x[8] hi_y[8] hi_z[8] child[8], f32 boxes rounded outwards
     const float4*   leaf_rec;    // n_leaves * kLeafK float4: kLeafK/2 pair-packed sphere records {cx0,cx1,cy0,cy1},{cz0,cz1,nk0,nk1}
-    const uint32_t* leaf_id;     // n_leaves * kLeafK: slot -> ORIGINAL sphere index (0xffffffff = padding)
-    const uint32_t* skip_pos;    // n: where the traversal can leave the sphere out (rtbvh::Records::skip_pos, rtk::kNoSkip)
+    const uint32_t* leaf_id;     // n_leaves * kLeafK: slot -> ORIGINAL sphere index (rtbvh::kPadId = padding)
+    const uint32_t* skip_pos;    // n: where the traversal can leave the sphere out (rtbvh::Records::skip_pos)
     const uint32_t* always;      // n_always sphere indices tested in f64 for every ray (not representable in the f32 frame)
     const float4*   filt;        // n_pairs * 2 float4: every sphere in list order, pair-packed (MODE_BRUTE)
     const double4*  geo;         // n: {cx,cy,cz,radius} exact f64
@@ -119,7 +117,7 @@ struct ResolveParams {
 struct RefitParams {
     const double4* geo;
     uint32_t n;
-    double gx, gy, gz;
+    double g[3];                 // recentring offset
     float* filt;                 // MODE_BRUTE: n_pairs * 8 flat records, else null
     const uint32_t* leaf_id;     // MODE_TREE from here on
     float* leaf_rec;

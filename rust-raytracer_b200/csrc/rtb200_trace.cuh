@@ -35,14 +35,14 @@ constexpr uint32_t kDeadLevel = 0xffffffffu;
 // Pool.shd bit: the slot's scatter sample is still being drawn; its hit record (bt/bi) and path state are those of the
 // vertex being shaded. The shadow depth in the low bits never exceeds max_shadow (<= 384), so the bit is free.
 constexpr uint32_t kScatterPending = 0x80000000u;
-constexpr uint32_t kLeafBit = 0x80000000u;
+using rtbvh::kLeafBit;
 constexpr unsigned long long kNoHitBits = 0x7ff0000000000000ull;   // +inf as the "no root yet" key (roots are > t_min > 0)
 constexpr uint32_t kNoSphere = 0xffffffffu;     // Pool.src: the ray does not start on a known sphere
 // skip_pos / WarpCtx.skip: where the traversal leaves the certified source sphere out. kSkipNodeBit | node * 8 + child: the
 // node step drops child `child` of `node` (a leaf holding only that sphere); else leaf * kLeafK + slot: the leaf step drops
 // the slot. kNoSkip: nothing (kNoSkip / kLeafK and (kNoSkip & ~kSkipNodeBit) / 8 are no leaf's or node's index, < 2^27).
-constexpr uint32_t kSkipNodeBit = 0x80000000u;
-constexpr uint32_t kNoSkip = 0xffffffffu;
+using rtbvh::kSkipNodeBit;
+using rtbvh::kNoSkip;
 constexpr uint32_t kSlotBytes = 7 * 8 + 10 * 4 + RT_SMEM_STACK * 4;   // shared memory per pool slot
 constexpr uint32_t kFrameSlotBytes = 4;                               // + Pool.frm per slot in a multi-frame launch
 
@@ -264,7 +264,7 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                             hit |= (fmaxf(fmax3(tnx1.x, tny1.x, tnz1.x), 0.f) <= fmin3(tfx1.x, tfy1.x, tfz1.x) ? 1u : 0u) << (4 * h + 2);
                             hit |= (fmaxf(fmax3(tnx1.y, tny1.y, tnz1.y), 0.f) <= fmin3(tfx1.y, tfy1.y, tfz1.y) ? 1u : 0u) << (4 * h + 3);
                         }
-                        const uint4 R0 = *reinterpret_cast<const uint4*>(N + 12), R1 = *reinterpret_cast<const uint4*>(N + 13);
+                        const uint4 R0 = *reinterpret_cast<const uint4*>(N + kChildVec), R1 = *reinterpret_cast<const uint4*>(N + kChildVec + 1);
                         leafbits = (R0.x >> 31) | ((R0.y >> 31) << 1) | ((R0.z >> 31) << 2) | ((R0.w >> 31) << 3) |
                                    ((R1.x >> 31) << 4) | ((R1.y >> 31) << 5) | ((R1.z >> 31) << 6) | ((R1.w >> 31) << 7);
                     }
@@ -291,7 +291,7 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                     if (act && (uint32_t)lane < k) {
                         const uint32_t exc = inc - packed;
                         uint32_t pi = (n_in - k) + (exc & 0xffffu), pl = n_lf + (exc >> 16);
-                        const uint32_t* refs = reinterpret_cast<const uint32_t*>(N + 12);
+                        const uint32_t* refs = reinterpret_cast<const uint32_t*>(N + kChildVec);
                         uint32_t mm = hit;
                         while (mm) {
                             const int c = __ffs(mm) - 1;

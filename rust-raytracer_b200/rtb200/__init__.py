@@ -384,6 +384,16 @@ def load_scene(path: str, base_dir: Optional[str] = None) -> Scene:
     return Scene.from_config(cfg, base_dir)
 
 
+def _record_views(info, nodes: np.ndarray, rec: np.ndarray, flat: np.ndarray) -> dict:
+    """The float arrays of rtb200_debug_bvh / rtb200_scene_debug_records, sized by their info[8], in their logical shapes:
+    a node is lo[3][8], hi[3][8], child[8]; a leaf holds k/2 pair-packed records; a flat pair is one record pair."""
+    n_nodes, n_leaves, depth, k, _, fpn, n_pairs, _ = (int(x) for x in info)
+    nd = nodes[: n_nodes * fpn].reshape(n_nodes, fpn)
+    return {"n_nodes": n_nodes, "n_leaves": n_leaves, "depth": depth,
+            "lo": nd[:, :24].reshape(n_nodes, 3, 8), "hi": nd[:, 24:48].reshape(n_nodes, 3, 8), "child": nd[:, 48:56].view(np.uint32),
+            "leaf_rec": rec[: n_leaves * k * 4].reshape(n_leaves, k // 2, 2, 4), "flat": flat[: n_pairs * 8].reshape(n_pairs, 2, 4)}
+
+
 def bvh_records(scene: "Scene") -> dict:
     """Host-side diagnostic: the hierarchy the closest-hit stage traverses (no GPU needed). See rtb200_debug_bvh."""
     n = scene.n_spheres
@@ -394,11 +404,8 @@ def bvh_records(scene: "Scene") -> dict:
     ids = np.zeros(max(n_leaves * k, 1), np.uint32); always = np.zeros(max(n_always, 1), np.uint32); flat = np.zeros(max(n_pairs * 8, 1), np.float32)
     _check(lib().rtb200_debug_bvh(C.byref(scene.c), g, info, nodes.ctypes.data, nodes.size, rec.ctypes.data, rec.size, ids.ctypes.data, ids.size,
                                   always.ctypes.data, always.size, flat.ctypes.data, flat.size))
-    nd = nodes[: n_nodes * fpn].reshape(n_nodes, fpn)
-    return {"n_nodes": n_nodes, "n_leaves": n_leaves, "depth": depth, "leaf_size": k, "recentre": np.array(g[:]), "n": n,
-            "lo": nd[:, :24].reshape(n_nodes, 3, 8), "hi": nd[:, 24:48].reshape(n_nodes, 3, 8), "child": nd[:, 48:56].view(np.uint32),
-            "leaf_rec": rec[: n_leaves * k * 4].reshape(n_leaves, k // 2, 2, 4), "leaf_id": ids[: n_leaves * k].reshape(n_leaves, k),
-            "always": always[:n_always], "flat": flat[: n_pairs * 8].reshape(n_pairs, 2, 4)}
+    return {**_record_views(info, nodes, rec, flat), "leaf_size": k, "recentre": np.array(g[:]), "n": n,
+            "leaf_id": ids[: n_leaves * k].reshape(n_leaves, k), "always": always[:n_always]}
 
 
 def make_options(device: int = -1, rank: int = 0, world: int = 1, band_rows: int = 1, variant: int = RT_VARIANT_AUTO,
@@ -555,11 +562,8 @@ class ResidentScene:
         flat = np.zeros(max(n_pairs * 8, 1), np.float32); geo = np.zeros(max(self.n * 4, 1), np.float64)
         _check(lib().rtb200_scene_debug_records(self.h, info, nodes.ctypes.data, nodes.size, rec.ctypes.data, rec.size,
                                                 flat.ctypes.data, flat.size, geo.ctypes.data, geo.size))
-        nd = nodes[: n_nodes * fpn].reshape(n_nodes, fpn)
-        b.update({"n_nodes": n_nodes, "n_leaves": n_leaves, "depth": depth,
-                  "lo": nd[:, :24].reshape(n_nodes, 3, 8), "hi": nd[:, 24:48].reshape(n_nodes, 3, 8), "child": nd[:, 48:56].view(np.uint32),
-                  "leaf_rec": rec[: n_leaves * k * 4].reshape(n_leaves, k // 2, 2, 4), "leaf_id": b["leaf_id"][:n_leaves],
-                  "always": b["always"][:n_always], "flat": flat[: n_pairs * 8].reshape(n_pairs, 2, 4), "geo": geo[: self.n * 4].reshape(self.n, 4)})
+        b.update(_record_views(info, nodes, rec, flat))
+        b.update({"leaf_id": b["leaf_id"][:n_leaves], "always": b["always"][:n_always], "geo": geo[: self.n * 4].reshape(self.n, 4)})
         return b
 
     def kernel_info(self) -> dict:

@@ -1,6 +1,6 @@
 // Host-side robustness harness, built with -fsanitize=address,undefined by tests/test_host_sanitizers.py (no GPU, no CUDA).
 // Exercises the three pieces of host code that consume untrusted or awkward input on the way to the render call:
-//   1. the hierarchy builder (csrc/rtb200_bvh.hpp) on degenerate scenes, checking every index it emits;
+//   1. the hierarchy builder (csrc/rtb200_bvh.hpp) on degenerate scenes, checking every index it emits and its level order;
 //   2. the baseline JPEG decoder (host/jpeg_decode.cpp) on mutated / truncated files;
 //   3. the scene reader (host/scene_json.cpp + json.hpp) on mutated / truncated / deeply nested JSON.
 // Exit code 0 and the line "host_sanitize: ok" = no sanitizer report, no escaped exception, no out-of-range index.
@@ -51,10 +51,24 @@ static void check_records(const char* what, const std::vector<rt_sphere>& sph, b
     REQUIRE(R.depth <= (uint32_t)rtbvh::kMaxDepth, "%s: depth %u", what, R.depth);
     std::vector<uint8_t> seen(n, 0), leaf_seen(R.n_leaves, 0), node_seen(R.n_nodes, 0);
     for (uint32_t a : R.always) { REQUIRE(a < n, "%s: always index", what); if (a < n) { REQUIRE(!seen[a], "%s: sphere twice", what); seen[a] = 1; } }
+    // level order: every node once, in groups (deepest level first) that match the depth
+    const size_t n_groups = R.level_off.empty() ? 0 : R.level_off.size() - 1;
+    REQUIRE(n_groups == R.depth, "%s: %zu level groups for depth %u", what, n_groups, R.depth);
+    REQUIRE(R.level_nodes.size() == R.n_nodes && (R.level_off.empty() ? R.n_nodes == 0 : R.level_off.front() == 0 && R.level_off.back() == R.n_nodes),
+            "%s: level order size", what);
+    std::vector<uint32_t> group(R.n_nodes, ~0u);
+    for (size_t g = 0; g < n_groups; ++g) {
+        REQUIRE(R.level_off[g] < R.level_off[g + 1], "%s: empty level group %zu", what, g);
+        for (uint32_t t = R.level_off[g]; t < R.level_off[g + 1] && t < R.level_nodes.size(); ++t) {
+            const uint32_t v = R.level_nodes[t];
+            REQUIRE(v < R.n_nodes, "%s: level order node %u of %u", what, v, R.n_nodes);
+            if (v < R.n_nodes) { REQUIRE(group[v] == ~0u, "%s: node %u twice in the level order", what, v); group[v] = (uint32_t)g; }
+        }
+    }
     if (R.n_nodes) node_seen[0] = 1;
     for (uint32_t k = 0; k < R.n_nodes; ++k) {
         for (int i = 0; i < rtbvh::kWide; ++i) {
-            uint32_t ref; std::memcpy(&ref, &R.nodes[(size_t)k * rtbvh::kNodeFloats + 48 + i], 4);
+            const uint32_t ref = rtbvh::child_of(&R.nodes[(size_t)k * rtbvh::kNodeFloats], i);
             if (ref == rtbvh::kEmptyChild) continue;
             if (ref & rtbvh::kLeafBit) {
                 const uint32_t l = ref & ~rtbvh::kLeafBit;
@@ -62,7 +76,10 @@ static void check_records(const char* what, const std::vector<rt_sphere>& sph, b
                 if (l < R.n_leaves) { REQUIRE(!leaf_seen[l], "%s: leaf referenced twice", what); leaf_seen[l] = 1; }
             } else {
                 REQUIRE(ref < R.n_nodes && ref > k, "%s: node reference %u from %u of %u", what, ref, k, R.n_nodes);
-                if (ref < R.n_nodes) { REQUIRE(!node_seen[ref], "%s: node referenced twice", what); node_seen[ref] = 1; }
+                if (ref < R.n_nodes) {
+                    REQUIRE(!node_seen[ref], "%s: node referenced twice", what); node_seen[ref] = 1;
+                    REQUIRE(group[ref] < group[k], "%s: node %u is not in a deeper level than its parent %u", what, ref, k);
+                }
             }
         }
     }

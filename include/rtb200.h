@@ -230,7 +230,7 @@ int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, u
  * h already enqueued, on any stream, and before every frame enqueued later; rtb200_scene_release waits for it. The first
  * update of a handle builds the refit's scratch and waits for the library's stream once.
  * Spheres that no longer fit the f32 frame (non-finite, or max|c - recentre| + |radius| >= 1e15) are tested in f64 by every
- * ray; the tree gets slower as spheres wander from where they were uploaded: upload again to rebuild it. */
+ * ray; the tree gets slower as spheres wander from where they were uploaded: rtb200_scene_rebuild gives it a new topology. */
 /* Replace spheres index[k] (k < n) of a resident scene by spheres[k]: centre, radius and material. Everything is checked on
  * the host before anything is enqueued (on error the scene is unchanged); n == 0 is a no-op. RT_ERR_INVALID: NULL arrays, an
  * index >= n_spheres, a repeated index, an unknown kind, a texture index outside the uploaded textures (or one whose image was
@@ -245,6 +245,31 @@ int rtb200_scene_update_geometry_device(rtb200_scene_handle h, const void* dev_c
  * {cx,cy,cz,radius}, laid out as rtb200_debug_bvh's (same info[]); arrays are filled up to their capacities (elements). */
 int rtb200_scene_debug_records(rtb200_scene_handle h, uint32_t info[8], float* nodes, uint64_t cap_nodes, float* leaf_rec,
                                uint64_t cap_leaf_rec, float* flat, uint64_t cap_flat, double* geo, uint64_t cap_geo);
+
+/* Rebuild the hierarchy of a resident RT_VARIANT_FILTERED / RT_VARIANT_AUTO scene from its current spheres, on the GPU
+ * (DESIGN.md §4.8): a refit keeps the upload's topology, which loosens as spheres wander; a rebuild gives a new one without a
+ * host build or a copy through host memory. Contract, the update's: after a rebuild every render of h is bit-identical, in
+ * linear f32, RGB8 and ray count, to the same render of a fresh upload of the current spheres (the diagnostic candidates /
+ * clusters / nodes counters may differ: the tree differs). The recentring offset (element n/2 of each sorted centre
+ * coordinate, 0 when not finite) and the always-list (the spheres outside the f32 frame, in increasing index order) equal a
+ * fresh upload's.
+ * Ordering: enqueued on `stream` (NULL: the library's stream) after the handle's last update and after every frame of h
+ * already enqueued, on any stream; every frame enqueued later traces the new tree, and later rtb200_scene_update_* calls refit
+ * it. Blocking: the call waits for those frames and for the new topology, reads back one small header (counts, depth, level
+ * sizes, recentring offset) and returns; the values of the new tree are computed on `stream` after it returns.
+ * Memory: one device block for n spheres, allocated at the first rebuild and kept until release: 576 * n + 88 * (n / 9 + 1)
+ * bytes (the tree bound is n leaves and n nodes, DESIGN.md §4.8) plus cub's sort and scan scratch; RT_ERR_OOM, with the scene
+ * unchanged, when it cannot be allocated. A no-op returning RT_OK for RT_VARIANT_EXACT_F64 / RT_VARIANT_BRUTE_FORCE handles (no hierarchy) and for
+ * n_spheres == 0. RT_ERR_INVALID for a NULL handle, before any device is touched. RT_ERR_UNSUPPORTED for a handle that stages
+ * its hierarchy in shared memory (RTB200_WF_SMEM bit 0 at upload): its launch layout is fixed by the upload's tree size. */
+int rtb200_scene_rebuild(rtb200_scene_handle h, void* stream);
+/* Diagnostic: the handle's current topology, the upload's or the last rebuild's: recentring offset, info[] as
+ * rtb200_debug_bvh's, leaf slot -> sphere index (n_leaves * leaf_size), the always-list (n_always), skip_pos (max(n, 1) entries
+ * of a hierarchy handle: kSkipNodeBit | node * 8 + child, leaf * leaf_size + slot, or 0xffffffff), the level order of the
+ * nodes, deepest level first (n_nodes) and its offsets (depth + 1). Arrays are filled up to their capacities (elements). */
+int rtb200_scene_debug_topology(rtb200_scene_handle h, double recentre[3], uint32_t info[8], uint32_t* leaf_id, uint64_t cap_leaf_id,
+                                uint32_t* always, uint64_t cap_always, uint32_t* skip_pos, uint64_t cap_skip_pos,
+                                uint32_t* level_nodes, uint64_t cap_level_nodes, uint32_t* level_off, uint64_t cap_level_off);
 
 /* load_texture_image — materials.rs:213-219, config.rs:36-47: decode a baseline JPEG file to RGB8 (host-side scene staging
  * helper for hosts without their own decoder; the reference uses the jpeg-decoder crate). *out_rgb8 is released with rtb200_free(). */

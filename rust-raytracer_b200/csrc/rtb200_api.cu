@@ -195,6 +195,8 @@ struct rtb200_scene_t {
     double* node_box = nullptr;          // n_nodes exact boxes {lo[3], hi[3]}
     double* leaf_box = nullptr;          // n_leaves exact boxes
     uint32_t* level_nodes_dev = nullptr;
+    // ---- rebuilt hierarchy (rtb200_scene_rebuild): its arrays and the refit's scratch, allocated at the first rebuild ----
+    void* rebuild = nullptr;             // RebuildBufs of tp.n spheres; once set, the tree arrays of tp and the refit scratch live here
     GrowBuf upd_in;                      // host form's input: geo, materials, indices
 };
 
@@ -287,6 +289,7 @@ int rtb200_scene_release(rtb200_scene_handle h) {
         else if (h->ctx->stream) cudaStreamSynchronize(h->ctx->stream);
         if (h->updated) { cudaEventSynchronize(h->updated); cudaEventDestroy(h->updated); }   // an update in flight writes them
         if (h->refit) cudaFree(h->refit);
+        if (h->rebuild) cudaFree(h->rebuild);
         if (h->upd_in.p) cudaFree(h->upd_in.p);
         for (cudaEvent_t e : h->ev) h->ctx->event_pool.push_back(e);
         if (h->arena) {
@@ -797,7 +800,7 @@ int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, u
 // and leaves, and the device copy of the builder's level order (an update never changes the topology).
 static int refit_prepare(rtb200_scene_handle h, cudaStream_t st) {
     const uint32_t nn = h->tp.n_nodes, nl = h->tp.n_leaves;
-    if (h->refit || h->mode != MODE_TREE || nn == 0) return RT_OK;
+    if (h->node_box || h->mode != MODE_TREE || nn == 0) return RT_OK;   // a rebuild brings its own scratch
     void* p = nullptr;
     CU(cudaMalloc(&p, ((size_t)nn + nl) * 6 * sizeof(double) + (size_t)nn * 4));
     h->refit = p;
@@ -829,7 +832,7 @@ static int update_finish(rtb200_scene_handle h, cudaStream_t st) {
     if (h->mode == MODE_BRUTE) {
         p.filt = (float*)h->tp.filt;
         CU(launch_refit_spheres(p, st));
-    } else if (h->mode == MODE_TREE && h->refit) {
+    } else if (h->mode == MODE_TREE && h->node_box) {
         p.leaf_id = h->tp.leaf_id; p.leaf_rec = (float*)h->tp.leaf_rec; p.leaf_box = h->leaf_box; p.n_leaves = h->tp.n_leaves;
         p.nodes = (float*)h->tp.nodes; p.node_box = h->node_box;
         CU(launch_refit_spheres(p, st));
@@ -931,6 +934,101 @@ int rtb200_scene_debug_records(rtb200_scene_handle h, uint32_t info[8], float* n
     if (rc == RT_OK) rc = get(flat, tp.filt, cap_flat, (uint64_t)info[6] * 8, 4);
     if (rc == RT_OK) rc = get(geo, tp.geo, cap_geo, (uint64_t)tp.n * 4, 8);
     if (rc != RT_OK) return rc;
+    CU(cudaStreamSynchronize(st));
+    return RT_OK;
+  });
+}
+
+// ---- rebuilding the hierarchy of a resident scene on the GPU (DESIGN.md §4.8) ----
+// The topology comes from rtb200_rebuild.cu, its values from the refit's kernels; the host reads back one header (counts,
+// depth, level sizes, recentring offset) between the two. The new arrays live in the handle's rebuild block, which frames
+// enqueued before the call may still read (after an earlier rebuild): the build waits for them.
+int rtb200_scene_rebuild(rtb200_scene_handle h, void* stream_in) {
+  return guarded([&]() -> int {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    if (h->mode != MODE_TREE || h->tp.n == 0) return RT_OK;   // no hierarchy to rebuild
+    if (h->tp.scene_in_smem & 1u)
+        return fail(RT_ERR_UNSUPPORTED, "the handle stages its hierarchy in shared memory (RTB200_WF_SMEM bit 0), whose launch layout is fixed at upload");
+    DeviceRestore restore;
+    DeviceCtx* ctx = h->ctx;
+    std::lock_guard<std::recursive_mutex> lk(ctx->mu);
+    CU(cudaSetDevice(h->device));
+    const uint32_t n = h->tp.n;
+    if (!h->rebuild) {
+        void* p = nullptr;
+        const size_t bytes = rebuild_carve(nullptr, n, nullptr);
+        const cudaError_t e = cudaMalloc(&p, bytes);
+        if (e != cudaSuccess) {
+            cudaGetLastError();
+            return fail(RT_ERR_OOM, "rebuild: cannot allocate " + std::to_string(bytes) + " bytes of device memory for " + std::to_string(n) + " spheres");
+        }
+        h->rebuild = p;
+    }
+    RebuildBufs b;
+    rebuild_carve(h->rebuild, n, &b);
+    cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
+    int rc = update_begin(h, st);
+    if (rc == RT_OK) rc = update_after_frames(h, st);
+    if (rc != RT_OK) return rc;
+    const char* ov = getenv("RTB200_REBUILD_OVERSIZE");   // benchmark hook: 0 keeps oversized spheres in the Morton order
+    CU(launch_rebuild_topology(b, h->tp.geo, n, ov ? atof(ov) : kRebuildOversize, st));
+    RebuildHeader H;
+    CU(cudaMemcpyAsync(&H, b.header, sizeof H, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (H.overflow || H.depth > (uint32_t)rtbvh::kMaxDepth)   // unreachable by the depth bound (DESIGN.md §4.8)
+        return fail(RT_ERR_CUDA, "internal error: the rebuilt hierarchy is deeper than the traversal stack reserve");
+    // the level order, deepest level first (Records::level_off)
+    std::vector<uint32_t> level_off(1, 0u);
+    for (uint32_t k = H.depth; k-- > 0;) level_off.push_back(level_off.back() + H.level_count[k]);
+    RefitParams p{};
+    p.geo = h->tp.geo; p.n = n; p.g[0] = H.g[0]; p.g[1] = H.g[1]; p.g[2] = H.g[2];
+    p.leaf_id = b.leaf_id; p.leaf_rec = b.leaf_rec; p.leaf_box = b.leaf_box; p.n_leaves = H.n_leaves;
+    p.nodes = b.nodes; p.node_box = b.node_box;
+    CU(launch_refit_spheres(p, st));
+    for (size_t k = 0; k + 1 < level_off.size(); ++k) CU(launch_refit_nodes(p, b.level_nodes + level_off[k], level_off[k + 1] - level_off[k], st));
+    CU(cudaEventRecord(h->updated, st));
+    // every frame enqueued from here on traces the new tree, and every update refits it
+    if (h->refit) { CU(cudaFree(h->refit)); h->refit = nullptr; }   // the stream synchronisation above covers the updates that used it
+    TraceParams& tp = h->tp;
+    tp.nodes = (const float4*)b.nodes; tp.leaf_rec = (const float4*)b.leaf_rec; tp.leaf_id = b.leaf_id;
+    tp.skip_pos = b.skip_pos; tp.always = b.always;
+    tp.n_nodes = H.n_nodes; tp.n_leaves = H.n_leaves; tp.n_always = H.n_always; tp.depth = H.depth;
+    tp.gx = H.g[0]; tp.gy = H.g[1]; tp.gz = H.g[2];
+    h->level_off = level_off;
+    h->level_nodes.clear();
+    h->node_box = b.node_box; h->leaf_box = b.leaf_box; h->level_nodes_dev = b.level_nodes;
+    return RT_OK;
+  });
+}
+
+// Diagnostic: the handle's current topology (the upload's, or the last rebuild's)
+int rtb200_scene_debug_topology(rtb200_scene_handle h, double recentre[3], uint32_t info[8], uint32_t* leaf_id, uint64_t cap_leaf_id,
+                                uint32_t* always, uint64_t cap_always, uint32_t* skip_pos, uint64_t cap_skip_pos,
+                                uint32_t* level_nodes, uint64_t cap_level_nodes, uint32_t* level_off, uint64_t cap_level_off) {
+  return guarded([&]() -> int {
+    if (!h || !info) return fail(RT_ERR_INVALID, "null argument");
+    const TraceParams& tp = h->tp;
+    bvh_info(info, tp.n_nodes, tp.n_leaves, tp.depth, tp.n_always, tp.filt ? tp.n_pairs : 0u);
+    if (recentre) { recentre[0] = tp.gx; recentre[1] = tp.gy; recentre[2] = tp.gz; }
+    if (level_off && cap_level_off) memcpy(level_off, h->level_off.data(), std::min<uint64_t>(cap_level_off, h->level_off.size()) * 4);
+    DeviceRestore restore;
+    std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
+    CU(cudaSetDevice(h->device));
+    cudaStream_t st = h->ctx->stream;   // after the upload; after the last update or rebuild:
+    if (h->updated) CU(cudaStreamWaitEvent(st, h->updated, 0));
+    auto get = [&](void* dst, const void* src, uint64_t cap, uint64_t count) -> int {
+        if (dst && src && cap && count) CU(cudaMemcpyAsync(dst, src, std::min(cap, count) * 4, cudaMemcpyDeviceToHost, st));
+        return RT_OK;
+    };
+    const bool tree = h->mode == MODE_TREE;
+    int rc = RT_OK;
+    if (rc == RT_OK) rc = get(leaf_id, tp.leaf_id, cap_leaf_id, (uint64_t)tp.n_leaves * rtbvh::kLeafK);
+    if (rc == RT_OK) rc = get(always, tp.always, cap_always, tp.n_always);
+    if (rc == RT_OK) rc = get(skip_pos, tp.skip_pos, cap_skip_pos, tree ? std::max<uint64_t>(tp.n, 1) : 0);
+    if (rc == RT_OK && h->rebuild) rc = get(level_nodes, h->level_nodes_dev, cap_level_nodes, tp.n_nodes);
+    if (rc != RT_OK) return rc;
+    if (level_nodes && cap_level_nodes && !h->rebuild)
+        memcpy(level_nodes, h->level_nodes.data(), std::min<uint64_t>(cap_level_nodes, h->level_nodes.size()) * 4);
     CU(cudaStreamSynchronize(st));
     return RT_OK;
   });

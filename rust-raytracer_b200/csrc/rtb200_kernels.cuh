@@ -127,6 +127,30 @@ struct RefitParams {
     double* node_box;            // n_nodes exact boxes (the union of the node's children)
 };
 
+// Rebuild of a resident scene's hierarchy on the GPU (rtb200_rebuild.cu, DESIGN.md §4.8). The header is what the host reads
+// back: the counts, the recentring offset and the level sizes it needs for TraceParams and for later refits.
+constexpr uint32_t kRebuildIdBits = 26;   // sphere index bits of a sort key (n < 2^26, validate_scene)
+struct RebuildHeader {
+    double g[3];                                     // recentring offset
+    double r_big;                                    // |radius| above which a sphere is oversized
+    unsigned long long box_lo[3], box_hi[3];         // Morton box of the centres (order-preserving integer form)
+    uint32_t n_in, n_always, n_nodes, n_leaves, depth, overflow;
+    uint32_t level_count[rtbvh::kMaxDepth + 1];      // nodes per wide level, root level first
+    uint32_t level_base[rtbvh::kMaxDepth + 2];       // the first node of each level: nodes are numbered level by level
+};
+struct RebuildBufs {
+    RebuildHeader* header;
+    // the new hierarchy (TraceParams) and the refit's scratch of its topology
+    float* nodes; float* leaf_rec; uint32_t* leaf_id; uint32_t* skip_pos; uint32_t* always;
+    double* node_box; double* leaf_box; uint32_t* level_nodes;
+    // scratch of the build
+    double* col; double* sorted; unsigned long long* keys; unsigned long long* keys_sorted;
+    uint32_t *out_flag, *always_pos, *leaf_start, *leaf_scan, *leaf_cnt;
+    uint2* tasks[2]; uint2* kids; uint32_t *n_inner, *off;
+    uint32_t cap;                                    // nodes per level at most
+    void* temp; size_t temp_bytes;                   // cub's temporary storage
+};
+
 struct KernelInfo { int registers, max_threads, const_bytes, local_bytes; char name[96]; };
 
 // `frames`: the multi-frame kernel (work ids span p.ftab's frames) instead of the single-frame one
@@ -142,6 +166,13 @@ cudaError_t launch_update_scatter(const uint32_t* idx, const double4* geo_in, co
 cudaError_t launch_refit_spheres(const RefitParams& p, cudaStream_t st);
 // the `count` nodes level_nodes[0, count) of one tree level; their children's exact boxes are final
 cudaError_t launch_refit_nodes(const RefitParams& p, const uint32_t* level_nodes, uint32_t count, cudaStream_t st);
+// the rebuild's arrays for n spheres carved out of `base` (null: only the size); returns the bytes they take
+size_t rebuild_carve(void* base, uint32_t n, RebuildBufs* b);
+// the topology of a new hierarchy over geo[0, n): header, child words, leaf members and padding, always-list, skip_pos and the
+// level order; the position-dependent values are then the refit's (launch_refit_spheres / launch_refit_nodes). A sphere whose
+// |radius| exceeds `oversize` times the median |radius| gets its own subtree near the root (oversize <= 0: none does).
+constexpr double kRebuildOversize = 16.0;
+cudaError_t launch_rebuild_topology(const RebuildBufs& b, const double4* geo, uint32_t n, double oversize, cudaStream_t st);
 
 // single-thread probes of the device routines (known-answer tests)
 cudaError_t probe_sphere_hit(const double* in /*12*/, double* out /*9*/, cudaStream_t st);

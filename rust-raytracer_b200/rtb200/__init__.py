@@ -114,6 +114,7 @@ ABI_SYMBOLS = [
     "rtb200_debug_bvh", "rtb200_probe_sphere_uv", "rtb200_device_count", "rtb200_render_rgb8_multi", "rtb200_scene_kernel_info",
     "rtb200_render_frames", "rtb200_render_frames_device",
     "rtb200_scene_update_spheres", "rtb200_scene_update_geometry_device", "rtb200_scene_debug_records",
+    "rtb200_scene_rebuild", "rtb200_scene_debug_topology",
 ]
 
 _lib = None
@@ -165,6 +166,8 @@ def lib() -> C.CDLL:
     L.rtb200_scene_update_geometry_device.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
     L.rtb200_scene_debug_records.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64,
                                              C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
+    L.rtb200_scene_rebuild.argtypes = [C.c_void_p, C.c_void_p]
+    L.rtb200_scene_debug_topology.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_uint32)] + [C.c_void_p, C.c_uint64] * 5
     _lib = L
     return L
 
@@ -494,9 +497,6 @@ class ResidentScene:
         self.rows = scene.c.height if (opts is None or opts.world <= 1) else shard_rows(scene.c.height, opts.rank, opts.world, opts.band_rows)
         self.n = scene.n_spheres
         self.device = opts.device if opts is not None and opts.device >= 0 else _current_device()   # None: unknown without torch
-        # the uploaded spheres: bvh_records() restates the upload's topology from them
-        self._uploaded = (rt_sphere * max(self.n, 1))()
-        C.memmove(self._uploaded, scene._spheres, self.n * C.sizeof(rt_sphere))
 
     def render(self, dev_rgb8_ptr: int = 0, dev_linear_ptr: int = 0, stream: int = 0) -> dict:
         st = rt_stats()
@@ -543,18 +543,39 @@ class ResidentScene:
             raise ValueError(f"update_geometry takes a contiguous float64 tensor of shape [{self.n}, 4], got {t.dtype} {tuple(t.shape)}")
         if self.device is not None and t.device.index != self.device:
             raise ValueError(f"the tensor is on cuda:{t.device.index}, the scene on cuda:{self.device}")
+        _check(lib().rtb200_scene_update_geometry_device(self.h, C.c_void_p(t.data_ptr()), C.c_void_p(self._stream(stream, t.device) or None)))
+
+    def _stream(self, stream, device):
+        """The cudaStream_t handle of `stream` (see :meth:`update_geometry`); None: torch's current stream on `device`."""
         if stream is None:
-            stream = torch.cuda.current_stream(t.device)
-        s = (stream.cuda_stream or CUDA_STREAM_LEGACY) if isinstance(stream, torch.cuda.Stream) else int(stream)
-        _check(lib().rtb200_scene_update_geometry_device(self.h, C.c_void_p(t.data_ptr()), C.c_void_p(s or None)))
+            import torch
+            stream = torch.cuda.current_stream(device)
+        return (stream.cuda_stream or CUDA_STREAM_LEGACY) if hasattr(stream, "cuda_stream") else int(stream)
+
+    def rebuild(self, stream=None):
+        """Rebuild the hierarchy from the current spheres on the GPU (rtb200_scene_rebuild): a new topology for spheres that
+        moved, ordered like an update on `stream` (as in :meth:`update_geometry`, by default torch's current stream). Returns
+        when the new tree exists; later frames trace it and later updates refit it. A no-op without a hierarchy."""
+        _check(lib().rtb200_scene_rebuild(self.h, C.c_void_p(self._stream(stream, self.device) or None)))
+
+    def topology(self) -> dict:
+        """The handle's current topology (rtb200_scene_debug_topology): recentre, leaf_id [n_leaves, k], always, skip_pos,
+        level_nodes (deepest level first) and level_off, the upload's or the last rebuild's."""
+        g = (C.c_double * 3)(); info = (C.c_uint32 * 8)()
+        _check(lib().rtb200_scene_debug_topology(self.h, g, info, None, 0, None, 0, None, 0, None, 0, None, 0))
+        n_nodes, n_leaves, depth, k, n_always = (int(x) for x in info[:5])
+        ids = np.zeros(max(n_leaves * k, 1), np.uint32); always = np.zeros(max(n_always, 1), np.uint32)
+        skip = np.zeros(max(self.n, 1), np.uint32); ln = np.zeros(max(n_nodes, 1), np.uint32); lo = np.zeros(depth + 1, np.uint32)
+        _check(lib().rtb200_scene_debug_topology(self.h, g, info, ids.ctypes.data, ids.size, always.ctypes.data, always.size,
+                                                 skip.ctypes.data, skip.size, ln.ctypes.data, ln.size, lo.ctypes.data, lo.size))
+        return {"n": self.n, "leaf_size": k, "n_nodes": n_nodes, "n_leaves": n_leaves, "depth": depth, "recentre": np.array(g[:]),
+                "leaf_id": ids[: n_leaves * k].reshape(n_leaves, k), "always": always[:n_always], "skip_pos": skip,
+                "level_nodes": ln[:n_nodes], "level_off": lo}
 
     def bvh_records(self) -> dict:
         """The handle's current arrays (rtb200_scene_debug_records) in the layout of :func:`bvh_records`, plus "geo"
-        (float64 [n, 4]). leaf_id, always and recentre are the upload's: an update never changes them."""
-        up = Scene()
-        up.c = rt_scene.from_buffer_copy(self.scene.c)
-        up.c.spheres = C.cast(self._uploaded, C.POINTER(rt_sphere)); up.c.n_spheres = self.n
-        b = bvh_records(up)
+        (float64 [n, 4]) and the topology of :meth:`topology` (leaf_id, always, recentre, skip_pos, level order)."""
+        b = self.topology()
         info = (C.c_uint32 * 8)()
         _check(lib().rtb200_scene_debug_records(self.h, info, None, 0, None, 0, None, 0, None, 0))
         n_nodes, n_leaves, depth, k, n_always, fpn, n_pairs, _ = (int(x) for x in info)
@@ -563,7 +584,7 @@ class ResidentScene:
         _check(lib().rtb200_scene_debug_records(self.h, info, nodes.ctypes.data, nodes.size, rec.ctypes.data, rec.size,
                                                 flat.ctypes.data, flat.size, geo.ctypes.data, geo.size))
         b.update(_record_views(info, nodes, rec, flat))
-        b.update({"leaf_id": b["leaf_id"][:n_leaves], "always": b["always"][:n_always], "geo": geo[: self.n * 4].reshape(self.n, 4)})
+        b["geo"] = geo[: self.n * 4].reshape(self.n, 4)
         return b
 
     def kernel_info(self) -> dict:

@@ -215,14 +215,28 @@ private:
     int sah_limit_ = 24;
     int area_levels_ = kAreaFirstLevels;
 
+    // g = element n/2 of each centre coordinate, 0 when that is not finite. The order is that of the GPU rebuild's stable
+    // radix sort (cub::DeviceRadixSort, rtb200_rebuild.cu): the sign-flipped IEEE bits with -0.0 ranked as +0.0, equal keys
+    // in index order. So a rebuild of unchanged spheres keeps g bit for bit, also when the median is a zero of mixed sign.
     void recentre() {
         const uint32_t n = R_.n;
         if (!n) return;
-        std::vector<double> tmp(n);
+        std::vector<uint64_t> key(n);
+        std::vector<uint32_t> idx(n);
         for (int c = 0; c < 3; ++c) {
-            for (uint32_t i = 0; i < n; ++i) tmp[i] = c == 0 ? s_->spheres[i].center.x : (c == 1 ? s_->spheres[i].center.y : s_->spheres[i].center.z);
-            std::nth_element(tmp.begin(), tmp.begin() + n / 2, tmp.end());
-            R_.g[c] = std::isfinite(tmp[n / 2]) ? tmp[n / 2] : 0.0;
+            auto coord = [&](uint32_t i) { return c == 0 ? s_->spheres[i].center.x : (c == 1 ? s_->spheres[i].center.y : s_->spheres[i].center.z); };
+            for (uint32_t i = 0; i < n; ++i) {
+                uint64_t u;
+                const double v = coord(i);
+                std::memcpy(&u, &v, 8);
+                if (u == 0x8000000000000000ull) u = 0;
+                key[i] = (u >> 63) ? ~u : (u | 0x8000000000000000ull);
+                idx[i] = i;
+            }
+            std::nth_element(idx.begin(), idx.begin() + n / 2, idx.end(),
+                             [&](uint32_t a, uint32_t b) { return key[a] != key[b] ? key[a] < key[b] : a < b; });
+            const double m = coord(idx[n / 2]);
+            R_.g[c] = std::isfinite(m) ? m : 0.0;
         }
     }
 

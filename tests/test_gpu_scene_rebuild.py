@@ -11,78 +11,24 @@ import oracle_py as O
 import rtb200 as R
 from rtb200 import scenes
 from synth import base_config, mixed_config, _v
-from test_bvh_cpu import _exact_hits, _traverse
+from rebuild_restatement import MAX_DEPTH, check_tree, skip_rule
 from test_gpu_scene_update import HOLD, _assert_same, _check, _fresh, _jitter, _light_scene, _positions, _render
-from test_scene_update_cpu import _rays, refit, same_bits
+from test_scene_update_cpu import refit, same_bits
 
 pytestmark = pytest.mark.gpu
-EMPTY, LEAF, SKIP_NODE, NO_SKIP = 0xFFFFFFFF, 0x80000000, 0x80000000, 0xFFFFFFFF
-MAX_DEPTH, K = 21, 8
-
-
-def _skip_rule(t, n):
-    """build_records' skip_pos rule on topology t: a member's leaf slot, or its parent slot when it is alone in its leaf."""
-    skip = np.full(max(n, 1), NO_SKIP, np.uint32)
-    ids = t["leaf_id"].ravel()
-    k = np.nonzero(ids != EMPTY)[0]
-    skip[ids[k]] = k
-    for node in range(t["n_nodes"]):
-        for c, ref in enumerate(t["child"][node]):
-            if ref != EMPTY and ref & LEAF:
-                m = t["leaf_id"][ref & 0x7FFFFFFF]
-                if (m != EMPTY).sum() == 1:
-                    skip[m[0]] = SKIP_NODE | (node * 8 + c)
-    return skip
+EXACT = R.make_options(variant=R.RT_VARIANT_EXACT_F64)
 
 
 def check_topology(rs, sc, rays=0):
-    """Every invariant of a rebuilt hierarchy, against the host scene sc (the handle's current spheres). Returns the records."""
+    """Every invariant of a rebuilt hierarchy (rebuild_restatement.check_tree) for the host scene sc (the handle's current
+    spheres), and the recentring offset (bit for bit) and always-list of a fresh upload of sc. Returns the records."""
     t = rs.bvh_records()
     c, r = _positions(sc)
-    n = sc.n_spheres
     host = R.bvh_records(sc)
     assert np.array_equal(t["always"], host["always"]), "always-list differs from a fresh upload's"
-    assert np.array_equal(t["recentre"], host["recentre"]), (t["recentre"], host["recentre"])
-    ids = t["leaf_id"].ravel()
-    assert sorted(np.concatenate([ids[ids != EMPTY], t["always"]]).tolist()) == list(range(n))   # in exactly one leaf or always
-    for leaf in range(t["n_leaves"]):
-        m = t["leaf_id"][leaf]
-        cnt = int((m != EMPTY).sum())
-        assert cnt >= 1 and np.all(m[cnt:] == EMPTY) and np.all(np.diff(m[:cnt].astype(np.int64)) > 0), (leaf, m)
-        nk = np.concatenate([t["leaf_rec"][leaf][:, 1, 2], t["leaf_rec"][leaf][:, 1, 3]]).reshape(2, -1).T.ravel()
-        assert np.all(nk[cnt:] == -np.inf), "padding records must never hit"
-    depth, nn = t["depth"], t["n_nodes"]
-    assert depth <= MAX_DEPTH and len(t["level_off"]) == depth + 1 and t["level_off"][-1] == nn
-    assert sorted(t["level_nodes"].tolist()) == list(range(nn))
-    level = np.empty(nn, np.int64)
-    for k in range(depth):                                     # deepest first
-        level[t["level_nodes"][t["level_off"][k]:t["level_off"][k + 1]]] = depth - 1 - k
-    seen_nodes, seen_leaves = np.zeros(nn, int), np.zeros(t["n_leaves"], int)
-    for node in range(nn):
-        for s, ref in enumerate(t["child"][node]):
-            if ref == EMPTY:
-                assert np.all(t["lo"][node][:, s] == np.inf) and np.all(t["hi"][node][:, s] == -np.inf)
-            elif ref & LEAF:
-                seen_leaves[ref & 0x7FFFFFFF] += 1
-            else:
-                assert ref > node and level[ref] == level[node] + 1
-                seen_nodes[ref] += 1
-    if nn:
-        assert level[0] == 0 and seen_nodes[0] == 0 and np.all(seen_nodes[1:] == 1) and np.all(seen_leaves == 1)
-    assert np.array_equal(t["skip_pos"], _skip_rule(t, n))
-    b = dict(t)
-    b["flat"] = np.zeros((max((n + 1) // 2, 1), 2, 4), np.float32)   # a hierarchy handle has no flat records
-    want = refit(b, c, r)
-    for key in ("lo", "hi", "leaf_rec"):
-        assert same_bits(t[key], want[key]), key
-    if rays and nn:
-        rng = np.random.default_rng(11)
-        cam = np.array([sc.c.camera.origin.x, sc.c.camera.origin.y, sc.c.camera.origin.z])
-        for i, (o, d) in enumerate(_rays(c, r, cam, rng, rays)):
-            with np.errstate(all="ignore"):
-                exact = _exact_hits(c, r, o, d)
-            cand, _ = _traverse(t, o, d)
-            assert not set(exact.tolist()) - cand, i
+    assert t["recentre"].view(np.uint64).tolist() == host["recentre"].view(np.uint64).tolist(), (t["recentre"], host["recentre"])
+    cam = [sc.c.camera.origin.x, sc.c.camera.origin.y, sc.c.camera.origin.z]
+    check_tree(t, c, r, rays=rays, cam=cam)
     return t
 
 
@@ -303,7 +249,9 @@ def test_adversarial_inputs(kind):
     rs.rebuild()
     t = check_topology(rs, sc, rays=40 if kind not in ("coincident",) else 0)
     assert t["depth"] <= MAX_DEPTH
-    _check(rs, sc, oracle=kind != "coincident", what=kind)      # a render that succeeds: the traversal guard never tripped
+    got = _check(rs, sc, oracle=kind != "coincident", what=kind)   # a render that succeeds: the traversal guard never tripped
+    if kind == "coincident":                                      # too many spheres per ray for the oracle: the exact variant
+        _assert_same(got, _fresh(sc, EXACT), "coincident vs EXACT_F64")
     rs.release()
 
 
@@ -338,7 +286,8 @@ def test_the_100k_sphere_scene():
     rs.rebuild()
     t = check_topology(rs, sc)
     assert t["depth"] <= MAX_DEPTH and sc.n_spheres > 90_000
-    _check(rs, sc, oracle=False, what="100k")
+    got = _check(rs, sc, oracle=False, what="100k")
+    _assert_same(got, _fresh(sc, EXACT), "100k vs EXACT_F64")
     rs.release()
 
 
@@ -370,7 +319,7 @@ def test_topology_of_a_handle_never_rebuilt_is_the_uploads():
     t, host = rs.bvh_records(), R.bvh_records(sc)
     for key in ("leaf_id", "always", "recentre", "child", "lo", "hi", "leaf_rec"):
         assert np.array_equal(t[key], host[key]), key
-    assert np.array_equal(t["skip_pos"], _skip_rule(host, sc.n_spheres))
+    assert np.array_equal(t["skip_pos"], skip_rule(host, sc.n_spheres))
     assert t["depth"] == host["depth"] and len(t["level_off"]) == host["depth"] + 1
     rs.release()
     info = (C.c_uint32 * 8)()

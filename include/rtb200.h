@@ -183,9 +183,12 @@ int rtb200_scene_upload(const rt_scene* scene, const rt_options* opts, rtb200_sc
  * own non-blocking stream (pass cudaStreamLegacy / cudaStreamPerThread explicitly to order against the default stream). */
 int rtb200_render_device(rtb200_scene_handle h, void* dev_rgb8, void* dev_linear_f32, void* stream, rt_stats* stats);
 /* Non-blocking form for frame loops: enqueue a frame on `stream` and return; rtb200_render_device_wait() blocks until the
- * frames enqueued so far are done and returns statistics. Successive frames alternate between two sets of work buffers, so a caller
- * that alternates two streams (and two output buffers) lets frame k+1 start while frame k drains its last paths; frames on the
- * same stream are ordered by it. One scene at a time may have asynchronous frames in flight on a device. */
+ * frames enqueued so far are done and returns statistics: rays, samples and the other counters are those of the last frame
+ * enqueued, times and frames are summed. A device has two sets of work buffers, shared by all its scenes: successive
+ * asynchronous frames of a scene alternate between them and every blocking render uses the first. A frame starts only after
+ * the previous frame that used the same set has finished with it, whatever its stream and scene, so any number of scenes may
+ * have frames in flight on any streams; a caller that alternates two streams (and two output buffers) lets frame k+1 start
+ * while frame k drains its last paths. */
 int rtb200_render_device_async(rtb200_scene_handle h, void* dev_rgb8, void* dev_linear_f32, void* stream);
 int rtb200_render_device_wait(rtb200_scene_handle h, rt_stats* stats);
 int rtb200_scene_release(rtb200_scene_handle h);

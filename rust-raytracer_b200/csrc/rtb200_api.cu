@@ -38,8 +38,11 @@ int fail_cuda(cudaError_t e, const char* what) {
 struct GrowBuf {
     void* p = nullptr;
     size_t cap = 0;
-    cudaError_t ensure(size_t bytes) {
+    // `busy`: recorded after the last use of the buffer on the device; a growth waits for it on the host before the old
+    // buffer is freed (cudaFree's own synchronisation is not relied on).
+    cudaError_t ensure(size_t bytes, cudaEvent_t busy = nullptr) {
         if (bytes <= cap) return cudaSuccess;
+        if (p && busy) { cudaError_t e = cudaEventSynchronize(busy); if (e != cudaSuccess) return e; }
         if (p) { cudaError_t e = cudaFree(p); if (e != cudaSuccess) return e; p = nullptr; cap = 0; }
         size_t want = bytes + bytes / 8;
         cudaError_t e = cudaMalloc(&p, want);
@@ -49,6 +52,9 @@ struct GrowBuf {
         return cudaSuccess;
     }
 };
+constexpr size_t kStatBytes = 256;      // a work set's stat block (32 counters), followed by its queue counters
+constexpr uint32_t kMaxPending = 64;    // submissions of one handle enqueued without a collect
+
 struct PinnedBuf {
     void* p = nullptr;
     size_t cap = 0;
@@ -70,9 +76,15 @@ struct DeviceCtx {
     int device = -1;
     int sm_count = 0;
     cudaStream_t stream = nullptr;
-    // Two sets of per-frame work buffers: a frame loop that alternates two streams lets frame k+1 start tracing while frame k
-    // drains its last paths and resolves (rtb200_render_device_async); blocking calls use set 0 only.
-    struct WorkSet { GrowBuf samplebuf, accum, stack, small, frames, lterm, ftab; } ws[2];   // ftab: the multi-frame kernel's frame table
+    // Two sets of per-frame work buffers, shared by every handle of the device: a frame loop that alternates two streams lets
+    // frame k+1 start tracing while frame k drains its last paths and resolves (rtb200_render_device_async); blocking calls
+    // use set 0 only. `done` is recorded after the last use of the set by the latest submission that took it, on that
+    // submission's stream; the next submission's stream waits for it, so submissions that share a set run one after the other
+    // whatever their streams and handles.
+    struct WorkSet {
+        GrowBuf samplebuf, accum, stack, small, frames, lterm, ftab;   // ftab: the multi-frame kernel's frame table
+        cudaEvent_t done = nullptr;
+    } ws[2];
     GrowBuf out_rgb8, out_lin, probe, frame;
     // scene arenas of released handles, kept for the next upload (a per-frame upload costs no cudaMalloc / cudaFree)
     struct Arena { void* p; size_t cap; };
@@ -111,6 +123,7 @@ int get_ctx(int device, DeviceCtx** out) {
         c.sm_count = prop.multiProcessorCount;
         CU(cudaStreamCreateWithFlags(&c.stream, cudaStreamNonBlocking));
         CU(cudaEventCreateWithFlags(&c.staging_free, cudaEventDisableTiming));
+        for (auto& W : c.ws) CU(cudaEventCreateWithFlags(&W.done, cudaEventDisableTiming));
         c.init = true;
     }
     *out = &c;
@@ -176,7 +189,6 @@ struct rtb200_scene_t {
     // What one render_enqueue put on a stream. Events: begin, end, and a pair around each trace launch (or black memset).
     struct Submission {
         cudaStream_t stream;
-        int set;                         // work set: its stat block holds the submission's counters
         uint32_t ev0, n_ev;              // n_ev = 0: a shard with no rows, nothing was enqueued
         uint32_t frames, batches, launches;
         int grid;                        // of the widest launch (print_diagnostics)
@@ -184,6 +196,9 @@ struct rtb200_scene_t {
         uint64_t ftab_bytes;             // frame table uploaded
     };
     std::vector<Submission> pending;     // enqueued since the last render_collect, oldest first
+    // device: the stat block of pending[i], copied out of its work set at the end of the submission (the set may be taken by
+    // another submission before the collect reads it)
+    unsigned long long* stat_snap = nullptr;
     uint32_t frame_counter = 0;
     uint64_t h2d_bytes = 0;
     // ---- moving spheres (rtb200_scene_update_*): what the upload fixed, and the refit's scratch built at the first update ----
@@ -437,6 +452,7 @@ static int scene_upload_records(const rt_scene* s, const rt_options& opts, uint3
     lights.push_back(0);
     upload_array(h, lights.data(), lights.size() * 4, (void**)&tp.lights);
     upload_array(h, nullptr, 16, (void**)&h->err);   // zero-filled error counters
+    upload_array(h, nullptr, kMaxPending * kStatBytes, (void**)&h->stat_snap);
     tp.err = nullptr;                                // patched after commit
     tp.gx = R.g[0]; tp.gy = R.g[1]; tp.gz = R.g[2];
     tp.er_coef = 1.0f - (float)(96.0 * rtbvh::kU);
@@ -506,20 +522,21 @@ int rtb200_scene_kernel_info(rtb200_scene_handle h, rt_kernel_info* out) {
 
 // Work buffers of W for launches of up to `threads_total` threads that trace paths up to `max_depth` deep, stage up to
 // `samplebuf_bytes` of per-sample radiance and take `n_counters` queue counters; points tp at them (stack_stride excepted).
+// A buffer that has to grow is freed only after the set's last submission has finished with it.
 static int prepare_work(DeviceCtx::WorkSet& W, TraceParams& tp, uint32_t threads_total, uint32_t max_depth,
                         size_t samplebuf_bytes, uint32_t n_counters) {
-    CU(W.samplebuf.ensure(samplebuf_bytes));
-    CU(W.accum.ensure((size_t)tp.npix_local * 12));
-    CU(W.stack.ensure((size_t)std::max<uint32_t>(max_depth, 1) * threads_total * 4));
-    CU(W.small.ensure(256 + (size_t)n_counters * 4));
+    CU(W.samplebuf.ensure(samplebuf_bytes, W.done));
+    CU(W.accum.ensure((size_t)tp.npix_local * 12, W.done));
+    CU(W.stack.ensure((size_t)std::max<uint32_t>(max_depth, 1) * threads_total * 4, W.done));
+    CU(W.small.ensure(kStatBytes + (size_t)n_counters * 4, W.done));
     if (tp.n_lights > 0) {
         // Nested light tests form a branching process: a vertex nests with probability 0.1 n and then spawns n shadow rays, so
         // depth d is reached with probability ~(0.1 n^2 P_hit)^d: harmless for 1-2 lights, near-critical for 3 (the reference
         // itself recurses hundreds of frames deep there) and super-critical beyond. Size the per-path frame stack accordingly;
         // an overflow is reported as an error, never rendered wrongly.
         tp.max_shadow = tp.n_lights == 1 ? 32u : tp.n_lights == 2 ? 96u : 384u;
-        CU(W.frames.ensure((size_t)tp.max_shadow * threads_total * sizeof(ShadowFrame)));
-        CU(W.lterm.ensure((size_t)6 * threads_total * 4));
+        CU(W.frames.ensure((size_t)tp.max_shadow * threads_total * sizeof(ShadowFrame), W.done));
+        CU(W.lterm.ensure((size_t)6 * threads_total * 4, W.done));
     }
     tp.frames = (ShadowFrame*)W.frames.p;
     tp.lterm = (float*)W.lterm.p;
@@ -531,7 +548,7 @@ static int prepare_work(DeviceCtx::WorkSet& W, TraceParams& tp, uint32_t threads
 
 // Zero the stat block and the first n_counters queue counters of W.
 static int clear_stats(DeviceCtx::WorkSet& W, uint32_t n_counters, cudaStream_t st) {
-    CU(cudaMemsetAsync(W.small.p, 0, 256 + (size_t)n_counters * 4, st));
+    CU(cudaMemsetAsync(W.small.p, 0, kStatBytes + (size_t)n_counters * 4, st));
     CU(cudaMemsetAsync((char*)W.small.p + 64, 0xff, 16, st));   // stat[8], stat[9]: minima (kernel start / first dry-queue time, ns)
     return RT_OK;
 }
@@ -576,10 +593,11 @@ static rt_frame own_frame(rtb200_scene_handle h) { return rt_frame{h->tp.cam, h-
 
 // Enqueue frames[0, n) of h on `stream_in` (NULL: the context's stream) with work set `set`, without waiting, and append the
 // submission to h->pending; the caller holds the context's lock. Frame i goes to output slice i (rows * width * 3 elements).
+// The submission starts after the previous one that took the same set, on any stream and of any handle, has finished with it.
 // A submission that fails part-way is not recorded.
 static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_t n, void* dev_rgb8, void* dev_linear_f32,
                           void* stream_in, int set) {
-    if (h->pending.size() >= 64) return fail(RT_ERR_INVALID, "more than 64 frames enqueued without rtb200_render_device_wait");
+    if (h->pending.size() >= kMaxPending) return fail(RT_ERR_INVALID, "more than 64 frames enqueued without rtb200_render_device_wait");
     DeviceCtx* ctx = h->ctx;
     DeviceCtx::WorkSet& W = ctx->ws[set];
     CU(cudaSetDevice(h->device));
@@ -587,7 +605,7 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
     if (st != ctx->stream) CU(cudaStreamWaitEvent(st, ctx->staging_free, 0));   // the scene upload ran on the context's stream
     if (h->updated) CU(cudaStreamWaitEvent(st, h->updated, 0));                 // and its last update on the update's stream
     const rtb200_scene_t::Submission* prev = h->pending.empty() ? nullptr : &h->pending.back();
-    rtb200_scene_t::Submission sub{st, set, prev ? prev->ev0 + prev->n_ev : 0u, 0, n, 0, 0, h->grid, 0, 0};
+    rtb200_scene_t::Submission sub{st, prev ? prev->ev0 + prev->n_ev : 0u, 0, n, 0, 0, h->grid, 0, 0};
     TraceParams tp = h->tp;   // the handle's own view stays as uploaded
     const uint64_t npl = tp.npix_local;
     if (npl == 0) { h->pending.push_back(sub); return RT_OK; }   // a shard with no rows: nothing to trace
@@ -616,13 +634,14 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
     const uint32_t threads_total = (uint32_t)sub.grid * (uint32_t)kBlock;   // ray slots of the widest grid: columns of the per-slot global arrays
     int rc = prepare_work(W, tp, threads_total, max_depth, sbuf, sub.batches);
     if (rc != RT_OK) return rc;
+    CU(cudaStreamWaitEvent(st, W.done, 0));   // nothing below touches the set before its previous submission is done with it
     if (grid_f) {   // the multi-frame kernel reads each frame's camera and key from this table
         std::vector<FrameRec> tab(n);
         for (uint32_t i = 0; i < n; ++i) {
             tab[i].cam = frames[i].camera; tab[i].key0 = (uint32_t)frames[i].seed; tab[i].key1 = (uint32_t)(frames[i].seed >> 32);
         }
         sub.ftab_bytes = (uint64_t)n * sizeof(FrameRec);
-        CU(W.ftab.ensure(sub.ftab_bytes));
+        CU(W.ftab.ensure(sub.ftab_bytes, W.done));
         CU(cudaMemcpyAsync(W.ftab.p, tab.data(), sub.ftab_bytes, cudaMemcpyHostToDevice, st));
     }
     sub.n_ev = 2 + 2 * sub.batches;
@@ -633,7 +652,7 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
         h->ev.push_back(e);
     }
     cudaEvent_t* ev = h->ev.data() + sub.ev0;
-    unsigned int* counters = (unsigned int*)((char*)W.small.p + 256);
+    unsigned int* counters = (unsigned int*)((char*)W.small.p + kStatBytes);
     if ((rc = clear_stats(W, sub.batches, st)) != RT_OK) return rc;
 
     CU(cudaEventRecord(ev[0], st));
@@ -686,6 +705,8 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
         b += 1; sub.launches += 1 + g.count;
     }
     CU(cudaEventRecord(ev[1], st));
+    CU(cudaMemcpyAsync(h->stat_snap + h->pending.size() * (kStatBytes / 8), W.small.p, kStatBytes, cudaMemcpyDeviceToDevice, st));
+    CU(cudaEventRecord(W.done, st));
     h->pending.push_back(sub);
     return RT_OK;
 }
@@ -713,17 +734,19 @@ static void print_diagnostics(const unsigned long long* hstat, int grid) {
 }
 
 // Wait for the pending submissions of h and report them (stats may be NULL). Counters, batches and the diagnostics are the
-// last submission's; times, frames, kernel launches and frame-table bytes are summed over the submissions.
+// last submission's (from its copy of the stat block); times, frames, kernel launches and frame-table bytes are summed over
+// the submissions.
 static int render_collect(rtb200_scene_handle h, rt_stats* stats) {
     if (stats) memset(stats, 0, sizeof *stats);
     if (h->pending.empty()) return RT_OK;
     CU(cudaSetDevice(h->device));
     const rtb200_scene_t::Submission last = h->pending.back();
     for (const auto& p : h->pending) if (p.stream != last.stream) CU(cudaStreamSynchronize(p.stream));
-    unsigned long long hstat[32] = {0}, herr[2] = {0, 0};   // the whole 256-byte stat block
+    unsigned long long hstat[kStatBytes / 8] = {0}, herr[2] = {0, 0};   // the whole stat block
     if (last.n_ev) {
         // error counters accumulate over every frame since the last collect (each frame adds to them; nothing clears them in between)
-        CU(cudaMemcpyAsync(hstat, h->ctx->ws[last.set].small.p, sizeof hstat, cudaMemcpyDeviceToHost, last.stream));
+        const unsigned long long* snap = h->stat_snap + (h->pending.size() - 1) * (kStatBytes / 8);
+        CU(cudaMemcpyAsync(hstat, snap, sizeof hstat, cudaMemcpyDeviceToHost, last.stream));
         CU(cudaMemcpyAsync(herr, h->err, sizeof herr, cudaMemcpyDeviceToHost, last.stream));
     }
     CU(cudaStreamSynchronize(last.stream));

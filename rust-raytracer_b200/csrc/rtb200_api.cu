@@ -403,6 +403,13 @@ static int normalise_options(const rt_options* opts_in, rt_options* o) {
     return RT_OK;
 }
 
+// TraceParams::albedo_nonfinite for a sphere: only Lambertian and Metal spheres carry their own albedo (Texture, Glass and
+// Light albedos are finite)
+static bool albedo_nonfinite(const rt_sphere& sp) {
+    return (sp.kind == RT_LAMBERTIAN || sp.kind == RT_METAL) &&
+           !(std::isfinite(sp.albedo[0]) && std::isfinite(sp.albedo[1]) && std::isfinite(sp.albedo[2]));
+}
+
 // `R` holds the host-side records (built once; the multi-GPU entry point shares them between its devices).
 static int scene_upload_records(const rt_scene* s, const rt_options& opts, uint32_t n_lights, const rtbvh::Records& R, rtb200_scene_handle* out) {
     *out = nullptr;
@@ -446,7 +453,10 @@ static int scene_upload_records(const rt_scene* s, const rt_options& opts, uint3
     }
     if (h->mode == MODE_TREE) { h->level_nodes = R.level_nodes; h->level_off = R.level_off; }
     std::vector<uint32_t> lights;
-    for (uint32_t i = 0; i < n; ++i) if (s->spheres[i].kind == RT_LIGHT) lights.push_back(i);
+    for (uint32_t i = 0; i < n; ++i) {
+        if (s->spheres[i].kind == RT_LIGHT) lights.push_back(i);
+        if (albedo_nonfinite(s->spheres[i])) tp.albedo_nonfinite = 1u;
+    }
     h->light_idx = lights;
     for (uint64_t t = 0; t < s->n_textures; ++t) h->tex_ok.push_back(image_ok(s->textures[t]));
     lights.push_back(0);
@@ -899,7 +909,11 @@ int rtb200_scene_update_spheres(rtb200_scene_handle h, const uint32_t* index, co
     CU(cudaEventSynchronize(ctx->staging_free));   // the previous copy has left the staging buffer
     CU(ctx->staging.ensure(bytes));
     char* S = (char*)ctx->staging.p;
-    for (uint32_t k = 0; k < n; ++k) rtbvh::sphere_exact(spheres[k], (double*)S + 4 * (size_t)k, ((rtbvh::Mat32*)(S + geo_b))[k]);
+    for (uint32_t k = 0; k < n; ++k) {
+        rtbvh::sphere_exact(spheres[k], (double*)S + 4 * (size_t)k, ((rtbvh::Mat32*)(S + geo_b))[k]);
+        // never cleared: the flag only selects the exact slow path, and frames already enqueued copied the old value
+        if (albedo_nonfinite(spheres[k])) h->tp.albedo_nonfinite = 1u;
+    }
     memcpy(S + geo_b + mat_b, index, (size_t)n * 4);
     CU(h->upd_in.ensure(bytes));
     char* D = (char*)h->upd_in.p;

@@ -100,6 +100,10 @@ struct TraceParams {
     // ---- multi-frame launches only (appended, so that the fields above keep their offsets) ----
     const FrameRec* ftab;        // [frames of the launch]: work id w belongs to frame w / frame_work
     uint32_t frame_work;         // work ids per frame = s_count * npix_local; total_work = frames * frame_work
+    // ---- appended after the multi-frame fields ----
+    // 1: a Lambertian or Metal sphere has, or once had, an infinite or NaN albedo component. A black path then has to unwind
+    // its albedo stack, and a nested shadow vertex has to read its albedo, because albedo * 0 is NaN for such an albedo.
+    uint32_t albedo_nonfinite;
 };
 
 struct ResolveParams {

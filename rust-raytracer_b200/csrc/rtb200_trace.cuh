@@ -620,8 +620,14 @@ RT_DEV bool shade_slot(const TraceParams& p, const SceneRefs& sc, const Pool& P,
                     if (level == p.max_depth) done = true;   // the next ray_color call returns black (raytracer.rs:80-82)
                 }
             } else {
-                // nested vertex without light contribution: clamp(0 + albedo * black), or white for a Light
+                // nested vertex without light contribution: clamp(0 + albedo * black), or white for a Light. That is 0 for a
+                // finite albedo; only a scene with a non-finite one reads it.
                 tr = tg = tb = is_light ? 1.f : 0.f;
+                if (p.albedo_nonfinite && !is_light) {
+                    float ar, ag, ab;
+                    albedo_of(code, mat, ar, ag, ab);
+                    tr = clampf(__fadd_rn(0.f, __fmul_rn(ar, 0.f))); tg = clampf(__fadd_rn(0.f, __fmul_rn(ag, 0.f))); tb = clampf(__fadd_rn(0.f, __fmul_rn(ab, 0.f)));
+                }
                 have_tc = true;
             }
         }
@@ -670,8 +676,9 @@ RT_DEV bool shade_slot(const TraceParams& p, const SceneRefs& sc, const Pool& P,
         P.shd[s] = shd;   // also clears kScatterPending
     }
     if (done) {
-        // unwind the recursion: c = clamp(light + albedo * c) per level, innermost first (raytracer.rs:117-122)
-        if (LIGHTS || cr != 0.f || cg != 0.f || cb != 0.f) {
+        // unwind the recursion: c = clamp(light + albedo * c) per level, innermost first (raytracer.rs:117-122). A black path
+        // without light terms stays black unless an albedo is non-finite (albedo * 0 = NaN).
+        if (LIGHTS || p.albedo_nonfinite || cr != 0.f || cg != 0.f || cb != 0.f) {
             for (int l = (int)level - 1; l >= 0; --l) {
                 float ar, ag, ab;
                 albedo_of(stack_get((uint32_t)l), mat, ar, ag, ab);

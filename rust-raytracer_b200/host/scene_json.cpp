@@ -1,5 +1,7 @@
 #include "scene_json.hpp"
 
+#include <cfloat>
+#include <cmath>
 #include <fstream>
 #include <stdexcept>
 
@@ -8,9 +10,16 @@
 namespace rthost {
 namespace {
 rt_vec3 vec3(const Json& j) { return rt_vec3{j.at("x").number(), j.at("y").number(), j.at("z").number()}; }   // point3d.rs:10-15
+// Rust `as f32`: round to nearest, +-inf from the halfway point 0x1.ffffffp127 above FLT_MAX on. A plain (float) cast of a
+// value beyond FLT_MAX is undefined behaviour in C++.
+float f64_as_f32(double x) {
+    if (std::fabs(x) >= 0x1.ffffffp127) return x > 0.0 ? INFINITY : -INFINITY;
+    if (std::fabs(x) > FLT_MAX) return x > 0.0 ? FLT_MAX : -FLT_MAX;
+    return (float)x;
+}
 void albedo(const Json& j, float out[3]) {                                                                  // SrgbAsArray, materials.rs:18-25
     if (j.kind != Json::Arr || j.arr.size() != 3) throw std::runtime_error("albedo: array of 3 numbers expected");
-    for (int i = 0; i < 3; ++i) out[i] = (float)j.arr[i].number();
+    for (int i = 0; i < 3; ++i) out[i] = f64_as_f32(j.arr[i].number());
 }
 // serde parses width/height/max_depth as usize and samples_per_pixel as u32 (config.rs:68-71): negative, fractional or
 // out-of-range numbers are parse errors there; casting them blindly would be undefined behaviour here.

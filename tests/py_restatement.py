@@ -78,6 +78,22 @@ def unit_vector(a):                          # three divisions, point3d.rs:67-70
     return (a[0] / l, a[1] / l, a[2] / l)
 
 
+def fdiv(a, b):                              # IEEE f64 division: x / 0 is +-inf or NaN, as in Rust, not an exception
+    if b == 0.0:
+        return math.nan if a == 0.0 or a != a else math.copysign(math.inf, a) * math.copysign(1.0, b)
+    return a / b
+
+
+def fsqrt(x):                                # f64::sqrt: NaN below 0
+    return math.sqrt(x) if x >= 0.0 else math.nan
+
+
+def as_usize(x):                             # Rust `as usize` of a float: saturating, NaN -> 0
+    if not x > 0.0:
+        return 0
+    return U64 if x >= 18446744073709551616.0 else int(x)
+
+
 def near_zero(a):
     e = 2.220446049250313e-16
     return abs(a[0]) < e and abs(a[1]) < e and abs(a[2]) < e
@@ -176,8 +192,10 @@ class World:
                 rot = rot - 1.0
             W, H = int(body["width"]), int(body["height"])
             uu, vv = rot * float(W), (1.0 - h["v"]) * float(H - 1)
-            base = 3 * (int(math.floor(vv)) * W + int(math.floor(uu)))
+            base = 3 * (as_usize(math.floor(vv)) * W + as_usize(math.floor(uu)))
             flat = tex.reshape(-1)
+            if base + 2 >= flat.size:                                                    # the reference panics (index out of bounds)
+                raise IndexError(f"texture index {base + 2} out of bounds for {flat.size} bytes")
             return ray, (f32(flat[base]) / f32(255.0), f32(flat[base + 1]) / f32(255.0), f32(flat[base + 2]) / f32(255.0))
         if kind == "Metal":                                                              # :111-129
             reflected = sub(d, mul(h["normal"], 2.0 * dot(d, h["normal"])))
@@ -187,13 +205,13 @@ class World:
             return "absorbed"
         if kind == "Glass":                                                              # :144-155, :176-199
             ior = float(body["index_of_refraction"])
-            ratio = 1.0 / ior if h["front"] else ior
+            ratio = fdiv(1.0, ior) if h["front"] else ior
             ud = unit_vector(d)
             cos_theta = min(dot(neg(ud), h["normal"]), 1.0)
-            sin_theta = math.sqrt(1.0 - cos_theta * cos_theta)
+            sin_theta = fsqrt(1.0 - cos_theta * cos_theta)
             reflect_it = ratio * sin_theta > 1.0
             if not reflect_it:
-                r0 = (1.0 - ratio) / (1.0 + ratio)
+                r0 = fdiv(1.0 - ratio, 1.0 + ratio)
                 r0 = r0 * r0
                 x = 1.0 - cos_theta
                 x2 = x * x
@@ -226,7 +244,7 @@ class World:
                 omt = (f32(1.0) - t) * f32(1.0)
                 return omt + t * f32(0.5), omt + t * f32(0.7), omt + t * f32(1.0)
             H, W = self.sky.shape[0], self.sky.shape[1]
-            x = int(u * f32(W - 1)); y = int((f32(1.0) - t) * f32(H - 1))
+            x = as_usize(u * f32(W - 1)); y = as_usize((f32(1.0) - t) * f32(H - 1))
             px = self.sky.reshape(-1)[(y * W + x) * 3: (y * W + x) * 3 + 3]
             return tuple(f32(0.7) * f32(px[k]) / f32(255.0) for k in range(3))
         sc = self.scatter(o, d, h, rng)
@@ -269,7 +287,7 @@ class World:
                     m = scale * acc[k]
                     lin[y, x, k] = m
                     # palette 0.6 Srgb<f32> -> u8: min(x*255, 255) + 2^23, low mantissa bits (round half even)
-                    scaled = min(np.sqrt(m) * f32(255.0), f32(255.0))
+                    scaled = np.fmin(np.sqrt(m) * f32(255.0), f32(255.0))                # f32::min: a NaN operand is dropped
                     bits = int(np.array([scaled + f32(8388608.0)], np.float32).view(np.uint32)[0])
                     img[y, x, k] = max(bits - 0x4B000000, 0) & 0xFF if bits >= 0x4B000000 else 0
         return lin, img, self.rays

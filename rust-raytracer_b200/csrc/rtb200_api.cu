@@ -139,7 +139,6 @@ struct DeviceRestore {
 
 struct V3 { double x, y, z; };
 inline V3 v3(const rt_vec3& a) { return V3{a.x, a.y, a.z}; }
-inline V3 operator+(V3 a, V3 b) { return V3{a.x + b.x, a.y + b.y, a.z + b.z}; }
 inline V3 operator-(V3 a, V3 b) { return V3{a.x - b.x, a.y - b.y, a.z - b.z}; }
 inline V3 operator*(V3 a, double s) { return V3{a.x * s, a.y * s, a.z * s}; }
 inline double vlen(V3 a) { return std::sqrt(a.x * a.x + a.y * a.y + a.z * a.z); }
@@ -403,6 +402,9 @@ static int normalise_options(const rt_options* opts_in, rt_options* o) {
     return RT_OK;
 }
 
+// bytes of per-sample radiance one launch may stage (rt_options.sample_buffer_bytes, 0: 1 GiB)
+static uint64_t sample_buffer_cap(const rt_options& o) { return o.sample_buffer_bytes ? o.sample_buffer_bytes : (1ull << 30); }
+
 // TraceParams::albedo_nonfinite for a sphere: only Lambertian and Metal spheres carry their own albedo (Texture, Glass and
 // Light albedos are finite)
 static bool albedo_nonfinite(const rt_sphere& sp) {
@@ -485,7 +487,7 @@ static int scene_upload_records(const rt_scene* s, const rt_options& opts, uint3
     h->grid = ctx->sm_count * occ;
 
     // ---- per-sample staging: samples per batch bounded by the buffer cap ----
-    uint64_t cap = opts.sample_buffer_bytes ? opts.sample_buffer_bytes : (1ull << 30);
+    uint64_t cap = sample_buffer_cap(opts);
     uint64_t per_spp = (uint64_t)std::max<uint32_t>(tp.npix_local, 1) * 16ull;
     uint64_t spb = std::max<uint64_t>(1, cap / per_spp);
     spb = std::min<uint64_t>(spb, s->samples_per_pixel);
@@ -601,6 +603,15 @@ static int check_frames(const rt_frame* frames, uint32_t n, uint64_t rows, uint6
 // The handle's own view (the camera, seed and depth it was uploaded with) as a frame.
 static rt_frame own_frame(rtb200_scene_handle h) { return rt_frame{h->tp.cam, h->tp.key0 | (uint64_t)h->tp.key1 << 32, h->tp.max_depth, 0}; }
 
+// The stream of a call on h, `stream_in` (NULL: the context's stream), made to wait for what last wrote the scene arrays:
+// the upload, which ran on the context's stream, and the last update or rebuild, on whichever stream it ran.
+static cudaError_t scene_stream(rtb200_scene_handle h, void* stream_in, cudaStream_t* out) {
+    const cudaStream_t st = stream_in ? (cudaStream_t)stream_in : h->ctx->stream;
+    *out = st;
+    if (st != h->ctx->stream) { cudaError_t e = cudaStreamWaitEvent(st, h->ctx->staging_free, 0); if (e != cudaSuccess) return e; }
+    return h->updated ? cudaStreamWaitEvent(st, h->updated, 0) : cudaSuccess;
+}
+
 // Enqueue frames[0, n) of h on `stream_in` (NULL: the context's stream) with work set `set`, without waiting, and append the
 // submission to h->pending; the caller holds the context's lock. Frame i goes to output slice i (rows * width * 3 elements).
 // The submission starts after the previous one that took the same set, on any stream and of any handle, has finished with it.
@@ -611,9 +622,8 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
     DeviceCtx* ctx = h->ctx;
     DeviceCtx::WorkSet& W = ctx->ws[set];
     CU(cudaSetDevice(h->device));
-    cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
-    if (st != ctx->stream) CU(cudaStreamWaitEvent(st, ctx->staging_free, 0));   // the scene upload ran on the context's stream
-    if (h->updated) CU(cudaStreamWaitEvent(st, h->updated, 0));                 // and its last update on the update's stream
+    cudaStream_t st;
+    CU(scene_stream(h, stream_in, &st));
     const rtb200_scene_t::Submission* prev = h->pending.empty() ? nullptr : &h->pending.back();
     rtb200_scene_t::Submission sub{st, prev ? prev->ev0 + prev->n_ev : 0u, 0, n, 0, 0, h->grid, 0, 0};
     TraceParams tp = h->tp;   // the handle's own view stays as uploaded
@@ -621,8 +631,11 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
     if (npl == 0) { h->pending.push_back(sub); return RT_OK; }   // a shard with no rows: nothing to trace
     const uint32_t spp = tp.spp, spb = h->spp_batch, n_batches = (spp + spb - 1) / spb;
     const uint64_t frame_work = (uint64_t)spp * npl;
-    const uint64_t cap = h->opts.sample_buffer_bytes ? h->opts.sample_buffer_bytes : (1ull << 30);
-    const std::vector<FrameGroup> groups = frame_groups(frames, n, frame_work, cap);
+    const std::vector<FrameGroup> groups = frame_groups(frames, n, frame_work, sample_buffer_cap(h->opts));
+    // A batch of a group holds spb samples of each of its frames. A group of F >= 2 frames is one batch: frame_groups admits
+    // it only when 2 * spp * npl * 16 bytes fit the cap and 2 * spp * npl < 2^31, and with these scene_upload_records made
+    // spp_batch == spp.
+    auto batches_of = [&](const FrameGroup& g) { return g.count > 1 ? 1u : n_batches; };
 
     // trace launches, work buffer sizes and the launch geometry of the multi-frame kernel (its pool also holds the slots' frames)
     size_t smem_f = 0;
@@ -630,8 +643,8 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
     uint32_t max_depth = 1;
     size_t sbuf = 0;
     for (const FrameGroup& g : groups) {
-        sub.batches += g.count > 1 ? 1u : n_batches;   // trace launches (or black memsets)
-        sbuf = std::max(sbuf, g.count > 1 ? (size_t)(g.count * frame_work * 16) : (size_t)spb * npl * 16);
+        sub.batches += batches_of(g);   // trace launches (or black memsets)
+        sbuf = std::max(sbuf, (size_t)g.count * spb * npl * 16);
         max_depth = std::max(max_depth, frames[g.first].max_depth);
         if (g.count > 1 && grid_f == 0) {
             smem_f = wavefront_smem_bytes(tp, h->mode, tp.scene_in_smem, true);
@@ -669,50 +682,39 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
     uint32_t b = 0;   // trace launch (or black memset) index: its queue counter and its event pair
     for (const FrameGroup& g : groups) {
         const rt_frame& f0 = frames[g.first];
+        const bool multi = g.count > 1;   // the multi-frame trace kernel, which reads each frame's camera and key from ftab
+        const uint32_t batches = batches_of(g);
+        const int grid = multi ? grid_f : h->grid;
+        const size_t smem = multi ? smem_f : h->smem;
         uint8_t* o8 = dev_rgb8 ? (uint8_t*)dev_rgb8 + (size_t)g.first * npl * 3 : nullptr;
         float* ol = dev_linear_f32 ? (float*)dev_linear_f32 + (size_t)g.first * npl * 3 : nullptr;
         TraceParams q = tp;
         q.max_depth = f0.max_depth;
-        if (g.count == 1) {
-            q.cam = f0.camera; q.key0 = (uint32_t)f0.seed; q.key1 = (uint32_t)(f0.seed >> 32);
-            q.stack_stride = (uint32_t)h->grid * (uint32_t)kBlock;
-            for (uint32_t k = 0; k < n_batches; ++k, ++b) {
-                q.s0 = k * spb;
-                q.s_count = std::min(spb, spp - q.s0);
-                q.total_work = q.s_count * q.npix_local;
-                q.work_counter = counters + b;
-                CU(cudaEventRecord(ev[2 + 2 * b], st));
-                if (q.max_depth == 0) {
-                    CU(cudaMemsetAsync(q.samplebuf, 0, (size_t)q.total_work * 16, st));   // ray_color(depth 0) = black, no ray (raytracer.rs:80-82)
-                } else {
-                    CU(launch_wavefront(q, h->mode, false, h->grid, h->smem, st));
-                }
-                CU(cudaEventRecord(ev[3 + 2 * b], st));
+        q.stack_stride = (uint32_t)grid * (uint32_t)kBlock;
+        if (multi) { q.ftab = (const FrameRec*)W.ftab.p + g.first; q.frame_work = (uint32_t)frame_work; }
+        else { q.cam = f0.camera; q.key0 = (uint32_t)f0.seed; q.key1 = (uint32_t)(f0.seed >> 32); }
+        for (uint32_t k = 0; k < batches; ++k, ++b) {
+            q.s0 = k * spb;
+            q.s_count = std::min(spb, spp - q.s0);
+            q.total_work = g.count * q.s_count * q.npix_local;
+            q.work_counter = counters + b;
+            CU(cudaEventRecord(ev[2 + 2 * b], st));
+            if (q.max_depth == 0) {
+                CU(cudaMemsetAsync(q.samplebuf, 0, (size_t)q.total_work * 16, st));   // ray_color(depth 0) = black, no ray (raytracer.rs:80-82)
+            } else {
+                CU(launch_wavefront(q, h->mode, multi, grid, smem, st));
+            }
+            CU(cudaEventRecord(ev[3 + 2 * b], st));
+            for (uint32_t j = 0; j < g.count; ++j) {   // samplebuf [frame][sample][pixel]
                 ResolveParams r{};
-                r.samplebuf = q.samplebuf; r.accum = (float*)W.accum.p; r.npix_local = q.npix_local; r.s_count = q.s_count;
-                r.first = k == 0; r.last = k + 1 == n_batches; r.spp = spp;
-                r.out_linear = ol; r.out_rgb8 = o8;
+                r.samplebuf = q.samplebuf + (size_t)j * q.s_count * npl; r.accum = (float*)W.accum.p; r.npix_local = q.npix_local;
+                r.s_count = q.s_count; r.first = k == 0; r.last = k + 1 == batches; r.spp = spp;
+                r.out_linear = ol ? ol + (size_t)j * npl * 3 : nullptr; r.out_rgb8 = o8 ? o8 + (size_t)j * npl * 3 : nullptr;
                 CU(launch_resolve(r, st));
             }
-            sub.launches += 2 * n_batches;
-            if (f0.max_depth == 0) sub.black_samples += frame_work;
-            continue;
         }
-        q.ftab = (const FrameRec*)W.ftab.p + g.first; q.frame_work = (uint32_t)frame_work;
-        q.s0 = 0; q.s_count = spp; q.total_work = (uint32_t)(g.count * frame_work);
-        q.work_counter = counters + b;
-        q.stack_stride = (uint32_t)grid_f * (uint32_t)kBlock;
-        CU(cudaEventRecord(ev[2 + 2 * b], st));
-        CU(launch_wavefront(q, h->mode, true, grid_f, smem_f, st));
-        CU(cudaEventRecord(ev[3 + 2 * b], st));
-        for (uint32_t k = 0; k < g.count; ++k) {   // samplebuf [frame][sample][pixel]: frame k's samples are one batch
-            ResolveParams r{};
-            r.samplebuf = q.samplebuf + (size_t)k * frame_work; r.accum = (float*)W.accum.p; r.npix_local = (uint32_t)npl; r.s_count = spp;
-            r.first = 1; r.last = 1; r.spp = spp;
-            r.out_linear = ol ? ol + (size_t)k * npl * 3 : nullptr; r.out_rgb8 = o8 ? o8 + (size_t)k * npl * 3 : nullptr;
-            CU(launch_resolve(r, st));
-        }
-        b += 1; sub.launches += 1 + g.count;
+        sub.launches += batches * (1 + g.count);
+        if (q.max_depth == 0) sub.black_samples += g.count * frame_work;
     }
     CU(cudaEventRecord(ev[1], st));
     CU(cudaMemcpyAsync(h->stat_snap + h->pending.size() * (kStatBytes / 8), W.small.p, kStatBytes, cudaMemcpyDeviceToDevice, st));
@@ -836,26 +838,34 @@ static int refit_prepare(rtb200_scene_handle h, cudaStream_t st) {
     if (h->node_box || h->mode != MODE_TREE || nn == 0) return RT_OK;   // a rebuild brings its own scratch
     void* p = nullptr;
     CU(cudaMalloc(&p, ((size_t)nn + nl) * 6 * sizeof(double) + (size_t)nn * 4));
-    h->refit = p;
-    h->node_box = (double*)p;
-    h->leaf_box = h->node_box + (size_t)nn * 6;
-    h->level_nodes_dev = (uint32_t*)(h->leaf_box + (size_t)nl * 6);
-    CU(cudaMemcpyAsync(h->level_nodes_dev, h->level_nodes.data(), (size_t)nn * 4, cudaMemcpyHostToDevice, st));
+    double* node_box = (double*)p;
+    double* leaf_box = node_box + (size_t)nn * 6;
+    uint32_t* level_nodes = (uint32_t*)(leaf_box + (size_t)nl * 6);
+    const cudaError_t e = cudaMemcpyAsync(level_nodes, h->level_nodes.data(), (size_t)nn * 4, cudaMemcpyHostToDevice, st);
+    if (e != cudaSuccess) { cudaFree(p); return fail_cuda(e, "cudaMemcpyAsync(level order)"); }
+    // node_box marks the handle as prepared: set only once the level order is on its way
+    h->refit = p; h->node_box = node_box; h->leaf_box = leaf_box; h->level_nodes_dev = level_nodes;
     return RT_OK;
 }
 
-// Order `st` after the upload and the previous update (which may still read upd_in).
-static int update_begin(rtb200_scene_handle h, cudaStream_t st) {
-    if (st != h->ctx->stream) CU(cudaStreamWaitEvent(st, h->ctx->staging_free, 0));
-    if (h->updated) CU(cudaStreamWaitEvent(st, h->updated, 0));
-    else CU(cudaEventCreateWithFlags(&h->updated, cudaEventDisableTiming));
-    return RT_OK;
+// The event every later frame of h waits for, created by the first update or rebuild.
+static cudaError_t update_begin(rtb200_scene_handle h) {
+    return h->updated ? cudaSuccess : cudaEventCreateWithFlags(&h->updated, cudaEventDisableTiming);
 }
 
 // Order `st` after the frames of h in flight, on any stream: they read the arrays the update writes.
 static int update_after_frames(rtb200_scene_handle h, cudaStream_t st) {
     for (const auto& p : h->pending) if (p.n_ev) CU(cudaStreamWaitEvent(st, h->ev[p.ev0 + 1], 0));
     return RT_OK;
+}
+
+// Enqueue the refit of the tree p describes: its leaf records and boxes, then one pass per level of the level order
+// `level_nodes` (device) with level k at [level_off[k], level_off[k + 1]), deepest first.
+static cudaError_t refit_tree(const RefitParams& p, const uint32_t* level_nodes, const std::vector<uint32_t>& level_off, cudaStream_t st) {
+    cudaError_t e = launch_refit_spheres(p, st);
+    for (size_t k = 0; e == cudaSuccess && k + 1 < level_off.size(); ++k)
+        e = launch_refit_nodes(p, level_nodes + level_off[k], level_off[k + 1] - level_off[k], st);
+    return e;
 }
 
 // Recompute the arrays of h's mode from its geo and record the end of the update: every frame enqueued later waits for it.
@@ -868,9 +878,7 @@ static int update_finish(rtb200_scene_handle h, cudaStream_t st) {
     } else if (h->mode == MODE_TREE && h->node_box) {
         p.leaf_id = h->tp.leaf_id; p.leaf_rec = (float*)h->tp.leaf_rec; p.leaf_box = h->leaf_box; p.n_leaves = h->tp.n_leaves;
         p.nodes = (float*)h->tp.nodes; p.node_box = h->node_box;
-        CU(launch_refit_spheres(p, st));
-        for (size_t k = 0; k + 1 < h->level_off.size(); ++k)
-            CU(launch_refit_nodes(p, h->level_nodes_dev + h->level_off[k], h->level_off[k + 1] - h->level_off[k], st));
+        CU(refit_tree(p, h->level_nodes_dev, h->level_off, st));
     }
     CU(cudaEventRecord(h->updated, st));
     return RT_OK;
@@ -900,9 +908,10 @@ int rtb200_scene_update_spheres(rtb200_scene_handle h, const uint32_t* index, co
     DeviceCtx* ctx = h->ctx;
     std::lock_guard<std::recursive_mutex> lk(ctx->mu);
     CU(cudaSetDevice(h->device));
-    cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
-    int rc = update_begin(h, st);
-    if (rc == RT_OK) rc = refit_prepare(h, st);
+    cudaStream_t st;   // after the previous update too: it may still read upd_in
+    CU(scene_stream(h, stream_in, &st));
+    CU(update_begin(h));
+    int rc = refit_prepare(h, st);
     if (rc != RT_OK) return rc;
     // input in the pinned staging buffer (geo, materials, indices), copied before this call returns
     const size_t geo_b = (size_t)n * 32, mat_b = (size_t)n * sizeof(DevMat), bytes = geo_b + mat_b + (size_t)n * 4;
@@ -939,14 +948,22 @@ int rtb200_scene_update_geometry_device(rtb200_scene_handle h, const void* dev_c
     if (!((a.type == cudaMemoryTypeDevice && a.device == h->device) || a.type == cudaMemoryTypeManaged))
         return fail(RT_ERR_INVALID, "dev_center_radius is not device or managed memory of device " + std::to_string(h->device));
     if (h->tp.n == 0) return RT_OK;
-    cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
-    int rc = update_begin(h, st);
-    if (rc == RT_OK) rc = refit_prepare(h, st);
+    cudaStream_t st;
+    CU(scene_stream(h, stream_in, &st));
+    CU(update_begin(h));
+    int rc = refit_prepare(h, st);
     if (rc == RT_OK) rc = update_after_frames(h, st);
     if (rc != RT_OK) return rc;
     CU(cudaMemcpyAsync((void*)h->tp.geo, dev_center_radius, (size_t)h->tp.n * 32, cudaMemcpyDeviceToDevice, st));
     return update_finish(h, st);
   });
+}
+
+// The first min(cap, count) elements of `elem` bytes of device array src into host array dst, enqueued on st (nothing when
+// either array is null or either count is 0).
+static cudaError_t copy_out(void* dst, const void* src, uint64_t cap, uint64_t count, size_t elem, cudaStream_t st) {
+    if (!dst || !src || !cap || !count) return cudaSuccess;
+    return cudaMemcpyAsync(dst, src, std::min(cap, count) * elem, cudaMemcpyDeviceToHost, st);
 }
 
 // Diagnostic: the handle's current arrays, laid out as rtb200_debug_bvh's (flat records only in RT_VARIANT_BRUTE_FORCE)
@@ -959,18 +976,12 @@ int rtb200_scene_debug_records(rtb200_scene_handle h, uint32_t info[8], float* n
     DeviceRestore restore;
     std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
     CU(cudaSetDevice(h->device));
-    cudaStream_t st = h->ctx->stream;   // after the upload; after the last update:
-    if (h->updated) CU(cudaStreamWaitEvent(st, h->updated, 0));
-    auto get = [&](void* dst, const void* src, uint64_t cap, uint64_t count, size_t elem) -> int {
-        if (dst && src && cap && count) CU(cudaMemcpyAsync(dst, src, std::min(cap, count) * elem, cudaMemcpyDeviceToHost, st));
-        return RT_OK;
-    };
-    int rc = RT_OK;
-    if (rc == RT_OK) rc = get(nodes, tp.nodes, cap_nodes, (uint64_t)tp.n_nodes * rtbvh::kNodeFloats, 4);
-    if (rc == RT_OK) rc = get(leaf_rec, tp.leaf_rec, cap_leaf_rec, (uint64_t)tp.n_leaves * rtbvh::kLeafK * 4, 4);
-    if (rc == RT_OK) rc = get(flat, tp.filt, cap_flat, (uint64_t)info[6] * 8, 4);
-    if (rc == RT_OK) rc = get(geo, tp.geo, cap_geo, (uint64_t)tp.n * 4, 8);
-    if (rc != RT_OK) return rc;
+    cudaStream_t st;
+    CU(scene_stream(h, nullptr, &st));
+    CU(copy_out(nodes, tp.nodes, cap_nodes, (uint64_t)tp.n_nodes * rtbvh::kNodeFloats, 4, st));
+    CU(copy_out(leaf_rec, tp.leaf_rec, cap_leaf_rec, (uint64_t)tp.n_leaves * rtbvh::kLeafK * 4, 4, st));
+    CU(copy_out(flat, tp.filt, cap_flat, (uint64_t)info[6] * 8, 4, st));
+    CU(copy_out(geo, tp.geo, cap_geo, (uint64_t)tp.n * 4, 8, st));
     CU(cudaStreamSynchronize(st));
     return RT_OK;
   });
@@ -1003,9 +1014,10 @@ int rtb200_scene_rebuild(rtb200_scene_handle h, void* stream_in) {
     }
     RebuildBufs b;
     rebuild_carve(h->rebuild, n, &b);
-    cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
-    int rc = update_begin(h, st);
-    if (rc == RT_OK) rc = update_after_frames(h, st);
+    cudaStream_t st;
+    CU(scene_stream(h, stream_in, &st));
+    CU(update_begin(h));
+    int rc = update_after_frames(h, st);
     if (rc != RT_OK) return rc;
     const char* ov = getenv("RTB200_REBUILD_OVERSIZE");   // benchmark hook: 0 keeps oversized spheres in the Morton order
     CU(launch_rebuild_topology(b, h->tp.geo, n, ov ? atof(ov) : kRebuildOversize, st));
@@ -1021,8 +1033,7 @@ int rtb200_scene_rebuild(rtb200_scene_handle h, void* stream_in) {
     p.geo = h->tp.geo; p.n = n; p.g[0] = H.g[0]; p.g[1] = H.g[1]; p.g[2] = H.g[2];
     p.leaf_id = b.leaf_id; p.leaf_rec = b.leaf_rec; p.leaf_box = b.leaf_box; p.n_leaves = H.n_leaves;
     p.nodes = b.nodes; p.node_box = b.node_box;
-    CU(launch_refit_spheres(p, st));
-    for (size_t k = 0; k + 1 < level_off.size(); ++k) CU(launch_refit_nodes(p, b.level_nodes + level_off[k], level_off[k + 1] - level_off[k], st));
+    CU(refit_tree(p, b.level_nodes, level_off, st));
     CU(cudaEventRecord(h->updated, st));
     // every frame enqueued from here on traces the new tree, and every update refits it
     if (h->refit) { CU(cudaFree(h->refit)); h->refit = nullptr; }   // the stream synchronisation above covers the updates that used it
@@ -1051,19 +1062,13 @@ int rtb200_scene_debug_topology(rtb200_scene_handle h, double recentre[3], uint3
     DeviceRestore restore;
     std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
     CU(cudaSetDevice(h->device));
-    cudaStream_t st = h->ctx->stream;   // after the upload; after the last update or rebuild:
-    if (h->updated) CU(cudaStreamWaitEvent(st, h->updated, 0));
-    auto get = [&](void* dst, const void* src, uint64_t cap, uint64_t count) -> int {
-        if (dst && src && cap && count) CU(cudaMemcpyAsync(dst, src, std::min(cap, count) * 4, cudaMemcpyDeviceToHost, st));
-        return RT_OK;
-    };
     const bool tree = h->mode == MODE_TREE;
-    int rc = RT_OK;
-    if (rc == RT_OK) rc = get(leaf_id, tp.leaf_id, cap_leaf_id, (uint64_t)tp.n_leaves * rtbvh::kLeafK);
-    if (rc == RT_OK) rc = get(always, tp.always, cap_always, tp.n_always);
-    if (rc == RT_OK) rc = get(skip_pos, tp.skip_pos, cap_skip_pos, tree ? std::max<uint64_t>(tp.n, 1) : 0);
-    if (rc == RT_OK && h->rebuild) rc = get(level_nodes, h->level_nodes_dev, cap_level_nodes, tp.n_nodes);
-    if (rc != RT_OK) return rc;
+    cudaStream_t st;
+    CU(scene_stream(h, nullptr, &st));
+    CU(copy_out(leaf_id, tp.leaf_id, cap_leaf_id, (uint64_t)tp.n_leaves * rtbvh::kLeafK, 4, st));
+    CU(copy_out(always, tp.always, cap_always, tp.n_always, 4, st));
+    CU(copy_out(skip_pos, tp.skip_pos, cap_skip_pos, tree ? std::max<uint64_t>(tp.n, 1) : 0, 4, st));
+    if (h->rebuild) CU(copy_out(level_nodes, h->level_nodes_dev, cap_level_nodes, tp.n_nodes, 4, st));
     if (level_nodes && cap_level_nodes && !h->rebuild)
         memcpy(level_nodes, h->level_nodes.data(), std::min<uint64_t>(cap_level_nodes, h->level_nodes.size()) * 4);
     CU(cudaStreamSynchronize(st));
@@ -1240,33 +1245,39 @@ int rtb200_render_rgb8_multi(const rt_scene* s, const rt_options* opts_in, int32
   });
 }
 
+}  // extern "C"
+
 // ---- probes ------------------------------------------------------------------------------------------
-static int probe_io(const void* in, size_t in_bytes, size_t out_bytes, DeviceCtx** pctx, void** din, void** dout) {
-    int rc = get_ctx(-1, pctx);
+// One probe on the current device: in_bytes of `in` to the device, `launch(din, dout, stream)` enqueues the probe kernel,
+// and the out_bytes it writes (zeroed first) come back into `out`. The probe buffer and the stream are the context's, so
+// the context's lock is held until the result is on the host.
+template <typename Launch>
+static int probe_run(const void* in, size_t in_bytes, void* out, size_t out_bytes, Launch&& launch) {
+    DeviceCtx* c = nullptr;
+    int rc = get_ctx(-1, &c);
     if (rc != RT_OK) return rc;
-    DeviceCtx* c = *pctx;
+    std::lock_guard<std::recursive_mutex> lk(c->mu);
     CU(c->probe.ensure(in_bytes + out_bytes + 512));
-    *din = c->probe.p;
-    *dout = (char*)c->probe.p + ((in_bytes + 255) / 256) * 256;
-    CU(cudaMemsetAsync(*dout, 0, out_bytes, c->stream));
-    if (in_bytes) CU(cudaMemcpyAsync(*din, in, in_bytes, cudaMemcpyHostToDevice, c->stream));
-    return RT_OK;
-}
-static int probe_finish(DeviceCtx* c, void* host_out, const void* dout, size_t out_bytes) {
-    CU(cudaMemcpyAsync(host_out, dout, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+    void* din = c->probe.p;
+    void* dout = (char*)c->probe.p + ((in_bytes + 255) / 256) * 256;
+    CU(cudaMemsetAsync(dout, 0, out_bytes, c->stream));
+    if (in_bytes) CU(cudaMemcpyAsync(din, in, in_bytes, cudaMemcpyHostToDevice, c->stream));
+    CU(launch(din, dout, c->stream));
+    CU(cudaMemcpyAsync(out, dout, out_bytes, cudaMemcpyDeviceToHost, c->stream));
     CU(cudaStreamSynchronize(c->stream));
     return RT_OK;
 }
+
+extern "C" {
 
 int rtb200_probe_sphere_hit(const rt_vec3* center, double radius, const rt_vec3* origin, const rt_vec3* dir, double t_min,
                             double t_max, int32_t* hit, double* t, rt_vec3* point, rt_vec3* normal, int32_t* front_face) {
     double in[12] = {center->x, center->y, center->z, radius, origin->x, origin->y, origin->z, dir->x, dir->y, dir->z, t_min, t_max};
     double out[9];
-    DeviceCtx* c; void *din, *dout;
-    int rc = probe_io(in, sizeof in, sizeof out, &c, &din, &dout);
+    int rc = probe_run(in, sizeof in, out, sizeof out, [](void* din, void* dout, cudaStream_t st) {
+        return probe_sphere_hit((const double*)din, (double*)dout, st);
+    });
     if (rc != RT_OK) return rc;
-    CU(probe_sphere_hit((const double*)din, (double*)dout, c->stream));
-    if ((rc = probe_finish(c, out, dout, sizeof out)) != RT_OK) return rc;
     *hit = out[0] != 0.0;
     if (*hit) {
         *t = out[1]; *point = rt_vec3{out[2], out[3], out[4]}; *normal = rt_vec3{out[5], out[6], out[7]};
@@ -1276,63 +1287,51 @@ int rtb200_probe_sphere_hit(const rt_vec3* center, double radius, const rt_vec3*
 }
 int rtb200_probe_refract(const rt_vec3* uv, const rt_vec3* n, double eta, rt_vec3* o) {
     double in[7] = {uv->x, uv->y, uv->z, n->x, n->y, n->z, eta}, out[3];
-    DeviceCtx* c; void *din, *dout;
-    int rc = probe_io(in, sizeof in, sizeof out, &c, &din, &dout);
+    int rc = probe_run(in, sizeof in, out, sizeof out, [](void* din, void* dout, cudaStream_t st) {
+        return probe_refract((const double*)din, (double*)dout, st);
+    });
     if (rc != RT_OK) return rc;
-    CU(probe_refract((const double*)din, (double*)dout, c->stream));
-    if ((rc = probe_finish(c, out, dout, sizeof out)) != RT_OK) return rc;
     *o = rt_vec3{out[0], out[1], out[2]};
     return RT_OK;
 }
 int rtb200_probe_reflectance(double cosine, double ref_idx, double* o) {
     double in[2] = {cosine, ref_idx};
-    DeviceCtx* c; void *din, *dout;
-    int rc = probe_io(in, sizeof in, 8, &c, &din, &dout);
-    if (rc != RT_OK) return rc;
-    CU(probe_reflectance((const double*)din, (double*)dout, c->stream));
-    return probe_finish(c, o, dout, 8);
+    return probe_run(in, sizeof in, o, 8, [](void* din, void* dout, cudaStream_t st) {
+        return probe_reflectance((const double*)din, (double*)dout, st);
+    });
 }
 int rtb200_probe_sky(const rt_vec3* dir, uint32_t sky_mode, float out_rgb[3]) {
     if (sky_mode == RT_SKY_TEXTURE) return fail(RT_ERR_INVALID, "probe_sky supports none/gradient only");
     double in[3] = {dir->x, dir->y, dir->z};
-    DeviceCtx* c; void *din, *dout;
-    int rc = probe_io(in, sizeof in, 12, &c, &din, &dout);
-    if (rc != RT_OK) return rc;
-    CU(probe_sky((const double*)din, sky_mode, (float*)dout, c->stream));
-    return probe_finish(c, out_rgb, dout, 12);
+    return probe_run(in, sizeof in, out_rgb, 12, [&](void* din, void* dout, cudaStream_t st) {
+        return probe_sky((const double*)din, sky_mode, (float*)dout, st);
+    });
 }
 int rtb200_probe_get_ray(const rt_camera* cam, double u, double v, rt_vec3* origin, rt_vec3* dir) {
     struct { rt_camera cam; double uv[2]; } in;
     in.cam = *cam; in.uv[0] = u; in.uv[1] = v;
     double out[6];
-    DeviceCtx* c; void *din, *dout;
-    int rc = probe_io(&in, sizeof in, sizeof out, &c, &din, &dout);
+    int rc = probe_run(&in, sizeof in, out, sizeof out, [](void* din, void* dout, cudaStream_t st) {
+        return probe_get_ray((const rt_camera*)din, (const double*)((char*)din + sizeof(rt_camera)), (double*)dout, st);
+    });
     if (rc != RT_OK) return rc;
-    CU(probe_get_ray((const rt_camera*)din, (const double*)((char*)din + sizeof(rt_camera)), (double*)dout, c->stream));
-    if ((rc = probe_finish(c, out, dout, sizeof out)) != RT_OK) return rc;
     *origin = rt_vec3{out[0], out[1], out[2]}; *dir = rt_vec3{out[3], out[4], out[5]};
     return RT_OK;
 }
 int rtb200_probe_rng(uint64_t seed, uint32_t pixel, uint32_t sample, uint32_t kind, uint32_t n, double* o) {
-    DeviceCtx* c; void *din, *dout;
-    int rc = probe_io(nullptr, 0, (size_t)n * 8, &c, &din, &dout);
-    if (rc != RT_OK) return rc;
-    CU(probe_rng(seed, pixel, sample, kind, n, (double*)dout, c->stream));
-    return probe_finish(c, o, dout, (size_t)n * 8);
+    return probe_run(nullptr, 0, o, (size_t)n * 8, [&](void*, void* dout, cudaStream_t st) {
+        return probe_rng(seed, pixel, sample, kind, n, (double*)dout, st);
+    });
 }
 int rtb200_probe_sphere_uv(const double* hp_xyz, uint32_t n, double* out_uv) {
-    DeviceCtx* c; void *din, *dout;
-    int rc = probe_io(hp_xyz, (size_t)n * 24, (size_t)n * 16, &c, &din, &dout);
-    if (rc != RT_OK) return rc;
-    CU(probe_sphere_uv((const double*)din, n, (double*)dout, c->stream));
-    return probe_finish(c, out_uv, dout, (size_t)n * 16);
+    return probe_run(hp_xyz, (size_t)n * 24, out_uv, (size_t)n * 16, [&](void* din, void* dout, cudaStream_t st) {
+        return probe_sphere_uv((const double*)din, n, (double*)dout, st);
+    });
 }
 int rtb200_probe_quantise(const float* mean_linear, uint32_t n, uint8_t* o) {
-    DeviceCtx* c; void *din, *dout;
-    int rc = probe_io(mean_linear, (size_t)n * 4, n, &c, &din, &dout);
-    if (rc != RT_OK) return rc;
-    CU(probe_quantise((const float*)din, n, (uint8_t*)dout, c->stream));
-    return probe_finish(c, o, dout, n);
+    return probe_run(mean_linear, (size_t)n * 4, o, n, [&](void* din, void* dout, cudaStream_t st) {
+        return probe_quantise((const float*)din, n, (uint8_t*)dout, st);
+    });
 }
 
 }  // extern "C"

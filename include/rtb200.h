@@ -274,6 +274,44 @@ int rtb200_scene_debug_topology(rtb200_scene_handle h, double recentre[3], uint3
                                 uint32_t* always, uint64_t cap_always, uint32_t* skip_pos, uint64_t cap_skip_pos,
                                 uint32_t* level_nodes, uint64_t cap_level_nodes, uint32_t* level_off, uint64_t cap_level_off);
 
+/* ---- adaptive rendering: stop sampling the pixels that have converged (DESIGN.md §4.9) -----------------------------------
+ * Parameters: m = samples_per_round >= 1, N = max_samples (0: the scene's samples_per_pixel), min_samples >= 1, and the f32
+ * tolerances abs_tol and rel_tol. Per pixel the state is n (samples taken) and, per channel c, the f32 sums in sample order
+ * S_c = sum of the sample radiances (the sum the one-shot render forms) and Q_c = sum of x_c * x_c.
+ * Round: every pixel still on the list traces samples [n, min(n + m, N)) (all listed pixels have the same n).
+ * Test after the round, every f32 operation rounded to nearest and never contracted: inv = 1/n and per channel
+ *     mean_c = inv*S_c   var_c = inv*Q_c - mean_c*mean_c   err_c = sqrt(max(var_c, 0)*inv)   tol_c = abs_tol + rel_tol*mean_c
+ * The pixel leaves the list if n == N, or if n >= min_samples, every S_c and Q_c is finite and err_c <= tol_c for all three
+ * channels. A pixel with a NaN or infinite sum therefore runs to N, and negative tolerances never stop a pixel early.
+ * Resolve: linear = mean_c, RGB8 = the one-shot quantisation of mean_c; a pixel with n == 0 is 0.
+ * Contract: a pixel that received n samples has exactly the linear f32 value, RGB8 value and rays of the one-shot render of the
+ * same scene at samples_per_pixel = n. */
+typedef struct {
+    uint32_t samples_per_round, max_samples, min_samples, reserved;   /* reserved must be 0 */
+    float    abs_tol, rel_tol;
+} rt_adaptive_params;     /* 24 bytes */
+
+/* Resident form: the state (about 40 bytes per pixel of the shard plus cub's scan scratch) lives in the scene handle; it is
+ * allocated at the first begin and freed with the handle. A shard handle (rank/world/band_rows) works on its own rows, every
+ * variant is supported. Outputs are compact like the other calls' (shard rows * width). All three calls are blocking.
+ * begin (re)starts: n = 0 everywhere, every pixel on the list. RT_ERR_INVALID, before any device work, for a NULL handle or
+ * params, samples_per_round or min_samples of 0, a NaN tolerance, a nonzero reserved, samples_per_round * pixels * 16 above the
+ * handle's sample-buffer cap (rt_options.sample_buffer_bytes) or samples_per_round * pixels >= 2^31.
+ * step enqueues `rounds` rounds with no host wait between them, then waits once, and reports the pixels still active and
+ * rt_stats summed over the rounds (rays, samples, device and trace time, kernel launches; batches = trace launches). Once no
+ * pixel is active a step is a no-op. It drains the handle's asynchronous frames first, takes work set 0 and orders its rounds
+ * after the previous user of that set like a blocking render (rtb200_render_device). RT_ERR_INVALID before any begin and after an
+ * rtb200_scene_update_* since the last begin (the sums would mix two scenes); a rebuild does not change renders and is allowed.
+ * resolve writes, for every pixel of the handle, the mean (dev_linear_f32, rows * width * 3 floats), its RGB8 value (dev_rgb8)
+ * and n (dev_counts_u32, rows * width); each output may be NULL. stream: as rtb200_render_device's. */
+int rtb200_adaptive_begin(rtb200_scene_handle h, const rt_adaptive_params* p, void* stream);
+int rtb200_adaptive_step(rtb200_scene_handle h, uint32_t rounds, void* stream, uint32_t* active_out, rt_stats* stats);
+int rtb200_adaptive_resolve(rtb200_scene_handle h, void* dev_rgb8, void* dev_linear_f32, void* dev_counts_u32, void* stream);
+/* Host form, like rtb200_render_frames: upload, run rounds until no pixel is active, copy back, release. Outputs are host
+ * buffers of rows * width * 3 bytes / floats and rows * width counts; each may be NULL. Same checks as begin. */
+int rtb200_render_adaptive(const rt_scene* scene, const rt_options* opts, const rt_adaptive_params* p,
+                           uint8_t* out_rgb8, float* out_linear_f32, uint32_t* out_counts, rt_stats* stats);
+
 /* load_texture_image — materials.rs:213-219, config.rs:36-47: decode a baseline JPEG file to RGB8 (host-side scene staging
  * helper for hosts without their own decoder; the reference uses the jpeg-decoder crate). *out_rgb8 is released with rtb200_free(). */
 int  rtb200_decode_jpeg_file(const char* path, uint8_t** out_rgb8, uint64_t* width, uint64_t* height);

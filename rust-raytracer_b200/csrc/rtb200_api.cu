@@ -85,12 +85,12 @@ struct DeviceCtx {
         GrowBuf samplebuf, accum, stack, small, frames, lterm, ftab;   // ftab: the multi-frame kernel's frame table
         cudaEvent_t done = nullptr;
     } ws[2];
-    GrowBuf out_rgb8, out_lin, probe, frame;
+    GrowBuf out_rgb8, out_lin, out_cnt, probe, frame;
     // scene arenas of released handles, kept for the next upload (a per-frame upload costs no cudaMalloc / cudaFree)
     struct Arena { void* p; size_t cap; };
     std::vector<Arena> arena_cache;
     std::vector<cudaEvent_t> event_pool;  // timing events of released handles (creating four events per one-shot render costs more than the upload)
-    struct OccKey { uint32_t mode; bool lights, frames; size_t smem; int occ; };
+    struct OccKey { uint32_t mode; bool lights; uint32_t queue; size_t smem; int occ; };
     std::vector<OccKey> occ_cache;        // cudaOccupancyMaxActiveBlocksPerMultiprocessor answers
     PinnedBuf staging;                    // host image of the arena being uploaded
     cudaEvent_t staging_free = nullptr;   // the last H2D copy out of `staging` has finished
@@ -160,10 +160,10 @@ uint32_t mode_of(uint32_t variant) {
 }
 
 // resident CTAs per SM of one trace kernel with `smem` bytes of dynamic shared memory (cached per context)
-int occupancy(DeviceCtx* ctx, uint32_t mode, bool lights, bool frames, size_t smem) {
-    for (auto& k : ctx->occ_cache) if (k.mode == mode && k.lights == lights && k.frames == frames && k.smem == smem) return k.occ;
-    const int occ = wavefront_max_ctas_per_sm(mode, lights, frames, smem);
-    ctx->occ_cache.push_back(DeviceCtx::OccKey{mode, lights, frames, smem, occ});
+int occupancy(DeviceCtx* ctx, uint32_t mode, bool lights, uint32_t queue, size_t smem) {
+    for (auto& k : ctx->occ_cache) if (k.mode == mode && k.lights == lights && k.queue == queue && k.smem == smem) return k.occ;
+    const int occ = wavefront_max_ctas_per_sm(mode, lights, queue, smem);
+    ctx->occ_cache.push_back(DeviceCtx::OccKey{mode, lights, queue, smem, occ});
     return occ;
 }
 
@@ -212,6 +212,27 @@ struct rtb200_scene_t {
     // ---- rebuilt hierarchy (rtb200_scene_rebuild): its arrays and the refit's scratch, allocated at the first rebuild ----
     void* rebuild = nullptr;             // RebuildBufs of tp.n spheres; once set, the tree arrays of tp and the refit scratch live here
     GrowBuf upd_in;                      // host form's input: geo, materials, indices
+    uint32_t updates = 0;                // rtb200_scene_update_* calls so far: an adaptive render refuses to step across one
+    // ---- adaptive rendering (rtb200_adaptive_*, DESIGN.md §4.9): one device block allocated at the first begin ----
+    struct Adaptive {
+        void* mem = nullptr;             // sum, sq, count, keep, list[2], list_n[2], cub's scratch
+        float* sum = nullptr;            // [npix_local][3] S_c
+        float* sq = nullptr;             // [npix_local][3] Q_c
+        uint32_t* count = nullptr;       // [npix_local] n
+        uint32_t* keep = nullptr;        // [npix_local] by list position
+        uint32_t* list[2] = {nullptr, nullptr};   // the list of the next round is list[cur], its length list_n[cur]
+        uint32_t* list_n = nullptr;
+        void* temp = nullptr;
+        size_t temp_bytes = 0;
+        uint32_t* active_host = nullptr; // pinned: list_n of the last step
+        bool begun = false;              // false before the first begin and after a step that failed part-way
+        rt_adaptive_params p{};
+        uint32_t N = 0;                  // max_samples resolved
+        uint32_t n = 0;                  // samples every listed pixel has
+        uint32_t cur = 0;
+        uint32_t active = 0;             // pixels on the list after the last step
+        uint32_t updates = 0;            // `updates` at begin
+    } ad;
 };
 
 // Releases a scene handle on scope exit; the error that made the scope return early survives the release.
@@ -305,6 +326,8 @@ int rtb200_scene_release(rtb200_scene_handle h) {
         if (h->refit) cudaFree(h->refit);
         if (h->rebuild) cudaFree(h->rebuild);
         if (h->upd_in.p) cudaFree(h->upd_in.p);
+        if (h->ad.mem) cudaFree(h->ad.mem);
+        if (h->ad.active_host) cudaFreeHost(h->ad.active_host);
         for (cudaEvent_t e : h->ev) h->ctx->event_pool.push_back(e);
         if (h->arena) {
             auto& cache = h->ctx->arena_cache;
@@ -480,8 +503,8 @@ static int scene_upload_records(const rt_scene* s, const rt_options& opts, uint3
     // records, bit1 geo, bit2 mat): for these small, hot arrays a larger L1 beats the staging (DESIGN.md §4.5).
     const char* es = getenv("RTB200_WF_SMEM");
     tp.scene_in_smem = es ? (uint32_t)atoi(es) : 0u;
-    h->smem = wavefront_smem_bytes(tp, h->mode, tp.scene_in_smem, false);
-    const int occ = occupancy(ctx, h->mode, n_lights > 0, false, h->smem);
+    h->smem = wavefront_smem_bytes(tp, h->mode, tp.scene_in_smem, Q_SINGLE);
+    const int occ = occupancy(ctx, h->mode, n_lights > 0, Q_SINGLE, h->smem);
     if (occ <= 0) return fail(RT_ERR_UNSUPPORTED, "no launch configuration fits shared memory");
     h->ctas_per_sm = occ;
     h->grid = ctx->sm_count * occ;
@@ -523,7 +546,7 @@ int rtb200_scene_kernel_info(rtb200_scene_handle h, rt_kernel_info* out) {
     CU(cudaSetDevice(h->device));
     memset(out, 0, sizeof *out);
     KernelInfo ki{};
-    CU(wavefront_info(h->mode, h->tp.n_lights > 0, false, &ki));
+    CU(wavefront_info(h->mode, h->tp.n_lights > 0, Q_SINGLE, &ki));
     out->registers = ki.registers; out->local_bytes = ki.local_bytes; out->smem_bytes = (uint32_t)h->smem; out->grid = (uint32_t)h->grid;
     out->block = (uint32_t)kBlock; out->pool_slots = (uint32_t)kBlock;
     out->ctas_per_sm = (uint32_t)h->ctas_per_sm; out->smem_mask = h->tp.scene_in_smem;
@@ -612,20 +635,67 @@ static cudaError_t scene_stream(rtb200_scene_handle h, void* stream_in, cudaStre
     return h->updated ? cudaStreamWaitEvent(st, h->updated, 0) : cudaSuccess;
 }
 
+// ---- submissions: what one call enqueues on one stream with one work set, reported by render_collect ----
+// A submission of h on `stream_in` (NULL: the context's stream) with work set `set` starts after the previous submission that
+// took the same set, on any stream and of any handle, has finished with it; the caller holds the context's lock.
+// submission_open picks the stream, submission_start sizes the set's buffers (prepare_work) and orders the stream after the
+// set's last user, submission_events takes sub->n_ev timing events (begin, end, a pair per trace launch), clears the stat
+// block and the sub->batches queue counters and records the begin event, submission_close records the end event, snapshots
+// the stat block and appends the submission to h->pending. A submission that fails part-way is not recorded.
+static int submission_open(rtb200_scene_handle h, void* stream_in, uint32_t frames, cudaStream_t* st, rtb200_scene_t::Submission* sub) {
+    if (h->pending.size() >= kMaxPending) return fail(RT_ERR_INVALID, "more than 64 frames enqueued without rtb200_render_device_wait");
+    CU(cudaSetDevice(h->device));
+    CU(scene_stream(h, stream_in, st));
+    const rtb200_scene_t::Submission* prev = h->pending.empty() ? nullptr : &h->pending.back();
+    *sub = rtb200_scene_t::Submission{*st, prev ? prev->ev0 + prev->n_ev : 0u, 0, frames, 0, 0, h->grid, 0, 0};
+    return RT_OK;
+}
+
+static int submission_start(DeviceCtx::WorkSet& W, cudaStream_t st, TraceParams& tp, const rtb200_scene_t::Submission& sub,
+                            uint32_t max_depth, size_t samplebuf_bytes) {
+    const uint32_t threads_total = (uint32_t)sub.grid * (uint32_t)kBlock;   // ray slots of the widest grid: columns of the per-slot global arrays
+    int rc = prepare_work(W, tp, threads_total, max_depth, samplebuf_bytes, sub.batches);
+    if (rc != RT_OK) return rc;
+    CU(cudaStreamWaitEvent(st, W.done, 0));   // nothing below touches the set before its previous submission is done with it
+    return RT_OK;
+}
+
+static int submission_events(rtb200_scene_handle h, DeviceCtx::WorkSet& W, cudaStream_t st, rtb200_scene_t::Submission& sub,
+                             cudaEvent_t** ev_out) {
+    DeviceCtx* ctx = h->ctx;
+    sub.n_ev = 2 + 2 * sub.batches;
+    while (h->ev.size() < (size_t)sub.ev0 + sub.n_ev) {
+        cudaEvent_t e;
+        if (!ctx->event_pool.empty()) { e = ctx->event_pool.back(); ctx->event_pool.pop_back(); }
+        else CU(cudaEventCreate(&e));
+        h->ev.push_back(e);
+    }
+    cudaEvent_t* ev = h->ev.data() + sub.ev0;
+    int rc = clear_stats(W, sub.batches, st);
+    if (rc != RT_OK) return rc;
+    CU(cudaEventRecord(ev[0], st));
+    *ev_out = ev;
+    return RT_OK;
+}
+
+static int submission_close(rtb200_scene_handle h, DeviceCtx::WorkSet& W, cudaStream_t st, const rtb200_scene_t::Submission& sub) {
+    CU(cudaEventRecord(h->ev[sub.ev0 + 1], st));
+    CU(cudaMemcpyAsync(h->stat_snap + h->pending.size() * (kStatBytes / 8), W.small.p, kStatBytes, cudaMemcpyDeviceToDevice, st));
+    CU(cudaEventRecord(W.done, st));
+    h->pending.push_back(sub);
+    return RT_OK;
+}
+
 // Enqueue frames[0, n) of h on `stream_in` (NULL: the context's stream) with work set `set`, without waiting, and append the
 // submission to h->pending; the caller holds the context's lock. Frame i goes to output slice i (rows * width * 3 elements).
-// The submission starts after the previous one that took the same set, on any stream and of any handle, has finished with it.
-// A submission that fails part-way is not recorded.
 static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_t n, void* dev_rgb8, void* dev_linear_f32,
                           void* stream_in, int set) {
-    if (h->pending.size() >= kMaxPending) return fail(RT_ERR_INVALID, "more than 64 frames enqueued without rtb200_render_device_wait");
     DeviceCtx* ctx = h->ctx;
     DeviceCtx::WorkSet& W = ctx->ws[set];
-    CU(cudaSetDevice(h->device));
     cudaStream_t st;
-    CU(scene_stream(h, stream_in, &st));
-    const rtb200_scene_t::Submission* prev = h->pending.empty() ? nullptr : &h->pending.back();
-    rtb200_scene_t::Submission sub{st, prev ? prev->ev0 + prev->n_ev : 0u, 0, n, 0, 0, h->grid, 0, 0};
+    rtb200_scene_t::Submission sub;
+    int rc = submission_open(h, stream_in, n, &st, &sub);
+    if (rc != RT_OK) return rc;
     TraceParams tp = h->tp;   // the handle's own view stays as uploaded
     const uint64_t npl = tp.npix_local;
     if (npl == 0) { h->pending.push_back(sub); return RT_OK; }   // a shard with no rows: nothing to trace
@@ -647,17 +717,14 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
         sbuf = std::max(sbuf, (size_t)g.count * spb * npl * 16);
         max_depth = std::max(max_depth, frames[g.first].max_depth);
         if (g.count > 1 && grid_f == 0) {
-            smem_f = wavefront_smem_bytes(tp, h->mode, tp.scene_in_smem, true);
-            const int occ = occupancy(ctx, h->mode, tp.n_lights > 0, true, smem_f);
+            smem_f = wavefront_smem_bytes(tp, h->mode, tp.scene_in_smem, Q_FRAMES);
+            const int occ = occupancy(ctx, h->mode, tp.n_lights > 0, Q_FRAMES, smem_f);
             if (occ <= 0) return fail(RT_ERR_UNSUPPORTED, "no launch configuration of the multi-frame trace kernel fits shared memory");
             grid_f = ctx->sm_count * occ;
         }
     }
     sub.grid = std::max(h->grid, grid_f);
-    const uint32_t threads_total = (uint32_t)sub.grid * (uint32_t)kBlock;   // ray slots of the widest grid: columns of the per-slot global arrays
-    int rc = prepare_work(W, tp, threads_total, max_depth, sbuf, sub.batches);
-    if (rc != RT_OK) return rc;
-    CU(cudaStreamWaitEvent(st, W.done, 0));   // nothing below touches the set before its previous submission is done with it
+    if ((rc = submission_start(W, st, tp, sub, max_depth, sbuf)) != RT_OK) return rc;
     if (grid_f) {   // the multi-frame kernel reads each frame's camera and key from this table
         std::vector<FrameRec> tab(n);
         for (uint32_t i = 0; i < n; ++i) {
@@ -667,18 +734,10 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
         CU(W.ftab.ensure(sub.ftab_bytes, W.done));
         CU(cudaMemcpyAsync(W.ftab.p, tab.data(), sub.ftab_bytes, cudaMemcpyHostToDevice, st));
     }
-    sub.n_ev = 2 + 2 * sub.batches;
-    while (h->ev.size() < (size_t)sub.ev0 + sub.n_ev) {
-        cudaEvent_t e;
-        if (!ctx->event_pool.empty()) { e = ctx->event_pool.back(); ctx->event_pool.pop_back(); }
-        else CU(cudaEventCreate(&e));
-        h->ev.push_back(e);
-    }
-    cudaEvent_t* ev = h->ev.data() + sub.ev0;
+    cudaEvent_t* ev = nullptr;
+    if ((rc = submission_events(h, W, st, sub, &ev)) != RT_OK) return rc;
     unsigned int* counters = (unsigned int*)((char*)W.small.p + kStatBytes);
-    if ((rc = clear_stats(W, sub.batches, st)) != RT_OK) return rc;
 
-    CU(cudaEventRecord(ev[0], st));
     uint32_t b = 0;   // trace launch (or black memset) index: its queue counter and its event pair
     for (const FrameGroup& g : groups) {
         const rt_frame& f0 = frames[g.first];
@@ -702,7 +761,7 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
             if (q.max_depth == 0) {
                 CU(cudaMemsetAsync(q.samplebuf, 0, (size_t)q.total_work * 16, st));   // ray_color(depth 0) = black, no ray (raytracer.rs:80-82)
             } else {
-                CU(launch_wavefront(q, h->mode, multi, grid, smem, st));
+                CU(launch_wavefront(q, h->mode, multi ? Q_FRAMES : Q_SINGLE, grid, smem, st));
             }
             CU(cudaEventRecord(ev[3 + 2 * b], st));
             for (uint32_t j = 0; j < g.count; ++j) {   // samplebuf [frame][sample][pixel]
@@ -716,11 +775,7 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
         sub.launches += batches * (1 + g.count);
         if (q.max_depth == 0) sub.black_samples += g.count * frame_work;
     }
-    CU(cudaEventRecord(ev[1], st));
-    CU(cudaMemcpyAsync(h->stat_snap + h->pending.size() * (kStatBytes / 8), W.small.p, kStatBytes, cudaMemcpyDeviceToDevice, st));
-    CU(cudaEventRecord(W.done, st));
-    h->pending.push_back(sub);
-    return RT_OK;
+    return submission_close(h, W, st, sub);
 }
 
 // RTB200_PRINT_TAIL / RTB200_PRINT_PHASES: the frame-tail and phase-clock counters of a stat block (stderr)
@@ -908,6 +963,7 @@ int rtb200_scene_update_spheres(rtb200_scene_handle h, const uint32_t* index, co
     DeviceCtx* ctx = h->ctx;
     std::lock_guard<std::recursive_mutex> lk(ctx->mu);
     CU(cudaSetDevice(h->device));
+    ++h->updates;
     cudaStream_t st;   // after the previous update too: it may still read upd_in
     CU(scene_stream(h, stream_in, &st));
     CU(update_begin(h));
@@ -948,6 +1004,7 @@ int rtb200_scene_update_geometry_device(rtb200_scene_handle h, const void* dev_c
     if (!((a.type == cudaMemoryTypeDevice && a.device == h->device) || a.type == cudaMemoryTypeManaged))
         return fail(RT_ERR_INVALID, "dev_center_radius is not device or managed memory of device " + std::to_string(h->device));
     if (h->tp.n == 0) return RT_OK;
+    ++h->updates;
     cudaStream_t st;
     CU(scene_stream(h, stream_in, &st));
     CU(update_begin(h));
@@ -1045,6 +1102,201 @@ int rtb200_scene_rebuild(rtb200_scene_handle h, void* stream_in) {
     h->level_off = level_off;
     h->level_nodes.clear();
     h->node_box = b.node_box; h->leaf_box = b.leaf_box; h->level_nodes_dev = b.level_nodes;
+    return RT_OK;
+  });
+}
+
+// ---- adaptive rendering (DESIGN.md §4.9) ----
+// The checks of rt_adaptive_params for a shard of npix_local pixels and a sample-buffer cap of `cap` bytes (no device is touched).
+static int check_adaptive(const rt_adaptive_params* p, uint64_t npix_local, uint64_t cap) {
+    if (!p) return fail(RT_ERR_INVALID, "null adaptive params");
+    if (p->samples_per_round == 0) return fail(RT_ERR_INVALID, "samples_per_round must be > 0");
+    if (p->min_samples == 0) return fail(RT_ERR_INVALID, "min_samples must be > 0");
+    if (p->reserved != 0) return fail(RT_ERR_INVALID, "rt_adaptive_params.reserved must be 0");
+    if (std::isnan(p->abs_tol) || std::isnan(p->rel_tol)) return fail(RT_ERR_INVALID, "abs_tol and rel_tol must not be NaN");
+    const uint64_t work = (uint64_t)p->samples_per_round * npix_local;
+    if (work >= (1ull << 31)) return fail(RT_ERR_INVALID, "samples_per_round * pixels must be below 2^31 (u32 work ids of a round)");
+    if (work * 16 > cap) return fail(RT_ERR_INVALID, "samples_per_round * pixels * 16 bytes exceed the sample-buffer cap (rt_options.sample_buffer_bytes)");
+    return RT_OK;
+}
+
+int rtb200_adaptive_begin(rtb200_scene_handle h, const rt_adaptive_params* p, void* stream_in) {
+  return guarded([&]() -> int {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    const uint32_t npl = h->tp.npix_local;
+    int rc = check_adaptive(p, npl, sample_buffer_cap(h->opts));
+    if (rc != RT_OK) return rc;
+    DeviceRestore restore;
+    std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
+    CU(cudaSetDevice(h->device));
+    auto& A = h->ad;
+    A.begun = false;
+    if (!A.mem && npl) {
+        auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+        const size_t b3 = al((size_t)npl * 12), b1 = al((size_t)npl * 4), temp = adaptive_compact_bytes(npl);
+        const size_t bytes = 2 * b3 + 4 * b1 + 256 + temp;
+        void* m = nullptr;
+        cudaError_t e = cudaMalloc(&m, bytes);
+        if (e != cudaSuccess) { cudaGetLastError(); return fail(RT_ERR_OOM, "adaptive: cannot allocate " + std::to_string(bytes) + " bytes of device memory"); }
+        e = cudaHostAlloc((void**)&A.active_host, 4, cudaHostAllocDefault);
+        if (e != cudaSuccess) { cudaFree(m); A.active_host = nullptr; return fail_cuda(e, "cudaHostAlloc"); }
+        char* c = (char*)m;
+        A.mem = m;
+        A.sum = (float*)c; c += b3;
+        A.sq = (float*)c; c += b3;
+        A.count = (uint32_t*)c; c += b1;   // sum, sq and count are contiguous: one memset clears them
+        A.keep = (uint32_t*)c; c += b1;
+        A.list[0] = (uint32_t*)c; c += b1;
+        A.list[1] = (uint32_t*)c; c += b1;
+        A.list_n = (uint32_t*)c; c += 256;
+        A.temp = c; A.temp_bytes = temp;
+    }
+    cudaStream_t st;
+    CU(scene_stream(h, stream_in, &st));
+    if (npl) {
+        CU(cudaMemsetAsync(A.sum, 0, (char*)A.keep - (char*)A.sum, st));
+        CU(launch_adaptive_list(A.list[0], A.list_n, npl, st));
+        CU(cudaStreamSynchronize(st));
+    }
+    A.p = *p;
+    A.N = p->max_samples ? p->max_samples : h->tp.spp;
+    A.n = 0; A.cur = 0; A.active = npl; A.updates = h->updates;
+    A.begun = true;
+    return RT_OK;
+  });
+}
+
+// One submission of `rounds` rounds (DESIGN.md §4.9): per round a Q_LIST trace launch (a black memset at max_depth 0), the
+// accumulate-and-test and the compaction into the other list buffer; then the active count is copied out and collected.
+int rtb200_adaptive_step(rtb200_scene_handle h, uint32_t rounds, void* stream_in, uint32_t* active_out, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (stats) memset(stats, 0, sizeof *stats);
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    auto& A = h->ad;
+    if (!A.begun) return fail(RT_ERR_INVALID, "no adaptive render on this handle: call rtb200_adaptive_begin");
+    if (A.updates != h->updates) return fail(RT_ERR_INVALID, "the scene was updated since rtb200_adaptive_begin: the sums would mix two scenes (begin again)");
+    auto wall0 = std::chrono::steady_clock::now();
+    const uint32_t m = A.p.samples_per_round;
+    const uint64_t left = A.active && A.n < A.N ? ((uint64_t)A.N - A.n + m - 1) / m : 0;   // rounds until every pixel has N
+    rounds = (uint32_t)std::min<uint64_t>(rounds, left);
+    if (active_out) *active_out = A.active;
+    if (rounds == 0) return RT_OK;   // finished: nothing to do
+    DeviceRestore restore;
+    DeviceCtx* ctx = h->ctx;
+    std::lock_guard<std::recursive_mutex> lk(ctx->mu);
+    int rc = render_collect(h, nullptr);   // the handle's asynchronous frames first, like a blocking render
+    if (rc != RT_OK) return rc;
+    DeviceCtx::WorkSet& W = ctx->ws[0];
+    cudaStream_t st;
+    rtb200_scene_t::Submission sub;
+    if ((rc = submission_open(h, stream_in, 1, &st, &sub)) != RT_OK) return rc;
+    TraceParams tp = h->tp;
+    const uint32_t npl = tp.npix_local;
+    const size_t smem = wavefront_smem_bytes(tp, h->mode, tp.scene_in_smem, Q_LIST);
+    const int occ = occupancy(ctx, h->mode, tp.n_lights > 0, Q_LIST, smem);
+    if (occ <= 0) return fail(RT_ERR_UNSUPPORTED, "no launch configuration of the list trace kernel fits shared memory");
+    const int grid = ctx->sm_count * occ;
+    sub.grid = grid;
+    sub.batches = rounds;
+    if ((rc = submission_start(W, st, tp, sub, tp.max_depth, (size_t)m * npl * 16)) != RT_OK) return rc;
+    cudaEvent_t* ev = nullptr;
+    if ((rc = submission_events(h, W, st, sub, &ev)) != RT_OK) return rc;
+    unsigned int* counters = (unsigned int*)((char*)W.small.p + kStatBytes);
+    const bool black = tp.max_depth == 0;
+    A.begun = false;   // until the rounds are enqueued: a step that fails part-way leaves the state unusable
+    for (uint32_t r = 0; r < rounds; ++r) {
+        TraceParams q = tp;
+        q.s0 = A.n;
+        q.s_count = std::min(m, A.N - A.n);
+        q.total_work = 0;   // Q_LIST: n_list * s_count, n_list read on the device
+        q.work_counter = counters + r;
+        q.stack_stride = (uint32_t)grid * (uint32_t)kBlock;
+        q.list = A.list[A.cur]; q.list_n = A.list_n + A.cur;
+        CU(cudaEventRecord(ev[2 + 2 * r], st));
+        if (black) CU(cudaMemsetAsync(q.samplebuf, 0, (size_t)q.s_count * npl * 16, st));   // ray_color(depth 0) = black, no ray
+        else CU(launch_wavefront(q, h->mode, Q_LIST, grid, smem, st));
+        CU(cudaEventRecord(ev[3 + 2 * r], st));
+        AdaptiveParams a{};
+        a.samplebuf = q.samplebuf; a.list = q.list; a.list_n = q.list_n;
+        a.sum = A.sum; a.sq = A.sq; a.count = A.count; a.keep = A.keep;
+        a.black_samples = black ? tp.stat + 3 : nullptr;
+        a.npix_local = npl; a.s_count = q.s_count; a.n_after = A.n + q.s_count;
+        a.max_samples = A.N; a.min_samples = A.p.min_samples; a.abs_tol = A.p.abs_tol; a.rel_tol = A.p.rel_tol;
+        CU(launch_adaptive_accumulate(a, st));
+        CU(launch_adaptive_compact(A.temp, A.temp_bytes, A.list[A.cur], A.keep, A.list[A.cur ^ 1u], A.list_n + (A.cur ^ 1u), npl, st));
+        A.cur ^= 1u;
+        A.n += q.s_count;
+        sub.launches += 3;   // trace (or black memset), accumulate, compaction
+    }
+    CU(cudaMemcpyAsync(A.active_host, A.list_n + A.cur, 4, cudaMemcpyDeviceToHost, st));
+    if ((rc = submission_close(h, W, st, sub)) != RT_OK) return rc;
+    if ((rc = render_collect(h, stats)) != RT_OK) return rc;
+    A.active = *A.active_host;
+    A.begun = true;
+    if (active_out) *active_out = A.active;
+    if (stats) stats->wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count();
+    return RT_OK;
+  });
+}
+
+int rtb200_adaptive_resolve(rtb200_scene_handle h, void* dev_rgb8, void* dev_linear_f32, void* dev_counts_u32, void* stream_in) {
+  return guarded([&]() -> int {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    if (!h->ad.begun) return fail(RT_ERR_INVALID, "no adaptive render on this handle: call rtb200_adaptive_begin");
+    if (h->tp.npix_local == 0 || (!dev_rgb8 && !dev_linear_f32 && !dev_counts_u32)) return RT_OK;
+    DeviceRestore restore;
+    std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
+    CU(cudaSetDevice(h->device));
+    cudaStream_t st;
+    CU(scene_stream(h, stream_in, &st));
+    AdaptiveResolveParams r{};
+    r.sum = h->ad.sum; r.count = h->ad.count; r.npix_local = h->tp.npix_local;
+    r.out_linear = (float*)dev_linear_f32; r.out_rgb8 = (uint8_t*)dev_rgb8; r.out_count = (uint32_t*)dev_counts_u32;
+    CU(launch_adaptive_resolve(r, st));
+    CU(cudaStreamSynchronize(st));
+    return RT_OK;
+  });
+}
+
+int rtb200_render_adaptive(const rt_scene* s, const rt_options* opts_in, const rt_adaptive_params* p, uint8_t* out_rgb8,
+                           float* out_lin, uint32_t* out_counts, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (!s) return fail(RT_ERR_INVALID, "null argument");
+    rt_options opts;
+    int rc = normalise_options(opts_in, &opts);
+    if (rc != RT_OK) return rc;
+    uint32_t n_lights = 0;
+    if ((rc = validate_scene(s, &n_lights)) != RT_OK) return rc;
+    const uint64_t npl = (uint64_t)rtb200_shard_rows(s->height, opts.rank, opts.world, opts.band_rows) * s->width;
+    if ((rc = check_adaptive(p, npl, sample_buffer_cap(opts))) != RT_OK) return rc;
+    auto wall0 = std::chrono::steady_clock::now();
+    DeviceRestore restore;
+    rtb200_scene_handle h = nullptr;
+    if ((rc = rtb200_scene_upload(s, &opts, &h)) != RT_OK) return rc;
+    ReleaseGuard rel{h};
+    DeviceCtx* ctx = h->ctx;
+    std::lock_guard<std::recursive_mutex> lk(ctx->mu);
+    CU(cudaSetDevice(h->device));
+    rt_stats st{};
+    uint32_t active = 0;
+    if ((rc = rtb200_adaptive_begin(h, p, nullptr)) != RT_OK) return rc;
+    if ((rc = rtb200_adaptive_step(h, 0xffffffffu, nullptr, &active, &st)) != RT_OK) return rc;
+    void *d8 = nullptr, *dl = nullptr, *dc = nullptr;
+    if (out_rgb8) { CU(ctx->out_rgb8.ensure(npl * 3 + 16)); d8 = ctx->out_rgb8.p; }
+    if (out_lin) { CU(ctx->out_lin.ensure(npl * 12 + 16)); dl = ctx->out_lin.p; }
+    if (out_counts) { CU(ctx->out_cnt.ensure(npl * 4 + 16)); dc = ctx->out_cnt.p; }
+    if ((rc = rtb200_adaptive_resolve(h, d8, dl, dc, nullptr)) != RT_OK) return rc;
+    if (npl) {
+        if (out_rgb8) CU(cudaMemcpyAsync(out_rgb8, d8, npl * 3, cudaMemcpyDeviceToHost, ctx->stream));
+        if (out_lin) CU(cudaMemcpyAsync(out_lin, dl, npl * 12, cudaMemcpyDeviceToHost, ctx->stream));
+        if (out_counts) CU(cudaMemcpyAsync(out_counts, dc, npl * 4, cudaMemcpyDeviceToHost, ctx->stream));
+        CU(cudaStreamSynchronize(ctx->stream));
+    }
+    st.frames = 1;
+    st.h2d_bytes += h->h2d_bytes;
+    st.d2h_bytes = (out_rgb8 ? npl * 3 : 0) + (out_lin ? npl * 12 : 0) + (out_counts ? npl * 4 : 0) + 128 + 16 + 4;
+    st.wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count();
+    if (stats) *stats = st;
     return RT_OK;
   });
 }

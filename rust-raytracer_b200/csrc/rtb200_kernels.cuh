@@ -54,8 +54,11 @@ struct ShadowFrame {
 static_assert(sizeof(ShadowFrame) == 88, "ShadowFrame layout");
 
 enum TraceMode : uint32_t { MODE_TREE = 0, MODE_BRUTE = 1, MODE_EXACT = 2 };
+// The work queue of a trace launch: every pixel of one frame, every pixel of several frames (TraceParams::ftab), or the
+// pixels of an adaptive render's list (TraceParams::list, DESIGN.md §4.9)
+enum TraceQueue : uint32_t { Q_SINGLE = 0, Q_FRAMES = 1, Q_LIST = 2 };
 
-// One frame of a multi-frame launch (rt_wavefront_kernel<.., FRAMES = true>): the view and the Philox key that replace
+// One frame of a multi-frame launch (rt_wavefront_kernel<.., Q_FRAMES>): the view and the Philox key that replace
 // TraceParams::cam / key0 / key1 for the work ids of that frame.
 struct FrameRec { rt_camera cam; uint32_t key0, key1; };
 static_assert(sizeof(FrameRec) == 104, "FrameRec layout");
@@ -104,6 +107,30 @@ struct TraceParams {
     // 1: a Lambertian or Metal sphere has, or once had, an infinite or NaN albedo component. A black path then has to unwind
     // its albedo stack, and a nested shadow vertex has to read its albedo, because albedo * 0 is NaN for such an albedo.
     uint32_t albedo_nonfinite;
+    // ---- Q_LIST launches only (appended after albedo_nonfinite) ----
+    const uint32_t* list;        // local pixel indices, increasing; samplebuf is [s_count][n_list]
+    const uint32_t* list_n;      // device: n_list, read once at kernel start; total_work = n_list * s_count
+};
+
+// An adaptive round's accumulate-and-test (rtb200_adaptive.cu, DESIGN.md §4.9): one thread per list position.
+struct AdaptiveParams {
+    const float4* samplebuf;     // [s_count][n_list] the round's samples
+    const uint32_t* list;        // [n_list] local pixel indices
+    const uint32_t* list_n;      // device: n_list
+    float* sum;                  // [npix_local][3] S_c, f32 in sample order
+    float* sq;                   // [npix_local][3] Q_c
+    uint32_t* count;             // [npix_local] n
+    uint32_t* keep;              // [npix_local] by list position: 1 = the pixel stays on the list (0 past n_list)
+    unsigned long long* black_samples;   // max_depth 0 rounds: stat[3], which no trace kernel counts; else null
+    uint32_t npix_local, s_count;
+    uint32_t n_after;            // samples of every listed pixel after the round
+    uint32_t max_samples, min_samples;
+    float abs_tol, rel_tol;
+};
+struct AdaptiveResolveParams {
+    const float* sum; const uint32_t* count;
+    uint32_t npix_local;
+    float* out_linear; uint8_t* out_rgb8; uint32_t* out_count;   // each may be null
 };
 
 struct ResolveParams {
@@ -157,12 +184,20 @@ struct RebuildBufs {
 
 struct KernelInfo { int registers, max_threads, const_bytes, local_bytes; char name[96]; };
 
-// `frames`: the multi-frame kernel (work ids span p.ftab's frames) instead of the single-frame one
-size_t wavefront_smem_bytes(const TraceParams& p, uint32_t mode, uint32_t smem_mask, bool frames);
-cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, bool frames, int grid, size_t smem, cudaStream_t st);
-int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, bool frames, size_t smem);   // 0 when the kernel cannot run on the current device
-cudaError_t wavefront_info(uint32_t mode, bool lights, bool frames, KernelInfo* out);
+// `queue` (TraceQueue): Q_FRAMES is the multi-frame kernel (work ids span p.ftab's frames), Q_LIST the adaptive round's
+size_t wavefront_smem_bytes(const TraceParams& p, uint32_t mode, uint32_t smem_mask, uint32_t queue);
+cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, uint32_t queue, int grid, size_t smem, cudaStream_t st);
+int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, uint32_t queue, size_t smem);   // 0 when the kernel cannot run on the current device
+cudaError_t wavefront_info(uint32_t mode, bool lights, uint32_t queue, KernelInfo* out);
 cudaError_t launch_resolve(const ResolveParams& p, cudaStream_t st);
+// adaptive rendering (rtb200_adaptive.cu): the round's accumulate-and-test, the list compaction (cub::DeviceSelect::Flagged,
+// keep[0, npix_local) over list_in, the count to *list_n_out), and the resolve
+cudaError_t launch_adaptive_list(uint32_t* list, uint32_t* list_n, uint32_t npix_local, cudaStream_t st);   // list = 0, 1, .., npix_local - 1
+cudaError_t launch_adaptive_accumulate(const AdaptiveParams& p, cudaStream_t st);
+size_t adaptive_compact_bytes(uint32_t npix_local);   // cub's temporary storage
+cudaError_t launch_adaptive_compact(void* temp, size_t temp_bytes, const uint32_t* list_in, const uint32_t* keep, uint32_t* list_out,
+                                    uint32_t* list_n_out, uint32_t npix_local, cudaStream_t st);
+cudaError_t launch_adaptive_resolve(const AdaptiveResolveParams& p, cudaStream_t st);
 // geo[idx[k]] = geo_in[k], mat[idx[k]] = mat_in[k] for k < n (idx has no repeats)
 cudaError_t launch_update_scatter(const uint32_t* idx, const double4* geo_in, const DevMat* mat_in, uint32_t n, double4* geo, DevMat* mat,
                                   cudaStream_t st);

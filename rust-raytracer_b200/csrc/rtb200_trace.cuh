@@ -447,9 +447,13 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
 // dry. Returns true when the slot received a new primary ray. raytracer.rs:199-201 + camera.rs:79-84.
 // FRAMES: the queue spans several frames, frame outermost; the frame's camera and key come from p.ftab (read once per
 // sample, off the bounce loop) and the frame is kept in Pool.frm for the shade stage's draws.
+// Q_LIST: the queue spans samples [s0, s0 + s_count) of the n_list pixels p.list[0, n_list) (an adaptive round, DESIGN.md
+// §4.9); n_list is read from p.list_n once per launch by the caller.
 // =====================================================================================================================
-template <bool LIGHTS, bool FRAMES>
-RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint32_t s, int lane, bool& exhausted, Stats& st) {
+template <bool LIGHTS, uint32_t QUEUE>
+RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint32_t s, int lane, bool& exhausted, Stats& st,
+                            uint32_t n_list = 0u) {
+    constexpr bool FRAMES = QUEUE == Q_FRAMES;
     const unsigned FULL = 0xffffffffu;
     want = want && !exhausted;
     unsigned need = __ballot_sync(FULL, want);
@@ -458,10 +462,10 @@ RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint
     unsigned base = 0;
     if (lane == leader) base = atomicAdd(p.work_counter, (unsigned)__popc(need));
     base = __shfl_sync(FULL, base, leader);
-    if (base + (unsigned)__popc(need) >= p.total_work) exhausted = true;
+    if (base + (unsigned)__popc(need) >= (QUEUE == Q_LIST ? n_list * p.s_count : p.total_work)) exhausted = true;
     if (!want) return false;
     unsigned my = base + __popc(need & ((1u << lane) - 1u));
-    if (my >= p.total_work) return false;
+    if (my >= (QUEUE == Q_LIST ? n_list * p.s_count : p.total_work)) return false;
     uint32_t f = 0u, k0 = p.key0, k1 = p.key1;
     if constexpr (FRAMES) { f = my / p.frame_work; my -= f * p.frame_work; k0 = p.ftab[f].key0; k1 = p.ftab[f].key1; }
     // Order of the global queue: image rows from the BOTTOM up, all samples of a row before the next row, x innermost.
@@ -469,10 +473,23 @@ RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint
     // sky, one ray per sample - so that the stragglers of the last expensive rows finish under the cover of cheap work
     // instead of holding nearly empty CTAs for ~50 iterations after the queue ran dry (DESIGN.md §5: 0.5 ms per launch).
     // The (pixel, sample) -> RNG stream and the samplebuf index do not depend on the order.
-    const uint32_t x = my % p.width, t_ = my / p.width;
-    const uint32_t s_local = t_ % p.s_count, rr = t_ / p.s_count;
-    const uint32_t y_local = p.rows_local - 1u - rr;
-    const uint32_t lp = y_local * p.width + x;
+    // Q_LIST: the list is in increasing pixel order and is handed out from its end, so bottom rows go first here too; the
+    // samples of one pixel are consecutive work ids.
+    uint32_t x, s_local, y_local, lp, k_list = 0u;
+    if constexpr (QUEUE == Q_LIST) {
+        s_local = my % p.s_count;
+        k_list = n_list - 1u - my / p.s_count;
+        lp = p.list[k_list];
+        y_local = lp / p.width;
+        x = lp - y_local * p.width;
+    } else {
+        x = my % p.width;
+        const uint32_t t_ = my / p.width;
+        s_local = t_ % p.s_count;
+        const uint32_t rr = t_ / p.s_count;
+        y_local = p.rows_local - 1u - rr;
+        lp = y_local * p.width + x;
+    }
     uint32_t band = y_local / p.band_rows;
     uint32_t y = (band * (uint32_t)p.world + (uint32_t)p.rank) * p.band_rows + (y_local - band * p.band_rows);
     Rng rng; rng_init(rng, y * p.width + x, p.s0 + s_local);
@@ -484,8 +501,9 @@ RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint
     if constexpr (FRAMES) get_ray(p.ftab[f].cam, u, v, o, d);
     else get_ray(p.cam, u, v, o, d);
     P.ox[s] = o.x; P.oy[s] = o.y; P.oz[s] = o.z; P.dx[s] = d.x; P.dy[s] = d.y; P.dz[s] = d.z;
-    // samplebuf index [sample][pixel], or [frame][sample][pixel]
+    // samplebuf index [sample][pixel], [frame][sample][pixel], or [sample][list position] (Q_LIST)
     if constexpr (FRAMES) { P.work[s] = (f * p.s_count + s_local) * p.npix_local + lp; P.frm[s] = f; }
+    else if constexpr (QUEUE == Q_LIST) P.work[s] = s_local * n_list + k_list;
     else P.work[s] = s_local * p.npix_local + lp;
     P.pix[s] = rng.pixel; P.smp[s] = rng.sample;
     P.blk[s] = (rng.blk << 1) | rng.has; P.clo[s] = rng.c_lo; P.chi[s] = rng.c_hi;

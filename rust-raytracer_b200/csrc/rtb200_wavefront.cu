@@ -8,8 +8,9 @@
 //
 // The three template modes share everything but the closest-hit stage: MODE_TREE (production: BVH traversal), MODE_BRUTE
 // (RT_VARIANT_BRUTE_FORCE: linear scan with the conservative sphere test) and MODE_EXACT (RT_VARIANT_EXACT_F64: every
-// sphere in f64) - the last two validate the first. Each mode has a single-frame kernel and a multi-frame one (FRAMES: the
-// queue spans several frames of the scene, each with its own camera and key; rtb200_render_frames, DESIGN.md §4.6).
+// sphere in f64) - the last two validate the first. Each mode has a single-frame kernel, a multi-frame one (Q_FRAMES: the
+// queue spans several frames of the scene, each with its own camera and key; rtb200_render_frames, DESIGN.md §4.6) and a list
+// one (Q_LIST: the queue spans the pixels still on an adaptive render's list; rtb200_adaptive_step, DESIGN.md §4.9).
 #include <cstdio>
 
 #include "rtb200_trace.cuh"
@@ -51,8 +52,8 @@ __host__ __device__ inline WfSmem wf_layout(uint32_t n, uint32_t n_pairs, uint32
 
 }  // namespace
 
-size_t wavefront_smem_bytes(const TraceParams& p, uint32_t mode, uint32_t smem_mask, bool frames) {
-    return wf_layout(p.n, p.n_pairs, p.n_nodes, p.n_leaves, mode, smem_mask, frames).total;
+size_t wavefront_smem_bytes(const TraceParams& p, uint32_t mode, uint32_t smem_mask, uint32_t queue) {
+    return wf_layout(p.n, p.n_pairs, p.n_nodes, p.n_leaves, mode, smem_mask, queue == Q_FRAMES).total;
 }
 
 // CTAs per SM each kernel's register budget is built for: 3 of 256 threads for the BVH path (80 registers), 2 for the
@@ -62,9 +63,11 @@ constexpr int wf_min_blocks(uint32_t mode) {
     return n > 0 ? n : 1;
 }
 
-// FRAMES: one launch renders several frames of the scene (TraceParams::ftab / frame_work, rtb200_render_frames)
-template <uint32_t MODE, bool LIGHTS, bool FRAMES>
+// Q_FRAMES: one launch renders several frames of the scene (TraceParams::ftab / frame_work, rtb200_render_frames)
+// Q_LIST: one launch traces a round of an adaptive render (TraceParams::list / list_n, rtb200_adaptive_step)
+template <uint32_t MODE, bool LIGHTS, uint32_t QUEUE>
 __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kernel(const __grid_constant__ TraceParams p) {
+    constexpr bool FRAMES = QUEUE == Q_FRAMES;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const WfSmem L = wf_layout(p.n, p.n_pairs, p.n_nodes, p.n_leaves, MODE, p.scene_in_smem, FRAMES);
     uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw);
@@ -112,7 +115,9 @@ __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kern
     bool exhausted = false;   // warp-uniform: this warp has seen the end of the queue
     bool stamped = false;
     uint32_t dry_iters = 0;   // iterations of this CTA after it first found the global queue dry
-    regenerate_slot<LIGHTS, FRAMES>(p, P, true, (uint32_t)tid, lane, exhausted, st);   // initial fill of the pool
+    uint32_t n_list = 0u;   // Q_LIST: the pixels on the list, fixed for the launch
+    if constexpr (QUEUE == Q_LIST) n_list = *p.list_n;
+    regenerate_slot<LIGHTS, QUEUE>(p, P, true, (uint32_t)tid, lane, exhausted, st, n_list);   // initial fill of the pool
     __syncthreads();
 
 #if RT_PHASE_CLOCKS
@@ -173,7 +178,7 @@ __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kern
             if (lane == 0) { ph[PH_ITERS] += 1ull; ph[PH_SCATTERS] += (unsigned)__popc(sm); ph[PH_DEFERRED] += (unsigned)__popc(dm); }
         }
 #endif
-        regenerate_slot<LIGHTS, FRAMES>(p, P, active && done, s, lane, exhausted, st);
+        regenerate_slot<LIGHTS, QUEUE>(p, P, active && done, s, lane, exhausted, st, n_list);
         if (exhausted && !stamped) { stamped = true; if (lane == 0) atomicMin(&p.stat[9], now_ns()); }
         if (stamped) ++dry_iters;
         const bool still_alive = active && (P.lvl[s] != kDeadLevel);
@@ -194,19 +199,20 @@ __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kern
     if (tid == 0) { atomicMax(&p.stat[10], now_ns()); atomicMax(&p.stat[11], (unsigned long long)dry_iters); atomicAdd(&p.stat[12], (unsigned long long)dry_iters); }
 }
 
-template <bool FRAMES, typename F>
+template <uint32_t QUEUE, typename F>
 static auto dispatch_mode(uint32_t mode, bool lights, F&& f) {
-    if (mode == MODE_EXACT) return lights ? f(rt_wavefront_kernel<MODE_EXACT, true, FRAMES>) : f(rt_wavefront_kernel<MODE_EXACT, false, FRAMES>);
-    if (mode == MODE_BRUTE) return lights ? f(rt_wavefront_kernel<MODE_BRUTE, true, FRAMES>) : f(rt_wavefront_kernel<MODE_BRUTE, false, FRAMES>);
-    return lights ? f(rt_wavefront_kernel<MODE_TREE, true, FRAMES>) : f(rt_wavefront_kernel<MODE_TREE, false, FRAMES>);
+    if (mode == MODE_EXACT) return lights ? f(rt_wavefront_kernel<MODE_EXACT, true, QUEUE>) : f(rt_wavefront_kernel<MODE_EXACT, false, QUEUE>);
+    if (mode == MODE_BRUTE) return lights ? f(rt_wavefront_kernel<MODE_BRUTE, true, QUEUE>) : f(rt_wavefront_kernel<MODE_BRUTE, false, QUEUE>);
+    return lights ? f(rt_wavefront_kernel<MODE_TREE, true, QUEUE>) : f(rt_wavefront_kernel<MODE_TREE, false, QUEUE>);
 }
 template <typename F>
-static auto dispatch(uint32_t mode, bool lights, bool frames, F&& f) {
-    return frames ? dispatch_mode<true>(mode, lights, f) : dispatch_mode<false>(mode, lights, f);
+static auto dispatch(uint32_t mode, bool lights, uint32_t queue, F&& f) {
+    if (queue == Q_LIST) return dispatch_mode<Q_LIST>(mode, lights, f);
+    return queue == Q_FRAMES ? dispatch_mode<Q_FRAMES>(mode, lights, f) : dispatch_mode<Q_SINGLE>(mode, lights, f);
 }
 
-cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, bool frames, int grid, size_t smem, cudaStream_t st) {
-    return dispatch(mode, p.n_lights > 0, frames, [&](auto kern) -> cudaError_t {
+cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, uint32_t queue, int grid, size_t smem, cudaStream_t st) {
+    return dispatch(mode, p.n_lights > 0, queue, [&](auto kern) -> cudaError_t {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
         kern<<<grid, kBlock, smem, st>>>(p);
@@ -214,8 +220,8 @@ cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, bool frames, i
     });
 }
 
-int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, bool frames, size_t smem) {
-    return dispatch(mode, lights, frames, [&](auto kern) -> int {
+int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, uint32_t queue, size_t smem) {
+    return dispatch(mode, lights, queue, [&](auto kern) -> int {
         int nb = 0;
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return 0; }
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kBlock, smem) != cudaSuccess) { cudaGetLastError(); return 0; }
@@ -223,14 +229,15 @@ int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, bool frames, size_t sm
     });
 }
 
-cudaError_t wavefront_info(uint32_t mode, bool lights, bool frames, KernelInfo* out) {
-    return dispatch(mode, lights, frames, [&](auto kern) -> cudaError_t {
+cudaError_t wavefront_info(uint32_t mode, bool lights, uint32_t queue, KernelInfo* out) {
+    return dispatch(mode, lights, queue, [&](auto kern) -> cudaError_t {
         cudaFuncAttributes a;
         cudaError_t e = cudaFuncGetAttributes(&a, kern);
         if (e != cudaSuccess) return e;
         out->registers = a.numRegs; out->max_threads = a.maxThreadsPerBlock; out->const_bytes = (int)a.constSizeBytes; out->local_bytes = (int)a.localSizeBytes;
         snprintf(out->name, sizeof out->name, "rt_wavefront_kernel<%s,%s%s>",
-                 mode == MODE_TREE ? "MODE_TREE" : mode == MODE_BRUTE ? "MODE_BRUTE" : "MODE_EXACT", lights ? "LIGHTS" : "NO_LIGHTS", frames ? ",FRAMES" : "");
+                 mode == MODE_TREE ? "MODE_TREE" : mode == MODE_BRUTE ? "MODE_BRUTE" : "MODE_EXACT", lights ? "LIGHTS" : "NO_LIGHTS",
+                 queue == Q_FRAMES ? ",FRAMES" : queue == Q_LIST ? ",LIST" : "");
         return cudaSuccess;
     });
 }

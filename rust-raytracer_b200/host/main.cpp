@@ -7,6 +7,10 @@
 // {"camera": {<the config's camera schema>}, "seed"?: n, "max_depth"?: n}, omitted fields are the scene's, and <output_file> is a
 // prefix: frame i is written to <prefix>_{i:03}.png (the reference's commented-out per-frame name, main.rs:17). Stdout gets
 // "\nRendering <file>" per frame and one "Frames time: <ms>ms for <n> frames" line.
+// RTB200_ADAPTIVE=<rel_tol>[,<abs_tol>[,<samples_per_round>[,<min_samples>]]] renders adaptively (rtb200_render_adaptive, defaults
+// 0, 8, 16) with max_samples = the scene's samples_per_pixel: a pixel stops once its standard error is within
+// abs_tol + rel_tol * mean in every channel (DESIGN.md §4.9). Same two stdout lines; RTB200_STATS also prints the samples
+// traced out of samples_per_pixel * width * height.
 #include <chrono>
 #include <cstdio>
 #include <cstdlib>
@@ -57,6 +61,24 @@ static int render_animation(const rt_scene& s, const char* frames_path, const st
     return 0;
 }
 
+// RTB200_ADAPTIVE: the scene rendered adaptively into `pixels`
+static int render_adaptive(const rt_scene& s, const char* spec, const rt_options& opts, uint8_t* pixels, rt_stats* st) {
+    rt_adaptive_params p{8u, 0u, 16u, 0u, 0.0f, 0.0f};
+    double v[4] = {0.0, 0.0, 8.0, 16.0};
+    int k = 0;
+    for (const char* c = spec; k < 4; ++k) {
+        char* end = nullptr;
+        v[k] = strtod(c, &end);
+        if (end == c || (*end != ',' && *end != 0)) { fprintf(stderr, "RTB200_ADAPTIVE: expected <rel_tol>[,<abs_tol>[,<samples_per_round>[,<min_samples>]]], got \"%s\"\n", spec); return 101; }
+        if (*end == 0) { ++k; break; }
+        c = end + 1;
+    }
+    if (v[2] < 1 || v[3] < 1 || v[2] > 4294967295.0 || v[3] > 4294967295.0) { fprintf(stderr, "RTB200_ADAPTIVE: samples_per_round and min_samples must be positive integers\n"); return 101; }
+    p.rel_tol = (float)v[0]; p.abs_tol = (float)v[1]; p.samples_per_round = (uint32_t)v[2]; p.min_samples = (uint32_t)v[3];
+    if (rtb200_render_adaptive(&s, &opts, &p, pixels, nullptr, nullptr, st) != 0) return -1;
+    return 0;
+}
+
 int main(int argc, char** argv) {
     if (argc != 3) {                                                       // main.rs:9-12
         printf("Usage: %s <config_file> <output_file>\n", argc > 0 ? argv[0] : "raytracer");
@@ -72,6 +94,11 @@ int main(int argc, char** argv) {
         rthost::load_scene_json(ss.str(), slash == std::string::npos ? std::string(".") : path.substr(0, slash), &holder);
     } catch (const std::exception& e) { fprintf(stderr, "Unable to parse config json: %s\n", e.what()); return 101; }   // main.rs:15
     if (const char* sd = getenv("RTB200_SEED")) holder.scene.seed = strtoull(sd, nullptr, 0);
+    const char* adaptive = getenv("RTB200_ADAPTIVE");
+    if (adaptive && (getenv("RTB200_GPUS") || getenv("RTB200_FRAMES"))) {
+        fprintf(stderr, "RTB200_ADAPTIVE with RTB200_GPUS or RTB200_FRAMES is not supported: adaptive renders are one frame on one GPU\n");
+        return 101;
+    }
     if (const char* fp = getenv("RTB200_FRAMES")) return render_animation(holder.scene, fp, argv[2]);
     printf("\nRendering %s\n", argv[2]);                                  // main.rs:18
     fflush(stdout);
@@ -82,14 +109,24 @@ int main(int argc, char** argv) {
     rt_stats st{};
     auto t0 = std::chrono::steady_clock::now();                           // raytracer.rs:259
     const char* gpus = getenv("RTB200_GPUS");
-    int rc = gpus ? rtb200_render_rgb8_multi(&s, &opts, atoi(gpus), pixels.data(), &st)   // replaces raytracer.rs:260-262
+    int rc = 0;
+    if (adaptive) {
+        rc = render_adaptive(s, adaptive, opts, pixels.data(), &st);
+        if (rc == 101) return rc;
+    } else {
+        rc = gpus ? rtb200_render_rgb8_multi(&s, &opts, atoi(gpus), pixels.data(), &st)   // replaces raytracer.rs:260-262
                   : rtb200_render_rgb8(&s, &opts, pixels.data(), &st);
+    }
     if (rc != 0) { fprintf(stderr, "render failed (%d): %s\n", rc, rtb200_last_error()); return 101; }
     long long ms = std::chrono::duration_cast<std::chrono::milliseconds>(std::chrono::steady_clock::now() - t0).count();
     printf("Frame time: %lldms\n", ms);                                   // raytracer.rs:263
     if (getenv("RTB200_STATS"))
         fprintf(stderr, "rays=%llu samples=%llu device_ms=%.3f Mrays/s=%.1f gpus=%d\n", (unsigned long long)st.rays, (unsigned long long)st.samples, st.device_ms,
                 st.device_ms > 0 ? st.rays / st.device_ms / 1e3 : 0.0, (int)st.gpus_used);
+    if (adaptive && getenv("RTB200_STATS")) {
+        const unsigned long long all = (unsigned long long)s.samples_per_pixel * s.width * s.height;
+        fprintf(stderr, "adaptive: %llu of %llu samples traced (%.1f %%)\n", (unsigned long long)st.samples, all, all ? 100.0 * st.samples / all : 0.0);
+    }
     std::string err;
     if (!rthost::write_png_rgb8(argv[2], pixels.data(), s.width, s.height, &err)) { fprintf(stderr, "error writing image: %s\n", err.c_str()); return 101; }   // raytracer.rs:265
     return 0;

@@ -102,7 +102,14 @@ class rt_frame(C.Structure):
     _fields_ = [("camera", rt_camera), ("seed", C.c_uint64), ("max_depth", C.c_uint32), ("reserved", C.c_uint32)]
 
 
-assert C.sizeof(rt_sphere) == 64 and C.sizeof(rt_frame) == 112
+class rt_adaptive_params(C.Structure):
+    """Adaptive rendering (rtb200_adaptive_*): samples per round, the sample budget (0: the scene's samples_per_pixel), the
+    samples before a pixel may stop, and the f32 tolerances of the stopping rule err_c <= abs_tol + rel_tol * mean_c."""
+    _fields_ = [("samples_per_round", C.c_uint32), ("max_samples", C.c_uint32), ("min_samples", C.c_uint32), ("reserved", C.c_uint32),
+                ("abs_tol", C.c_float), ("rel_tol", C.c_float)]
+
+
+assert C.sizeof(rt_sphere) == 64 and C.sizeof(rt_frame) == 112 and C.sizeof(rt_adaptive_params) == 24
 
 # every symbol include/rtb200.h declares (tests check that the library exports all of them)
 ABI_SYMBOLS = [
@@ -115,6 +122,7 @@ ABI_SYMBOLS = [
     "rtb200_render_frames", "rtb200_render_frames_device",
     "rtb200_scene_update_spheres", "rtb200_scene_update_geometry_device", "rtb200_scene_debug_records",
     "rtb200_scene_rebuild", "rtb200_scene_debug_topology",
+    "rtb200_adaptive_begin", "rtb200_adaptive_step", "rtb200_adaptive_resolve", "rtb200_render_adaptive",
 ]
 
 _lib = None
@@ -168,6 +176,11 @@ def lib() -> C.CDLL:
                                              C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64]
     L.rtb200_scene_rebuild.argtypes = [C.c_void_p, C.c_void_p]
     L.rtb200_scene_debug_topology.argtypes = [C.c_void_p, C.POINTER(C.c_double), C.POINTER(C.c_uint32)] + [C.c_void_p, C.c_uint64] * 5
+    L.rtb200_adaptive_begin.argtypes = [C.c_void_p, C.POINTER(rt_adaptive_params), C.c_void_p]
+    L.rtb200_adaptive_step.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(rt_stats)]
+    L.rtb200_adaptive_resolve.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    L.rtb200_render_adaptive.argtypes = [C.POINTER(rt_scene), C.POINTER(rt_options), C.POINTER(rt_adaptive_params), C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.POINTER(rt_stats)]
     _lib = L
     return L
 
@@ -477,6 +490,25 @@ def render_frames(scene: Scene, frames: Sequence[rt_frame], opts: Optional[rt_op
     return out, st.as_dict()
 
 
+def make_adaptive(rel_tol: float, abs_tol: float = 0.0, samples_per_round: int = 8, min_samples: int = 16,
+                  max_samples: int = 0) -> rt_adaptive_params:
+    return rt_adaptive_params(int(samples_per_round), int(max_samples), int(min_samples), 0, float(abs_tol), float(rel_tol))
+
+
+def render_adaptive(scene: Scene, params: rt_adaptive_params, opts: Optional[rt_options] = None):
+    """Render adaptively (rtb200_render_adaptive): rounds of params.samples_per_round samples of the pixels that have not
+    converged, until none is left. A pixel that received n samples equals the one-shot render at samples_per_pixel = n.
+    Returns (uint8 [rows,w,3], float32 linear [rows,w,3], uint32 counts [rows,w], stats dict)."""
+    rows = scene.c.height if (opts is None or opts.world <= 1) else shard_rows(scene.c.height, opts.rank, opts.world, opts.band_rows)
+    img = np.empty((rows, scene.c.width, 3), dtype=np.uint8)
+    lin = np.empty((rows, scene.c.width, 3), dtype=np.float32)
+    cnt = np.empty((rows, scene.c.width), dtype=np.uint32)
+    st = rt_stats()
+    _check(lib().rtb200_render_adaptive(C.byref(scene.c), C.byref(opts) if opts is not None else None, C.byref(params),
+                                        img.ctypes.data, lin.ctypes.data, cnt.ctypes.data, C.byref(st)))
+    return img, lin, cnt, st.as_dict()
+
+
 def _current_device() -> Optional[int]:
     """The caller's current CUDA device, which an upload without opts.device uses (None when torch is not installed)."""
     try:
@@ -557,6 +589,35 @@ class ResidentScene:
         moved, ordered like an update on `stream` (as in :meth:`update_geometry`, by default torch's current stream). Returns
         when the new tree exists; later frames trace it and later updates refit it. A no-op without a hierarchy."""
         _check(lib().rtb200_scene_rebuild(self.h, C.c_void_p(self._stream(stream, self.device) or None)))
+
+    def adaptive_begin(self, params: rt_adaptive_params, stream=None):
+        """(Re)start an adaptive render of the handle (rtb200_adaptive_begin): n = 0 everywhere, every pixel active. `stream`
+        as in :meth:`update_geometry`."""
+        _check(lib().rtb200_adaptive_begin(self.h, C.byref(params), C.c_void_p(self._stream(stream, self.device) or None)))
+
+    def adaptive_step(self, rounds: int = 1, stream=None):
+        """Run up to `rounds` rounds and wait (rtb200_adaptive_step). Returns (pixels still active, stats summed over the
+        rounds)."""
+        active = C.c_uint32(); st = rt_stats()
+        _check(lib().rtb200_adaptive_step(self.h, int(rounds), C.c_void_p(self._stream(stream, self.device) or None), C.byref(active), C.byref(st)))
+        return int(active.value), st.as_dict()
+
+    def adaptive_resolve(self, rgb8=None, linear=None, counts=None, stream=None):
+        """Write the current adaptive image into CUDA tensors (rtb200_adaptive_resolve), each optional: uint8 rgb8 and float32
+        linear of rows * w * 3 elements, int32 or uint32-sized counts of rows * w elements, on the handle's device."""
+        import torch
+        n = self.rows * self.scene.c.width
+        ptrs = []
+        for t, dt, size in ((rgb8, (torch.uint8,), 3 * n), (linear, (torch.float32,), 3 * n), (counts, (torch.int32,), n)):
+            if t is None:
+                ptrs.append(None)
+                continue
+            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype not in dt or t.numel() != size or not t.is_contiguous():
+                raise ValueError(f"adaptive_resolve takes contiguous CUDA tensors of {dt[0]} with {size} elements")
+            if self.device is not None and t.device.index != self.device:
+                raise ValueError(f"the tensor is on cuda:{t.device.index}, the scene on cuda:{self.device}")
+            ptrs.append(C.c_void_p(t.data_ptr()))
+        _check(lib().rtb200_adaptive_resolve(self.h, *ptrs, C.c_void_p(self._stream(stream, self.device) or None)))
 
     def topology(self) -> dict:
         """The handle's current topology (rtb200_scene_debug_topology): recentre, leaf_id [n_leaves, k], always, skip_pos,

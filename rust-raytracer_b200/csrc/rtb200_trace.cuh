@@ -25,9 +25,10 @@ using namespace rtd;
 #endif
 #ifndef RT_SMEM_STACK
 // Albedo-stack levels kept in shared memory per slot; deeper levels live in global memory, and every bounce there costs a
-// global store and, when the path is unwound, a dependent global load. 12 levels (65.1 KB per CTA) still leave 3 CTAs per
-// SM; on C2 on an H100 each step from 3 to 5, 8 and 12 levels was faster (DESIGN.md §4.3).
-#define RT_SMEM_STACK 12
+// global store and, when the path is unwound, a dependent global load. On C2 on an H100 each step from 3 to 5, 8 and 12
+// levels was faster (DESIGN.md §4.3), but 12 levels (67,152 B per CTA) need the 228 KiB shared-memory carveout for 3 CTAs
+// per SM and leave 28 KiB of L1; 10 levels (65,104 B) fit the 196 KiB carveout and leave 60 KiB, which is faster (§4.5).
+#define RT_SMEM_STACK 10
 #endif
 
 enum : uint32_t { CLS_MISS = 0, CLS_DIFFUSE = 1, CLS_METAL = 2, CLS_GLASS = 3, CLS_LIGHT = 4, CLS_DEAD = 5, N_CLS = 6 };

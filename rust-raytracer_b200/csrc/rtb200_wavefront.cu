@@ -12,6 +12,7 @@
 // queue spans several frames of the scene, each with its own camera and key; rtb200_render_frames, DESIGN.md §4.6) and a list
 // one (Q_LIST: the queue spans the pixels still on an adaptive render's list; rtb200_adaptive_step, DESIGN.md §4.9).
 #include <cstdio>
+#include <cstdlib>
 
 #include "rtb200_trace.cuh"
 
@@ -31,8 +32,8 @@ struct WfSmem {
 
 // mask: bit0 hierarchy (MODE_TREE) / flat records (MODE_BRUTE), bit1 exact geometry, bit2 materials in shared memory
 // frames: the multi-frame kernel's pool also holds Pool.frm
-__host__ __device__ inline WfSmem wf_layout(uint32_t n, uint32_t n_pairs, uint32_t n_nodes, uint32_t n_leaves, uint32_t mode, uint32_t mask, bool frames) {
-    WfSmem L;
+__host__ __device__ constexpr WfSmem wf_layout(uint32_t n, uint32_t n_pairs, uint32_t n_nodes, uint32_t n_leaves, uint32_t mode, uint32_t mask, bool frames) {
+    WfSmem L{};
     uint32_t off = 16;   // mbarrier
     L.nodes_off = off;   if (mode == MODE_TREE && (mask & 1u)) off += n_nodes * (uint32_t)(kNodeVec * 16);
     L.leafrec_off = off; if (mode == MODE_TREE && (mask & 1u)) off += n_leaves * (uint32_t)(kLeafK * 16);
@@ -61,6 +62,39 @@ size_t wavefront_smem_bytes(const TraceParams& p, uint32_t mode, uint32_t smem_m
 constexpr int wf_min_blocks(uint32_t mode) {
     const int n = (mode == MODE_TREE ? 3 : 2) * 256 / kBlock;
     return n > 0 ? n : 1;
+}
+
+// Shared memory and L1 share the SM's 256 KiB, and every scene load and local-memory spill of the trace kernel goes through
+// L1. The H100 sets the shared-memory side in steps (..., 164, 196, 228 KiB), allocates a CTA's shared memory in 128 B units
+// and reserves 1 KiB per CTA. Three tree CTAs therefore leave 60 KiB of L1 when each takes at most 65,792 B of dynamic shared
+// memory, and 28 KiB when it takes more; on C2 the same kernel ran 3.3 % faster with 60 KiB (DESIGN.md §4.5). (The
+// stage-clock build's per-warp table does not fit.)
+constexpr uint32_t smem_alloc(uint32_t bytes) { return (bytes + 127u) / 128u * 128u + 1024u; }
+static_assert(RT_PHASE_CLOCKS || 3u * smem_alloc(wf_layout(0, 0, 0, 0, MODE_TREE, 0u, false).total) <= 196u * 1024u,
+              "three single-frame tree CTAs per SM must fit the 196 KiB carveout");
+
+// Give the kernel the smallest carveout that holds the CTAs per SM its register budget is built for (wf_min_blocks), so that
+// L1 keeps the rest whatever the driver would pick. A percentage is rounded up to the next carveout step, so the rounded-down
+// percentage of what the CTAs need is tried first, and one percent more only when the occupancy says that step is too small.
+// RTB200_WF_CARVEOUT=<percent> sets the preference instead (experiments: tools/l1_probe.py). Needs the kernel's
+// cudaFuncAttributeMaxDynamicSharedMemorySize set to `smem`.
+template <typename K>
+static cudaError_t set_carveout(K kern, uint32_t mode, size_t smem) {
+    static const char* forced = getenv("RTB200_WF_CARVEOUT");
+    if (forced) return cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, atoi(forced));
+    int dev = 0, max_sm = 0, reserved = 0;
+    cudaError_t e = cudaGetDevice(&dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&max_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
+    if (e == cudaSuccess) e = cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev);
+    if (e != cudaSuccess) return e;
+    const size_t need = (size_t)wf_min_blocks(mode) * ((smem + 127u) / 128u * 128u + (size_t)reserved);
+    const int pct = need >= (size_t)max_sm ? 100 : (int)(need * 100u / (size_t)max_sm);
+    e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
+    if (e != cudaSuccess || pct == 100) return e;
+    int nb = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kBlock, smem);
+    if (e != cudaSuccess || nb >= wf_min_blocks(mode)) return e;
+    return cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, pct + 1);
 }
 
 // Q_FRAMES: one launch renders several frames of the scene (TraceParams::ftab / frame_work, rtb200_render_frames)
@@ -214,6 +248,7 @@ static auto dispatch(uint32_t mode, bool lights, uint32_t queue, F&& f) {
 cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, uint32_t queue, int grid, size_t smem, cudaStream_t st) {
     return dispatch(mode, p.n_lights > 0, queue, [&](auto kern) -> cudaError_t {
         cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+        if (e == cudaSuccess) e = set_carveout(kern, mode, smem);
         if (e != cudaSuccess) return e;
         kern<<<grid, kBlock, smem, st>>>(p);
         return cudaGetLastError();
@@ -224,6 +259,7 @@ int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, uint32_t queue, size_t
     return dispatch(mode, lights, queue, [&](auto kern) -> int {
         int nb = 0;
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return 0; }
+        if (set_carveout(kern, mode, smem) != cudaSuccess) { cudaGetLastError(); return 0; }
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kBlock, smem) != cudaSuccess) { cudaGetLastError(); return 0; }
         return nb;
     });

@@ -75,7 +75,9 @@ struct WarpCtx {
     uint32_t *skip;                // [32] per ray: skip_pos of the certified source sphere, or kNoSkip
     uint32_t *l_in, *l_lf, *l_cd;  // work lists: (ray, node), (ray, leaf), (ray, sphere); entries id << 5 | ray
 };
-constexpr uint32_t kWarpCtxBytes = 3 * 32 * 16 + 32 * 4 + (uint32_t)(kCapIn + kCapLf + kCapCd) * 4;
+// Rounded up to 16 B: the contexts of a CTA's warps lie back to back, and each one's float4 constants (then the pool's
+// doubles after the last one) must stay aligned whatever the list capacities add up to.
+constexpr uint32_t kWarpCtxBytes = (3 * 32 * 16 + 32 * 4 + (uint32_t)(kCapIn + kCapLf + kCapCd) * 4 + 15u) & ~15u;
 RT_DEV WarpCtx warpctx_at(unsigned char* base) {
     WarpCtx W;
     W.cA = reinterpret_cast<float4*>(base); W.cB = W.cA + 32; W.cC = W.cB + 32;

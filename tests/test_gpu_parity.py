@@ -93,11 +93,14 @@ def test_device_quantisation_is_the_oracle_quantisation():
 
 
 # ---- images -----------------------------------------------------------------------------------------
-@pytest.mark.parametrize("name,mk", [
+GOLDEN = [   # (tests/golden/<name>.npz, the scene it was rendered from)
     ("cover_40x30_s4", lambda: scenes.cover_scene(40, 30, 4)),
     ("cover_64x48_s2_d3", lambda: scenes.cover_scene(64, 48, 2, depth=3)),
     ("mixed_48x36_s3", lambda: R.Scene.from_config(mixed_config(48, 36, 3, 12, seed=11), scenes.SCENES_DIR)),
-])
+]
+
+
+@pytest.mark.parametrize("name,mk", GOLDEN)
 def test_gpu_matches_committed_golden(name, mk):
     g = np.load(os.path.join(GOLD, name + ".npz"))
     sc = mk()

@@ -4,7 +4,7 @@ renders that overlap on one device. Every comparison is bit-exact: linear f32, R
 A device has two work sets (sample buffer, accumulator, albedo stack, stat block and queue counters, shadow frames, light
 terms, frame table), shared by every handle on it. Asynchronous frames of a handle alternate between them; every blocking
 render takes set 0. The first part traces lit scenes inside a closed room, where nearly every path runs to max_depth: the
-albedo stack past its shared-memory levels (RT_SMEM_STACK = 12) in the lights kernels, next to deep shadow frames. The second
+albedo stack past its shared-memory levels (RT_SMEM_STACK = 10) in the lights kernels, next to deep shadow frames. The second
 part forces submissions that share a set to overlap on different streams, from one handle or from several."""
 import numpy as np
 import pytest
@@ -51,9 +51,9 @@ def _one_shot_vs_oracle(sc, opts=None):
 
 # ---- 1. lit scenes that use every buffer of a work set ----------------------------------------------------------------
 
-@pytest.mark.parametrize("n_lights,depth", [(1, 12), (2, 13), (3, 50)])
+@pytest.mark.parametrize("n_lights,depth", [(1, 10), (2, 11), (3, 50)])
 def test_deep_lit_room_matches_the_oracle(n_lights, depth):
-    """max_depth 12 and 13 sit on the shared/global boundary of the albedo stack; 50 goes far past it."""
+    """max_depth 10 and 11 sit on the shared/global boundary of the albedo stack; 50 goes far past it."""
     st_o, _, _ = _one_shot_vs_oracle(R.Scene.from_config(_room_cfg(n_lights, depth)))
     assert _deep(st_o, depth) >= 10_000, st_o["path_len_hist"]              # most paths run to max_depth
     if depth == 50:
@@ -90,12 +90,16 @@ def _frames_vs_oracle(sc, frames, opts=None):
     return st
 
 
+def _room_frames(sc):
+    """Three views of the room, each with its own seed."""
+    return [R.make_frame(sc, seed=5), R.make_frame(sc, look_from=[-9.0, 3.0, 7.0], seed=6),
+            R.make_frame(sc, look_from=[4.0, 8.0, -12.0], look_at=[0.0, 1.0, 0.0], seed=7)]
+
+
 def test_deep_lit_frames_in_one_launch():
-    """The LIGHTS + FRAMES kernel past albedo-stack level 12: three views of the room in one trace launch."""
+    """The LIGHTS + FRAMES kernel past albedo-stack level 10: three views of the room in one trace launch."""
     sc = R.Scene.from_config(_room_cfg(3, 50))
-    frames = [R.make_frame(sc, seed=5), R.make_frame(sc, look_from=[-9.0, 3.0, 7.0], seed=6),
-              R.make_frame(sc, look_from=[4.0, 8.0, -12.0], look_at=[0.0, 1.0, 0.0], seed=7)]
-    st = _frames_vs_oracle(sc, frames)
+    st = _frames_vs_oracle(sc, _room_frames(sc))
     assert st["batches"] == 1 and st["frames"] == 3 and st["kernel_launches"] == 1 + 3
 
 
@@ -108,12 +112,16 @@ def test_deep_lit_sample_batches():
     assert _deep(st_o, 30) >= 10_000
 
 
-def test_deep_textured_room():
-    """The textured test scene (its own light, textured spheres, sky texture) closed in by the room sphere at max_depth 50:
-    texel codes go onto the albedo stack past its shared-memory levels (a fifth of the paths reach level 13)."""
+def _textured_room():
+    """The textured test scene (its own light, textured spheres, sky texture) closed in by the room sphere at max_depth 50."""
     cfg = scenes._variant(scenes.test_scene_config(), 80, 60, 4, 50)
     cfg["objects"].append({"center": _v(0, 0, 0), "radius": 40.0, "material": {"Lambertian": {"albedo": [0.9, 0.9, 0.9]}}})
-    st_o, _, _ = _one_shot_vs_oracle(R.Scene.from_config(cfg, scenes.SCENES_DIR))
+    return R.Scene.from_config(cfg, scenes.SCENES_DIR)
+
+
+def test_deep_textured_room():
+    """Texel codes go onto the albedo stack past its shared-memory levels (a fifth of the paths reach level 13)."""
+    st_o, _, _ = _one_shot_vs_oracle(_textured_room())
     assert _deep(st_o, 13) >= 2_000 and st_o["hits"][R.RT_TEXTURE] > 0, st_o["path_len_hist"]
 
 

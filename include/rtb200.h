@@ -312,6 +312,44 @@ int rtb200_adaptive_resolve(rtb200_scene_handle h, void* dev_rgb8, void* dev_lin
 int rtb200_render_adaptive(const rt_scene* scene, const rt_options* opts, const rt_adaptive_params* p,
                            uint8_t* out_rgb8, float* out_linear_f32, uint32_t* out_counts, rt_stats* stats);
 
+/* ---- closest-hit queries on a resident scene (DESIGN.md §4.10) -----------------------------------------------------------
+ * Contract: for ray i with origin o = origin[3i..3i+2], direction d = direction[3i..3i+2] (any f64 values, not necessarily
+ * normalised) and bound t_max_i = t_max[i] (f64::MAX when t_max is NULL; a bound above f64::MAX, i.e. +inf, counts as
+ * f64::MAX), the result is hit_world(world, Ray{o, d}, 0.001, t_max_i) (raytracer.rs:44-59) over the handle's CURRENT spheres:
+ * the upload's, or those of the last update or rebuild enqueued before the query. Every output equals the reference's bit for
+ * bit, for every variant:
+ *   sphere      index of the hit sphere (on equal t the first in list order), 0xffffffff for a miss;
+ *   t           the accepted root;
+ *   point       ray.at(t) (ray.rs:18-20);
+ *   normal      (point - centre) / radius, flipped against the ray, as HitRecord.normal (sphere.rs:59-76);
+ *   front_face  1 when the ray hits the outside, else 0;
+ *   uv          u_v_from_sphere_hit_point (sphere.rs:35-43), whose f64::atan2 is the explicit algorithm the texture path and
+ *               the oracle share (DESIGN.md §3), not the platform's: the last bit of u may differ from a host libm's.
+ * A miss writes sphere = 0xffffffff, t = +inf, zeros in point, normal and uv, and front_face = 0. t_min is always 0.001. */
+typedef struct {
+    const double* origin;     /* n x 3 */
+    const double* direction;  /* n x 3 */
+    const double* t_max;      /* n, or NULL: f64::MAX for every ray */
+} rt_rays;                    /* 24 bytes */
+typedef struct {              /* every pointer may be NULL: that output is not written */
+    double* t; uint32_t* sphere; double* point /* n x 3 */; double* normal /* n x 3 */; double* uv /* n x 2 */; uint8_t* front_face;
+} rt_hits;                    /* 48 bytes */
+/* Device buffers (of h's device, or managed memory), stream-ordered, without waiting for the GPU. The query runs on `stream`
+ * (NULL: the library's stream) after the upload and after the last update or rebuild of h enqueued before it, on any stream;
+ * every rtb200_scene_update_* and rtb200_scene_rebuild enqueued after it waits for it, and rtb200_scene_release waits for it.
+ * Queries only read the scene and take no work set: they neither wait for frames nor make frames wait, and queries on any
+ * streams may overlap each other and frames. The buffers must stay valid until the query has run on `stream`. A traversal-guard
+ * trip is counted with the handle's frames' and reported when its next frames are collected (rtb200_render_device_wait or a
+ * blocking render).
+ * RT_ERR_INVALID, before any device work, for a NULL handle, NULL rays, out, origin or direction, an out with every output NULL,
+ * or a pointer that is not device memory of h's device or managed memory. n == 0 is a no-op. */
+int rtb200_scene_intersect_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_hits* out, void* stream);
+/* Host buffers, blocking: the same query, through the same kernel, on the library's stream with copies in and out. stats (may
+ * be NULL): rays = n, candidates (f64 sphere tests), clusters (leaves visited), nodes (nodes visited), device_ms (copies and
+ * kernel), trace_ms (the kernel), wall_ms, h2d_bytes, d2h_bytes and kernel_launches. Same checks as the device form, bar the
+ * memory kind; a traversal-guard trip fails the call with RT_ERR_CUDA. */
+int rtb200_scene_intersect(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_hits* out, rt_stats* stats);
+
 /* load_texture_image — materials.rs:213-219, config.rs:36-47: decode a baseline JPEG file to RGB8 (host-side scene staging
  * helper for hosts without their own decoder; the reference uses the jpeg-decoder crate). *out_rgb8 is released with rtb200_free(). */
 int  rtb200_decode_jpeg_file(const char* path, uint8_t** out_rgb8, uint64_t* width, uint64_t* height);

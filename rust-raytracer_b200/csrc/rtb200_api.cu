@@ -94,6 +94,11 @@ struct DeviceCtx {
     std::vector<OccKey> occ_cache;        // cudaOccupancyMaxActiveBlocksPerMultiprocessor answers
     PinnedBuf staging;                    // host image of the arena being uploaded
     cudaEvent_t staging_free = nullptr;   // the last H2D copy out of `staging` has finished
+    // the host form of rtb200_scene_intersect: rays, hits and counters on the device, its timing events (created at its first
+    // call), and the resident CTAs per SM of the query kernel of each mode (0: not asked yet)
+    GrowBuf query;
+    cudaEvent_t query_ev[4] = {nullptr, nullptr, nullptr, nullptr};
+    int query_occ[3] = {0, 0, 0};
 };
 DeviceCtx g_ctx[64];
 std::mutex g_ctx_mu;
@@ -213,6 +218,11 @@ struct rtb200_scene_t {
     void* rebuild = nullptr;             // RebuildBufs of tp.n spheres; once set, the tree arrays of tp and the refit scratch live here
     GrowBuf upd_in;                      // host form's input: geo, materials, indices
     uint32_t updates = 0;                // rtb200_scene_update_* calls so far: an adaptive render refuses to step across one
+    // ---- closest-hit queries (rtb200_scene_intersect_device): queries[0, n_queries) hold the last query of each stream enqueued
+    // since the last update or rebuild, which the next update or rebuild waits for; the rest are spare events ----
+    struct QueryMark { cudaStream_t stream; cudaEvent_t done; };
+    std::vector<QueryMark> queries;
+    uint32_t n_queries = 0;
     // ---- adaptive rendering (rtb200_adaptive_*, DESIGN.md §4.9): one device block allocated at the first begin ----
     struct Adaptive {
         void* mem = nullptr;             // sum, sq, count, keep, list[2], list_n[2], cub's scratch
@@ -323,6 +333,7 @@ int rtb200_scene_release(rtb200_scene_handle h) {
         if (!h->pending.empty()) render_collect(h, nullptr);   // frames still in flight read the scene arrays
         else if (h->ctx->stream) cudaStreamSynchronize(h->ctx->stream);
         if (h->updated) { cudaEventSynchronize(h->updated); cudaEventDestroy(h->updated); }   // an update in flight writes them
+        for (const auto& q : h->queries) { cudaEventSynchronize(q.done); cudaEventDestroy(q.done); }   // queries in flight read them
         if (h->refit) cudaFree(h->refit);
         if (h->rebuild) cudaFree(h->rebuild);
         if (h->upd_in.p) cudaFree(h->upd_in.p);
@@ -908,9 +919,12 @@ static cudaError_t update_begin(rtb200_scene_handle h) {
     return h->updated ? cudaSuccess : cudaEventCreateWithFlags(&h->updated, cudaEventDisableTiming);
 }
 
-// Order `st` after the frames of h in flight, on any stream: they read the arrays the update writes.
+// Order `st` after the frames and the queries of h in flight, on any stream: they read the arrays the update writes. Every
+// later update or rebuild waits for this one (h->updated, scene_stream), so the queries waited for here are forgotten.
 static int update_after_frames(rtb200_scene_handle h, cudaStream_t st) {
     for (const auto& p : h->pending) if (p.n_ev) CU(cudaStreamWaitEvent(st, h->ev[p.ev0 + 1], 0));
+    for (uint32_t k = 0; k < h->n_queries; ++k) CU(cudaStreamWaitEvent(st, h->queries[k].done, 0));
+    h->n_queries = 0;
     return RT_OK;
 }
 
@@ -1102,6 +1116,132 @@ int rtb200_scene_rebuild(rtb200_scene_handle h, void* stream_in) {
     h->level_off = level_off;
     h->level_nodes.clear();
     h->node_box = b.node_box; h->leaf_box = b.leaf_box; h->level_nodes_dev = b.level_nodes;
+    return RT_OK;
+  });
+}
+
+// ---- closest-hit queries on a resident scene (DESIGN.md §4.10) ----
+// The argument checks both forms share (no device is touched).
+static int check_query(rtb200_scene_handle h, const rt_rays* rays, const rt_hits* out) {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    if (!rays || !out) return fail(RT_ERR_INVALID, "rays or out is null");
+    if (!rays->origin || !rays->direction) return fail(RT_ERR_INVALID, "rays->origin or rays->direction is null");
+    if (!out->t && !out->sphere && !out->point && !out->normal && !out->uv && !out->front_face)
+        return fail(RT_ERR_INVALID, "every output of out is null");
+    return RT_OK;
+}
+
+// The one path of both forms: enqueue the query of the n rays `rays` into `out` (device buffers) on `st`, which the caller has
+// ordered after the scene's last writer (scene_stream). Guard trips go to err[1], the counters to stat (null: not counted).
+static int query_enqueue(rtb200_scene_handle h, const rt_rays& rays, uint32_t n, const rt_hits& out, unsigned long long* stat,
+                         unsigned long long* err, cudaStream_t st) {
+    int& occ = h->ctx->query_occ[h->mode];
+    if (occ == 0) occ = query_max_ctas_per_sm(h->mode);
+    if (occ <= 0) { occ = 0; return fail(RT_ERR_UNSUPPORTED, "no launch configuration of the query kernel fits shared memory"); }
+    QueryParams q{};
+    q.p = h->tp; q.p.stat = stat; q.p.err = err;
+    q.origin = rays.origin; q.direction = rays.direction; q.t_max = rays.t_max;
+    q.t = out.t; q.sphere = out.sphere; q.point = out.point; q.normal = out.normal; q.uv = out.uv; q.front_face = out.front_face;
+    q.n = n;
+    CU(launch_query(q, h->mode, h->ctx->sm_count * occ, st));
+    return RT_OK;
+}
+
+int rtb200_scene_intersect_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_hits* out, void* stream_in) {
+  return guarded([&]() -> int {
+    int rc = check_query(h, rays, out);
+    if (rc != RT_OK) return rc;
+    if (n == 0) return RT_OK;
+    DeviceRestore restore;
+    std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
+    CU(cudaSetDevice(h->device));
+    const struct { const void* p; const char* name; } ptrs[] = {
+        {rays->origin, "rays->origin"}, {rays->direction, "rays->direction"}, {rays->t_max, "rays->t_max"}, {out->t, "out->t"},
+        {out->sphere, "out->sphere"}, {out->point, "out->point"}, {out->normal, "out->normal"}, {out->uv, "out->uv"},
+        {out->front_face, "out->front_face"}};
+    for (const auto& q : ptrs) {
+        if (!q.p) continue;
+        cudaPointerAttributes a{};
+        if (cudaPointerGetAttributes(&a, q.p) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+        if (!((a.type == cudaMemoryTypeDevice && a.device == h->device) || a.type == cudaMemoryTypeManaged))
+            return fail(RT_ERR_INVALID, std::string(q.name) + " is not device or managed memory of device " + std::to_string(h->device));
+    }
+    cudaStream_t st;
+    CU(scene_stream(h, stream_in, &st));
+    if ((rc = query_enqueue(h, *rays, n, *out, nullptr, h->err, st)) != RT_OK) return rc;
+    // the next update or rebuild waits for the last query of each stream
+    uint32_t k = 0;
+    while (k < h->n_queries && h->queries[k].stream != st) ++k;
+    if (k == h->n_queries) {
+        if (k == h->queries.size()) {
+            cudaEvent_t e;
+            CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+            h->queries.push_back(rtb200_scene_t::QueryMark{st, e});
+        }
+        h->queries[k].stream = st;
+        ++h->n_queries;
+    }
+    CU(cudaEventRecord(h->queries[k].done, st));
+    return RT_OK;
+  });
+}
+
+int rtb200_scene_intersect(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_hits* out, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (stats) memset(stats, 0, sizeof *stats);
+    int rc = check_query(h, rays, out);
+    if (rc != RT_OK) return rc;
+    if (n == 0) return RT_OK;
+    auto wall0 = std::chrono::steady_clock::now();
+    DeviceRestore restore;
+    DeviceCtx* ctx = h->ctx;
+    std::lock_guard<std::recursive_mutex> lk(ctx->mu);
+    CU(cudaSetDevice(h->device));
+    for (auto& e : ctx->query_ev) if (!e) CU(cudaEventCreate(&e));
+    // device image: counters (kStatBytes; the guard counters at stat[30..31]), then rays and hits, 256-byte aligned
+    const uint64_t N = n;
+    const uint64_t in_b[3] = {N * 24, N * 24, rays->t_max ? N * 8 : 0};
+    const uint64_t out_b[6] = {out->t ? N * 8 : 0, out->sphere ? N * 4 : 0, out->point ? N * 24 : 0, out->normal ? N * 24 : 0,
+                               out->uv ? N * 16 : 0, out->front_face ? N : 0};
+    auto al = [](uint64_t b) { return (b + 255) & ~(uint64_t)255; };
+    uint64_t bytes = kStatBytes;
+    for (uint64_t b : in_b) bytes += al(b);
+    for (uint64_t b : out_b) bytes += al(b);
+    CU(ctx->query.ensure(bytes));   // the last host-form query has finished: it waited for its stream
+    char* D = (char*)ctx->query.p;
+    unsigned long long* stat = (unsigned long long*)D;
+    char* din[3]; char* dout[6];
+    uint64_t off = kStatBytes;
+    for (int k = 0; k < 3; ++k) { din[k] = in_b[k] ? D + off : nullptr; off += al(in_b[k]); }
+    for (int k = 0; k < 6; ++k) { dout[k] = out_b[k] ? D + off : nullptr; off += al(out_b[k]); }
+    cudaStream_t st;
+    CU(scene_stream(h, nullptr, &st));
+    cudaEvent_t* ev = ctx->query_ev;
+    CU(cudaEventRecord(ev[0], st));
+    CU(cudaMemsetAsync(stat, 0, kStatBytes, st));
+    const void* src_in[3] = {rays->origin, rays->direction, rays->t_max};
+    uint64_t h2d = 0, d2h = kStatBytes;
+    for (int k = 0; k < 3; ++k) if (in_b[k]) { CU(cudaMemcpyAsync(din[k], src_in[k], in_b[k], cudaMemcpyHostToDevice, st)); h2d += in_b[k]; }
+    const rt_rays drays{(const double*)din[0], (const double*)din[1], (const double*)din[2]};
+    const rt_hits dhits{(double*)dout[0], (uint32_t*)dout[1], (double*)dout[2], (double*)dout[3], (double*)dout[4], (uint8_t*)dout[5]};
+    CU(cudaEventRecord(ev[1], st));
+    if ((rc = query_enqueue(h, drays, n, dhits, stat, stat + 30, st)) != RT_OK) return rc;
+    CU(cudaEventRecord(ev[2], st));
+    void* dst_out[6] = {out->t, out->sphere, out->point, out->normal, out->uv, out->front_face};
+    for (int k = 0; k < 6; ++k) if (out_b[k]) { CU(cudaMemcpyAsync(dst_out[k], dout[k], out_b[k], cudaMemcpyDeviceToHost, st)); d2h += out_b[k]; }
+    unsigned long long hstat[kStatBytes / 8];
+    CU(cudaMemcpyAsync(hstat, stat, kStatBytes, cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(ev[3], st));
+    CU(cudaStreamSynchronize(st));
+    if (hstat[31] != 0) return fail(RT_ERR_CUDA, "internal error: the traversal guard tripped; the query results are not valid");
+    if (!stats) return RT_OK;
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, ev[0], ev[3])); stats->device_ms = ms;
+    CU(cudaEventElapsedTime(&ms, ev[1], ev[2])); stats->trace_ms = ms;
+    stats->rays = hstat[0]; stats->candidates = hstat[1]; stats->clusters = hstat[4]; stats->nodes = hstat[6];
+    stats->kernel_launches = 1; stats->batches = 1; stats->gpus_used = 1;
+    stats->h2d_bytes = h2d; stats->d2h_bytes = d2h;
+    stats->wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count();
     return RT_OK;
   });
 }

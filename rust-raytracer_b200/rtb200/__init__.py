@@ -109,7 +109,22 @@ class rt_adaptive_params(C.Structure):
                 ("abs_tol", C.c_float), ("rel_tol", C.c_float)]
 
 
+class rt_rays(C.Structure):
+    """Rays of a closest-hit query (rtb200_scene_intersect[_device]): origin and direction n x 3 f64, t_max n f64 or NULL."""
+    _fields_ = [("origin", C.c_void_p), ("direction", C.c_void_p), ("t_max", C.c_void_p)]
+
+
+class rt_hits(C.Structure):
+    """Outputs of a closest-hit query, each NULL or n (t, sphere, front_face), n x 3 (point, normal) or n x 2 (uv) elements."""
+    _fields_ = [("t", C.c_void_p), ("sphere", C.c_void_p), ("point", C.c_void_p), ("normal", C.c_void_p), ("uv", C.c_void_p),
+                ("front_face", C.c_void_p)]
+
+
+HIT_FIELDS = (("t", 1, np.float64), ("sphere", 1, np.int32), ("point", 3, np.float64), ("normal", 3, np.float64),
+              ("uv", 2, np.float64), ("front_face", 1, np.uint8))   # rt_hits: name, values per ray, dtype (sphere -1 = 0xffffffff)
+
 assert C.sizeof(rt_sphere) == 64 and C.sizeof(rt_frame) == 112 and C.sizeof(rt_adaptive_params) == 24
+assert C.sizeof(rt_rays) == 24 and C.sizeof(rt_hits) == 48
 
 # every symbol include/rtb200.h declares (tests check that the library exports all of them)
 ABI_SYMBOLS = [
@@ -123,6 +138,7 @@ ABI_SYMBOLS = [
     "rtb200_scene_update_spheres", "rtb200_scene_update_geometry_device", "rtb200_scene_debug_records",
     "rtb200_scene_rebuild", "rtb200_scene_debug_topology",
     "rtb200_adaptive_begin", "rtb200_adaptive_step", "rtb200_adaptive_resolve", "rtb200_render_adaptive",
+    "rtb200_scene_intersect_device", "rtb200_scene_intersect",
 ]
 
 _lib = None
@@ -181,6 +197,8 @@ def lib() -> C.CDLL:
     L.rtb200_adaptive_resolve.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     L.rtb200_render_adaptive.argtypes = [C.POINTER(rt_scene), C.POINTER(rt_options), C.POINTER(rt_adaptive_params), C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.POINTER(rt_stats)]
+    L.rtb200_scene_intersect_device.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.POINTER(rt_hits), C.c_void_p]
+    L.rtb200_scene_intersect.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.POINTER(rt_hits), C.POINTER(rt_stats)]
     _lib = L
     return L
 
@@ -618,6 +636,63 @@ class ResidentScene:
                 raise ValueError(f"the tensor is on cuda:{t.device.index}, the scene on cuda:{self.device}")
             ptrs.append(C.c_void_p(t.data_ptr()))
         _check(lib().rtb200_adaptive_resolve(self.h, *ptrs, C.c_void_p(self._stream(stream, self.device) or None)))
+
+    def intersect(self, origin, direction, t_max=None, stream=None, outputs=None) -> dict:
+        """Closest hits of caller-supplied rays on the handle's current spheres: for ray i, hit_world(world, Ray{origin[i],
+        direction[i]}, 0.001, t_max[i]) (f64::MAX without t_max) as include/rtb200.h states it, bit for bit, in every variant.
+
+        CUDA tensors (contiguous float64 [n, 3], [n, 3] and [n], on the handle's device) use the device form
+        (rtb200_scene_intersect_device) on `stream` (as in :meth:`update_geometry`, by default torch's current stream), without
+        waiting: the query sees every update enqueued before it, and updates enqueued after it wait for it. numpy arrays use
+        the blocking host form (rtb200_scene_intersect) and the result also holds "stats".
+
+        Returns a dict of tensors or arrays, one per name of `outputs` (default: all): "t" [n] (+inf: miss), "sphere" int32 [n]
+        (-1: miss, the bits of 0xffffffff), "point" and "normal" [n, 3], "uv" [n, 2], "front_face" uint8 [n]."""
+        names = [f[0] for f in HIT_FIELDS] if outputs is None else list(outputs)
+        unknown = [k for k in names if k not in dict((f[0], f) for f in HIT_FIELDS)]
+        if unknown or not names:
+            raise ValueError(f"intersect outputs are a non-empty subset of {[f[0] for f in HIT_FIELDS]}, got {names}")
+        if isinstance(origin, np.ndarray):
+            return self._intersect_host(origin, direction, t_max, names)
+        import torch
+        args = [("origin", origin, 2), ("direction", direction, 2)] + ([("t_max", t_max, 1)] if t_max is not None else [])
+        n = origin.shape[0] if isinstance(origin, torch.Tensor) and origin.dim() == 2 else -1
+        for name, t, dim in args:
+            if not isinstance(t, torch.Tensor) or not t.is_cuda:
+                raise ValueError(f"intersect takes CUDA tensors (or numpy arrays): {name} is {type(t).__name__}")
+            shape = (n, 3) if dim == 2 else (n,)
+            if t.dtype != torch.float64 or tuple(t.shape) != shape or n < 0 or not t.is_contiguous():
+                raise ValueError(f"intersect: {name} must be a contiguous float64 tensor of shape {list(shape) if n >= 0 else '[n, 3]'}, got {t.dtype} {tuple(t.shape)}")
+            if self.device is not None and t.device.index != self.device:
+                raise ValueError(f"the tensor {name} is on cuda:{t.device.index}, the scene on cuda:{self.device}")
+            if t.device != origin.device:
+                raise ValueError(f"origin is on {origin.device}, {name} on {t.device}")
+        dt = {np.float64: torch.float64, np.int32: torch.int32, np.uint8: torch.uint8}
+        # outputs belong to the query's stream when it is a torch stream (the caching allocator orders their reuse after it)
+        with torch.cuda.stream(stream) if isinstance(stream, torch.cuda.Stream) else torch.cuda.device(origin.device):
+            out = {k: torch.empty((n, c) if c > 1 else (n,), dtype=dt[ty], device=origin.device) for k, c, ty in HIT_FIELDS if k in names}
+        if n == 0:
+            return out
+        rays = rt_rays(origin.data_ptr(), direction.data_ptr(), t_max.data_ptr() if t_max is not None else None)
+        hits = rt_hits(*(out[k].data_ptr() if k in out else None for k, _, _ in HIT_FIELDS))
+        _check(lib().rtb200_scene_intersect_device(self.h, C.byref(rays), n, C.byref(hits), C.c_void_p(self._stream(stream, origin.device) or None)))
+        return out
+
+    def _intersect_host(self, origin, direction, t_max, names) -> dict:
+        n = origin.shape[0] if origin.ndim == 2 else -1
+        for name, a, shape in (("origin", origin, (n, 3)), ("direction", direction, (n, 3)), ("t_max", t_max, (n,))):
+            if name == "t_max" and a is None:
+                continue
+            if not isinstance(a, np.ndarray) or a.dtype != np.float64 or a.shape != shape or n < 0 or not a.flags.c_contiguous:
+                raise ValueError(f"intersect: {name} must be a C-contiguous float64 array of shape {list(shape) if n >= 0 else '[n, 3]'}, "
+                                 f"got {getattr(a, 'dtype', type(a).__name__)} {getattr(a, 'shape', '')}")
+        out = {k: np.empty((n, c) if c > 1 else (n,), dtype=ty) for k, c, ty in HIT_FIELDS if k in names}
+        rays = rt_rays(origin.ctypes.data, direction.ctypes.data, t_max.ctypes.data if t_max is not None else None)
+        hits = rt_hits(*(out[k].ctypes.data if k in out else None for k, _, _ in HIT_FIELDS))
+        st = rt_stats()
+        _check(lib().rtb200_scene_intersect(self.h, C.byref(rays), n, C.byref(hits), C.byref(st)))
+        out["stats"] = st.as_dict()
+        return out
 
     def topology(self) -> dict:
         """The handle's current topology (rtb200_scene_debug_topology): recentre, leaf_id [n_leaves, k], always, skip_pos,

@@ -30,6 +30,16 @@ struct WfSmem {
     uint32_t total;
 };
 
+// A staged segment is copied with one cp.async.bulk, whose shared and global addresses must be 16-byte aligned and whose
+// size must be a multiple of 16. Every segment therefore starts at a multiple of 16 and is copied (and counted by the
+// mbarrier) at its size rounded up to 16: stage_bytes of `count` elements of UNIT bytes. The nodes (224 B), leaf records
+// (kLeafK * 16 B), flat record pairs, geometry and materials (32 B) are whole 16 B blocks already. Only the leaf-id block can
+// be short (UNIT = kLeafK * 4 with kLeafK / 2 odd, and an odd leaf count: 8 B short); its copy then reads 8 B past the
+// array, inside the array's 256 B upload block (commit_uploads). A UNIT that is a multiple of 16 compiles to no rounding:
+// the default build's leaves of 8 keep their code.
+template <uint32_t UNIT>
+__host__ __device__ constexpr uint32_t stage_bytes(uint32_t count) { return UNIT % 16u == 0u ? count * UNIT : (count * UNIT + 15u) & ~15u; }
+
 // mask: bit0 hierarchy (MODE_TREE) / flat records (MODE_BRUTE), bit1 exact geometry, bit2 materials in shared memory
 // frames: the multi-frame kernel's pool also holds Pool.frm
 __host__ __device__ constexpr WfSmem wf_layout(uint32_t n, uint32_t n_pairs, uint32_t n_nodes, uint32_t n_leaves, uint32_t mode, uint32_t mask, bool frames) {
@@ -37,7 +47,7 @@ __host__ __device__ constexpr WfSmem wf_layout(uint32_t n, uint32_t n_pairs, uin
     uint32_t off = 16;   // mbarrier
     L.nodes_off = off;   if (mode == MODE_TREE && (mask & 1u)) off += n_nodes * (uint32_t)(kNodeVec * 16);
     L.leafrec_off = off; if (mode == MODE_TREE && (mask & 1u)) off += n_leaves * (uint32_t)(kLeafK * 16);
-    L.leafid_off = off;  if (mode == MODE_TREE && (mask & 1u)) off += n_leaves * (uint32_t)(kLeafK * 4);
+    L.leafid_off = off;  if (mode == MODE_TREE && (mask & 1u)) off += stage_bytes<kLeafK * 4>(n_leaves);
     L.filt_off = off;    if (mode == MODE_BRUTE && (mask & 1u)) off += n_pairs * 32u;
     L.geo_off = off; if (mask & 2u) off += n * 32u;
     L.mat_off = off; if (mask & 4u) off += n * 32u;
@@ -126,10 +136,10 @@ __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kern
     if (tid < 16) s_cnt[tid] = 0;
     P.lvl[tid] = kDeadLevel;
     __syncthreads();
-    if (tid == 0) {
+    if (tid == 0) {   // the segment sizes of wf_layout, which the mbarrier counts
         const uint32_t b_nodes = (MODE == MODE_TREE && tree_smem) ? p.n_nodes * (uint32_t)(kNodeVec * 16) : 0u;
         const uint32_t b_lrec = (MODE == MODE_TREE && tree_smem) ? p.n_leaves * (uint32_t)(kLeafK * 16) : 0u;
-        const uint32_t b_lid = (MODE == MODE_TREE && tree_smem) ? p.n_leaves * (uint32_t)(kLeafK * 4) : 0u;
+        const uint32_t b_lid = (MODE == MODE_TREE && tree_smem) ? stage_bytes<kLeafK * 4>(p.n_leaves) : 0u;
         const uint32_t b_filt = (MODE == MODE_BRUTE && tree_smem) ? p.n_pairs * 32u : 0u;
         const uint32_t b_geo = (p.scene_in_smem & 2u) ? p.n * 32u : 0u, b_mat = (p.scene_in_smem & 4u) ? p.n * 32u : 0u;
         mbar_arrive_expect_tx(bar, b_nodes + b_lrec + b_lid + b_filt + b_geo + b_mat);

@@ -3,10 +3,13 @@ so each build runs in a process of its own) and writes what it rendered to an .n
 
     python tests/build_worker.py <out.npz>
 
-For every case: "<case>.linear", "<case>.rgb8" (one frame, or [frames, ...]) and, for the adaptive case, "<case>.counts";
-"meta" holds a JSON dict with each case's rays, samples and candidates, the kernel_info() and leaf size of the build, the
-depth of the rebuilt tree, and every case that raised ("errors", with its traceback). The process exits 1 when a case raised.
-The scene makers are the suite's own; CASES is shared with the parent test, which renders the references."""
+For every case: "<case>.linear", "<case>.rgb8" (one frame, or [frames, ...]) and, for the adaptive cases, "<case>.counts";
+"meta" holds a JSON dict with each case's rays, samples and candidates (and the depth of a rebuilt tree; the shared memory
+staging adds and the hierarchy the build stages, for a staged one-frame case), the kernel_info() and leaf size of the build,
+and every case that raised ("errors", with its traceback). The "topology" cases render nothing: they rebuild a scene and hold
+the device's topology to the numpy restatement at the build's leaf size, and raise when it differs. The process exits 1
+when a case raised. The scene makers are the suite's own; CASES is shared with the parent test, which renders the
+references."""
 import json
 import os
 import sys
@@ -24,9 +27,11 @@ import rtb200 as R  # noqa: E402
 from rtb200 import scenes  # noqa: E402
 from test_gpu_adaptive import SCENES as ADAPTIVE_SCENES, _params  # noqa: E402
 from test_gpu_parity import GOLDEN  # noqa: E402
-from test_gpu_rebuild_restatement import _coincident, _deep_dense, _render_stats  # noqa: E402
+from test_gpu_rebuild_restatement import _coincident, _deep_dense, _drifted, _geometry, _render_stats, _scene, rebuilt  # noqa: E402
+from test_gpu_scene_rebuild import _adversarial  # noqa: E402
 from test_gpu_scene_update import _jitter, _light_scene  # noqa: E402
 from test_gpu_work_sets import _room_cfg, _room_frames, _textured_room  # noqa: E402
+from test_rebuild_restatement_cpu import deep_spheres  # noqa: E402
 
 FILTERED, BRUTE, EXACT = R.RT_VARIANT_FILTERED, R.RT_VARIANT_BRUTE_FORCE, R.RT_VARIANT_EXACT_F64
 
@@ -47,33 +52,105 @@ def _unmoved_scene():
     return _light_scene(1, 6, seed=46)
 
 
-# case -> (kind, scene maker, variant). Kinds: "one_shot" (render_linear and render_rgb8), "rebuilt" (a resident handle after
-# rebuild()), "update" (a resident handle after update_spheres), "frames" (render_frames of _room_frames), "adaptive"
-# (render_adaptive with test_gpu_adaptive's parameters).
+# case -> (kind, scene maker, variant, RTB200_WF_SMEM mask). Kinds: "one_shot" (render_linear and render_rgb8), "rebuilt" (a
+# resident handle after rebuild()), "update" (a resident handle after update_spheres), "frames" (render_frames of
+# _room_frames), "adaptive" (render_adaptive with test_gpu_adaptive's parameters), "topology" (see the module docstring).
 CASES = {
-    **{f"golden_{name}": ("one_shot", mk, FILTERED) for name, mk in GOLDEN},
-    "room_3_lights_depth_50": ("one_shot", lambda: R.Scene.from_config(_room_cfg(3, 50)), FILTERED),
-    "room_1_light_depth_10": ("one_shot", lambda: R.Scene.from_config(_room_cfg(1, 10)), FILTERED),
-    "textured_room": ("one_shot", _textured_room, FILTERED),
-    "coincident_10k_1_light": ("one_shot", lambda: _coincident(1), FILTERED),
-    "deep_32768_rebuilt": ("rebuilt", lambda: _deep_dense(32_768, 0), FILTERED),
-    "rtiow_10k_filtered": ("one_shot", _rtiow_10k, FILTERED),
-    "rtiow_10k_brute_force": ("one_shot", _rtiow_10k, BRUTE),
-    "resident_update": ("update", _unmoved_scene, FILTERED),
-    "room_frames": ("frames", lambda: R.Scene.from_config(_room_cfg(3, 50)), FILTERED),
-    "adaptive_mixed_2_lights": ("adaptive", ADAPTIVE_SCENES["mixed_2_lights"], FILTERED),
-    "room_exact_f64": ("one_shot", lambda: R.Scene.from_config(_room_cfg(3, 50)), EXACT),
+    **{f"golden_{name}": ("one_shot", mk, FILTERED, 0) for name, mk in GOLDEN},
+    "room_3_lights_depth_50": ("one_shot", lambda: R.Scene.from_config(_room_cfg(3, 50)), FILTERED, 0),
+    "room_1_light_depth_10": ("one_shot", lambda: R.Scene.from_config(_room_cfg(1, 10)), FILTERED, 0),
+    "textured_room": ("one_shot", _textured_room, FILTERED, 0),
+    "coincident_10k_1_light": ("one_shot", lambda: _coincident(1), FILTERED, 0),
+    # after the rebuild every leaf of the coincident spheres is full (the host builder fills at most 20 of 32 slots): at
+    # leaves of 32 one ray's leaf step yields 32 candidates, RT_CAP_CD of the smallest lists
+    "coincident_10k_rebuilt": ("rebuilt", lambda: _coincident(1), FILTERED, 0),
+    "deep_32768_rebuilt": ("rebuilt", lambda: _deep_dense(32_768, 0), FILTERED, 0),
+    "rtiow_10k_filtered": ("one_shot", _rtiow_10k, FILTERED, 0),
+    "rtiow_10k_brute_force": ("one_shot", _rtiow_10k, BRUTE, 0),
+    "resident_update": ("update", _unmoved_scene, FILTERED, 0),
+    "room_frames": ("frames", lambda: R.Scene.from_config(_room_cfg(3, 50)), FILTERED, 0),
+    "adaptive_mixed_2_lights": ("adaptive", ADAPTIVE_SCENES["mixed_2_lights"], FILTERED, 0),
+    "room_exact_f64": ("one_shot", lambda: R.Scene.from_config(_room_cfg(3, 50)), EXACT, 0),
 }
+
+# Scene staging (RTB200_WF_SMEM) on every build: every mask in both modes that stage bit 0, on scenes whose hierarchy has an
+# odd number of leaves at leaves of 2 (the room) and of 6 (the cover scene), where the leaf-id block is not a whole number
+# of 16 B blocks (tests/test_stress_builds_cpu.py holds that parity); and the multi-frame and list kernels with everything
+# staged. Each renders the frames of the unstaged case it names in BASE.
+STAGE_SCENES = ("golden_cover_40x30_s4", "room_1_light_depth_10")
+BASE = {"rtiow_10k_brute_force": "rtiow_10k_filtered", "room_exact_f64": "room_3_lights_depth_50",
+        "coincident_10k_rebuilt": "coincident_10k_1_light"}
+for _base in STAGE_SCENES:
+    for _mode, _variant in (("tree", FILTERED), ("brute_force", BRUTE)):
+        for _mask in range(1, 8):
+            _name = f"staged_{_base}_{_mode}_m{_mask}"
+            CASES[_name] = ("one_shot", CASES[_base][1], _variant, _mask)
+            BASE[_name] = _base
+for _base in ("room_frames", "adaptive_mixed_2_lights"):
+    CASES[f"staged_{_base}_m7"] = CASES[_base][:3] + (7,)
+    BASE[f"staged_{_base}_m7"] = _base
+
+
+def _drifted_c4():
+    sc = R.Scene.from_config(scenes._variant(scenes.rtiow_config(50), 32, 18, 1, 4))
+    return sc, lambda rs: _geometry(rs, sc, _drifted(sc, 7))
+
+
+# The GPU rebuild at the build's leaf size k against its restatement (tests/test_gpu_rebuild_restatement.py): case ->
+# (k -> the scene, and what to do to the handle before the rebuild, or None)
+TOPOLOGY = {
+    "topology_n_k": lambda k: (_adversarial(f"n{k}"), None),
+    "topology_n_k_plus_1": lambda k: (_adversarial(f"n{k + 1}"), None),
+    "topology_coincident": lambda k: (_adversarial("coincident"), None),
+    "topology_deep_32768": lambda k: (_scene(*deep_spheres(32_768)), None),
+    "topology_c4_drifted": lambda k: _drifted_c4(),
+}
+CASES.update({name: ("topology", mk, FILTERED, 0) for name, mk in TOPOLOGY.items()})
 
 
 def _stats(st):
     return {k: int(st[k]) for k in ("rays", "samples", "candidates")}
 
 
-def run_case(name, out, meta):
-    kind, mk, variant = CASES[name]
+def _kernel_info(sc, variant, mask):
+    rs = R.ResidentScene(sc, R.make_options(variant=variant))
+    try:
+        return rs.kernel_info()
+    finally:
+        rs.release()
+
+
+def run_case(name, out, meta, leaf_size):
+    kind, mk, variant, mask = CASES[name]
+    if kind == "topology":
+        sc, prepare = mk(leaf_size)
+        rs = R.ResidentScene(sc)
+        try:
+            if prepare:
+                prepare(rs)
+            meta[name] = {"depth": int(rebuilt(rs, sc, leaf_size=leaf_size)["depth"])}
+        finally:
+            rs.release()
+        return
     opts = R.make_options(variant=variant)
     sc = mk()
+    if mask:
+        base = _kernel_info(sc, variant, 0)
+        os.environ["RTB200_WF_SMEM"] = str(mask)   # read at every upload
+    try:
+        if mask:
+            ki = _kernel_info(sc, variant, mask)
+            t = R.bvh_records(sc)
+            staged = dict(smem_mask=int(ki["smem_mask"]), smem_staged=int(ki["smem_bytes"] - base["smem_bytes"]),
+                          records={k: int(t[k]) for k in ("n_nodes", "n_leaves", "leaf_size")})
+        render_case(name, kind, sc, opts, out, meta)
+    finally:
+        os.environ.pop("RTB200_WF_SMEM", None)
+    if mask:
+        meta[name].update(staged)
+
+
+def render_case(name, kind, sc, opts, out, meta):
     if kind == "one_shot":
         lin, st = R.render_linear(sc, opts)
         img, st8 = R.render_rgb8(sc, opts)
@@ -81,14 +158,15 @@ def run_case(name, out, meta):
     elif kind in ("rebuilt", "update"):
         rs = R.ResidentScene(sc, opts)
         try:
+            extra = {}
             if kind == "rebuilt":
                 rs.rebuild()
-                meta["rebuilt_depth"] = int(rs.topology()["depth"])
+                extra["depth"] = int(rs.topology()["depth"])
             else:
                 _, idx, recs = moved_scene()
                 rs.update_spheres(idx, recs)
             (img, lin, _), st = _render_stats(rs)
-            meta[name] = _stats(st)
+            meta[name] = dict(_stats(st), **extra)
         finally:
             rs.release()
     elif kind == "frames":
@@ -108,13 +186,14 @@ def run_case(name, out, meta):
 
 def main(path):
     out, meta = {}, {"errors": {}}
+    os.environ.pop("RTB200_WF_SMEM", None)
     info = R.ResidentScene(scenes.cover_scene(32, 24, 1), R.make_options(variant=FILTERED))
     meta["kernel_info"] = info.kernel_info()
     info.release()
     meta["leaf_size"] = int(R.bvh_records(scenes.cover_scene(32, 24, 1))["leaf_size"])
     for name in CASES:
         try:
-            run_case(name, out, meta)
+            run_case(name, out, meta, meta["leaf_size"])
         except Exception:
             meta["errors"][name] = traceback.format_exc()
             print(f"[build_worker] {name} raised:\n{meta['errors'][name]}", file=sys.stderr, flush=True)

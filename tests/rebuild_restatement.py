@@ -4,7 +4,8 @@ columns, frame membership and the always-list, the 64-bit keys (oversized bit | 
 (radix split points on the first 13 wide levels, three rounds of halving below) and the numbering by scans. rebuild()
 returns a dict in the layout of ResidentScene.bvh_records(), with placeholder boxes and records that
 test_scene_update_cpu.refit fills in. check_tree() holds every invariant of a rebuilt topology that the traversal, the refit
-and the rebuild's own buffer sizes (rebuild_carve) rely on; it is used on the restatement and on the device's arrays."""
+and the rebuild's own buffer sizes (rebuild_carve) rely on; it is used on the restatement and on the device's arrays. Both
+take the leaf size of the library (RT_LEAF_K, bvh_records()["leaf_size"]) as an argument; the node width is fixed."""
 import bisect
 
 import numpy as np
@@ -12,7 +13,8 @@ import numpy as np
 from test_bvh_cpu import _exact_hits, _traverse
 from test_scene_update_cpu import refit, same_bits, sphere_boxes
 
-K = WIDE = 8                        # leaf size and node width
+K = 8                               # the default build's leaf size (RT_LEAF_K)
+WIDE = 8                            # node width
 MAX_DEPTH = 21                      # wide levels the trace's node stack reserve allows
 RADIX_LEVELS = 13                   # wide levels split at radix split points; halving below
 ID_BITS = 26                        # sphere index bits of a key
@@ -80,13 +82,13 @@ def _split_point(keys, f, l):
     return bisect.bisect_left(keys, ((keys[f] >> b) | 1) << b, f, l + 1) - f
 
 
-def _children(keys, level, f, cnt):
+def _children(keys, level, f, cnt, k):
     ch = [(f, cnt)]
     if level < RADIX_LEVELS:
         while len(ch) < WIDE:
             best = None                                  # shortest common prefix, then the larger range
             for i, (cf, cc) in enumerate(ch):
-                if cc > K:
+                if cc > k:
                     rank = (_prefix(keys, cf, cf + cc - 1), -cc)
                     if best is None or rank < best[0]:
                         best = (rank, i)
@@ -100,17 +102,19 @@ def _children(keys, level, f, cnt):
         for _ in range(3):
             for i in range(len(ch) - 1, -1, -1):         # right to left: the new right part is not revisited this round
                 cf, cc = ch[i]
-                if cc > K:
+                if cc > k:
                     left = cc - cc // 2
                     ch[i:i + 1] = [(cf, left), (cf + left, cc - left)]
     return ch
 
 
-def rebuild(c, r, oversize=OVERSIZE):
-    """The topology the GPU rebuild makes of spheres (c [n, 3], r [n]) in the layout of ResidentScene.bvh_records(), with
-    lo/hi (+inf, -inf) everywhere, leaf records zero with nk = -inf in padding slots, and "level_count" (nodes per level,
+def rebuild(c, r, oversize=OVERSIZE, leaf_size=K):
+    """The topology the GPU rebuild of a library with leaves of `leaf_size` makes of spheres (c [n, 3], r [n]) in the
+    layout of ResidentScene.bvh_records(), with lo/hi (+inf, -inf) everywhere, leaf records zero with nk = -inf in padding slots, and "level_count" (nodes per level,
     root first) and "r_big" for the tests. Levels are built until no node is left: a depth above MAX_DEPTH is reported,
     not cut."""
+    k = leaf_size
+    assert k % 2 == 0 and 2 <= k <= 32, k
     c = np.asarray(c, np.float64).reshape(-1, 3)
     r = np.asarray(r, np.float64)
     n = len(r)
@@ -124,8 +128,8 @@ def rebuild(c, r, oversize=OVERSIZE):
         base, nxt = len(rows), []
         for f, cnt in tasks:
             row = [EMPTY] * WIDE
-            for s, (cf, cc) in enumerate(_children(keys, level, f, cnt)):
-                if cc > K:
+            for s, (cf, cc) in enumerate(_children(keys, level, f, cnt, k)):
+                if cc > k:
                     row[s] = base + len(tasks) + len(nxt)
                     nxt.append((cf, cc))
                 else:
@@ -138,22 +142,22 @@ def rebuild(c, r, oversize=OVERSIZE):
     nl = len(leaves)
     child = np.array(rows, np.uint32).reshape(nn, WIDE)
     ids = (skeys & np.uint64((1 << ID_BITS) - 1)).astype(np.int64)
-    leaf_id = np.full((nl, K), EMPTY, np.uint32)
+    leaf_id = np.full((nl, k), EMPTY, np.uint32)
     skip = np.full(max(n, 1), NO_SKIP, np.uint32)
     for leaf, (f, cnt, node, s) in enumerate(leaves):
         child[node, s] = LEAF | leaf
         m = np.sort(ids[f:f + cnt])
         leaf_id[leaf, :cnt] = m
-        skip[m] = leaf * K + np.arange(cnt)
+        skip[m] = leaf * k + np.arange(cnt)
         if cnt == 1:
             skip[m[0]] = SKIP_NODE | (node * WIDE + s)
-    leaf_rec = np.zeros((nl, K // 2, 2, 4), np.float32)
-    for j in range(K):
+    leaf_rec = np.zeros((nl, k // 2, 2, 4), np.float32)
+    for j in range(k):
         leaf_rec[:, j // 2, 1, 2 + j % 2] = np.where(leaf_id[:, j] == EMPTY, -np.inf, 0.0)
     starts = np.concatenate([[0], np.cumsum(level_count)]).astype(np.int64)
-    level_nodes = np.concatenate([np.arange(starts[k], starts[k + 1]) for k in range(depth - 1, -1, -1)] or [np.zeros(0)])
+    level_nodes = np.concatenate([np.arange(starts[j], starts[j + 1]) for j in range(depth - 1, -1, -1)] or [np.zeros(0)])
     level_off = np.concatenate([[0], np.cumsum(level_count[::-1])])
-    return {"n": n, "leaf_size": K, "recentre": g, "r_big": r_big, "always": always, "n_nodes": nn, "n_leaves": nl,
+    return {"n": n, "leaf_size": k, "recentre": g, "r_big": r_big, "always": always, "n_nodes": nn, "n_leaves": nl,
             "depth": depth, "level_count": level_count, "child": child, "leaf_id": leaf_id, "skip_pos": skip,
             "level_nodes": level_nodes.astype(np.uint32), "level_off": level_off.astype(np.uint32),
             "lo": np.full((nn, 3, WIDE), np.inf, np.float32), "hi": np.full((nn, 3, WIDE), -np.inf, np.float32),
@@ -180,15 +184,16 @@ def skip_rule(t, n):
     return skip
 
 
-def check_tree(t, c, r, rays=0, cam=None, seed=11):
-    """Every invariant of a rebuilt topology t (a dict in the layout of ResidentScene.bvh_records()) for spheres (c, r):
-    each sphere in exactly one leaf or on the always-list, members in increasing index, padding records that never hit,
-    the level order and its depth, children deeper than their parents, the skip_pos rule, the sizes rebuild_carve
-    allocates (n_leaves <= n, n_nodes <= max(n, 1), at most n // 9 + 1 inner nodes per level), and values equal to the
-    numpy refit. With rays, the float32 traversal emulation must reach every sphere the exact f64 test accepts."""
+def check_tree(t, c, r, rays=0, cam=None, seed=11, leaf_size=K):
+    """Every invariant of a rebuilt topology t (a dict in the layout of ResidentScene.bvh_records()) with leaves of
+    `leaf_size` for spheres (c, r): leaves of that size, each sphere in exactly one leaf or on the always-list, members in
+    increasing index, padding records that never hit, the level order and its depth, children deeper than their parents,
+    the skip_pos rule, the sizes rebuild_carve allocates (n_leaves <= n, n_nodes <= max(n, 1), at most
+    n // (leaf_size + 1) + 1 inner nodes per level), and values equal to the numpy refit. With rays, the float32 traversal emulation must reach every sphere the exact f64 test accepts."""
     c = np.asarray(c, np.float64).reshape(-1, 3)
     r = np.asarray(r, np.float64)
     n = len(r)
+    assert t["leaf_size"] == leaf_size and t["leaf_id"].shape == (t["n_leaves"], leaf_size), (t["leaf_size"], t["leaf_id"].shape)
     ids = t["leaf_id"].ravel()
     assert sorted(np.concatenate([ids[ids != EMPTY], t["always"]]).tolist()) == list(range(n))   # in exactly one leaf or always
     assert np.all(np.diff(t["always"].astype(np.int64)) > 0), "the always-list is in increasing index order"
@@ -202,7 +207,7 @@ def check_tree(t, c, r, rays=0, cam=None, seed=11):
     assert depth <= MAX_DEPTH and len(t["level_off"]) == depth + 1 and t["level_off"][-1] == nn
     assert t["n_leaves"] <= n and nn <= max(n, 1)
     per_level = np.diff(t["level_off"].astype(np.int64))
-    assert np.all(per_level >= 1) and np.all(per_level <= n // (K + 1) + 1), per_level
+    assert np.all(per_level >= 1) and np.all(per_level <= n // (leaf_size + 1) + 1), per_level
     assert sorted(t["level_nodes"].tolist()) == list(range(nn))
     level = np.empty(nn, np.int64)
     for k in range(depth):                                     # deepest first

@@ -5,8 +5,11 @@ stacks, deferred scatters - through every kernel (one frame, many frames, the ad
 
 The library is chosen when rtb200 is imported (RTB200_LIB), so each build renders in a process of its own
 (tests/build_worker.py); this process renders the references once per module. Each build also proves that it is the build
-its DEFS describe: its block size, its shared-memory layout (wf_layout restated below), its leaf size, and, for lists_min,
-that its edges were reached."""
+its DEFS describe: its block size, its shared-memory layout (wf_layout restated below, and the staged arrays of
+test_gpu_scene_staging.staged_bytes), its leaf size, the depth the restatement gives its rebuilt deep tree, and, for the
+builds with the smallest lists, that their edges were reached. Every build also stages the scene in shared memory (every
+RTB200_WF_SMEM mask) and rebuilds topologies the numpy restatement checks at its leaf size (build_worker's "topology"
+cases)."""
 import json
 import os
 import re
@@ -20,14 +23,16 @@ import adaptive_restatement as A
 import build_worker as BW
 import oracle_py as O
 from test_gpu_adaptive import M, MIN, N, _samples
+from test_gpu_scene_staging import staged_bytes
 from test_gpu_shading_edges import assert_frames_match
 from test_gpu_work_sets import _deep, _room_frames, _view
+from test_rebuild_restatement_cpu import DEEP_AT
 
 pytestmark = pytest.mark.gpu
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 STRESS = os.path.join(REPO, "rust-raytracer_b200", "stress")
 GOLD = os.path.join(REPO, "tests", "golden")
-BUILDS = ["lists_min", "leaf2", "block128_leaf16"]
+BUILDS = ["lists_min", "leaf2", "block128_leaf16", "leaf6", "leaf32_lists_min"]
 TIMEOUT = 900   # seconds per build; every case of a build takes well under a minute on an H100
 
 # the constants as the sources define them when DEFS leave them alone
@@ -57,16 +62,15 @@ def test_the_default_layout_is_the_one_design_md_gives():
 
 
 # ---- references, rendered once per module ----
-SAME_SCENE = {"room_exact_f64": "room_3_lights_depth_50", "rtiow_10k_brute_force": "rtiow_10k_filtered"}
 _REF = {}
 
 
 def reference(name):
     """{linear, rgb8, rays, samples[, counts]} that case `name` must render; frames carry a leading frame axis."""
-    name = SAME_SCENE.get(name, name)
+    name = BW.BASE.get(name, name)
     if name in _REF:
         return _REF[name]
-    kind, mk, _ = BW.CASES[name]
+    kind, mk = BW.CASES[name][:2]
     if name.startswith("golden_"):
         g = np.load(os.path.join(GOLD, name[len("golden_"):] + ".npz"))
         sc = mk()
@@ -148,20 +152,38 @@ def test_stress_build_renders_the_oracle_frames(build, tmp_path):
 
     failures = []
     for name in BW.CASES:
+        if BW.CASES[name][0] == "topology":   # checked in the worker: a difference raises there
+            continue
         try:
             compare(name, z, meta)
         except AssertionError as e:
             failures.append(f"{name}: {e}")
-    per_ray = {name: round(meta[name]["candidates"] / max(meta[name]["rays"], 1), 1) for name in BW.CASES}
+    rendered = [name for name in BW.CASES if BW.CASES[name][0] != "topology"]
+    per_ray = {name: round(meta[name]["candidates"] / max(meta[name]["rays"], 1), 1) for name in rendered}
     scatters = sum(int(x) for x in re.findall(r"scatters=(\d+)", stderr))
     deferred = sum(int(x) for x in re.findall(r"deferred=(\d+)", stderr))
-    print(f"{build}: {c}\n  candidates per ray {per_ray}\n  rebuilt depth {meta['rebuilt_depth']}; "
+    depths = {name: meta[name]["depth"] for name in BW.CASES if "depth" in meta[name]}
+    print(f"{build}: {c}\n  candidates per ray {per_ray}\n  rebuilt depths {depths}; "
           f"scatters {scatters}, deferred {deferred} ({deferred / max(scatters, 1):.4f})")
     assert not failures, "\n".join(failures)
 
+    k = c["RT_LEAF_K"]
+    for name in BW.CASES:   # staging added exactly the arrays of the hierarchy this build makes, in whole 16 B blocks
+        kind, mk, variant, mask = BW.CASES[name]
+        if mask and kind == "one_shot":
+            m = meta[name]
+            assert m["records"]["leaf_size"] == k and m["smem_mask"] == mask, (name, m)
+            assert m["smem_staged"] == staged_bytes(mk(), variant, mask, m["records"]), (name, m)
+    if k * 4 % 16:   # the staged leaf-id block was 8 B short of a 16 B multiple in a staged scene
+        assert any(meta[f"staged_{s}_tree_m1"]["records"]["n_leaves"] % 2 for s in BW.STAGE_SCENES)
+    # the rebuilt deep tree is as deep as the restatement's at this leaf size
+    assert depths["deep_32768_rebuilt"] == depths["topology_deep_32768"] == DEEP_AT[k][32_768], depths
+
+    if c["RT_CAP_CD"] == 32:   # the smallest lists: a ray's candidates overflow the candidate list many times over
+        for name in ("coincident_10k_1_light", "coincident_10k_rebuilt"):
+            assert per_ray[name] >= 300 > c["RT_CAP_CD"], per_ray
     if build == "lists_min":   # the edges this build is made for were reached
-        assert per_ray["coincident_10k_1_light"] >= 300 > c["RT_CAP_CD"], per_ray
-        assert meta["rebuilt_depth"] >= 14, meta["rebuilt_depth"]   # fat_in = 187 - 7 * 14 - 8 = 81 node-stack entries
+        assert depths["deep_32768_rebuilt"] >= 14, depths   # fat_in = 187 - 7 * 14 - 8 = 81 node-stack entries
         # One trip is two rejection trials, both missing the unit sphere with probability (1 - pi/6)^2 = 0.2270. Over these
         # cases an H100 (at its default power limit) measured 3,211,706 deferred of 14,154,171 scatters: 0.2269.
         assert scatters > 0 and 0.20 <= deferred / scatters <= 0.25, (scatters, deferred, stderr[-2000:])

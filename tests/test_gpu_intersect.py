@@ -370,12 +370,22 @@ def test_device_form_refuses_host_pointers():
         rs.release()
 
 
-def test_stress_builds_answer_queries_exactly(tmp_path):
+def test_stress_builds_answer_dense_and_rebuilt_queries_exactly(tmp_path):
+    """Every stress build answers the 10k-sphere scene's queries, and the dense scenes' as uploaded and after rebuild(), bit
+    for bit like the oracle; with the smallest lists the coincident spheres overflow the candidate list many times over."""
+    from test_gpu_build_invariance import constants
     manifest = json.load(open(os.path.join(STRESS, "manifest.json")))
     sc = IW.c4_scene()
     o, d = IW.c4_rays(sc)
     want = IR.oracle(sc, o, d)
+    wants = {}
+    for name, (mk, rays, _) in IW.SETS.items():
+        s = mk()
+        so, sd = rays(s)
+        wants[name] = IR.oracle(s, so, sd)
+        assert (wants[name]["sphere"] >= 0).sum() > 1000, name
     for name in manifest:
+        c = constants(manifest[name])
         out = tmp_path / f"{name}.npz"
         env = dict(os.environ, RTB200_LIB=os.path.join(STRESS, f"librtb200_{name}.so"))
         subprocess.run([sys.executable, os.path.join(REPO, "tests", "intersect_worker.py"), str(out)], env=env, check=True, timeout=900)
@@ -384,4 +394,10 @@ def test_stress_builds_answer_queries_exactly(tmp_path):
         for v in ("filtered", "brute"):
             IR.assert_hits_equal({k: z[f"{v}.{k}"] for k in IR.FIELDS}, want, f"{name}/{v}")
             assert meta[v]["rays"] == len(o)
-        assert meta["leaf_size"] == (2 if name == "leaf2" else 16 if name == "block128_leaf16" else 8)
+        for s, w in wants.items():
+            IR.assert_hits_equal({k: z[f"{s}.{k}"] for k in IR.FIELDS}, w, f"{name}/{s}")
+            assert meta[s]["rays"] == len(w["sphere"])
+        assert meta["leaf_size"] == c["RT_LEAF_K"]
+        if c["RT_CAP_CD"] == 32:
+            for s in ("coincident", "coincident_rebuilt"):
+                assert meta[s]["candidates"] / meta[s]["rays"] > c["RT_CAP_CD"], (name, s, meta[s])

@@ -11,7 +11,7 @@ import pytest
 import oracle_py as O
 import rtb200 as R
 from rtb200 import scenes
-from rebuild_restatement import check_tree, rebuild
+from rebuild_restatement import K, check_tree, rebuild
 from synth import base_config, mixed_config
 from test_gpu_scene_rebuild import _adversarial, _move_all, _objs
 from test_gpu_scene_update import _assert_same, _fresh, _positions
@@ -33,12 +33,12 @@ def assert_same_topology(dev, want):
         assert not len(bad), (key, f"{len(bad)} words differ, first at {np.unravel_index(bad[0], a.shape)}")
 
 
-def rebuilt(rs, sc, oversize=None):
+def rebuilt(rs, sc, oversize=None, leaf_size=K):
     """Rebuild rs, whose spheres are sc's, and check the device's topology against the restatement and its values
-    against the numpy refit; returns the device's records."""
+    against the numpy refit, at the library's leaf size; returns the device's records."""
     if oversize is None:
         rs.rebuild()
-        want = rebuild(*_positions(sc))
+        want = rebuild(*_positions(sc), leaf_size=leaf_size)
     else:
         old = os.environ.get("RTB200_REBUILD_OVERSIZE")
         os.environ["RTB200_REBUILD_OVERSIZE"] = str(oversize)
@@ -49,10 +49,10 @@ def rebuilt(rs, sc, oversize=None):
                 del os.environ["RTB200_REBUILD_OVERSIZE"]
             else:
                 os.environ["RTB200_REBUILD_OVERSIZE"] = old
-        want = rebuild(*_positions(sc), oversize=oversize)
+        want = rebuild(*_positions(sc), oversize=oversize, leaf_size=leaf_size)
     dev = rs.bvh_records()
     assert_same_topology(dev, want)
-    check_tree(dev, *_positions(sc))
+    check_tree(dev, *_positions(sc), leaf_size=leaf_size)
     return dev
 
 

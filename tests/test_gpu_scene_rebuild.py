@@ -217,7 +217,7 @@ def _objs(centres, radii):
 
 def _adversarial(kind):
     rng = np.random.default_rng(21)
-    if kind in ("n1", "n8", "n9"):
+    if kind[1:].isdigit():                            # n<m>: m spheres (n1, and n = leaf size and one more)
         m = int(kind[1:])
         c = rng.uniform(-2, 2, size=(m, 3)); c[:, 1] = np.abs(c[:, 1]); r = rng.uniform(0.2, 0.6, m)
     elif kind == "coincident":

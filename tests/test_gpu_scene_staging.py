@@ -29,14 +29,20 @@ def oracle(name):
     return _ORACLE[name]
 
 
-def staged_bytes(sc, variant, mask):
-    """The arrays wf_layout adds for `mask`: 224 B per node and 8 * (16 + 4) B per leaf of the hierarchy (MODE_TREE) or 32 B
-    per flat record pair (MODE_BRUTE) for bit 0, 32 B per sphere for bits 1 and 2."""
+def _round16(b):
+    return (b + 15) // 16 * 16
+
+
+def staged_bytes(sc, variant, mask, t=None):
+    """The arrays wf_layout adds for `mask`: 224 B per node, k * 16 B of records and k * 4 B of ids per leaf of k spheres
+    (MODE_TREE) or 32 B per flat record pair (MODE_BRUTE) for bit 0, 32 B per sphere for bits 1 and 2. Each array is staged
+    with one bulk copy, so it takes a multiple of 16 B: the leaf ids of an odd number of leaves of 2, 6, 10, ... spheres
+    take 8 B more. t: the scene's hierarchy as the library that stages it builds it (default: R.bvh_records(sc))."""
     n = sc.n_spheres
     b = 0
     if mask & 1 and variant == FILTERED:
-        t = R.bvh_records(sc)
-        b += t["n_nodes"] * 224 + t["n_leaves"] * t["leaf_size"] * 20
+        t = R.bvh_records(sc) if t is None else t
+        b += t["n_nodes"] * 224 + t["n_leaves"] * t["leaf_size"] * 16 + _round16(t["n_leaves"] * t["leaf_size"] * 4)
     if mask & 1 and variant == BRUTE:
         b += max(((n + 1) // 2 + 7) // 8 * 8, 8) * 32
     return b + (32 * n if mask & 2 else 0) + (32 * n if mask & 4 else 0)

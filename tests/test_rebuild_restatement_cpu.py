@@ -3,7 +3,8 @@
 be as deep as the key layout allows, the rebuilt tree keeps the depth bound the trace's node stack relies on and the sizes
 rebuild_carve allocates, and the float32 traversal of the refitted tree never drops a sphere the exact f64 test accepts.
 The host builder chooses the same recentring offset as the rebuild. The GPU tests compare the device's topology with this
-restatement byte for byte."""
+restatement byte for byte. The edge cases and the deep constructions also run at every leaf size the stress builds use.
+"""
 import numpy as np
 import pytest
 
@@ -158,6 +159,64 @@ def test_deep_constructions_reach_their_depth(n):
     assert max(t["level_count"]) <= n // (K + 1) + 1 and t["n_leaves"] <= n and t["n_nodes"] <= n
     if n <= 32_768:
         check_tree(filled(t, c, r), c, r)
+
+
+LEAF_SIZES = [2, 6, 8, 16, 32]   # RT_LEAF_K of the default build (8) and of the stress builds
+# depth of the rebuilt tree of deep_spheres(n) at each leaf size: below leaves of 8 the peeled octants split further; from
+# leaves of 16 up the 8 spheres of a peeled octant fit one leaf and the last cell needs fewer levels
+DEEP_AT = {2: {4_096: 14, 32_768: 15, 262_144: 16}, 6: {4_096: 14, 32_768: 15, 262_144: 16},
+           8: {4_096: 13, 32_768: 14, 262_144: 15}, 16: {4_096: 8, 32_768: 9, 262_144: 10},
+           32: {4_096: 7, 32_768: 8, 262_144: 9}}
+
+
+def _edge_case(kind, k):
+    if kind == "n_k":
+        return _uniform(k)
+    if kind == "n_k_plus_1":
+        return _uniform(k + 1)
+    return _case(kind)
+
+
+@pytest.mark.parametrize("kind", ["n_k", "n_k_plus_1", "coincident", "exponential", "line"])
+@pytest.mark.parametrize("k", LEAF_SIZES)
+def test_the_rebuilt_tree_at_every_leaf_size(k, kind):
+    c, r = _edge_case(kind, k)
+    t = filled(rebuild(c, r, leaf_size=k), c, r)
+    n = len(r)
+    check_tree(t, c, r, leaf_size=k)
+    assert t["leaf_size"] == k and t["leaf_id"].shape == (t["n_leaves"], k)
+    assert max(t["level_count"]) <= n // (k + 1) + 1 and t["depth"] <= MAX_DEPTH
+    if kind == "n_k":          # one leaf under the root holds them all
+        assert (t["n_nodes"], t["n_leaves"], t["depth"]) == (1, 1, 1)
+    if kind == "n_k_plus_1":   # the root splits them
+        assert t["n_nodes"] == 1 and t["n_leaves"] >= 2
+    if kind != "coincident":
+        assert sound(t, c, r, 40, [13.0, 2.0, 3.0] if kind[0] == "n" else [0.3, 2.0, 6.0]) > 0
+
+
+def test_the_rebuild_fills_the_coincident_leaves_of_32():
+    """10,000 coincident spheres rebuild into leaves of 32 that are all full but the remainder of 16 (and, in the
+    build-invariance case coincident_10k_rebuilt, the light's own leaf): a ray through them makes one leaf step yield 32
+    candidates, which fills RT_CAP_CD = 32 of the smallest lists exactly."""
+    c = np.tile([[0.0, 0.5, 0.0]], (10_000, 1))
+    r = np.full(10_000, 0.5)
+    for light, leaves, fills in ((False, 313, [16] + [32] * 312), (True, 314, [1, 16] + [32] * 312)):
+        if light:
+            c, r = np.concatenate([c, [[2.0, 3.0, 0.0]]]), np.concatenate([r, [0.7]])
+        t = rebuild(c, r, leaf_size=32)
+        fill = (t["leaf_id"] != 0xFFFFFFFF).sum(axis=1)
+        assert t["n_leaves"] == leaves and sorted(fill.tolist()) == fills, (t["n_leaves"], np.bincount(fill))
+
+
+@pytest.mark.parametrize("n", [4_096, 32_768, 262_144])
+@pytest.mark.parametrize("k", LEAF_SIZES)
+def test_deep_constructions_at_every_leaf_size(k, n):
+    c, r = deep_spheres(n)
+    t = rebuild(c, r, leaf_size=k)
+    assert t["depth"] == DEEP_AT[k][n], t["level_count"]
+    assert max(t["level_count"]) <= n // (k + 1) + 1 and t["n_leaves"] <= n and t["n_nodes"] <= n
+    if n == 4_096:
+        check_tree(filled(t, c, r), c, r, leaf_size=k)
 
 
 def _drift(c, r, rng, scale):

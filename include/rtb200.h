@@ -350,6 +350,13 @@ int rtb200_scene_intersect_device(rtb200_scene_handle h, const rt_rays* rays, ui
  * memory kind; a traversal-guard trip fails the call with RT_ERR_CUDA. */
 int rtb200_scene_intersect(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_hits* out, rt_stats* stats);
 
+/* Occlusion queries on a resident scene (DESIGN.md §4.11). For ray i (origin, direction, t_max as in rt_rays; a NULL t_max is
+ * f64::MAX, a bound above f64::MAX counts as f64::MAX) occluded[i] = 1 if hit_world(world, Ray{o, d}, 0.001, t_max_i) is Some
+ * over the handle's CURRENT spheres, else 0, in every variant. Same ordering, memory-kind checks and guard-trip reporting as
+ * rtb200_scene_intersect[_device]; n == 0 is a no-op. */
+int rtb200_scene_occluded_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, uint8_t* occluded, void* stream);
+int rtb200_scene_occluded(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, uint8_t* occluded, rt_stats* stats);
+
 /* load_texture_image — materials.rs:213-219, config.rs:36-47: decode a baseline JPEG file to RGB8 (host-side scene staging
  * helper for hosts without their own decoder; the reference uses the jpeg-decoder crate). *out_rgb8 is released with rtb200_free(). */
 int  rtb200_decode_jpeg_file(const char* path, uint8_t** out_rgb8, uint64_t* width, uint64_t* height);

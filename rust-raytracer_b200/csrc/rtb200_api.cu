@@ -94,11 +94,11 @@ struct DeviceCtx {
     std::vector<OccKey> occ_cache;        // cudaOccupancyMaxActiveBlocksPerMultiprocessor answers
     PinnedBuf staging;                    // host image of the arena being uploaded
     cudaEvent_t staging_free = nullptr;   // the last H2D copy out of `staging` has finished
-    // the host form of rtb200_scene_intersect: rays, hits and counters on the device, its timing events (created at its first
-    // call), and the resident CTAs per SM of the query kernel of each mode (0: not asked yet)
+    // the host form of rtb200_scene_intersect and rtb200_scene_occluded: rays, outputs and counters on the device, its timing
+    // events (created at its first call), and the resident CTAs per SM of the query kernel of each kind and mode (0: not asked yet)
     GrowBuf query;
     cudaEvent_t query_ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    int query_occ[3] = {0, 0, 0};
+    int query_occ[2][3] = {{0, 0, 0}, {0, 0, 0}};   // [closest-hit, occlusion][mode]
 };
 DeviceCtx g_ctx[64];
 std::mutex g_ctx_mu;
@@ -1120,51 +1120,87 @@ int rtb200_scene_rebuild(rtb200_scene_handle h, void* stream_in) {
   });
 }
 
-// ---- closest-hit queries on a resident scene (DESIGN.md §4.10) ----
-// The argument checks both forms share (no device is touched).
-static int check_query(rtb200_scene_handle h, const rt_rays* rays, const rt_hits* out) {
+// ---- closest-hit and occlusion queries on a resident scene (DESIGN.md §4.10, §4.11) ----
+// What a query writes: the outputs of rt_hits (closest-hit), or the occlusion bits. Output k is ptr[k], bytes[k] per ray.
+struct QueryOut {
+    bool any;             // occlusion
+    rt_hits hits;         // closest-hit
+    uint8_t* occluded;    // occlusion
+    int count;
+    void* ptr[6];
+    uint32_t bytes[6];
+    const char* name[6];
+};
+static QueryOut hits_out(const rt_hits& o) {
+    QueryOut q{false, o, nullptr, 6, {o.t, o.sphere, o.point, o.normal, o.uv, o.front_face}, {8, 4, 24, 24, 16, 1},
+               {"out->t", "out->sphere", "out->point", "out->normal", "out->uv", "out->front_face"}};
+    return q;
+}
+static QueryOut occluded_out(uint8_t* o) {
+    QueryOut q{true, rt_hits{}, o, 1, {o}, {1}, {"occluded"}};
+    return q;
+}
+// the same outputs at other addresses (the host form's device image)
+static QueryOut with_ptrs(const QueryOut& o, char* const* p) {
+    if (o.any) return occluded_out((uint8_t*)p[0]);
+    return hits_out(rt_hits{(double*)p[0], (uint32_t*)p[1], (double*)p[2], (double*)p[3], (double*)p[4], (uint8_t*)p[5]});
+}
+
+// The argument checks both forms of both kinds share (no device is touched).
+static int check_query(rtb200_scene_handle h, const rt_rays* rays, const QueryOut* out) {
     if (!h) return fail(RT_ERR_INVALID, "null scene handle");
     if (!rays || !out) return fail(RT_ERR_INVALID, "rays or out is null");
     if (!rays->origin || !rays->direction) return fail(RT_ERR_INVALID, "rays->origin or rays->direction is null");
-    if (!out->t && !out->sphere && !out->point && !out->normal && !out->uv && !out->front_face)
-        return fail(RT_ERR_INVALID, "every output of out is null");
+    bool any_out = false;
+    for (int k = 0; k < out->count; ++k) any_out = any_out || out->ptr[k];
+    if (!any_out) return fail(RT_ERR_INVALID, out->any ? "occluded is null" : "every output of out is null");
     return RT_OK;
 }
 
 // The one path of both forms: enqueue the query of the n rays `rays` into `out` (device buffers) on `st`, which the caller has
 // ordered after the scene's last writer (scene_stream). Guard trips go to err[1], the counters to stat (null: not counted).
-static int query_enqueue(rtb200_scene_handle h, const rt_rays& rays, uint32_t n, const rt_hits& out, unsigned long long* stat,
+static int query_enqueue(rtb200_scene_handle h, const rt_rays& rays, uint32_t n, const QueryOut& out, unsigned long long* stat,
                          unsigned long long* err, cudaStream_t st) {
-    int& occ = h->ctx->query_occ[h->mode];
-    if (occ == 0) occ = query_max_ctas_per_sm(h->mode);
+    int& occ = h->ctx->query_occ[out.any ? 1 : 0][h->mode];
+    if (occ == 0) occ = query_max_ctas_per_sm(h->mode, out.any);
     if (occ <= 0) { occ = 0; return fail(RT_ERR_UNSUPPORTED, "no launch configuration of the query kernel fits shared memory"); }
+    const int max_grid = h->ctx->sm_count * occ;
+    if (out.any) {
+        OcclusionParams q{};
+        q.p = h->tp; q.p.stat = stat; q.p.err = err;
+        q.origin = rays.origin; q.direction = rays.direction; q.t_max = rays.t_max;
+        q.occluded = out.occluded;
+        q.n = n;
+        CU(launch_occluded(q, h->mode, max_grid, st));
+        return RT_OK;
+    }
     QueryParams q{};
     q.p = h->tp; q.p.stat = stat; q.p.err = err;
     q.origin = rays.origin; q.direction = rays.direction; q.t_max = rays.t_max;
-    q.t = out.t; q.sphere = out.sphere; q.point = out.point; q.normal = out.normal; q.uv = out.uv; q.front_face = out.front_face;
+    const rt_hits& o = out.hits;
+    q.t = o.t; q.sphere = o.sphere; q.point = o.point; q.normal = o.normal; q.uv = o.uv; q.front_face = o.front_face;
     q.n = n;
-    CU(launch_query(q, h->mode, h->ctx->sm_count * occ, st));
+    CU(launch_query(q, h->mode, max_grid, st));
     return RT_OK;
 }
 
-int rtb200_scene_intersect_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_hits* out, void* stream_in) {
-  return guarded([&]() -> int {
+// The device form of both kinds.
+static int query_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const QueryOut* out, void* stream_in) {
     int rc = check_query(h, rays, out);
     if (rc != RT_OK) return rc;
     if (n == 0) return RT_OK;
     DeviceRestore restore;
     std::lock_guard<std::recursive_mutex> lk(h->ctx->mu);
     CU(cudaSetDevice(h->device));
-    const struct { const void* p; const char* name; } ptrs[] = {
-        {rays->origin, "rays->origin"}, {rays->direction, "rays->direction"}, {rays->t_max, "rays->t_max"}, {out->t, "out->t"},
-        {out->sphere, "out->sphere"}, {out->point, "out->point"}, {out->normal, "out->normal"}, {out->uv, "out->uv"},
-        {out->front_face, "out->front_face"}};
+    std::vector<std::pair<const void*, const char*>> ptrs = {{rays->origin, "rays->origin"}, {rays->direction, "rays->direction"},
+                                                             {rays->t_max, "rays->t_max"}};
+    for (int k = 0; k < out->count; ++k) ptrs.push_back({out->ptr[k], out->name[k]});
     for (const auto& q : ptrs) {
-        if (!q.p) continue;
+        if (!q.first) continue;
         cudaPointerAttributes a{};
-        if (cudaPointerGetAttributes(&a, q.p) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+        if (cudaPointerGetAttributes(&a, q.first) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
         if (!((a.type == cudaMemoryTypeDevice && a.device == h->device) || a.type == cudaMemoryTypeManaged))
-            return fail(RT_ERR_INVALID, std::string(q.name) + " is not device or managed memory of device " + std::to_string(h->device));
+            return fail(RT_ERR_INVALID, std::string(q.second) + " is not device or managed memory of device " + std::to_string(h->device));
     }
     cudaStream_t st;
     CU(scene_stream(h, stream_in, &st));
@@ -1183,11 +1219,10 @@ int rtb200_scene_intersect_device(rtb200_scene_handle h, const rt_rays* rays, ui
     }
     CU(cudaEventRecord(h->queries[k].done, st));
     return RT_OK;
-  });
 }
 
-int rtb200_scene_intersect(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_hits* out, rt_stats* stats) {
-  return guarded([&]() -> int {
+// The host form of both kinds.
+static int query_host(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const QueryOut* out, rt_stats* stats) {
     if (stats) memset(stats, 0, sizeof *stats);
     int rc = check_query(h, rays, out);
     if (rc != RT_OK) return rc;
@@ -1198,11 +1233,11 @@ int rtb200_scene_intersect(rtb200_scene_handle h, const rt_rays* rays, uint32_t 
     std::lock_guard<std::recursive_mutex> lk(ctx->mu);
     CU(cudaSetDevice(h->device));
     for (auto& e : ctx->query_ev) if (!e) CU(cudaEventCreate(&e));
-    // device image: counters (kStatBytes; the guard counters at stat[30..31]), then rays and hits, 256-byte aligned
+    // device image: counters (kStatBytes; the guard counters at stat[30..31]), then rays and outputs, 256-byte aligned
     const uint64_t N = n;
     const uint64_t in_b[3] = {N * 24, N * 24, rays->t_max ? N * 8 : 0};
-    const uint64_t out_b[6] = {out->t ? N * 8 : 0, out->sphere ? N * 4 : 0, out->point ? N * 24 : 0, out->normal ? N * 24 : 0,
-                               out->uv ? N * 16 : 0, out->front_face ? N : 0};
+    uint64_t out_b[6] = {0, 0, 0, 0, 0, 0};
+    for (int k = 0; k < out->count; ++k) out_b[k] = out->ptr[k] ? N * out->bytes[k] : 0;
     auto al = [](uint64_t b) { return (b + 255) & ~(uint64_t)255; };
     uint64_t bytes = kStatBytes;
     for (uint64_t b : in_b) bytes += al(b);
@@ -1223,12 +1258,10 @@ int rtb200_scene_intersect(rtb200_scene_handle h, const rt_rays* rays, uint32_t 
     uint64_t h2d = 0, d2h = kStatBytes;
     for (int k = 0; k < 3; ++k) if (in_b[k]) { CU(cudaMemcpyAsync(din[k], src_in[k], in_b[k], cudaMemcpyHostToDevice, st)); h2d += in_b[k]; }
     const rt_rays drays{(const double*)din[0], (const double*)din[1], (const double*)din[2]};
-    const rt_hits dhits{(double*)dout[0], (uint32_t*)dout[1], (double*)dout[2], (double*)dout[3], (double*)dout[4], (uint8_t*)dout[5]};
     CU(cudaEventRecord(ev[1], st));
-    if ((rc = query_enqueue(h, drays, n, dhits, stat, stat + 30, st)) != RT_OK) return rc;
+    if ((rc = query_enqueue(h, drays, n, with_ptrs(*out, dout), stat, stat + 30, st)) != RT_OK) return rc;
     CU(cudaEventRecord(ev[2], st));
-    void* dst_out[6] = {out->t, out->sphere, out->point, out->normal, out->uv, out->front_face};
-    for (int k = 0; k < 6; ++k) if (out_b[k]) { CU(cudaMemcpyAsync(dst_out[k], dout[k], out_b[k], cudaMemcpyDeviceToHost, st)); d2h += out_b[k]; }
+    for (int k = 0; k < out->count; ++k) if (out_b[k]) { CU(cudaMemcpyAsync(out->ptr[k], dout[k], out_b[k], cudaMemcpyDeviceToHost, st)); d2h += out_b[k]; }
     unsigned long long hstat[kStatBytes / 8];
     CU(cudaMemcpyAsync(hstat, stat, kStatBytes, cudaMemcpyDeviceToHost, st));
     CU(cudaEventRecord(ev[3], st));
@@ -1243,6 +1276,33 @@ int rtb200_scene_intersect(rtb200_scene_handle h, const rt_rays* rays, uint32_t 
     stats->h2d_bytes = h2d; stats->d2h_bytes = d2h;
     stats->wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count();
     return RT_OK;
+}
+
+int rtb200_scene_intersect_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_hits* out, void* stream_in) {
+  return guarded([&]() -> int {
+    const QueryOut o = hits_out(out ? *out : rt_hits{});
+    return query_device(h, rays, n, out ? &o : nullptr, stream_in);
+  });
+}
+
+int rtb200_scene_intersect(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_hits* out, rt_stats* stats) {
+  return guarded([&]() -> int {
+    const QueryOut o = hits_out(out ? *out : rt_hits{});
+    return query_host(h, rays, n, out ? &o : nullptr, stats);
+  });
+}
+
+int rtb200_scene_occluded_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, uint8_t* occluded, void* stream_in) {
+  return guarded([&]() -> int {
+    const QueryOut o = occluded_out(occluded);
+    return query_device(h, rays, n, &o, stream_in);
+  });
+}
+
+int rtb200_scene_occluded(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, uint8_t* occluded, rt_stats* stats) {
+  return guarded([&]() -> int {
+    const QueryOut o = occluded_out(occluded);
+    return query_host(h, rays, n, &o, stats);
   });
 }
 

@@ -193,6 +193,16 @@ struct QueryParams {
     uint32_t n;
 };
 
+// Occlusion queries on caller-supplied rays (rtb200_query.cu, DESIGN.md §4.11): `p`, the rays and n as in QueryParams.
+struct OcclusionParams {
+    TraceParams p;
+    const double* origin;        // [n][3]
+    const double* direction;     // [n][3]
+    const double* t_max;         // [n] or null: DBL_MAX
+    uint8_t* occluded;           // [n]
+    uint32_t n;
+};
+
 struct KernelInfo { int registers, max_threads, const_bytes, local_bytes; char name[96]; };
 
 // `queue` (TraceQueue): Q_FRAMES is the multi-frame kernel (work ids span p.ftab's frames), Q_LIST the adaptive round's
@@ -201,10 +211,11 @@ cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, uint32_t queue
 int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, uint32_t queue, size_t smem);   // 0 when the kernel cannot run on the current device
 cudaError_t wavefront_info(uint32_t mode, bool lights, uint32_t queue, KernelInfo* out);
 cudaError_t launch_resolve(const ResolveParams& p, cudaStream_t st);
-// closest-hit queries: resident CTAs per SM of the query kernel of `mode` (0 when it cannot run on the current device), and a
-// launch of at most `max_grid` CTAs (no more than the rays need)
-int query_max_ctas_per_sm(uint32_t mode);
+// closest-hit (any = false) and occlusion (any = true) queries: resident CTAs per SM of the query kernel of that kind and
+// `mode` (0 when it cannot run on the current device), and a launch of at most `max_grid` CTAs (no more than the rays need)
+int query_max_ctas_per_sm(uint32_t mode, bool any);
 cudaError_t launch_query(const QueryParams& q, uint32_t mode, int max_grid, cudaStream_t st);
+cudaError_t launch_occluded(const OcclusionParams& q, uint32_t mode, int max_grid, cudaStream_t st);
 // adaptive rendering (rtb200_adaptive.cu): the round's accumulate-and-test, the list compaction (cub::DeviceSelect::Flagged,
 // keep[0, npix_local) over list_in, the count to *list_n_out), and the resolve
 cudaError_t launch_adaptive_list(uint32_t* list, uint32_t* list_n, uint32_t npix_local, cudaStream_t st);   // list = 0, 1, .., npix_local - 1

@@ -8,6 +8,11 @@
 //
 // t_max costs nothing in the traversal: closest_hit finds the unbounded closest hit (r*, j*) under f64::MAX and the kernel
 // reports it only when r* < t_max (Sphere::hit's strict bound). That equals hit_world under t_max (DESIGN.md §4.10).
+//
+// rt_occluded_kernel<MODE> answers occlusion queries (rtb200_scene_occluded[_device], DESIGN.md §4.11) with the same CTA, chunks
+// and slots: it calls the any-hit kind of the same stage, closest_hit<MODE, true>, under each ray's own bound
+// T = min(t_max, f64::MAX), which prunes boxes beyond T and stops at the first sphere that accepts a root below T. A ray with
+// !(T > 0.001) cannot be occluded (an accepted root is > 0.001 and < T) and does not enter the stage.
 #include <algorithm>
 
 #include "rtb200_trace.cuh"
@@ -25,6 +30,12 @@ __host__ __device__ constexpr uint32_t query_warp_bytes(uint32_t mode) {
     return (mode == MODE_TREE ? kWarpCtxBytes : 0u) + 32u * kQuerySlotBytes;
 }
 constexpr size_t query_smem_bytes(uint32_t mode) { return (size_t)kQueryWarps * query_warp_bytes(mode); }
+// occlusion queries: the traversal context is followed by the 32 rays' f32 bounds T~ (MODE_TREE), then the slots
+constexpr uint32_t kTcapBytes = 32u * 4u;
+__host__ __device__ constexpr uint32_t occluded_warp_bytes(uint32_t mode) {
+    return query_warp_bytes(mode) + (mode == MODE_TREE ? kTcapBytes : 0u);
+}
+constexpr size_t occluded_smem_bytes(uint32_t mode) { return (size_t)kQueryWarps * occluded_warp_bytes(mode); }
 
 template <uint32_t MODE>
 __global__ void __launch_bounds__(kQueryBlock) rt_query_kernel(const __grid_constant__ QueryParams q) {
@@ -82,36 +93,97 @@ __global__ void __launch_bounds__(kQueryBlock) rt_query_kernel(const __grid_cons
     if (q.p.stat) flush_stats(q.p, st, lane);
 }
 
+template <uint32_t MODE>
+__global__ void __launch_bounds__(kQueryBlock) rt_occluded_kernel(const __grid_constant__ OcclusionParams q) {
+    extern __shared__ __align__(16) unsigned char smem_raw[];
+    const int lane = threadIdx.x & 31;
+    const uint32_t warp = threadIdx.x >> 5;
+    unsigned char* base = smem_raw + warp * occluded_warp_bytes(MODE);
+    const WarpCtx W = warpctx_at(base);   // read by MODE_TREE only
+    float* tcap = reinterpret_cast<float*>(base + kWarpCtxBytes);   // MODE_TREE only
+    double* dbl = reinterpret_cast<double*>(base + (MODE == MODE_TREE ? kWarpCtxBytes + kTcapBytes : 0u));
+    uint32_t* u32 = reinterpret_cast<uint32_t*>(dbl + 7 * 32);
+    Pool P{};   // the slots of rt_query_kernel
+    P.ox = dbl; P.oy = dbl + 32; P.oz = dbl + 64; P.dx = dbl + 96; P.dy = dbl + 128; P.dz = dbl + 160; P.bt = dbl + 192;
+    P.bi = u32; P.src = u32 + 32;
+    P.n_slots = 32u;
+    SceneRefs sc;
+    sc.nodes = q.p.nodes; sc.leaf_rec = q.p.leaf_rec; sc.leaf_id = q.p.leaf_id; sc.filt = q.p.filt; sc.geo = q.p.geo; sc.mat = q.p.mat;
+    Stats st;
+    const uint64_t chunks = ((uint64_t)q.n + 31u) / 32u;
+    for (uint64_t c = (uint64_t)blockIdx.x * kQueryWarps + warp; c < chunks; c += (uint64_t)gridDim.x * kQueryWarps) {
+        const uint64_t i = c * 32u + (uint64_t)lane;
+        const bool alive = i < q.n;   // the last chunk has dead lanes
+        double tb = DBL_MAX;   // T
+        if (alive) {
+            P.ox[lane] = q.origin[3 * i]; P.oy[lane] = q.origin[3 * i + 1]; P.oz[lane] = q.origin[3 * i + 2];
+            P.dx[lane] = q.direction[3 * i]; P.dy[lane] = q.direction[3 * i + 1]; P.dz[lane] = q.direction[3 * i + 2];
+            P.src[lane] = kNoSphere;
+            if (q.t_max) { const double t = q.t_max[i]; tb = t > DBL_MAX ? DBL_MAX : t; }   // +inf counts as f64::MAX; NaN stays NaN
+        }
+        const bool live = alive && tb > 0.001;   // else no root can be accepted: 0 without a traversal
+        __syncwarp();   // the exact step reads the other lanes' rays
+        closest_hit<MODE, true>(q.p, sc, P, W, live, (uint32_t)lane, lane, st, live ? tb : DBL_MAX, tcap);
+        if (alive) {
+            q.occluded[i] = live && P.bi[lane] != kNoSphere ? 1u : 0u;
+            if (!live) ++st.rays;
+        }
+        __syncwarp();   // every lane is done with the slots before the next chunk overwrites them
+    }
+    if (q.p.stat) flush_stats(q.p, st, lane);
+}
+
 template <typename F>
 static auto dispatch_query(uint32_t mode, F&& f) {
     if (mode == MODE_EXACT) return f(rt_query_kernel<MODE_EXACT>);
     if (mode == MODE_BRUTE) return f(rt_query_kernel<MODE_BRUTE>);
     return f(rt_query_kernel<MODE_TREE>);
 }
-
-}  // namespace
-
-int query_max_ctas_per_sm(uint32_t mode) {
-    return dispatch_query(mode, [&](auto kern) -> int {
-        const size_t smem = query_smem_bytes(mode);
-        int nb = 0;
-        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return 0; }
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kQueryBlock, smem) != cudaSuccess) { cudaGetLastError(); return 0; }
-        return nb;
-    });
+template <typename F>
+static auto dispatch_occluded(uint32_t mode, F&& f) {
+    if (mode == MODE_EXACT) return f(rt_occluded_kernel<MODE_EXACT>);
+    if (mode == MODE_BRUTE) return f(rt_occluded_kernel<MODE_BRUTE>);
+    return f(rt_occluded_kernel<MODE_TREE>);
 }
 
-cudaError_t launch_query(const QueryParams& q, uint32_t mode, int max_grid, cudaStream_t st) {
+// one query kind's kernel of `mode` and its dynamic shared memory
+template <typename F>
+static auto dispatch_kind(bool any, uint32_t mode, F&& f) {
+    if (any) return dispatch_occluded(mode, [&](auto kern) { return f(kern, occluded_smem_bytes(mode)); });
+    return dispatch_query(mode, [&](auto kern) { return f(kern, query_smem_bytes(mode)); });
+}
+
+template <typename K>
+static int max_ctas_per_sm(K kern, size_t smem) {
+    int nb = 0;
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return 0; }
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kQueryBlock, smem) != cudaSuccess) { cudaGetLastError(); return 0; }
+    return nb;
+}
+
+template <typename K, typename Q>
+static cudaError_t launch(K kern, size_t smem, const Q& q, int max_grid, cudaStream_t st) {
     if (q.n == 0) return cudaSuccess;
     const uint64_t ctas = ((uint64_t)q.n + 32u * kQueryWarps - 1u) / (32u * kQueryWarps);
     const int grid = (int)std::min<uint64_t>(ctas, (uint64_t)std::max(max_grid, 1));
-    return dispatch_query(mode, [&](auto kern) -> cudaError_t {
-        const size_t smem = query_smem_bytes(mode);
-        cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-        kern<<<grid, kQueryBlock, smem, st>>>(q);
-        return cudaGetLastError();
-    });
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    if (e != cudaSuccess) return e;
+    kern<<<grid, kQueryBlock, smem, st>>>(q);
+    return cudaGetLastError();
+}
+
+}  // namespace
+
+int query_max_ctas_per_sm(uint32_t mode, bool any) {
+    return dispatch_kind(any, mode, [&](auto kern, size_t smem) -> int { return max_ctas_per_sm(kern, smem); });
+}
+
+cudaError_t launch_query(const QueryParams& q, uint32_t mode, int max_grid, cudaStream_t st) {
+    return dispatch_query(mode, [&](auto kern) { return launch(kern, query_smem_bytes(mode), q, max_grid, st); });
+}
+
+cudaError_t launch_occluded(const OcclusionParams& q, uint32_t mode, int max_grid, cudaStream_t st) {
+    return dispatch_occluded(mode, [&](auto kern) { return launch(kern, occluded_smem_bytes(mode), q, max_grid, st); });
 }
 
 }  // namespace rtk

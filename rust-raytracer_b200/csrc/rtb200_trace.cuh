@@ -160,9 +160,16 @@ RT_DEV uint32_t class_of(uint32_t kind) {
 // hit_world (raytracer.rs:44-59) keeps the closest root and, on equal t, the first sphere in list order; because
 // Sphere::hit(t_max) accepts exactly r < t_max with r the first root beyond t_min, that fold equals the lexicographic
 // minimum of (r, index) over all spheres - so spheres may be tested in any order, by any lane.
+//
+// ANY (occlusion queries, DESIGN.md §4.11): the same traversal asks only whether some sphere accepts a root below the ray's
+// bound t_hi (0.001 < t_hi <= f64::MAX). On return P.bi[slot] is one such sphere (which one depends on the order of the
+// steps), or 0xffffffff; P.bt is not meaningful. The node step also drops children that lie wholly beyond the ray's f32
+// bound tcap[lane] (written here), the first acceptance marks the ray done, entries of done rays are popped without work,
+// and the warp leaves the traversal once every ray in it is done. The thread-private loops stop at their first acceptance.
 // =====================================================================================================================
-template <uint32_t MODE>
-RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Pool& P, const WarpCtx& W, bool alive, uint32_t slot, int lane, Stats& st) {
+template <uint32_t MODE, bool ANY = false>
+RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Pool& P, const WarpCtx& W, bool alive, uint32_t slot, int lane, Stats& st,
+                            double t_hi = DBL_MAX, float* tcap = nullptr) {
     const unsigned FULL = 0xffffffffu;
     uint32_t cls = CLS_DEAD;
     if (__ballot_sync(FULL, alive) == 0u) return cls;   // a warp without rays skips the stage (frame tail)
@@ -170,14 +177,17 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
     unsigned long long* btu = reinterpret_cast<unsigned long long*>(P.bt);
     const D3 o = mk(P.ox[slot], P.oy[slot], P.oz[slot]), d = mk(P.dx[slot], P.dy[slot], P.dz[slot]);
     const double a = length_squared(d);
+    const double thi = ANY ? t_hi : DBL_MAX;   // the bound of every exact test
     bool ovf = false;
+    uint32_t done = 0u;   // ANY: the rays (by owning lane) with a proven hit below their bound; warp-uniform
     // thread-private exact f64 confirmation (fallback paths: every sphere / the always-list / MODE_BRUTE candidates)
     double best_t = DBL_MAX;
     int best = -1;
     auto confirm = [&](int j) {
+        if constexpr (ANY) { if (best >= 0) return; }   // one acceptance answers the ray
         double4 gq = sc.geo[j];
         double root;
-        if (sphere_root(mk(gq.x, gq.y, gq.z), gq.w, o, d, a, 0.001, DBL_MAX, root)) {
+        if (sphere_root(mk(gq.x, gq.y, gq.z), gq.w, o, d, a, 0.001, thi, root)) {
             if (best < 0 || root < best_t || (root == best_t && j < best)) { best_t = root; best = j; }
         }
         ++st.cand;
@@ -205,6 +215,9 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
             W.cA[lane] = make_float4(ofx, ofy, ofz, mray);
             W.cB[lane] = make_float4(__frcp_rn(ax), __frcp_rn(ay), __frcp_rn(az), thr);
             W.cC[lane] = make_float4(dnx, dny, dnz, nod);
+            // ANY: the bound on the distance along d^, T~ >= t_hi * |d| (DESIGN.md §4.11): the f64 product rounded up, a 2^-40
+            // margin for the rounding of a = |d|^2, then rounded up to f32 (+inf when it exceeds the f32 range: no pruning)
+            if constexpr (ANY) tcap[lane] = __double2float_ru(__dmul_ru(__dmul_ru(t_hi, __dsqrt_ru(a)), 1.0 + 0x1p-40));
             // The sphere the ray starts on is left out of its candidates when a cheap f64 certificate proves that the exact
             // test rejects it (a ray leaving the surface outwards; DESIGN.md §4.2). The certificate is evaluated on this ray's
             // own o and d, so even a wrong Pool.src could only cost a missed skip, never a wrong hit.
@@ -238,8 +251,13 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                     const uint32_t ray = e & 31u, node = e >> 5;
                     uint32_t hit = 0u, leafbits = 0u;
                     const float4* N = sc.nodes + (size_t)node * kNodeVec;
-                    if (act) {
+                    bool test = act;   // ANY: a done ray's entry is popped without a test
+                    if constexpr (ANY) test = act && !((done >> ray) & 1u);
+                    if (test) {
                         const float4 A = W.cA[ray], B = W.cB[ray];
+                        float tcr = 0.f;
+                        if constexpr (ANY) tcr = tcap[ray];
+                        auto far_ = [&](float f) { if constexpr (ANY) return fminf(f, tcr); else return f; };   // ANY: min(t_far, T~)
                         // near/far plane of each axis by the sign of d^; planes shifted outwards by the per-ray margin
                         const uint32_t sx = __float_as_uint(B.x) >> 31, sy = __float_as_uint(B.y) >> 31, sz = __float_as_uint(B.z) >> 31;
                         const float mx = copysignf(A.w, B.x), my = copysignf(A.w, B.y), mz = copysignf(A.w, B.z);
@@ -262,10 +280,10 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                             const float2 tfy0 = fma2_rn(make_float2(FY.x, FY.y), iy2, cfy2), tfy1 = fma2_rn(make_float2(FY.z, FY.w), iy2, cfy2);
                             const float2 tfz0 = fma2_rn(make_float2(FZ.x, FZ.y), iz2, cfz2), tfz1 = fma2_rn(make_float2(FZ.z, FZ.w), iz2, cfz2);
                             // hit iff max(t_near, 0) <= t_far
-                            hit |= (fmaxf(fmax3(tnx0.x, tny0.x, tnz0.x), 0.f) <= fmin3(tfx0.x, tfy0.x, tfz0.x) ? 1u : 0u) << (4 * h + 0);
-                            hit |= (fmaxf(fmax3(tnx0.y, tny0.y, tnz0.y), 0.f) <= fmin3(tfx0.y, tfy0.y, tfz0.y) ? 1u : 0u) << (4 * h + 1);
-                            hit |= (fmaxf(fmax3(tnx1.x, tny1.x, tnz1.x), 0.f) <= fmin3(tfx1.x, tfy1.x, tfz1.x) ? 1u : 0u) << (4 * h + 2);
-                            hit |= (fmaxf(fmax3(tnx1.y, tny1.y, tnz1.y), 0.f) <= fmin3(tfx1.y, tfy1.y, tfz1.y) ? 1u : 0u) << (4 * h + 3);
+                            hit |= (fmaxf(fmax3(tnx0.x, tny0.x, tnz0.x), 0.f) <= far_(fmin3(tfx0.x, tfy0.x, tfz0.x)) ? 1u : 0u) << (4 * h + 0);
+                            hit |= (fmaxf(fmax3(tnx0.y, tny0.y, tnz0.y), 0.f) <= far_(fmin3(tfx0.y, tfy0.y, tfz0.y)) ? 1u : 0u) << (4 * h + 1);
+                            hit |= (fmaxf(fmax3(tnx1.x, tny1.x, tnz1.x), 0.f) <= far_(fmin3(tfx1.x, tfy1.x, tfz1.x)) ? 1u : 0u) << (4 * h + 2);
+                            hit |= (fmaxf(fmax3(tnx1.y, tny1.y, tnz1.y), 0.f) <= far_(fmin3(tfx1.y, tfy1.y, tfz1.y)) ? 1u : 0u) << (4 * h + 3);
                         }
                         const uint4 R0 = *reinterpret_cast<const uint4*>(N + kChildVec), R1 = *reinterpret_cast<const uint4*>(N + kChildVec + 1);
                         leafbits = (R0.x >> 31) | ((R0.y >> 31) << 1) | ((R0.z >> 31) << 2) | ((R0.w >> 31) << 3) |
@@ -303,7 +321,7 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                             if (ref & kLeafBit) W.l_lf[pl++] = (ref << 5) | ray;   // the shift drops the leaf bit
                             else W.l_in[pi++] = (ref << 5) | ray;
                         }
-                        ++st.nodes;
+                        if constexpr (ANY) st.nodes += test ? 1u : 0u; else ++st.nodes;
                     }
                     n_in = n_in - k + (tot & 0xffffu);
                     n_lf += tot >> 16;
@@ -318,7 +336,9 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                     const uint32_t e = act ? W.l_lf[n_lf - 1u - (uint32_t)lane] : 0u;
                     const uint32_t ray = e & 31u, leaf = e >> 5;
                     uint32_t hit = 0u;
-                    if (act) {
+                    bool test = act;   // ANY: a done ray's entry is popped without a test
+                    if constexpr (ANY) test = act && !((done >> ray) & 1u);
+                    if (test) {
                         const float4 A = W.cA[ray], C = W.cC[ray];
                         const float th = W.cB[ray].w;
                         const float2 dx2 = make_float2(C.x, C.x), dy2 = make_float2(C.y, C.y), dz2 = make_float2(C.z, C.z);
@@ -355,7 +375,7 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                             mm &= mm - 1u;
                             W.l_cd[pc++] = (ids[c] << 5) | ray;
                         }
-                        ++st.leaves;
+                        if constexpr (ANY) st.leaves += test ? 1u : 0u; else ++st.leaves;
                     }
                     n_lf -= k;
                     n_cd += tot;
@@ -369,29 +389,51 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                     const bool act = (uint32_t)lane < m;
                     const uint32_t e = act ? W.l_cd[n_cd - 1u - (uint32_t)lane] : 0u;
                     const uint32_t rs = __shfl_sync(FULL, slot, (int)(e & 31u)), sph = e >> 5;   // pool slot of the candidate's ray
-                    unsigned long long key = ~0ull;
-                    if (act) {
-                        const D3 ro = mk(P.ox[rs], P.oy[rs], P.oz[rs]), rd = mk(P.dx[rs], P.dy[rs], P.dz[rs]);
-                        const double4 gq = sc.geo[sph];
-                        double root;
-                        if (sphere_root(mk(gq.x, gq.y, gq.z), gq.w, ro, rd, length_squared(rd), 0.001, DBL_MAX, root)) key = (unsigned long long)__double_as_longlong(root);
-                        ++st.cand;
+                    if constexpr (ANY) {
+                        // Sphere::hit under the ray's own bound; one acceptance answers the ray, in whatever order it comes
+                        const uint32_t ray = e & 31u;
+                        const double tr = __shfl_sync(FULL, t_hi, (int)ray);
+                        bool acc = false;
+                        if (act && !((done >> ray) & 1u)) {
+                            const D3 ro = mk(P.ox[rs], P.oy[rs], P.oz[rs]), rd = mk(P.dx[rs], P.dy[rs], P.dz[rs]);
+                            const double4 gq = sc.geo[sph];
+                            double root;
+                            acc = sphere_root(mk(gq.x, gq.y, gq.z), gq.w, ro, rd, length_squared(rd), 0.001, tr, root);
+                            ++st.cand;
 #if RT_PHASE_CLOCKS
-                        ++st.exact_tests;
+                            ++st.exact_tests;
 #endif
+                        }
+                        if (acc) P.bi[rs] = sph;   // lanes of one ray may race here: any of their spheres will do
+                        done |= __reduce_or_sync(FULL, acc ? 1u << ray : 0u);
+                        n_cd -= m;
+                        __syncwarp();
+                        if ((em & ~done) == 0u) break;   // every ray of the warp is answered
+                    } else {
+                        unsigned long long key = ~0ull;
+                        if (act) {
+                            const D3 ro = mk(P.ox[rs], P.oy[rs], P.oz[rs]), rd = mk(P.dx[rs], P.dy[rs], P.dz[rs]);
+                            const double4 gq = sc.geo[sph];
+                            double root;
+                            if (sphere_root(mk(gq.x, gq.y, gq.z), gq.w, ro, rd, length_squared(rd), 0.001, DBL_MAX, root)) key = (unsigned long long)__double_as_longlong(root);
+                            ++st.cand;
+#if RT_PHASE_CLOCKS
+                            ++st.exact_tests;
+#endif
+                        }
+                        // per-ray lexicographic minimum of (root, sphere index): roots are positive, so their bit patterns order like the values
+                        const bool h = key != ~0ull;
+                        const unsigned long long before = h ? btu[rs] : 0ull;
+                        __syncwarp();
+                        if (h && key < before) atomicMin(&btu[rs], key);
+                        __syncwarp();
+                        const bool mine = h && key == btu[rs];
+                        if (mine && key < before) atomicMax(&P.bi[rs], 0xffffffffu);   // the root got smaller in this step: forget the old index
+                        __syncwarp();
+                        if (mine) atomicMin(&P.bi[rs], sph);
+                        n_cd -= m;
+                        __syncwarp();
                     }
-                    // per-ray lexicographic minimum of (root, sphere index): roots are positive, so their bit patterns order like the values
-                    const bool h = key != ~0ull;
-                    const unsigned long long before = h ? btu[rs] : 0ull;
-                    __syncwarp();
-                    if (h && key < before) atomicMin(&btu[rs], key);
-                    __syncwarp();
-                    const bool mine = h && key == btu[rs];
-                    if (mine && key < before) atomicMax(&P.bi[rs], 0xffffffffu);   // the root got smaller in this step: forget the old index
-                    __syncwarp();
-                    if (mine) atomicMin(&P.bi[rs], sph);
-                    n_cd -= m;
-                    __syncwarp();
 #if RT_PHASE_CLOCKS
                     if (lane == 0) { st.t_exact += clock64() - t_step; ++st.exact_steps; }
 #endif
@@ -416,6 +458,7 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
                         if (Dv[q].x >= thr && j < p.n) confirm((int)j);
                         if (Dv[q].y >= thr && j + 1u < p.n) confirm((int)j + 1);
                     }
+                    if constexpr (ANY) { if (best >= 0) break; }
                 }
             }
         }
@@ -423,11 +466,23 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
         ovf = alive;
     }
     if (alive) {
+        if constexpr (ANY) { if ((done >> lane) & 1u) best = (int)P.bi[slot]; }   // answered by the traversal
         if (ovf) {   // MODE_EXACT, or a ray outside the f32 frame's safe range: every sphere in f64
             ++st.ovf;
-            for (int k = 0; k < (int)p.n; ++k) confirm(k);
+            for (int k = 0; k < (int)p.n; ++k) {
+                confirm(k);
+                if constexpr (ANY) { if (best >= 0) break; }
+            }
         } else if (MODE == MODE_TREE) {
-            for (uint32_t k = 0; k < p.n_always; ++k) confirm((int)p.always[k]);
+            for (uint32_t k = 0; k < p.n_always; ++k) {
+                if constexpr (ANY) { if (best >= 0) break; }
+                confirm((int)p.always[k]);
+            }
+        }
+        if constexpr (ANY) {
+            if (best >= 0) P.bi[slot] = (uint32_t)best;
+            ++st.rays;
+            return CLS_MISS;   // the caller reads P.bi
         }
         // merge the thread-private result with the traversal's (this slot is only touched by its own thread now)
         const unsigned long long tb = btu[slot];

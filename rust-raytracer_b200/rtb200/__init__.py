@@ -139,6 +139,7 @@ ABI_SYMBOLS = [
     "rtb200_scene_rebuild", "rtb200_scene_debug_topology",
     "rtb200_adaptive_begin", "rtb200_adaptive_step", "rtb200_adaptive_resolve", "rtb200_render_adaptive",
     "rtb200_scene_intersect_device", "rtb200_scene_intersect",
+    "rtb200_scene_occluded_device", "rtb200_scene_occluded",
 ]
 
 _lib = None
@@ -199,6 +200,8 @@ def lib() -> C.CDLL:
                                          C.c_void_p, C.POINTER(rt_stats)]
     L.rtb200_scene_intersect_device.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.POINTER(rt_hits), C.c_void_p]
     L.rtb200_scene_intersect.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.POINTER(rt_hits), C.POINTER(rt_stats)]
+    L.rtb200_scene_occluded_device.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.c_void_p, C.c_void_p]
+    L.rtb200_scene_occluded.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.c_void_p, C.POINTER(rt_stats)]
     _lib = L
     return L
 
@@ -652,17 +655,53 @@ class ResidentScene:
         unknown = [k for k in names if k not in dict((f[0], f) for f in HIT_FIELDS)]
         if unknown or not names:
             raise ValueError(f"intersect outputs are a non-empty subset of {[f[0] for f in HIT_FIELDS]}, got {names}")
+        fields = [f for f in HIT_FIELDS if f[0] in names]
         if isinstance(origin, np.ndarray):
-            return self._intersect_host(origin, direction, t_max, names)
+            out, rays, n = self._query_host_args("intersect", origin, direction, t_max, fields)
+            hits = rt_hits(*(out[k].ctypes.data if k in out else None for k, _, _ in HIT_FIELDS))
+            st = rt_stats()
+            _check(lib().rtb200_scene_intersect(self.h, C.byref(rays), n, C.byref(hits), C.byref(st)))
+            out["stats"] = st.as_dict()
+            return out
+        out, rays, n = self._query_device_args("intersect", origin, direction, t_max, stream, fields)
+        if n:
+            hits = rt_hits(*(out[k].data_ptr() if k in out else None for k, _, _ in HIT_FIELDS))
+            _check(lib().rtb200_scene_intersect_device(self.h, C.byref(rays), n, C.byref(hits), C.c_void_p(self._stream(stream, origin.device) or None)))
+        return out
+
+    def occluded(self, origin, direction, t_max=None, stream=None) -> dict:
+        """Occlusion of caller-supplied rays on the handle's current spheres: for ray i, 1 if hit_world(world, Ray{origin[i],
+        direction[i]}, 0.001, t_max[i]) (f64::MAX without t_max) is Some, else 0, as include/rtb200.h states it, in every
+        variant. It equals intersect(...)["sphere"] != -1 under the same t_max, but the traversal skips boxes beyond t_max and
+        stops at the first sphere that is hit below it. A segment from a to b is origin a, direction b - a, t_max 1.
+
+        CUDA tensors use the device form (rtb200_scene_occluded_device) and numpy arrays the blocking host form
+        (rtb200_scene_occluded), with the same arguments, checks and stream ordering as :meth:`intersect`. Returns
+        {"occluded": uint8 [n]}, and with numpy arrays also "stats"."""
+        fields = [("occluded", 1, np.uint8)]
+        if isinstance(origin, np.ndarray):
+            out, rays, n = self._query_host_args("occluded", origin, direction, t_max, fields)
+            st = rt_stats()
+            _check(lib().rtb200_scene_occluded(self.h, C.byref(rays), n, C.c_void_p(out["occluded"].ctypes.data), C.byref(st)))
+            out["stats"] = st.as_dict()
+            return out
+        out, rays, n = self._query_device_args("occluded", origin, direction, t_max, stream, fields)
+        if n:
+            _check(lib().rtb200_scene_occluded_device(self.h, C.byref(rays), n, C.c_void_p(out["occluded"].data_ptr()),
+                                                      C.c_void_p(self._stream(stream, origin.device) or None)))
+        return out
+
+    def _query_device_args(self, what, origin, direction, t_max, stream, fields):
+        """Checks of a query's CUDA tensors; returns the outputs `fields` (name, values per ray, numpy dtype), rt_rays and n."""
         import torch
         args = [("origin", origin, 2), ("direction", direction, 2)] + ([("t_max", t_max, 1)] if t_max is not None else [])
         n = origin.shape[0] if isinstance(origin, torch.Tensor) and origin.dim() == 2 else -1
         for name, t, dim in args:
             if not isinstance(t, torch.Tensor) or not t.is_cuda:
-                raise ValueError(f"intersect takes CUDA tensors (or numpy arrays): {name} is {type(t).__name__}")
+                raise ValueError(f"{what} takes CUDA tensors (or numpy arrays): {name} is {type(t).__name__}")
             shape = (n, 3) if dim == 2 else (n,)
             if t.dtype != torch.float64 or tuple(t.shape) != shape or n < 0 or not t.is_contiguous():
-                raise ValueError(f"intersect: {name} must be a contiguous float64 tensor of shape {list(shape) if n >= 0 else '[n, 3]'}, got {t.dtype} {tuple(t.shape)}")
+                raise ValueError(f"{what}: {name} must be a contiguous float64 tensor of shape {list(shape) if n >= 0 else '[n, 3]'}, got {t.dtype} {tuple(t.shape)}")
             if self.device is not None and t.device.index != self.device:
                 raise ValueError(f"the tensor {name} is on cuda:{t.device.index}, the scene on cuda:{self.device}")
             if t.device != origin.device:
@@ -670,29 +709,22 @@ class ResidentScene:
         dt = {np.float64: torch.float64, np.int32: torch.int32, np.uint8: torch.uint8}
         # outputs belong to the query's stream when it is a torch stream (the caching allocator orders their reuse after it)
         with torch.cuda.stream(stream) if isinstance(stream, torch.cuda.Stream) else torch.cuda.device(origin.device):
-            out = {k: torch.empty((n, c) if c > 1 else (n,), dtype=dt[ty], device=origin.device) for k, c, ty in HIT_FIELDS if k in names}
-        if n == 0:
-            return out
+            out = {k: torch.empty((n, c) if c > 1 else (n,), dtype=dt[ty], device=origin.device) for k, c, ty in fields}
         rays = rt_rays(origin.data_ptr(), direction.data_ptr(), t_max.data_ptr() if t_max is not None else None)
-        hits = rt_hits(*(out[k].data_ptr() if k in out else None for k, _, _ in HIT_FIELDS))
-        _check(lib().rtb200_scene_intersect_device(self.h, C.byref(rays), n, C.byref(hits), C.c_void_p(self._stream(stream, origin.device) or None)))
-        return out
+        return out, rays, n
 
-    def _intersect_host(self, origin, direction, t_max, names) -> dict:
+    def _query_host_args(self, what, origin, direction, t_max, fields):
+        """Checks of a query's numpy arrays; returns the outputs `fields`, rt_rays and n."""
         n = origin.shape[0] if origin.ndim == 2 else -1
         for name, a, shape in (("origin", origin, (n, 3)), ("direction", direction, (n, 3)), ("t_max", t_max, (n,))):
             if name == "t_max" and a is None:
                 continue
             if not isinstance(a, np.ndarray) or a.dtype != np.float64 or a.shape != shape or n < 0 or not a.flags.c_contiguous:
-                raise ValueError(f"intersect: {name} must be a C-contiguous float64 array of shape {list(shape) if n >= 0 else '[n, 3]'}, "
+                raise ValueError(f"{what}: {name} must be a C-contiguous float64 array of shape {list(shape) if n >= 0 else '[n, 3]'}, "
                                  f"got {getattr(a, 'dtype', type(a).__name__)} {getattr(a, 'shape', '')}")
-        out = {k: np.empty((n, c) if c > 1 else (n,), dtype=ty) for k, c, ty in HIT_FIELDS if k in names}
+        out = {k: np.empty((n, c) if c > 1 else (n,), dtype=ty) for k, c, ty in fields}
         rays = rt_rays(origin.ctypes.data, direction.ctypes.data, t_max.ctypes.data if t_max is not None else None)
-        hits = rt_hits(*(out[k].ctypes.data if k in out else None for k, _, _ in HIT_FIELDS))
-        st = rt_stats()
-        _check(lib().rtb200_scene_intersect(self.h, C.byref(rays), n, C.byref(hits), C.byref(st)))
-        out["stats"] = st.as_dict()
-        return out
+        return out, rays, n
 
     def topology(self) -> dict:
         """The handle's current topology (rtb200_scene_debug_topology): recentre, leaf_id [n_leaves, k], always, skip_pos,

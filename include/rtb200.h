@@ -357,6 +357,43 @@ int rtb200_scene_intersect(rtb200_scene_handle h, const rt_rays* rays, uint32_t 
 int rtb200_scene_occluded_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, uint8_t* occluded, void* stream);
 int rtb200_scene_occluded(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, uint8_t* occluded, rt_stats* stats);
 
+/* ---- radiance of caller-supplied primary rays on a resident scene (DESIGN.md §4.12) --------------------------------------
+ * Contract: for ray i (origin, direction as in rt_rays, any f64 values; rays->t_max must be NULL) and sample j < samples, the
+ * sample's radiance is ray_color(Ray{o, d}, max_depth, max_depth) (raytracer.rs:71-165) over the handle's CURRENT spheres. It
+ * draws from the Philox stream of (pixel = stream0 + i, sample = sample0 + j) under the key `seed`, starting at the stream's
+ * third f64 draw: the two draws a render spends on the pixel jitter (raytracer.rs:199-200) are skipped. The outputs are the
+ * render's resolve with spp = samples: S_c the f32 sum of the samples in sample order, linear = (1.0f / samples) * S_c,
+ * rgb8 = the render's quantisation of sqrt(linear). Bit for bit in every variant, with or without lights, every sky, textures,
+ * shard handles (rank / world do not affect rays) and shared-memory-staged handles. So when ray p of a call with sample0 = s
+ * and samples = 1 is the render's primary ray of (pixel p, sample s), its output is that sample's radiance, and the f32 sum of
+ * such calls in sample order times 1.0f / spp is the render's linear image. */
+typedef struct {
+    uint64_t seed;        /* Philox key, as rt_scene.seed */
+    uint32_t samples;     /* samples of every ray, >= 1 */
+    uint32_t sample0;     /* sample index of the first sample */
+    uint32_t stream0;     /* ray i draws from the stream of pixel stream0 + i */
+    uint32_t max_depth;   /* as rt_scene.max_depth; 0: black, no ray */
+    uint32_t reserved[2]; /* must be 0 */
+} rt_trace_params;        /* 32 bytes */
+/* Device buffers (of h's device, or managed memory): dev_linear_f32 and dev_rgb8 hold n x 3 floats / bytes, either may be NULL,
+ * not both. Blocking, like rtb200_render_device: drains the handle's asynchronous frames, takes work set 0 like a blocking render,
+ * runs on `stream` (NULL: the library's stream) after the last update or rebuild of h, and returns when the outputs are
+ * written. The samples are traced in batches of spb samples of every ray with n * spb * 16 bytes <= the handle's sample-buffer
+ * cap (rt_options.sample_buffer_bytes) and n * spb < 2^31; the sums carry across batches. stats (may be NULL): rays (hit_world
+ * calls), samples = n * samples, candidates, clusters, nodes, device_ms, trace_ms, wall_ms, kernel_launches, batches (trace
+ * launches, or black batches at max_depth 0) and frames = 1. Shadow-frame-stack overflows (RT_ERR_UNSUPPORTED) and
+ * traversal-guard trips (RT_ERR_CUDA) fail the call as they fail a render.
+ * RT_ERR_INVALID, before any device work, for a NULL handle, rays, params, origin or direction, a non-NULL rays->t_max, both
+ * outputs NULL, samples == 0, a nonzero reserved, stream0 + n or sample0 + samples above 2^32, n >= 2^31, n * 16 above the
+ * sample-buffer cap (one sample of every ray must fit), or a pointer that is not device memory of h's device or managed
+ * memory. n == 0 is a no-op. */
+int rtb200_scene_trace_rays_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_trace_params* params,
+                                   float* dev_linear_f32, uint8_t* dev_rgb8, void* stream, rt_stats* stats);
+/* Host buffers: the same through the same path on the library's stream, with the rays copied in and the outputs copied out
+ * (h2d_bytes = 48 n, d2h_bytes = 12 n with linear + 3 n with rgb8). Same checks, bar the memory kind. */
+int rtb200_scene_trace_rays(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_trace_params* params,
+                            float* out_linear_f32, uint8_t* out_rgb8, rt_stats* stats);
+
 /* load_texture_image — materials.rs:213-219, config.rs:36-47: decode a baseline JPEG file to RGB8 (host-side scene staging
  * helper for hosts without their own decoder; the reference uses the jpeg-decoder crate). *out_rgb8 is released with rtb200_free(). */
 int  rtb200_decode_jpeg_file(const char* path, uint8_t** out_rgb8, uint64_t* width, uint64_t* height);

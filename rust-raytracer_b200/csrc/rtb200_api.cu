@@ -1184,6 +1184,19 @@ static int query_enqueue(rtb200_scene_handle h, const rt_rays& rays, uint32_t n,
     return RT_OK;
 }
 
+// RT_ERR_INVALID unless every non-null pointer of `ptrs` (pointer, name) is device memory of h's device or managed memory.
+// The caller has made h's device current.
+static int check_device_ptrs(rtb200_scene_handle h, const std::vector<std::pair<const void*, const char*>>& ptrs) {
+    for (const auto& q : ptrs) {
+        if (!q.first) continue;
+        cudaPointerAttributes a{};
+        if (cudaPointerGetAttributes(&a, q.first) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
+        if (!((a.type == cudaMemoryTypeDevice && a.device == h->device) || a.type == cudaMemoryTypeManaged))
+            return fail(RT_ERR_INVALID, std::string(q.second) + " is not device or managed memory of device " + std::to_string(h->device));
+    }
+    return RT_OK;
+}
+
 // The device form of both kinds.
 static int query_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const QueryOut* out, void* stream_in) {
     int rc = check_query(h, rays, out);
@@ -1195,13 +1208,7 @@ static int query_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, 
     std::vector<std::pair<const void*, const char*>> ptrs = {{rays->origin, "rays->origin"}, {rays->direction, "rays->direction"},
                                                              {rays->t_max, "rays->t_max"}};
     for (int k = 0; k < out->count; ++k) ptrs.push_back({out->ptr[k], out->name[k]});
-    for (const auto& q : ptrs) {
-        if (!q.first) continue;
-        cudaPointerAttributes a{};
-        if (cudaPointerGetAttributes(&a, q.first) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
-        if (!((a.type == cudaMemoryTypeDevice && a.device == h->device) || a.type == cudaMemoryTypeManaged))
-            return fail(RT_ERR_INVALID, std::string(q.second) + " is not device or managed memory of device " + std::to_string(h->device));
-    }
+    if ((rc = check_device_ptrs(h, ptrs)) != RT_OK) return rc;
     cudaStream_t st;
     CU(scene_stream(h, stream_in, &st));
     if ((rc = query_enqueue(h, *rays, n, *out, nullptr, h->err, st)) != RT_OK) return rc;
@@ -1304,6 +1311,141 @@ int rtb200_scene_occluded(rtb200_scene_handle h, const rt_rays* rays, uint32_t n
     const QueryOut o = occluded_out(occluded);
     return query_host(h, rays, n, &o, stats);
   });
+}
+
+// ---- radiance of caller-supplied primary rays on a resident scene (DESIGN.md §4.12) ----
+// The argument checks both forms share (no device is touched).
+static int check_trace_rays(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_trace_params* p, const void* lin, const void* rgb) {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    if (!rays || !p) return fail(RT_ERR_INVALID, "rays or params is null");
+    if (!rays->origin || !rays->direction) return fail(RT_ERR_INVALID, "rays->origin or rays->direction is null");
+    if (rays->t_max) return fail(RT_ERR_INVALID, "rays->t_max must be null: ray_color traces its rays unbounded");
+    if (!lin && !rgb) return fail(RT_ERR_INVALID, "the linear and rgb8 outputs are both null");
+    if (p->samples == 0) return fail(RT_ERR_INVALID, "params->samples must be > 0");
+    if (p->reserved[0] != 0 || p->reserved[1] != 0) return fail(RT_ERR_INVALID, "rt_trace_params.reserved must be 0");
+    if ((uint64_t)p->stream0 + n > (1ull << 32)) return fail(RT_ERR_INVALID, "stream0 + n exceeds 2^32 (u32 RNG streams)");
+    if ((uint64_t)p->sample0 + p->samples > (1ull << 32)) return fail(RT_ERR_INVALID, "sample0 + samples exceeds 2^32 (u32 sample indices)");
+    if (n >= (1u << 31)) return fail(RT_ERR_INVALID, "n must be below 2^31 (u32 work ids of one sample of every ray)");
+    if ((uint64_t)n * 16 > sample_buffer_cap(h->opts))
+        return fail(RT_ERR_INVALID, "n * 16 bytes exceed the sample-buffer cap (rt_options.sample_buffer_bytes): one sample of every ray must fit");
+    return RT_OK;
+}
+
+// Enqueue the samples of the n rays `rays` (device buffers) on work set 0 and append the submission to h->pending; the caller
+// holds the context's lock and has collected h's asynchronous frames. Per batch of spb samples of every ray one launch of the
+// Q_RAYS trace kernel (a black memset at max_depth 0) and one resolve, which carries the f32 sums across batches as
+// render_enqueue's does. *st_out is the stream the submission runs on.
+static int trace_rays_enqueue(rtb200_scene_handle h, const rt_rays& rays, uint32_t n, const rt_trace_params& tr, float* lin,
+                              uint8_t* rgb, void* stream_in, cudaStream_t* st_out) {
+    DeviceCtx* ctx = h->ctx;
+    DeviceCtx::WorkSet& W = ctx->ws[0];
+    cudaStream_t st;
+    rtb200_scene_t::Submission sub;
+    int rc = submission_open(h, stream_in, 1, &st, &sub);
+    if (rc != RT_OK) return rc;
+    *st_out = st;
+    TraceParams tp = h->tp;
+    tp.npix_local = n;   // Q_RAYS: the rays, which are also the resolve's pixels
+    tp.max_depth = tr.max_depth;
+    tp.key0 = (uint32_t)tr.seed; tp.key1 = (uint32_t)(tr.seed >> 32);
+    tp.stream0 = tr.stream0;
+    tp.ray_o = rays.origin; tp.ray_d = rays.direction;
+    const uint32_t m = tr.samples;
+    uint64_t spb = std::max<uint64_t>(1, sample_buffer_cap(h->opts) / ((uint64_t)n * 16));
+    spb = std::min<uint64_t>(spb, m);
+    while (spb > 1 && spb * n >= (1ull << 31)) spb /= 2;
+    const uint32_t n_batches = (uint32_t)((m + spb - 1) / spb);
+    const size_t smem = wavefront_smem_bytes(tp, h->mode, tp.scene_in_smem, Q_RAYS);
+    const int occ = occupancy(ctx, h->mode, tp.n_lights > 0, Q_RAYS, smem);
+    if (occ <= 0) return fail(RT_ERR_UNSUPPORTED, "no launch configuration of the rays trace kernel fits shared memory");
+    const int grid = ctx->sm_count * occ;
+    sub.grid = grid;
+    sub.batches = n_batches;
+    if ((rc = submission_start(W, st, tp, sub, tp.max_depth, (size_t)spb * n * 16)) != RT_OK) return rc;
+    cudaEvent_t* ev = nullptr;
+    if ((rc = submission_events(h, W, st, sub, &ev)) != RT_OK) return rc;
+    unsigned int* counters = (unsigned int*)((char*)W.small.p + kStatBytes);
+    for (uint32_t b = 0; b < n_batches; ++b) {
+        TraceParams q = tp;
+        const uint32_t first = b * (uint32_t)spb;
+        q.s0 = tr.sample0 + first;
+        q.s_count = (uint32_t)std::min<uint64_t>(spb, m - first);
+        q.total_work = q.s_count * n;
+        q.work_counter = counters + b;
+        q.stack_stride = (uint32_t)grid * (uint32_t)kBlock;
+        CU(cudaEventRecord(ev[2 + 2 * b], st));
+        if (q.max_depth == 0) CU(cudaMemsetAsync(q.samplebuf, 0, (size_t)q.total_work * 16, st));   // ray_color(depth 0) = black, no ray
+        else CU(launch_wavefront(q, h->mode, Q_RAYS, grid, smem, st));
+        CU(cudaEventRecord(ev[3 + 2 * b], st));
+        ResolveParams r{};
+        r.samplebuf = q.samplebuf; r.accum = (float*)W.accum.p; r.npix_local = n;
+        r.s_count = q.s_count; r.first = b == 0; r.last = b + 1 == n_batches; r.spp = m;
+        r.out_linear = lin; r.out_rgb8 = rgb;
+        CU(launch_resolve(r, st));
+    }
+    sub.launches = 2 * n_batches;
+    if (tp.max_depth == 0) sub.black_samples = (uint64_t)n * m;
+    return submission_close(h, W, st, sub);
+}
+
+// Both forms: the device form checks the memory kind of the caller's buffers and traces them on `stream_in`; the host form
+// copies the rays into the context's query block, traces on the library's stream and copies the outputs back.
+static int trace_rays_blocking(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_trace_params* p, float* lin,
+                               uint8_t* rgb, void* stream_in, bool host, rt_stats* stats) {
+    if (stats) memset(stats, 0, sizeof *stats);
+    int rc = check_trace_rays(h, rays, n, p, lin, rgb);
+    if (rc != RT_OK) return rc;
+    if (n == 0) return RT_OK;
+    auto wall0 = std::chrono::steady_clock::now();
+    DeviceRestore restore;
+    DeviceCtx* ctx = h->ctx;
+    std::lock_guard<std::recursive_mutex> lk(ctx->mu);
+    CU(cudaSetDevice(h->device));
+    if (!host && (rc = check_device_ptrs(h, {{rays->origin, "rays->origin"}, {rays->direction, "rays->direction"},
+                                             {lin, "dev_linear_f32"}, {rgb, "dev_rgb8"}})) != RT_OK)
+        return rc;
+    if ((rc = render_collect(h, nullptr)) != RT_OK) return rc;   // the handle's asynchronous frames first, like a blocking render
+    rt_rays drays = *rays;
+    float* dlin = lin;
+    uint8_t* drgb = rgb;
+    const uint64_t N = n;
+    uint64_t h2d = 0, d2h = 0;
+    if (host) {   // device image: origins, directions, linear, rgb8, 256-byte aligned (the last host-form user waited for it)
+        auto al = [](uint64_t b) { return (b + 255) & ~(uint64_t)255; };
+        CU(ctx->query.ensure(2 * al(N * 24) + (lin ? al(N * 12) : 0) + (rgb ? al(N * 3) : 0)));
+        char* D = (char*)ctx->query.p;
+        drays = rt_rays{(const double*)D, (const double*)(D + al(N * 24)), nullptr};
+        char* o = D + 2 * al(N * 24);
+        if (lin) { dlin = (float*)o; o += al(N * 12); }
+        if (rgb) drgb = (uint8_t*)o;
+        cudaStream_t st;
+        CU(scene_stream(h, nullptr, &st));   // the stream the submission takes
+        CU(cudaMemcpyAsync((void*)drays.origin, rays->origin, N * 24, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync((void*)drays.direction, rays->direction, N * 24, cudaMemcpyHostToDevice, st));
+        h2d = N * 48;
+    }
+    cudaStream_t st = nullptr;
+    if ((rc = trace_rays_enqueue(h, drays, n, *p, dlin, drgb, host ? nullptr : stream_in, &st)) != RT_OK) return rc;
+    if (host) {
+        if (lin) { CU(cudaMemcpyAsync(lin, dlin, N * 12, cudaMemcpyDeviceToHost, st)); d2h += N * 12; }
+        if (rgb) { CU(cudaMemcpyAsync(rgb, drgb, N * 3, cudaMemcpyDeviceToHost, st)); d2h += N * 3; }
+    }
+    if ((rc = render_collect(h, stats)) != RT_OK) return rc;
+    if (stats) {
+        stats->h2d_bytes += h2d; stats->d2h_bytes += d2h;
+        stats->wall_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - wall0).count();
+    }
+    return RT_OK;
+}
+
+int rtb200_scene_trace_rays_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_trace_params* params,
+                                   float* dev_linear_f32, uint8_t* dev_rgb8, void* stream_in, rt_stats* stats) {
+  return guarded([&]() -> int { return trace_rays_blocking(h, rays, n, params, dev_linear_f32, dev_rgb8, stream_in, false, stats); });
+}
+
+int rtb200_scene_trace_rays(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_trace_params* params,
+                            float* out_linear_f32, uint8_t* out_rgb8, rt_stats* stats) {
+  return guarded([&]() -> int { return trace_rays_blocking(h, rays, n, params, out_linear_f32, out_rgb8, nullptr, true, stats); });
 }
 
 // ---- adaptive rendering (DESIGN.md §4.9) ----

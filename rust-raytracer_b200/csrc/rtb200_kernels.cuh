@@ -54,9 +54,10 @@ struct ShadowFrame {
 static_assert(sizeof(ShadowFrame) == 88, "ShadowFrame layout");
 
 enum TraceMode : uint32_t { MODE_TREE = 0, MODE_BRUTE = 1, MODE_EXACT = 2 };
-// The work queue of a trace launch: every pixel of one frame, every pixel of several frames (TraceParams::ftab), or the
-// pixels of an adaptive render's list (TraceParams::list, DESIGN.md §4.9)
-enum TraceQueue : uint32_t { Q_SINGLE = 0, Q_FRAMES = 1, Q_LIST = 2 };
+// The work queue of a trace launch: every pixel of one frame, every pixel of several frames (TraceParams::ftab), the
+// pixels of an adaptive render's list (TraceParams::list, DESIGN.md §4.9), or caller-supplied primary rays
+// (TraceParams::ray_o / ray_d, rtb200_scene_trace_rays, DESIGN.md §4.12)
+enum TraceQueue : uint32_t { Q_SINGLE = 0, Q_FRAMES = 1, Q_LIST = 2, Q_RAYS = 3 };
 
 // One frame of a multi-frame launch (rt_wavefront_kernel<.., Q_FRAMES>): the view and the Philox key that replace
 // TraceParams::cam / key0 / key1 for the work ids of that frame.
@@ -102,14 +103,26 @@ struct TraceParams {
     unsigned long long* err;     // per scene handle, accumulated over frames: [0]=shadow-frame-stack overflows [1]=traversal guard trips (must stay 0)
     // ---- multi-frame launches only (appended, so that the fields above keep their offsets) ----
     const FrameRec* ftab;        // [frames of the launch]: work id w belongs to frame w / frame_work
-    uint32_t frame_work;         // work ids per frame = s_count * npix_local; total_work = frames * frame_work
+    union {
+        uint32_t frame_work;     // Q_FRAMES: work ids per frame = s_count * npix_local; total_work = frames * frame_work
+        uint32_t stream0;        // Q_RAYS: ray i draws from the RNG stream of pixel stream0 + i
+    };
     // ---- appended after the multi-frame fields ----
     // 1: a Lambertian or Metal sphere has, or once had, an infinite or NaN albedo component. A black path then has to unwind
     // its albedo stack, and a nested shadow vertex has to read its albedo, because albedo * 0 is NaN for such an albedo.
     uint32_t albedo_nonfinite;
     // ---- Q_LIST launches only (appended after albedo_nonfinite) ----
-    const uint32_t* list;        // local pixel indices, increasing; samplebuf is [s_count][n_list]
-    const uint32_t* list_n;      // device: n_list, read once at kernel start; total_work = n_list * s_count
+    // Q_RAYS launches share these slots (a queue reads only its own member): appending the ray arrays instead would move the
+    // fields that QueryParams and OcclusionParams place after their TraceParams, and with them the query kernels' code.
+    // Q_RAYS: npix_local is the number of rays n; work id w is ray w % n, sample s0 + w / n, samplebuf index w.
+    union {
+        const uint32_t* list;    // Q_LIST: local pixel indices, increasing; samplebuf is [s_count][n_list]
+        const double* ray_o;     // Q_RAYS: [n][3] ray origins
+    };
+    union {
+        const uint32_t* list_n;  // Q_LIST: device: n_list, read once at kernel start; total_work = n_list * s_count
+        const double* ray_d;     // Q_RAYS: [n][3] ray directions
+    };
 };
 
 // An adaptive round's accumulate-and-test (rtb200_adaptive.cu, DESIGN.md §4.9): one thread per list position.
@@ -205,7 +218,8 @@ struct OcclusionParams {
 
 struct KernelInfo { int registers, max_threads, const_bytes, local_bytes; char name[96]; };
 
-// `queue` (TraceQueue): Q_FRAMES is the multi-frame kernel (work ids span p.ftab's frames), Q_LIST the adaptive round's
+// `queue` (TraceQueue): Q_FRAMES is the multi-frame kernel (work ids span p.ftab's frames), Q_LIST the adaptive round's,
+// Q_RAYS the caller-supplied rays' (work ids span samples x rays)
 size_t wavefront_smem_bytes(const TraceParams& p, uint32_t mode, uint32_t smem_mask, uint32_t queue);
 cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, uint32_t queue, int grid, size_t smem, cudaStream_t st);
 int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, uint32_t queue, size_t smem);   // 0 when the kernel cannot run on the current device

@@ -8,7 +8,8 @@
 //   shade_slot<LIGHTS>  ray_color's body for one path vertex (raytracer.rs:71-165): Material::scatter of all five
 //                       materials, the sky, the stochastic light test with its shadow-frame stack, and - when the path
 //                       ends - the backwards unwinding of the albedo stack that reproduces the recursion's f32 products;
-//   regenerate_slot     render_line's per-sample set-up (raytracer.rs:199-201) + Camera::get_ray (camera.rs:79-84).
+//   regenerate_slot     render_line's per-sample set-up (raytracer.rs:199-201) + Camera::get_ray (camera.rs:79-84), or a
+//                       caller-supplied primary ray (Q_RAYS).
 //
 // Ray state lives in shared memory, SoA over the slots of a CTA's pool (struct Pool).
 #pragma once
@@ -507,6 +508,8 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
 // sample, off the bounce loop) and the frame is kept in Pool.frm for the shade stage's draws.
 // Q_LIST: the queue spans samples [s0, s0 + s_count) of the n_list pixels p.list[0, n_list) (an adaptive round, DESIGN.md
 // §4.9); n_list is read from p.list_n once per launch by the caller.
+// Q_RAYS: the queue spans samples [s0, s0 + s_count) of the n = p.npix_local caller-supplied rays p.ray_o / p.ray_d (DESIGN.md
+// §4.12); the slot gets the ray itself instead of a camera ray.
 // =====================================================================================================================
 template <bool LIGHTS, uint32_t QUEUE>
 RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint32_t s, int lane, bool& exhausted, Stats& st,
@@ -525,43 +528,58 @@ RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint
     unsigned my = base + __popc(need & ((1u << lane) - 1u));
     if (my >= (QUEUE == Q_LIST ? n_list * p.s_count : p.total_work)) return false;
     uint32_t f = 0u, k0 = p.key0, k1 = p.key1;
-    if constexpr (FRAMES) { f = my / p.frame_work; my -= f * p.frame_work; k0 = p.ftab[f].key0; k1 = p.ftab[f].key1; }
-    // Order of the global queue: image rows from the BOTTOM up, all samples of a row before the next row, x innermost.
-    // The long paths of these scenes start at the ground / the spheres; the rows handed out last are the top of the image -
-    // sky, one ray per sample - so that the stragglers of the last expensive rows finish under the cover of cheap work
-    // instead of holding nearly empty CTAs for ~50 iterations after the queue ran dry (DESIGN.md §5: 0.5 ms per launch).
-    // The (pixel, sample) -> RNG stream and the samplebuf index do not depend on the order.
-    // Q_LIST: the list is in increasing pixel order and is handed out from its end, so bottom rows go first here too; the
-    // samples of one pixel are consecutive work ids.
     uint32_t x, s_local, y_local, lp, k_list = 0u;
-    if constexpr (QUEUE == Q_LIST) {
-        s_local = my % p.s_count;
-        k_list = n_list - 1u - my / p.s_count;
-        lp = p.list[k_list];
-        y_local = lp / p.width;
-        x = lp - y_local * p.width;
-    } else {
-        x = my % p.width;
-        const uint32_t t_ = my / p.width;
-        s_local = t_ % p.s_count;
-        const uint32_t rr = t_ / p.s_count;
-        y_local = p.rows_local - 1u - rr;
-        lp = y_local * p.width + x;
-    }
-    uint32_t band = y_local / p.band_rows;
-    uint32_t y = (band * (uint32_t)p.world + (uint32_t)p.rank) * p.band_rows + (y_local - band * p.band_rows);
-    Rng rng; rng_init(rng, y * p.width + x, p.s0 + s_local);
-    double xi1 = rng_f64(rng, k0, k1);
-    double u = __ddiv_rn(__dadd_rn((double)x, xi1), __dsub_rn((double)p.width, 1.0));
-    double xi2 = rng_f64(rng, k0, k1);
-    double v = __ddiv_rn(__dsub_rn((double)p.height, __dadd_rn((double)y, xi2)), __dsub_rn((double)p.height, 1.0));
+    Rng rng;
     D3 o, d;
-    if constexpr (FRAMES) get_ray(p.ftab[f].cam, u, v, o, d);
-    else get_ray(p.cam, u, v, o, d);
+    if constexpr (QUEUE == Q_RAYS) {
+        // Ray index innermost: neighbouring lanes take neighbouring, usually coherent, rays, and every sample of the launch
+        // re-reads its ray. Ray i's sample s0 + j draws from the stream of the render's (pixel stream0 + i, sample s0 + j)
+        // past the two jitter draws of raytracer.rs:199-200, which are the two u64 of the stream's first Philox block.
+        const uint32_t i = my % p.npix_local;
+        rng_init(rng, p.stream0 + i, p.s0 + my / p.npix_local);
+        rng.blk = 1u;
+        const double* ro = p.ray_o + 3 * (size_t)i;
+        const double* rd = p.ray_d + 3 * (size_t)i;
+        o = mk(ro[0], ro[1], ro[2]);
+        d = mk(rd[0], rd[1], rd[2]);
+    } else {
+        if constexpr (FRAMES) { f = my / p.frame_work; my -= f * p.frame_work; k0 = p.ftab[f].key0; k1 = p.ftab[f].key1; }
+        // Order of the global queue: image rows from the BOTTOM up, all samples of a row before the next row, x innermost.
+        // The long paths of these scenes start at the ground / the spheres; the rows handed out last are the top of the image -
+        // sky, one ray per sample - so that the stragglers of the last expensive rows finish under the cover of cheap work
+        // instead of holding nearly empty CTAs for ~50 iterations after the queue ran dry (DESIGN.md §5: 0.5 ms per launch).
+        // The (pixel, sample) -> RNG stream and the samplebuf index do not depend on the order.
+        // Q_LIST: the list is in increasing pixel order and is handed out from its end, so bottom rows go first here too; the
+        // samples of one pixel are consecutive work ids.
+        if constexpr (QUEUE == Q_LIST) {
+            s_local = my % p.s_count;
+            k_list = n_list - 1u - my / p.s_count;
+            lp = p.list[k_list];
+            y_local = lp / p.width;
+            x = lp - y_local * p.width;
+        } else {
+            x = my % p.width;
+            const uint32_t t_ = my / p.width;
+            s_local = t_ % p.s_count;
+            const uint32_t rr = t_ / p.s_count;
+            y_local = p.rows_local - 1u - rr;
+            lp = y_local * p.width + x;
+        }
+        uint32_t band = y_local / p.band_rows;
+        uint32_t y = (band * (uint32_t)p.world + (uint32_t)p.rank) * p.band_rows + (y_local - band * p.band_rows);
+        rng_init(rng, y * p.width + x, p.s0 + s_local);
+        double xi1 = rng_f64(rng, k0, k1);
+        double u = __ddiv_rn(__dadd_rn((double)x, xi1), __dsub_rn((double)p.width, 1.0));
+        double xi2 = rng_f64(rng, k0, k1);
+        double v = __ddiv_rn(__dsub_rn((double)p.height, __dadd_rn((double)y, xi2)), __dsub_rn((double)p.height, 1.0));
+        if constexpr (FRAMES) get_ray(p.ftab[f].cam, u, v, o, d);
+        else get_ray(p.cam, u, v, o, d);
+    }
     P.ox[s] = o.x; P.oy[s] = o.y; P.oz[s] = o.z; P.dx[s] = d.x; P.dy[s] = d.y; P.dz[s] = d.z;
-    // samplebuf index [sample][pixel], [frame][sample][pixel], or [sample][list position] (Q_LIST)
+    // samplebuf index [sample][pixel], [frame][sample][pixel], [sample][list position] (Q_LIST) or [sample][ray] (Q_RAYS)
     if constexpr (FRAMES) { P.work[s] = (f * p.s_count + s_local) * p.npix_local + lp; P.frm[s] = f; }
     else if constexpr (QUEUE == Q_LIST) P.work[s] = s_local * n_list + k_list;
+    else if constexpr (QUEUE == Q_RAYS) P.work[s] = my;
     else P.work[s] = s_local * p.npix_local + lp;
     P.pix[s] = rng.pixel; P.smp[s] = rng.sample;
     P.blk[s] = (rng.blk << 1) | rng.has; P.clo[s] = rng.c_lo; P.chi[s] = rng.c_hi;

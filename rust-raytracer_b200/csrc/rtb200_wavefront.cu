@@ -9,8 +9,9 @@
 // The three template modes share everything but the closest-hit stage: MODE_TREE (production: BVH traversal), MODE_BRUTE
 // (RT_VARIANT_BRUTE_FORCE: linear scan with the conservative sphere test) and MODE_EXACT (RT_VARIANT_EXACT_F64: every
 // sphere in f64) - the last two validate the first. Each mode has a single-frame kernel, a multi-frame one (Q_FRAMES: the
-// queue spans several frames of the scene, each with its own camera and key; rtb200_render_frames, DESIGN.md §4.6) and a list
-// one (Q_LIST: the queue spans the pixels still on an adaptive render's list; rtb200_adaptive_step, DESIGN.md §4.9).
+// queue spans several frames of the scene, each with its own camera and key; rtb200_render_frames, DESIGN.md §4.6), a list
+// one (Q_LIST: the queue spans the pixels still on an adaptive render's list; rtb200_adaptive_step, DESIGN.md §4.9) and a rays
+// one (Q_RAYS: the queue spans samples of caller-supplied primary rays; rtb200_scene_trace_rays, DESIGN.md §4.12).
 #include <cstdio>
 #include <cstdlib>
 
@@ -109,6 +110,7 @@ static cudaError_t set_carveout(K kern, uint32_t mode, size_t smem) {
 
 // Q_FRAMES: one launch renders several frames of the scene (TraceParams::ftab / frame_work, rtb200_render_frames)
 // Q_LIST: one launch traces a round of an adaptive render (TraceParams::list / list_n, rtb200_adaptive_step)
+// Q_RAYS: one launch traces a batch of samples of caller-supplied rays (TraceParams::ray_o / ray_d, rtb200_scene_trace_rays)
 template <uint32_t MODE, bool LIGHTS, uint32_t QUEUE>
 __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kernel(const __grid_constant__ TraceParams p) {
     constexpr bool FRAMES = QUEUE == Q_FRAMES;
@@ -251,6 +253,7 @@ static auto dispatch_mode(uint32_t mode, bool lights, F&& f) {
 }
 template <typename F>
 static auto dispatch(uint32_t mode, bool lights, uint32_t queue, F&& f) {
+    if (queue == Q_RAYS) return dispatch_mode<Q_RAYS>(mode, lights, f);
     if (queue == Q_LIST) return dispatch_mode<Q_LIST>(mode, lights, f);
     return queue == Q_FRAMES ? dispatch_mode<Q_FRAMES>(mode, lights, f) : dispatch_mode<Q_SINGLE>(mode, lights, f);
 }
@@ -283,7 +286,7 @@ cudaError_t wavefront_info(uint32_t mode, bool lights, uint32_t queue, KernelInf
         out->registers = a.numRegs; out->max_threads = a.maxThreadsPerBlock; out->const_bytes = (int)a.constSizeBytes; out->local_bytes = (int)a.localSizeBytes;
         snprintf(out->name, sizeof out->name, "rt_wavefront_kernel<%s,%s%s>",
                  mode == MODE_TREE ? "MODE_TREE" : mode == MODE_BRUTE ? "MODE_BRUTE" : "MODE_EXACT", lights ? "LIGHTS" : "NO_LIGHTS",
-                 queue == Q_FRAMES ? ",FRAMES" : queue == Q_LIST ? ",LIST" : "");
+                 queue == Q_FRAMES ? ",FRAMES" : queue == Q_LIST ? ",LIST" : queue == Q_RAYS ? ",RAYS" : "");
         return cudaSuccess;
     });
 }

@@ -120,11 +120,18 @@ class rt_hits(C.Structure):
                 ("front_face", C.c_void_p)]
 
 
+class rt_trace_params(C.Structure):
+    """Radiance of caller-supplied rays (rtb200_scene_trace_rays[_device]): the Philox key, samples per ray, the first sample
+    index, the RNG stream of ray 0 (ray i draws from pixel stream stream0 + i) and the depth of ray_color."""
+    _fields_ = [("seed", C.c_uint64), ("samples", C.c_uint32), ("sample0", C.c_uint32), ("stream0", C.c_uint32),
+                ("max_depth", C.c_uint32), ("reserved", C.c_uint32 * 2)]
+
+
 HIT_FIELDS = (("t", 1, np.float64), ("sphere", 1, np.int32), ("point", 3, np.float64), ("normal", 3, np.float64),
               ("uv", 2, np.float64), ("front_face", 1, np.uint8))   # rt_hits: name, values per ray, dtype (sphere -1 = 0xffffffff)
 
 assert C.sizeof(rt_sphere) == 64 and C.sizeof(rt_frame) == 112 and C.sizeof(rt_adaptive_params) == 24
-assert C.sizeof(rt_rays) == 24 and C.sizeof(rt_hits) == 48
+assert C.sizeof(rt_rays) == 24 and C.sizeof(rt_hits) == 48 and C.sizeof(rt_trace_params) == 32
 
 # every symbol include/rtb200.h declares (tests check that the library exports all of them)
 ABI_SYMBOLS = [
@@ -140,6 +147,7 @@ ABI_SYMBOLS = [
     "rtb200_adaptive_begin", "rtb200_adaptive_step", "rtb200_adaptive_resolve", "rtb200_render_adaptive",
     "rtb200_scene_intersect_device", "rtb200_scene_intersect",
     "rtb200_scene_occluded_device", "rtb200_scene_occluded",
+    "rtb200_scene_trace_rays_device", "rtb200_scene_trace_rays",
 ]
 
 _lib = None
@@ -202,6 +210,10 @@ def lib() -> C.CDLL:
     L.rtb200_scene_intersect.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.POINTER(rt_hits), C.POINTER(rt_stats)]
     L.rtb200_scene_occluded_device.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.c_void_p, C.c_void_p]
     L.rtb200_scene_occluded.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.c_void_p, C.POINTER(rt_stats)]
+    L.rtb200_scene_trace_rays_device.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.POINTER(rt_trace_params), C.c_void_p,
+                                                 C.c_void_p, C.c_void_p, C.POINTER(rt_stats)]
+    L.rtb200_scene_trace_rays.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.POINTER(rt_trace_params), C.c_void_p,
+                                          C.c_void_p, C.POINTER(rt_stats)]
     _lib = L
     return L
 
@@ -691,6 +703,41 @@ class ResidentScene:
                                                       C.c_void_p(self._stream(stream, origin.device) or None)))
         return out
 
+    def trace_rays(self, origin, direction, samples: int = 1, *, sample0: int = 0, stream0: int = 0, seed: Optional[int] = None,
+                   max_depth: Optional[int] = None, linear: bool = True, rgb8: bool = False, stream=None) -> dict:
+        """Radiance of caller-supplied primary rays on the handle's current spheres, as include/rtb200.h states it: `samples`
+        samples of ray_color(Ray{origin[i], direction[i]}, max_depth, max_depth) per ray, sample j drawing from the RNG stream
+        of (pixel stream0 + i, sample sample0 + j) past the render's two jitter draws, resolved like a render with spp =
+        samples. Bit for bit in every variant; seed and max_depth default to the scene's own.
+
+        CUDA tensors (contiguous float64 [n, 3], on the handle's device) use the device form (rtb200_scene_trace_rays_device)
+        on `stream` (as in :meth:`update_geometry`, by default torch's current stream); numpy arrays use the host form
+        (rtb200_scene_trace_rays). Both block until the outputs are written. Returns {"linear": float32 [n, 3]} and/or
+        {"rgb8": uint8 [n, 3]}, whichever is asked for, and "stats"."""
+        if not (linear or rgb8):
+            raise ValueError("trace_rays: ask for linear, rgb8 or both")
+        fields = ([("linear", 3, np.float32)] if linear else []) + ([("rgb8", 3, np.uint8)] if rgb8 else [])
+        p = rt_trace_params(self.scene.seed if seed is None else int(seed), int(samples), int(sample0), int(stream0),
+                            self.scene.c.max_depth if max_depth is None else int(max_depth))
+        st = rt_stats()
+        host = isinstance(origin, np.ndarray)
+        if host:
+            out, rays, n = self._query_host_args("trace_rays", origin, direction, None, fields)
+        else:
+            out, rays, n = self._query_device_args("trace_rays", origin, direction, None, stream, fields)
+        ptr = (lambda a: a.ctypes.data) if host else (lambda t: t.data_ptr())
+        lin_p = C.c_void_p(ptr(out["linear"])) if linear else None
+        rgb_p = C.c_void_p(ptr(out["rgb8"])) if rgb8 else None
+        if n == 0:   # nothing to trace (the library's no-op)
+            pass
+        elif host:
+            _check(lib().rtb200_scene_trace_rays(self.h, C.byref(rays), n, C.byref(p), lin_p, rgb_p, C.byref(st)))
+        else:
+            _check(lib().rtb200_scene_trace_rays_device(self.h, C.byref(rays), n, C.byref(p), lin_p, rgb_p,
+                                                        C.c_void_p(self._stream(stream, origin.device) or None), C.byref(st)))
+        out["stats"] = st.as_dict()
+        return out
+
     def _query_device_args(self, what, origin, direction, t_max, stream, fields):
         """Checks of a query's CUDA tensors; returns the outputs `fields` (name, values per ray, numpy dtype), rt_rays and n."""
         import torch
@@ -706,7 +753,7 @@ class ResidentScene:
                 raise ValueError(f"the tensor {name} is on cuda:{t.device.index}, the scene on cuda:{self.device}")
             if t.device != origin.device:
                 raise ValueError(f"origin is on {origin.device}, {name} on {t.device}")
-        dt = {np.float64: torch.float64, np.int32: torch.int32, np.uint8: torch.uint8}
+        dt = {np.float64: torch.float64, np.float32: torch.float32, np.int32: torch.int32, np.uint8: torch.uint8}
         # outputs belong to the query's stream when it is a torch stream (the caching allocator orders their reuse after it)
         with torch.cuda.stream(stream) if isinstance(stream, torch.cuda.Stream) else torch.cuda.device(origin.device):
             out = {k: torch.empty((n, c) if c > 1 else (n,), dtype=dt[ty], device=origin.device) for k, c, ty in fields}

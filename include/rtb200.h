@@ -237,8 +237,9 @@ int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, u
 /* Replace spheres index[k] (k < n) of a resident scene by spheres[k]: centre, radius and material. Everything is checked on
  * the host before anything is enqueued (on error the scene is unchanged); n == 0 is a no-op. RT_ERR_INVALID: NULL arrays, an
  * index >= n_spheres, a repeated index, an unknown kind, a texture index outside the uploaded textures (or one whose image was
- * empty). RT_ERR_UNSUPPORTED: making a sphere a light or a light something else (the light set is fixed at upload; a light may
- * move). The input is copied into pinned staging memory before the call returns. */
+ * empty). RT_ERR_UNSUPPORTED: making a sphere a light or a light something else (a light may move; to change the set of lights,
+ * remove and insert the spheres with rtb200_scene_edit_spheres). The input is copied into pinned staging memory before the
+ * call returns. */
 int rtb200_scene_update_spheres(rtb200_scene_handle h, const uint32_t* index, const rt_sphere* spheres, uint32_t n, void* stream);
 /* Replace the centre and radius of EVERY sphere from device memory: n_spheres x {cx, cy, cz, radius} f64 (the layout of the geo
  * array); materials stay. Any values are accepted. RT_ERR_INVALID for a NULL pointer or one that is not device memory of h's
@@ -273,6 +274,33 @@ int rtb200_scene_rebuild(rtb200_scene_handle h, void* stream);
 int rtb200_scene_debug_topology(rtb200_scene_handle h, double recentre[3], uint32_t info[8], uint32_t* leaf_id, uint64_t cap_leaf_id,
                                 uint32_t* always, uint64_t cap_always, uint32_t* skip_pos, uint64_t cap_skip_pos,
                                 uint32_t* level_nodes, uint64_t cap_level_nodes, uint32_t* level_off, uint64_t cap_level_off);
+
+/* Insert and remove spheres of a resident scene, on the GPU (DESIGN.md §4.13). The edited list is the old list without the
+ * spheres remove[0, n_remove) (indices into the old list, distinct, < n_spheres), with insert[k] placed just before old sphere
+ * at[k] for every k < n_insert. at is non-decreasing with values in [0, n_spheres]; n_spheres appends, and at == NULL appends
+ * every insert; inserts with equal at keep their order. So a kept old sphere i lands at kept(< i) + #{k : at[k] <= i} and
+ * insert k at kept(< at[k]) + k, where kept(< j) counts the kept old spheres below j (also when at[k] names a removed sphere).
+ * Lights are the Light spheres of the new list in its order, so an edit may change them.
+ * Contract, the update's: after an edit every call on h is bit-identical to the same call on a fresh upload of the edited list
+ * with the same textures, sky, camera, seed and options: renders, frames, adaptive renders and trace_rays (linear f32, RGB8,
+ * rays) and every output of the queries, with the new sphere indices (the diagnostic candidates / clusters / nodes counters
+ * may differ: a RT_VARIANT_FILTERED / AUTO handle gets the rebuild's hierarchy of the new list, as rtb200_scene_rebuild).
+ * Everything is checked on the host before anything is enqueued; on error the scene is unchanged. RT_ERR_INVALID: a NULL
+ * handle, a NULL remove with n_remove > 0 or insert with n_insert > 0, a remove index >= n_spheres or repeated, an at that
+ * decreases or exceeds n_spheres, an insert that rtb200_scene_update_spheres would refuse as INVALID. RT_ERR_UNSUPPORTED: a
+ * list of 2^26 spheres or more, 10 or more lights, a handle that stages the scene in shared memory (any RTB200_WF_SMEM bit at
+ * upload). RT_ERR_OOM: device memory for the new arrays cannot be allocated. n_remove == n_insert == 0 is a no-op.
+ * Ordering and blocking, like rtb200_scene_rebuild: on `stream` (NULL: the library's stream) after the handle's last update,
+ * rebuild or edit and after every frame and query of h already enqueued, on any stream; every frame, query, update and rebuild
+ * enqueued later sees the new list. The call returns when the new list and its topology exist. It counts as an update (an
+ * adaptive render begun before it refuses to step). Host work and copies are O(n_remove + n_insert): the indices and the
+ * inserted records go through pinned staging memory.
+ * Memory: the new list lives in a per-handle block of two halves (the list and the next edit's target) for up to cap spheres,
+ * about 2 * 64 B per sphere (+ 2 * 16 B in RT_VARIANT_BRUTE_FORCE) plus 12 B of skip and scan arrays, allocated at the first
+ * edit and replaced by one of at least twice the size when an edit needs more; a hierarchy handle grows its rebuild block
+ * by half when the new list needs more. Both are freed at release; the upload's arrays stay as they are. */
+int rtb200_scene_edit_spheres(rtb200_scene_handle h, const uint32_t* remove, uint32_t n_remove, const uint32_t* at,
+                              const rt_sphere* insert, uint32_t n_insert, void* stream);
 
 /* ---- adaptive rendering: stop sampling the pixels that have converged (DESIGN.md §4.9) -----------------------------------
  * Parameters: m = samples_per_round >= 1, N = max_samples (0: the scene's samples_per_pixel), min_samples >= 1, and the f32

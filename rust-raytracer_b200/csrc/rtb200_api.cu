@@ -215,8 +215,24 @@ struct rtb200_scene_t {
     double* leaf_box = nullptr;          // n_leaves exact boxes
     uint32_t* level_nodes_dev = nullptr;
     // ---- rebuilt hierarchy (rtb200_scene_rebuild): its arrays and the refit's scratch, allocated at the first rebuild ----
-    void* rebuild = nullptr;             // RebuildBufs of tp.n spheres; once set, the tree arrays of tp and the refit scratch live here
-    GrowBuf upd_in;                      // host form's input: geo, materials, indices
+    void* rebuild = nullptr;             // RebuildBufs of rebuild_n spheres; once set, the tree arrays of tp and the refit scratch live here
+    uint32_t rebuild_n = 0;
+    GrowBuf upd_in;                      // host form's input: geo, materials, indices (an edit's: remove, at, geo, materials)
+    // ---- edited list (rtb200_scene_edit_spheres, DESIGN.md §4.13): one device block for up to cap spheres, allocated at the
+    // first edit and replaced by a larger one when an edit needs more. The list lives in half ed_cur (-1: still in the upload
+    // arena) and the next edit writes the other half: frames enqueued before an edit keep reading the arrays they were
+    // enqueued with ----
+    struct EditBlock {
+        void* mem = nullptr;
+        uint32_t cap = 0;
+        struct Half { double4* geo; DevMat* mat; float* filt; uint32_t* lights; } half[2] = {};   // filt: MODE_BRUTE only
+        uint32_t* skip_pos = nullptr;    // cap x kNoSkip: the skip_pos of a list without a hierarchy
+        uint32_t* keep = nullptr;        // cap + 1 words each: the keep flags of the old list and their scan
+        uint32_t* pos = nullptr;
+        void* temp = nullptr;            // cub's scan scratch
+        size_t temp_bytes = 0;
+    } ed;
+    int ed_cur = -1;
     uint32_t updates = 0;                // rtb200_scene_update_* calls so far: an adaptive render refuses to step across one
     // ---- closest-hit queries (rtb200_scene_intersect_device): queries[0, n_queries) hold the last query of each stream enqueued
     // since the last update or rebuild, which the next update or rebuild waits for; the rest are spare events ----
@@ -336,6 +352,7 @@ int rtb200_scene_release(rtb200_scene_handle h) {
         for (const auto& q : h->queries) { cudaEventSynchronize(q.done); cudaEventDestroy(q.done); }   // queries in flight read them
         if (h->refit) cudaFree(h->refit);
         if (h->rebuild) cudaFree(h->rebuild);
+        if (h->ed.mem) cudaFree(h->ed.mem);
         if (h->upd_in.p) cudaFree(h->upd_in.p);
         if (h->ad.mem) cudaFree(h->ad.mem);
         if (h->ad.active_host) cudaFreeHost(h->ad.active_host);
@@ -953,6 +970,15 @@ static int update_finish(rtb200_scene_handle h, cudaStream_t st) {
     return RT_OK;
 }
 
+// The checks of one sphere a resident scene takes, sphere k of the caller's array `what` (updates and edits): a known kind, and
+// a Texture index of an uploaded texture whose image was not empty.
+static int check_sphere(rtb200_scene_handle h, const rt_sphere& sp, const char* what, uint32_t k) {
+    if (sp.kind > RT_LIGHT) return fail(RT_ERR_INVALID, "unknown material kind (" + std::string(what) + "[" + std::to_string(k) + "])");
+    if (sp.kind == RT_TEXTURE && (sp.texture < 0 || (size_t)sp.texture >= h->tex_ok.size() || !h->tex_ok[sp.texture]))
+        return fail(RT_ERR_INVALID, "texture index out of range, or its image was empty at upload (" + std::string(what) + "[" + std::to_string(k) + "])");
+    return RT_OK;
+}
+
 int rtb200_scene_update_spheres(rtb200_scene_handle h, const uint32_t* index, const rt_sphere* spheres, uint32_t n, void* stream_in) {
   return guarded([&]() -> int {
     if (n && (!index || !spheres)) return fail(RT_ERR_INVALID, "index or spheres is null");
@@ -966,9 +992,8 @@ int rtb200_scene_update_spheres(rtb200_scene_handle h, const uint32_t* index, co
         if (sorted[k] == sorted[k - 1]) return fail(RT_ERR_INVALID, "sphere " + std::to_string(sorted[k]) + " is listed twice");
     for (uint32_t k = 0; k < n; ++k) {
         const rt_sphere& sp = spheres[k];
-        if (sp.kind > RT_LIGHT) return fail(RT_ERR_INVALID, "unknown material kind (spheres[" + std::to_string(k) + "])");
-        if (sp.kind == RT_TEXTURE && (sp.texture < 0 || (size_t)sp.texture >= h->tex_ok.size() || !h->tex_ok[sp.texture]))
-            return fail(RT_ERR_INVALID, "texture index out of range, or its image was empty at upload (spheres[" + std::to_string(k) + "])");
+        int rc = check_sphere(h, sp, "spheres", k);
+        if (rc != RT_OK) return rc;
         const bool was_light = std::binary_search(h->light_idx.begin(), h->light_idx.end(), index[k]);
         if (was_light != (sp.kind == RT_LIGHT))
             return fail(RT_ERR_UNSUPPORTED, "sphere " + std::to_string(index[k]) + ": the set of lights is fixed at upload (upload the scene again to change it)");
@@ -1059,37 +1084,39 @@ int rtb200_scene_debug_records(rtb200_scene_handle h, uint32_t info[8], float* n
 }
 
 // ---- rebuilding the hierarchy of a resident scene on the GPU (DESIGN.md §4.8) ----
-// The topology comes from rtb200_rebuild.cu, its values from the refit's kernels; the host reads back one header (counts,
-// depth, level sizes, recentring offset) between the two. The new arrays live in the handle's rebuild block, which frames
-// enqueued before the call may still read (after an earlier rebuild): the build waits for them.
-int rtb200_scene_rebuild(rtb200_scene_handle h, void* stream_in) {
-  return guarded([&]() -> int {
-    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
-    if (h->mode != MODE_TREE || h->tp.n == 0) return RT_OK;   // no hierarchy to rebuild
-    if (h->tp.scene_in_smem & 1u)
-        return fail(RT_ERR_UNSUPPORTED, "the handle stages its hierarchy in shared memory (RTB200_WF_SMEM bit 0), whose launch layout is fixed at upload");
-    DeviceRestore restore;
-    DeviceCtx* ctx = h->ctx;
-    std::lock_guard<std::recursive_mutex> lk(ctx->mu);
-    CU(cudaSetDevice(h->device));
-    const uint32_t n = h->tp.n;
-    if (!h->rebuild) {
-        void* p = nullptr;
-        const size_t bytes = rebuild_carve(nullptr, n, nullptr);
-        const cudaError_t e = cudaMalloc(&p, bytes);
-        if (e != cudaSuccess) {
-            cudaGetLastError();
-            return fail(RT_ERR_OOM, "rebuild: cannot allocate " + std::to_string(bytes) + " bytes of device memory for " + std::to_string(n) + " spheres");
-        }
-        h->rebuild = p;
+// A device allocation a call makes before it enqueues anything, freed on return unless the call took it over (take).
+struct FreshBlock {
+    void* p = nullptr;
+    uint32_t cap = 0;                    // spheres it is carved for
+    ~FreshBlock() { if (p) cudaFree(p); }
+    void* take() { void* q = p; p = nullptr; return q; }
+};
+
+// The rebuild block a hierarchy of n spheres needs: h->rebuild when it holds them, else a new block in *fresh, which
+// rebuild_tree installs (frames in flight may still read the old one). The first block holds n spheres; a block that has to
+// grow for an edit takes half as much again, so that a run of appends does not allocate on every call.
+static int rebuild_reserve(rtb200_scene_handle h, uint32_t n, FreshBlock* fresh) {
+    if (h->rebuild && n <= h->rebuild_n) return RT_OK;
+    const uint32_t cap = h->rebuild ? (uint32_t)std::min<uint64_t>(std::max<uint64_t>(n, (uint64_t)h->rebuild_n * 3 / 2), (1u << 26) - 1) : n;
+    const size_t bytes = rebuild_carve(nullptr, cap, nullptr);
+    const cudaError_t e = cudaMalloc(&fresh->p, bytes);
+    if (e != cudaSuccess) {
+        cudaGetLastError();
+        fresh->p = nullptr;
+        return fail(RT_ERR_OOM, "rebuild: cannot allocate " + std::to_string(bytes) + " bytes of device memory for " + std::to_string(cap) + " spheres");
     }
+    fresh->cap = cap;
+    return RT_OK;
+}
+
+// A new hierarchy over tp.geo[0, n), n > 0, enqueued on st, which the caller has ordered after h's last writer and after the
+// frames and queries of h in flight (update_after_frames), and installed in tp. The topology comes from rtb200_rebuild.cu, its
+// values from the refit's kernels; the host reads back one header (counts, depth, level sizes, recentring offset) between the
+// two, so st has passed those frames when this returns. The arrays live in the rebuild block (`fresh` when rebuild_reserve
+// made one; the old block is freed once st has passed the frames that may read it).
+static int rebuild_tree(rtb200_scene_handle h, uint32_t n, FreshBlock& fresh, cudaStream_t st) {
     RebuildBufs b;
-    rebuild_carve(h->rebuild, n, &b);
-    cudaStream_t st;
-    CU(scene_stream(h, stream_in, &st));
-    CU(update_begin(h));
-    int rc = update_after_frames(h, st);
-    if (rc != RT_OK) return rc;
+    rebuild_carve(fresh.p ? fresh.p : h->rebuild, fresh.p ? fresh.cap : h->rebuild_n, &b);
     const char* ov = getenv("RTB200_REBUILD_OVERSIZE");   // benchmark hook: 0 keeps oversized spheres in the Morton order
     CU(launch_rebuild_topology(b, h->tp.geo, n, ov ? atof(ov) : kRebuildOversize, st));
     RebuildHeader H;
@@ -1108,6 +1135,11 @@ int rtb200_scene_rebuild(rtb200_scene_handle h, void* stream_in) {
     CU(cudaEventRecord(h->updated, st));
     // every frame enqueued from here on traces the new tree, and every update refits it
     if (h->refit) { CU(cudaFree(h->refit)); h->refit = nullptr; }   // the stream synchronisation above covers the updates that used it
+    if (fresh.p) {
+        if (h->rebuild) CU(cudaFree(h->rebuild));   // and the frames that read the old block
+        h->rebuild_n = fresh.cap;
+        h->rebuild = fresh.take();
+    }
     TraceParams& tp = h->tp;
     tp.nodes = (const float4*)b.nodes; tp.leaf_rec = (const float4*)b.leaf_rec; tp.leaf_id = b.leaf_id;
     tp.skip_pos = b.skip_pos; tp.always = b.always;
@@ -1116,6 +1148,189 @@ int rtb200_scene_rebuild(rtb200_scene_handle h, void* stream_in) {
     h->level_off = level_off;
     h->level_nodes.clear();
     h->node_box = b.node_box; h->leaf_box = b.leaf_box; h->level_nodes_dev = b.level_nodes;
+    return RT_OK;
+}
+
+int rtb200_scene_rebuild(rtb200_scene_handle h, void* stream_in) {
+  return guarded([&]() -> int {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    if (h->mode != MODE_TREE || h->tp.n == 0) return RT_OK;   // no hierarchy to rebuild
+    if (h->tp.scene_in_smem & 1u)
+        return fail(RT_ERR_UNSUPPORTED, "the handle stages its hierarchy in shared memory (RTB200_WF_SMEM bit 0), whose launch layout is fixed at upload");
+    DeviceRestore restore;
+    DeviceCtx* ctx = h->ctx;
+    std::lock_guard<std::recursive_mutex> lk(ctx->mu);
+    CU(cudaSetDevice(h->device));
+    FreshBlock fresh;
+    int rc = rebuild_reserve(h, h->tp.n, &fresh);
+    if (rc != RT_OK) return rc;
+    cudaStream_t st;
+    CU(scene_stream(h, stream_in, &st));
+    CU(update_begin(h));
+    if ((rc = update_after_frames(h, st)) != RT_OK) return rc;
+    return rebuild_tree(h, h->tp.n, fresh, st);
+  });
+}
+
+// ---- inserting and removing spheres of a resident scene (DESIGN.md §4.13) ----
+// The edit block of `cap` spheres carved out of `base` (null: only the size); returns the bytes. `flat`: the halves carry flat
+// records (MODE_BRUTE).
+static size_t edit_carve(void* base, uint32_t cap, bool flat, rtb200_scene_t::EditBlock* out) {
+    size_t off = 0;
+    char* p = (char*)base;
+    auto take = [&](size_t bytes) -> void* { void* q = p ? p + off : nullptr; off += (bytes + 255) & ~(size_t)255; return q; };
+    rtb200_scene_t::EditBlock b;
+    b.mem = base; b.cap = cap;
+    for (auto& H : b.half) {
+        H.geo = (double4*)take((size_t)cap * 32);
+        H.mat = (DevMat*)take((size_t)cap * sizeof(DevMat));
+        H.filt = flat ? (float*)take((size_t)rtbvh::flat_pairs(cap) * 32) : nullptr;
+        H.lights = (uint32_t*)take(16 * 4);   // at most 9 lights and the trailing 0 of the upload's list
+    }
+    b.skip_pos = (uint32_t*)take((size_t)cap * 4);
+    b.keep = (uint32_t*)take(((size_t)cap + 1) * 4);
+    b.pos = (uint32_t*)take(((size_t)cap + 1) * 4);
+    b.temp_bytes = edit_scan_bytes(cap);
+    b.temp = take(b.temp_bytes);
+    if (out) *out = b;
+    return off;
+}
+
+int rtb200_scene_edit_spheres(rtb200_scene_handle h, const uint32_t* remove, uint32_t n_remove, const uint32_t* at,
+                              const rt_sphere* insert, uint32_t n_insert, void* stream_in) {
+  return guarded([&]() -> int {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    if (n_remove && !remove) return fail(RT_ERR_INVALID, "remove is null");
+    if (n_insert && !insert) return fail(RT_ERR_INVALID, "insert is null");
+    if (n_remove == 0 && n_insert == 0) return RT_OK;
+    // everything is checked before anything is enqueued: on error the scene is unchanged
+    const uint32_t n_old = h->tp.n;
+    std::vector<uint32_t> rem(remove, remove + n_remove);
+    std::sort(rem.begin(), rem.end());
+    if (n_remove && rem.back() >= n_old)
+        return fail(RT_ERR_INVALID, "remove index " + std::to_string(rem.back()) + " is not a sphere of the scene (n_spheres = " + std::to_string(n_old) + ")");
+    for (uint32_t k = 1; k < n_remove; ++k)
+        if (rem[k] == rem[k - 1]) return fail(RT_ERR_INVALID, "sphere " + std::to_string(rem[k]) + " is listed twice in remove");
+    std::vector<uint32_t> at_v(n_insert, n_old);   // at == NULL: every insert is appended
+    for (uint32_t k = 0; k < n_insert; ++k) {
+        if (at) {
+            if (at[k] > n_old) return fail(RT_ERR_INVALID, "at[" + std::to_string(k) + "] = " + std::to_string(at[k]) + " exceeds n_spheres = " + std::to_string(n_old));
+            if (k && at[k] < at[k - 1]) return fail(RT_ERR_INVALID, "at decreases at at[" + std::to_string(k) + "]");
+            at_v[k] = at[k];
+        }
+        int rc = check_sphere(h, insert[k], "insert", k);
+        if (rc != RT_OK) return rc;
+    }
+    const uint64_t n_new64 = (uint64_t)n_old - n_remove + n_insert;
+    if (n_new64 >= (1ull << 26)) return fail(RT_ERR_UNSUPPORTED, "2^26 or more spheres (list entries carry 27-bit ids)");
+    const uint32_t n_new = (uint32_t)n_new64;
+    // the lights in the new list order: a kept old sphere i goes to kept(< i) + #{k : at[k] <= i}, insert k to kept(< at[k]) + k
+    auto kept_below = [&](uint32_t j) { return j - (uint32_t)(std::lower_bound(rem.begin(), rem.end(), j) - rem.begin()); };
+    std::vector<uint32_t> lights;
+    for (uint32_t i : h->light_idx)
+        if (!std::binary_search(rem.begin(), rem.end(), i))
+            lights.push_back(kept_below(i) + (uint32_t)(std::upper_bound(at_v.begin(), at_v.end(), i) - at_v.begin()));
+    for (uint32_t k = 0; k < n_insert; ++k)
+        if (insert[k].kind == RT_LIGHT) lights.push_back(kept_below(at_v[k]) + k);
+    std::sort(lights.begin(), lights.end());
+    if (lights.size() >= 10) return fail(RT_ERR_UNSUPPORTED, "10 or more lights: the reference's light recursion (raytracer.rs:99-114) does not terminate when n_lights * 0.1 >= 1");
+    if (h->tp.scene_in_smem)
+        return fail(RT_ERR_UNSUPPORTED, "the handle stages the scene in shared memory (RTB200_WF_SMEM), whose launch layout is fixed at upload");
+
+    DeviceRestore restore;
+    DeviceCtx* ctx = h->ctx;
+    std::lock_guard<std::recursive_mutex> lk(ctx->mu);
+    CU(cudaSetDevice(h->device));
+    TraceParams& tp = h->tp;
+    // the single-frame kernel is another template with lights than without: its launch geometry follows n_lights > 0
+    int occ = h->ctas_per_sm;
+    if (lights.empty() != (tp.n_lights == 0)) {
+        occ = occupancy(ctx, h->mode, !lights.empty(), Q_SINGLE, h->smem);
+        if (occ <= 0) return fail(RT_ERR_UNSUPPORTED, "no launch configuration fits shared memory");
+    }
+    // device memory before anything is enqueued: a larger edit block, the rebuild block, the input
+    const uint32_t need = std::max(std::max(n_old, n_new), 1u);
+    FreshBlock fresh_ed, fresh_rb;
+    rtb200_scene_t::EditBlock E = h->ed;
+    if (need > E.cap) {   // grows geometrically: a run of single appends allocates once in a while, not on every call
+        const uint32_t cap = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(std::max<uint64_t>(need + need / 2, 2ull * E.cap), 64), 1u << 26);
+        const size_t bytes = edit_carve(nullptr, cap, h->mode == MODE_BRUTE, nullptr);
+        if (cudaMalloc(&fresh_ed.p, bytes) != cudaSuccess) {
+            cudaGetLastError();
+            fresh_ed.p = nullptr;
+            return fail(RT_ERR_OOM, "edit: cannot allocate " + std::to_string(bytes) + " bytes of device memory for " + std::to_string(cap) + " spheres");
+        }
+        edit_carve(fresh_ed.p, cap, h->mode == MODE_BRUTE, &E);
+    }
+    int rc = RT_OK;
+    if (h->mode == MODE_TREE && n_new > 0 && (rc = rebuild_reserve(h, n_new, &fresh_rb)) != RT_OK) return rc;
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    const size_t at_off = al((size_t)n_remove * 4), geo_off = at_off + al((size_t)n_insert * 4), mat_off = geo_off + al((size_t)n_insert * 32),
+                 in_bytes = mat_off + al((size_t)n_insert * sizeof(DevMat));
+    CU(h->upd_in.ensure(in_bytes, h->updated));   // after the last update, which read it
+    const int tgt = fresh_ed.p || h->ed_cur != 0 ? 0 : 1;   // the half that does not hold the current list
+    const auto& T = E.half[tgt];
+
+    ++h->updates;
+    cudaStream_t st;   // after the previous update or edit too: it may still read upd_in and the target half
+    CU(scene_stream(h, stream_in, &st));
+    CU(update_begin(h));
+    // input in the pinned staging buffer (remove, at, the inserts' geo and materials; the light list), copied before this
+    // call returns
+    lights.push_back(0);
+    CU(cudaEventSynchronize(ctx->staging_free));   // the previous copy has left the staging buffer
+    CU(ctx->staging.ensure(in_bytes + lights.size() * 4));
+    char* S = (char*)ctx->staging.p;
+    memcpy(S, rem.data(), (size_t)n_remove * 4);
+    memcpy(S + at_off, at_v.data(), (size_t)n_insert * 4);
+    bool nonfinite = false;
+    for (uint32_t k = 0; k < n_insert; ++k) {
+        rtbvh::sphere_exact(insert[k], (double*)(S + geo_off) + 4 * (size_t)k, ((rtbvh::Mat32*)(S + mat_off))[k]);
+        nonfinite = nonfinite || albedo_nonfinite(insert[k]);
+    }
+    memcpy(S + in_bytes, lights.data(), lights.size() * 4);
+    char* D = (char*)h->upd_in.p;
+    CU(cudaMemcpyAsync(D, S, in_bytes, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(T.lights, S + in_bytes, lights.size() * 4, cudaMemcpyHostToDevice, st));
+    CU(cudaEventRecord(ctx->staging_free, st));   // before the wait for the frames pending now (DESIGN.md §4.7, Ordering)
+    if ((rc = update_after_frames(h, st)) != RT_OK) return rc;
+    if (fresh_ed.p) CU(cudaMemsetAsync(E.skip_pos, 0xff, (size_t)E.cap * 4, st));   // rtbvh::kNoSkip
+    EditParams p{};
+    p.geo_old = tp.geo; p.mat_old = tp.mat; p.n_old = n_old;
+    p.remove = (const uint32_t*)D; p.n_remove = n_remove;
+    p.at = (const uint32_t*)(D + at_off); p.geo_in = (const double4*)(D + geo_off); p.mat_in = (const DevMat*)(D + mat_off); p.n_insert = n_insert;
+    p.keep = E.keep; p.pos = E.pos; p.temp = E.temp; p.temp_bytes = E.temp_bytes;
+    p.geo = T.geo; p.mat = T.mat;
+    p.filt = T.filt; p.n_pairs = rtbvh::flat_pairs(n_new);
+    CU(launch_edit_spheres(p, st));
+
+    // every frame, query, update and rebuild enqueued from here on sees the new list
+    void* retired = fresh_ed.p ? h->ed.mem : nullptr;   // freed once st has passed the frames that may read it
+    if (fresh_ed.p) { h->ed = E; fresh_ed.take(); }
+    h->ed_cur = tgt;
+    lights.pop_back();
+    tp.n = n_new; tp.n_pairs = p.n_pairs;
+    tp.geo = T.geo; tp.mat = T.mat; tp.lights = T.lights; tp.n_lights = (uint32_t)lights.size();
+    if (nonfinite) tp.albedo_nonfinite = 1u;   // never cleared, as in an update
+    if (h->mode == MODE_BRUTE) tp.filt = (const float4*)T.filt;
+    if (h->mode != MODE_TREE || n_new == 0) tp.skip_pos = E.skip_pos;
+    h->light_idx = lights;
+    h->ctas_per_sm = occ;
+    h->grid = ctx->sm_count * occ;
+    if (h->mode == MODE_TREE && n_new > 0) {
+        if ((rc = rebuild_tree(h, n_new, fresh_rb, st)) != RT_OK) return rc;   // returns when st has passed the frames
+    } else {
+        if (h->mode == MODE_TREE) {   // no spheres: the hierarchy of an empty upload
+            tp.n_nodes = tp.n_leaves = tp.n_always = tp.depth = 0;
+            tp.gx = tp.gy = tp.gz = 0.0;
+            h->level_off.clear(); h->level_nodes.clear();
+            h->node_box = h->leaf_box = nullptr; h->level_nodes_dev = nullptr;
+        }
+        if ((rc = update_finish(h, st)) != RT_OK) return rc;   // MODE_BRUTE: the flat records at the handle's recentring offset
+        CU(cudaStreamSynchronize(st));
+        if (h->refit) { CU(cudaFree(h->refit)); h->refit = nullptr; }
+    }
+    if (retired) CU(cudaFree(retired));
     return RT_OK;
   });
 }

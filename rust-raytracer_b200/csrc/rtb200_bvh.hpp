@@ -148,6 +148,12 @@ inline void sphere_exact(const rt_sphere& sp, double G[4], Mat32& m) {
     else { m.r = m.g = m.b = 1.0f; }   // Glass/Light attenuation is (1,1,1) (materials.rs:67,179); Texture uses texels
 }
 
+// Record pairs of the flat array for n spheres: the scan loop consumes blocks of 4 pairs; padding records never hit.
+inline uint32_t flat_pairs(uint32_t n) {
+    const uint32_t n_pairs = ((n + 1) / 2 + 7) / 8 * 8;
+    return n_pairs ? n_pairs : 8;
+}
+
 struct Box {
     double lo[3] = {INFINITY, INFINITY, INFINITY}, hi[3] = {-INFINITY, -INFINITY, -INFINITY};
     void grow(const Box& o) { for (int a = 0; a < 3; ++a) { lo[a] = std::min(lo[a], o.lo[a]); hi[a] = std::max(hi[a], o.hi[a]); } }
@@ -242,8 +248,7 @@ private:
 
     void flat_and_exact() {
         const uint32_t n = R_.n;
-        uint32_t n_pairs = ((n + 1) / 2 + 7) / 8 * 8;   // the scan loop consumes blocks of 4 pairs; padding records never hit
-        if (n_pairs == 0) n_pairs = 8;
+        const uint32_t n_pairs = flat_pairs(n);
         R_.n_pairs = n_pairs;
         R_.flat.assign((size_t)n_pairs * 8, 0.f);
         R_.geo.assign((size_t)std::max<uint32_t>(n, 1) * 4, 0.0);

@@ -195,6 +195,24 @@ struct RebuildBufs {
     void* temp; size_t temp_bytes;                   // cub's temporary storage
 };
 
+// Insert and remove spheres of a resident scene (rtb200_edit.cu, DESIGN.md §4.13): the old list without remove[0, n_remove),
+// with insert k placed just before old sphere at[k] (at non-decreasing, at most n_old), written to geo / mat, which are not the
+// old arrays. keep and pos hold n_old + 1 words.
+struct EditParams {
+    const double4* geo_old; const DevMat* mat_old;
+    uint32_t n_old;
+    const uint32_t* remove;      // [n_remove] distinct, below n_old
+    uint32_t n_remove;
+    const uint32_t* at;          // [n_insert]
+    const double4* geo_in; const DevMat* mat_in;
+    uint32_t n_insert;
+    uint32_t* keep; uint32_t* pos;   // keep[i]: old sphere i stays; pos[j] = kept(< j), the exclusive scan of keep
+    void* temp; size_t temp_bytes;   // cub's scan scratch (edit_scan_bytes)
+    double4* geo; DevMat* mat;
+    float* filt;                 // MODE_BRUTE: the new flat records, whose slots [n_old - n_remove + n_insert, 2 * n_pairs) get
+    uint32_t n_pairs;            // the builder's padding; else null
+};
+
 // Closest-hit queries on caller-supplied rays (rtb200_query.cu, DESIGN.md §4.10). `p` is the handle's TraceParams: closest_hit
 // reads the scene fields of it, err (guard trips) and stat (the counters; null: not counted). The outputs of rt_hits may be null.
 struct QueryParams {
@@ -252,6 +270,9 @@ size_t rebuild_carve(void* base, uint32_t n, RebuildBufs* b);
 // |radius| exceeds `oversize` times the median |radius| gets its own subtree near the root (oversize <= 0: none does).
 constexpr double kRebuildOversize = 16.0;
 cudaError_t launch_rebuild_topology(const RebuildBufs& b, const double4* geo, uint32_t n, double oversize, cudaStream_t st);
+// the edited list (EditParams): keep flags, their scan, every kept and inserted record at its new position, flat padding
+size_t edit_scan_bytes(uint32_t n_old);   // cub's scan scratch for n_old + 1 flags
+cudaError_t launch_edit_spheres(const EditParams& p, cudaStream_t st);
 
 // single-thread probes of the device routines (known-answer tests)
 cudaError_t probe_sphere_hit(const double* in /*12*/, double* out /*9*/, cudaStream_t st);

@@ -148,6 +148,7 @@ ABI_SYMBOLS = [
     "rtb200_scene_intersect_device", "rtb200_scene_intersect",
     "rtb200_scene_occluded_device", "rtb200_scene_occluded",
     "rtb200_scene_trace_rays_device", "rtb200_scene_trace_rays",
+    "rtb200_scene_edit_spheres",
 ]
 
 _lib = None
@@ -214,6 +215,7 @@ def lib() -> C.CDLL:
                                                  C.c_void_p, C.c_void_p, C.POINTER(rt_stats)]
     L.rtb200_scene_trace_rays.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.POINTER(rt_trace_params), C.c_void_p,
                                           C.c_void_p, C.POINTER(rt_stats)]
+    L.rtb200_scene_edit_spheres.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
     _lib = L
     return L
 
@@ -272,6 +274,40 @@ def _decode_jpeg(path: str) -> np.ndarray:
     finally:
         lib().rtb200_free(buf)
     return arr
+
+
+def _set_material(s: rt_sphere, material):
+    """Give sphere record s a JSON material ({"Metal": {"albedo": [...], "fuzz": f}}, ...; a Texture names one of the scene's
+    textures by index: {"Texture": {"albedo": [...], "h_offset": f, "texture": k}}) or the material of an rt_sphere."""
+    if isinstance(material, rt_sphere):
+        s.kind, s.param, s.texture = material.kind, material.param, material.texture
+        s.albedo[:] = list(material.albedo)
+        return
+    (kind, body), = material.items()
+    s.texture, s.param = -1, 0.0
+    s.albedo[:] = [np.float32(a) for a in body.get("albedo", [0.0, 0.0, 0.0])]
+    if kind == "Lambertian":
+        s.kind = RT_LAMBERTIAN
+    elif kind == "Metal":
+        s.kind = RT_METAL; s.param = float(body["fuzz"])
+    elif kind == "Glass":
+        s.kind = RT_GLASS; s.param = float(body["index_of_refraction"])
+    elif kind == "Texture":
+        s.kind = RT_TEXTURE; s.param = float(body["h_offset"]); s.texture = int(body["texture"])
+    elif kind == "Light":
+        s.kind = RT_LIGHT
+    else:
+        raise ValueError(f"unknown material {kind}")
+
+
+def make_sphere(center, radius: float, material) -> rt_sphere:
+    """A sphere record (for ResidentScene.edit_spheres and Scene.edited) from a centre, a radius and a material in the forms
+    Scene.set_sphere takes."""
+    s = rt_sphere()
+    s.center = vec3(center)
+    s.radius = float(radius)
+    _set_material(s, material)
+    return s
 
 
 class Scene:
@@ -377,26 +413,38 @@ class Scene:
             s.center = vec3(center)
         if radius is not None:
             s.radius = float(radius)
-        if isinstance(material, rt_sphere):
-            s.kind, s.param, s.texture = material.kind, material.param, material.texture
-            s.albedo[:] = list(material.albedo)
-        elif material is not None:
-            (kind, body), = material.items()
-            s.texture, s.param = -1, 0.0
-            s.albedo[:] = [np.float32(a) for a in body.get("albedo", [0.0, 0.0, 0.0])]
-            if kind == "Lambertian":
-                s.kind = RT_LAMBERTIAN
-            elif kind == "Metal":
-                s.kind = RT_METAL; s.param = float(body["fuzz"])
-            elif kind == "Glass":
-                s.kind = RT_GLASS; s.param = float(body["index_of_refraction"])
-            elif kind == "Texture":
-                s.kind = RT_TEXTURE; s.param = float(body["h_offset"]); s.texture = int(body["texture"])
-            elif kind == "Light":
-                s.kind = RT_LIGHT
-            else:
-                raise ValueError(f"unknown material {kind}")
+        if material is not None:
+            _set_material(s, material)
         return rt_sphere.from_buffer_copy(s)
+
+    def edited(self, remove: Sequence[int] = (), insert: Sequence[rt_sphere] = (), at: Optional[Sequence[int]] = None) -> "Scene":
+        """A new host scene with the edited sphere list of ResidentScene.edit_spheres: this list without the spheres `remove`,
+        with insert[k] placed just before old sphere at[k] (None: every insert appended). It shares the textures, sky, camera,
+        size, samples, depth and seed of this scene, so a fresh upload of it and the oracle render what an edited handle does."""
+        n = self.n_spheres
+        rem = [int(i) for i in remove]
+        if any(not 0 <= i < n for i in rem) or len(set(rem)) != len(rem):
+            raise ValueError(f"remove holds distinct indices below {n}, got {rem}")
+        at = [n] * len(insert) if at is None else [int(j) for j in at]
+        if len(at) != len(insert):
+            raise ValueError(f"{len(at)} positions for {len(insert)} inserts")
+        if any(not 0 <= j <= n for j in at) or any(a > b for a, b in zip(at, at[1:])):
+            raise ValueError(f"at is non-decreasing with values in [0, {n}], got {at}")
+        gone, before = set(rem), {}
+        for k, j in enumerate(at):
+            before.setdefault(j, []).append(insert[k])
+        spheres = []
+        for j in range(n + 1):
+            spheres += [rt_sphere.from_buffer_copy(s) for s in before.get(j, [])]
+            if j < n and j not in gone:
+                spheres.append(rt_sphere.from_buffer_copy(self._spheres[j]))
+        sc = Scene()
+        C.memmove(C.byref(sc.c), C.byref(self.c), C.sizeof(rt_scene))
+        sc._tex_arrays, sc._tex_structs, sc._sky_array = self._tex_arrays, self._tex_structs, self._sky_array
+        sc.camera_params = dict(self.camera_params) if self.camera_params is not None else None
+        sc._spheres = (rt_sphere * max(len(spheres), 1))(*spheres)
+        sc.c.spheres = C.cast(sc._spheres, C.POINTER(rt_sphere)); sc.c.n_spheres = len(spheres)
+        return sc
 
     @property
     def n_spheres(self):
@@ -622,6 +670,20 @@ class ResidentScene:
         moved, ordered like an update on `stream` (as in :meth:`update_geometry`, by default torch's current stream). Returns
         when the new tree exists; later frames trace it and later updates refit it. A no-op without a hierarchy."""
         _check(lib().rtb200_scene_rebuild(self.h, C.c_void_p(self._stream(stream, self.device) or None)))
+
+    def edit_spheres(self, remove: Sequence[int] = (), insert: Sequence[rt_sphere] = (), at: Optional[Sequence[int]] = None, stream=None):
+        """Remove the spheres `remove` and place insert[k] just before old sphere at[k] (None: append every insert), on the GPU
+        (rtb200_scene_edit_spheres): the list of :meth:`Scene.edited`, lights included. Ordered like :meth:`rebuild` on
+        `stream`; returns when the new list and its hierarchy exist, and later calls see n spheres of the new list."""
+        rem = np.ascontiguousarray(remove, dtype=np.uint32)
+        pos = None if at is None else np.ascontiguousarray(at, dtype=np.uint32)
+        if pos is not None and pos.size != len(insert):
+            raise ValueError(f"{pos.size} positions for {len(insert)} inserts")
+        arr = (rt_sphere * max(len(insert), 1))(*insert)
+        _check(lib().rtb200_scene_edit_spheres(self.h, rem.ctypes.data if rem.size else None, rem.size,
+                                               pos.ctypes.data if pos is not None and pos.size else None, arr, len(insert),
+                                               C.c_void_p(self._stream(stream, self.device) or None)))
+        self.n += len(insert) - rem.size
 
     def adaptive_begin(self, params: rt_adaptive_params, stream=None):
         """(Re)start an adaptive render of the handle (rtb200_adaptive_begin): n = 0 everywhere, every pixel active. `stream`

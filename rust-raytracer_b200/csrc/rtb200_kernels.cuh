@@ -1,4 +1,4 @@
-// rtb200_kernels.cuh — parameter blocks and launch wrappers shared by the kernels and rtb200_api.cu
+// rtb200_kernels.cuh — parameter blocks and launch wrappers shared by the kernels and the host code of the C ABI
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -263,6 +263,15 @@ cudaError_t launch_update_scatter(const uint32_t* idx, const double4* geo_in, co
 cudaError_t launch_refit_spheres(const RefitParams& p, cudaStream_t st);
 // the `count` nodes level_nodes[0, count) of one tree level; their children's exact boxes are final
 cudaError_t launch_refit_nodes(const RefitParams& p, const uint32_t* level_nodes, uint32_t count, cudaStream_t st);
+// Lays out arrays one after another in a block, each at a 256-byte boundary, in the order they are taken. With a null base
+// take returns null and `off` ends as the block's size.
+struct Carver {
+    char* base;
+    size_t off = 0;
+    explicit Carver(void* b = nullptr) : base((char*)b) {}
+    size_t offset(size_t bytes) { const size_t o = off; off += (bytes + 255) & ~(size_t)255; return o; }
+    void* take(size_t bytes) { const size_t o = offset(bytes); return base ? base + o : nullptr; }
+};
 // the rebuild's arrays for n spheres carved out of `base` (null: only the size); returns the bytes they take
 size_t rebuild_carve(void* base, uint32_t n, RebuildBufs* b);
 // the topology of a new hierarchy over geo[0, n): header, child words, leaf members and padding, always-list, skip_pos and the

@@ -276,38 +276,36 @@ size_t cub_bytes(uint32_t n, uint32_t cap) {
 // inner nodes of one level own disjoint ranges of more than kLeafK spheres: at most n / (kLeafK + 1) + 1 per level.
 size_t rebuild_carve(void* base, uint32_t n, RebuildBufs* b) {
     const size_t n1 = std::max<uint32_t>(n, 1), cap = n / (kLeafK + 1) + 1;
-    size_t off = 0;
-    char* p = (char*)base;
-    auto take = [&](size_t bytes) -> void* { void* q = p ? p + off : nullptr; off += (bytes + 255) & ~(size_t)255; return q; };
+    Carver c(base);
     RebuildBufs r{};
     r.cap = (uint32_t)cap;
-    r.header = (RebuildHeader*)take(sizeof(RebuildHeader));
-    r.nodes = (float*)take(n1 * rtbvh::kNodeFloats * 4);
-    r.leaf_rec = (float*)take(n1 * kLeafK * 16);
-    r.leaf_id = (uint32_t*)take(n1 * kLeafK * 4);
-    r.skip_pos = (uint32_t*)take(n1 * 4);
-    r.always = (uint32_t*)take(n1 * 4);
-    r.node_box = (double*)take(n1 * 48);
-    r.leaf_box = (double*)take(n1 * 48);
-    r.level_nodes = (uint32_t*)take(n1 * 4);
-    r.col = (double*)take(n1 * 32);            // the four columns; then the keys and the sorted keys
-    r.sorted = (double*)take(n1 * 32);
+    r.header = (RebuildHeader*)c.take(sizeof(RebuildHeader));
+    r.nodes = (float*)c.take(n1 * rtbvh::kNodeFloats * 4);
+    r.leaf_rec = (float*)c.take(n1 * kLeafK * 16);
+    r.leaf_id = (uint32_t*)c.take(n1 * kLeafK * 4);
+    r.skip_pos = (uint32_t*)c.take(n1 * 4);
+    r.always = (uint32_t*)c.take(n1 * 4);
+    r.node_box = (double*)c.take(n1 * 48);
+    r.leaf_box = (double*)c.take(n1 * 48);
+    r.level_nodes = (uint32_t*)c.take(n1 * 4);
+    r.col = (double*)c.take(n1 * 32);            // the four columns; then the keys and the sorted keys
+    r.sorted = (double*)c.take(n1 * 32);
     r.keys = (unsigned long long*)r.col;
     r.keys_sorted = (unsigned long long*)r.col + n1;
-    r.out_flag = (uint32_t*)take(n1 * 4);
-    r.always_pos = (uint32_t*)take(n1 * 4);
-    r.leaf_start = (uint32_t*)take(n1 * 4);
-    r.leaf_scan = (uint32_t*)take(n1 * 4);
-    r.leaf_cnt = (uint32_t*)take(n1 * 4);
-    r.tasks[0] = (uint2*)take(cap * 8);
-    r.tasks[1] = (uint2*)take(cap * 8);
-    r.kids = (uint2*)take(cap * kWide * 8);
-    r.n_inner = (uint32_t*)take(cap * 4);
-    r.off = (uint32_t*)take(cap * 4);
+    r.out_flag = (uint32_t*)c.take(n1 * 4);
+    r.always_pos = (uint32_t*)c.take(n1 * 4);
+    r.leaf_start = (uint32_t*)c.take(n1 * 4);
+    r.leaf_scan = (uint32_t*)c.take(n1 * 4);
+    r.leaf_cnt = (uint32_t*)c.take(n1 * 4);
+    r.tasks[0] = (uint2*)c.take(cap * 8);
+    r.tasks[1] = (uint2*)c.take(cap * 8);
+    r.kids = (uint2*)c.take(cap * kWide * 8);
+    r.n_inner = (uint32_t*)c.take(cap * 4);
+    r.off = (uint32_t*)c.take(cap * 4);
     r.temp_bytes = cub_bytes(n, (uint32_t)cap);
-    r.temp = take(r.temp_bytes);
+    r.temp = c.take(r.temp_bytes);
     if (b) *b = r;
-    return off;
+    return c.off;
 }
 
 cudaError_t launch_rebuild_topology(const RebuildBufs& b, const double4* geo, uint32_t n, double oversize, cudaStream_t st) {

@@ -422,6 +422,49 @@ int rtb200_scene_trace_rays_device(rtb200_scene_handle h, const rt_rays* rays, u
 int rtb200_scene_trace_rays(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_trace_params* params,
                             float* out_linear_f32, uint8_t* out_rgb8, rt_stats* stats);
 
+/* ---- auxiliary buffers of a resident scene's camera samples (DESIGN.md §4.14) ---------------------------------------------
+ * Denoiser guides (albedo, normal), coverage, object ids and hit points of the render's own samples. Contract: for every pixel
+ * (x, y) of the handle's rows and every sample s in [sample0, sample0 + samples):
+ *   ray      the render's primary ray of (pixel y * width + x, sample s) under the view's camera and seed: the two jitter
+ *            draws of raytracer.rs:199-200 from that Philox stream, then Camera::get_ray (camera.rs:79-84);
+ *   H        hit_world(world, ray, 0.001, f64::MAX) over the handle's CURRENT spheres (those after the last update, rebuild or
+ *            edit enqueued before the call);
+ *   albedo_s the attenuation Material::scatter returns at H, without drawing a random number: a Lambertian's or Metal's albedo
+ *            as stored (non-finite values included, also where a Metal's scatter would absorb), a Texture's
+ *            texture_get_albedo at H's (u, v) with its h_offset (materials.rs:236-253), (1, 1, 1) for Glass and Light; on a
+ *            miss the sky of the ray (raytracer.rs:134-163; black for RT_SKY_NONE);
+ *   normal_s HitRecord.normal (flipped against the ray, sphere.rs:59-76) with each component rounded to f32; 0 on a miss.
+ * Outputs per pixel, compact rows * width and top row first like every output (a shard handle writes its own rows), with the
+ * render's resolve arithmetic (f32 sums in sample order, every operation rounded, never contracted):
+ *   albedo   3 x f32: (1.0f / samples) * S_c, S_c the f32 sum of albedo_s in sample order;
+ *   normal   3 x f32: the same mean of normal_s, not renormalised (mixed surfaces or misses give a shorter vector);
+ *   hits     u32: the samples whose H is Some (coverage = hits / samples);
+ *   sphere   u32: the hit sphere of sample sample0 (first in list order on equal t), 0xffffffff on a miss;
+ *   point    3 x f64: ray.at(t) of sample sample0, 0 on a miss (its distance from the camera origin is the depth).
+ * sphere and point equal rtb200_scene_intersect of sample sample0's primary ray bit for bit. Every output is bit for bit the
+ * same in every variant, on shard and shared-memory-staged handles, and after updates, rebuilds and edits equals a fresh
+ * upload of the same spheres. max_depth plays no part (a handle uploaded with max_depth 0 has AOVs too).
+ * view: NULL for the handle's own camera and seed; else view->camera and view->seed, so that the buffers of an animation frame
+ * match that frame of rtb200_render_frames[_device]; view->max_depth is ignored. */
+typedef struct { uint32_t samples, sample0; uint32_t reserved[2]; } rt_aov_params;   /* 16 bytes; samples >= 1, reserved must be 0 */
+typedef struct {              /* every pointer may be NULL: that output is not written */
+    float* albedo /* rows x width x 3 */; float* normal /* rows x width x 3 */; uint32_t* hits; uint32_t* sphere;
+    double* point /* rows x width x 3 */;
+} rt_aov_out;                 /* 40 bytes */
+/* Device buffers (of h's device, or managed memory), stream-ordered like rtb200_scene_intersect_device: runs on `stream` (NULL:
+ * the library's stream) after the upload and the last update, rebuild or edit of h enqueued before it, without waiting for the
+ * GPU; every later update, rebuild and edit and rtb200_scene_release wait for it. It takes no work set and no sample buffer (the
+ * sums live in registers). A traversal-guard trip is reported with the handle's next collected frames.
+ * RT_ERR_INVALID, before any device work, for a NULL handle, params or out, an out with every output NULL, samples == 0,
+ * sample0 + samples above 2^32, a nonzero params->reserved or view->reserved, or a pointer that is not device memory of h's
+ * device or managed memory. A shard with no rows is a no-op. */
+int rtb200_scene_aov_device(rtb200_scene_handle h, const rt_aov_params* p, const rt_frame* view, const rt_aov_out* out, void* stream);
+/* Host buffers, blocking: the same through the same kernel on the library's stream, copied back. stats (may be NULL): rays =
+ * samples = pixels * samples, candidates, clusters, nodes, device_ms, trace_ms, wall_ms, d2h_bytes (the outputs asked for plus a
+ * 256-byte counter block), kernel_launches = batches = frames = gpus_used = 1. Same checks, bar the memory kind; a
+ * traversal-guard trip fails the call with RT_ERR_CUDA. */
+int rtb200_scene_aov(rtb200_scene_handle h, const rt_aov_params* p, const rt_frame* view, const rt_aov_out* out, rt_stats* stats);
+
 /* load_texture_image — materials.rs:213-219, config.rs:36-47: decode a baseline JPEG file to RGB8 (host-side scene staging
  * helper for hosts without their own decoder; the reference uses the jpeg-decoder crate). *out_rgb8 is released with rtb200_free(). */
 int  rtb200_decode_jpeg_file(const char* path, uint8_t** out_rgb8, uint64_t* width, uint64_t* height);

@@ -1,6 +1,7 @@
 // rtb200_api_query.cu — closest-hit and occlusion queries of caller-supplied rays on a resident scene through the C ABI
-// (DESIGN.md §4.10, §4.11), in both forms: device buffers on the caller's stream, or host buffers staged through the
-// context's query block (HostStage, which the host form of rtb200_scene_trace_rays uses too).
+// (DESIGN.md §4.10, §4.11), and the auxiliary buffers of its camera samples (§4.14), in both forms: device buffers on the
+// caller's stream, or host buffers staged through the context's query block (HostStage, which the host form of
+// rtb200_scene_trace_rays uses too).
 
 #include "rtb200_host.cuh"
 
@@ -94,20 +95,9 @@ static int query_enqueue(rtb200_scene_handle h, const rt_rays& rays, uint32_t n,
     return RT_OK;
 }
 
-// The device form of both kinds.
-static int query_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const QueryOut* out, void* stream_in) {
-    int rc = check_query(h, rays, out);
-    if (rc != RT_OK) return rc;
-    if (n == 0) return RT_OK;
-    HANDLE_PROLOGUE(h);
-    std::vector<std::pair<const void*, const char*>> ptrs = {{rays->origin, "rays->origin"}, {rays->direction, "rays->direction"},
-                                                             {rays->t_max, "rays->t_max"}};
-    for (int k = 0; k < out->count; ++k) ptrs.push_back({out->ptr[k], out->name[k]});
-    if ((rc = check_device_ptrs(h, ptrs)) != RT_OK) return rc;
-    cudaStream_t st;
-    CU(scene_stream(h, stream_in, &st));
-    if ((rc = query_enqueue(h, *rays, n, *out, nullptr, h->err, st)) != RT_OK) return rc;
-    // the next update or rebuild waits for the last query of each stream
+// After a stream-ordered reader of h's scene (a query, an AOV pass) enqueued on `st`: the next update, rebuild or edit and the
+// release wait for the last one of each stream.
+static int mark_query(rtb200_scene_handle h, cudaStream_t st) {
     uint32_t k = 0;
     while (k < h->n_queries && h->queries[k].stream != st) ++k;
     if (k == h->n_queries) {
@@ -121,6 +111,22 @@ static int query_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, 
     }
     CU(cudaEventRecord(h->queries[k].done, st));
     return RT_OK;
+}
+
+// The device form of both kinds.
+static int query_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const QueryOut* out, void* stream_in) {
+    int rc = check_query(h, rays, out);
+    if (rc != RT_OK) return rc;
+    if (n == 0) return RT_OK;
+    HANDLE_PROLOGUE(h);
+    std::vector<std::pair<const void*, const char*>> ptrs = {{rays->origin, "rays->origin"}, {rays->direction, "rays->direction"},
+                                                             {rays->t_max, "rays->t_max"}};
+    for (int k = 0; k < out->count; ++k) ptrs.push_back({out->ptr[k], out->name[k]});
+    if ((rc = check_device_ptrs(h, ptrs)) != RT_OK) return rc;
+    cudaStream_t st;
+    CU(scene_stream(h, stream_in, &st));
+    if ((rc = query_enqueue(h, *rays, n, *out, nullptr, h->err, st)) != RT_OK) return rc;
+    return mark_query(h, st);
 }
 
 // The host form of both kinds.
@@ -197,3 +203,109 @@ int rtb200_scene_occluded(rtb200_scene_handle h, const rt_rays* rays, uint32_t n
   });
 }
 
+
+// ---- auxiliary buffers of the camera samples (DESIGN.md §4.14) ----
+
+// The outputs of rt_aov_out: output k is ptr[k], bytes[k] per pixel.
+struct AovOut {
+    void* ptr[5];
+    const char* name[5];
+};
+static const uint32_t kAovBytes[5] = {12, 12, 4, 4, 24};
+static AovOut aov_out(const rt_aov_out& o) {
+    return AovOut{{o.albedo, o.normal, o.hits, o.sphere, o.point}, {"out->albedo", "out->normal", "out->hits", "out->sphere", "out->point"}};
+}
+
+// The argument checks of both forms (no device is touched).
+static int check_aov(rtb200_scene_handle h, const rt_aov_params* p, const rt_frame* view, const rt_aov_out* out) {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    if (!p) return fail(RT_ERR_INVALID, "params is null");
+    if (!out) return fail(RT_ERR_INVALID, "out is null");
+    const AovOut o = aov_out(*out);
+    if (std::none_of(o.ptr, o.ptr + 5, [](void* q) { return q != nullptr; })) return fail(RT_ERR_INVALID, "every output of out is null");
+    if (p->samples == 0) return fail(RT_ERR_INVALID, "rt_aov_params.samples must be >= 1");
+    if ((uint64_t)p->sample0 + p->samples > (1ull << 32)) return fail(RT_ERR_INVALID, "rt_aov_params.sample0 + samples exceeds 2^32");
+    if (p->reserved[0] != 0 || p->reserved[1] != 0) return fail(RT_ERR_INVALID, "rt_aov_params.reserved must be 0");
+    if (view && view->reserved != 0) return fail(RT_ERR_INVALID, "view->reserved must be 0");
+    return RT_OK;
+}
+
+// The one path of both forms: enqueue the pass over every local pixel of h into `out` (device buffers) on `st`, which the caller
+// has ordered after the scene's last writer (scene_stream). Guard trips go to err[1], the counters to stat (null: not counted).
+static int aov_enqueue(rtb200_scene_handle h, const rt_aov_params& prm, const rt_frame* view, const AovOut& out,
+                       unsigned long long* stat, unsigned long long* err, cudaStream_t st) {
+    int& occ = h->ctx->query_occ[2][h->mode];
+    if (occ == 0) occ = aov_max_ctas_per_sm(h->mode);
+    if (occ <= 0) { occ = 0; return fail(RT_ERR_UNSUPPORTED, "no launch configuration of the aov kernel fits shared memory"); }
+    AovParams q{};
+    q.p = h->tp; q.p.stat = stat; q.p.err = err;
+    if (view) { q.p.cam = view->camera; q.p.key0 = (uint32_t)view->seed; q.p.key1 = (uint32_t)(view->seed >> 32); }
+    q.albedo = (float*)out.ptr[0]; q.normal = (float*)out.ptr[1]; q.hits = (uint32_t*)out.ptr[2]; q.sphere = (uint32_t*)out.ptr[3];
+    q.point = (double*)out.ptr[4];
+    q.samples = prm.samples; q.sample0 = prm.sample0;
+    q.n = h->tp.npix_local;
+    CU(launch_aov(q, h->mode, h->ctx->sm_count * occ, st));
+    return RT_OK;
+}
+
+int rtb200_scene_aov_device(rtb200_scene_handle h, const rt_aov_params* p, const rt_frame* view, const rt_aov_out* out, void* stream_in) {
+  return guarded([&]() -> int {
+    int rc = check_aov(h, p, view, out);
+    if (rc != RT_OK) return rc;
+    HANDLE_PROLOGUE(h);
+    const AovOut o = aov_out(*out);
+    std::vector<std::pair<const void*, const char*>> ptrs;
+    for (int k = 0; k < 5; ++k) ptrs.push_back({o.ptr[k], o.name[k]});
+    if ((rc = check_device_ptrs(h, ptrs)) != RT_OK) return rc;
+    if (h->tp.npix_local == 0) return RT_OK;
+    cudaStream_t st;
+    CU(scene_stream(h, stream_in, &st));
+    if ((rc = aov_enqueue(h, *p, view, o, nullptr, h->err, st)) != RT_OK) return rc;
+    return mark_query(h, st);
+  });
+}
+
+int rtb200_scene_aov(rtb200_scene_handle h, const rt_aov_params* p, const rt_frame* view, const rt_aov_out* out, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (stats) memset(stats, 0, sizeof *stats);
+    int rc = check_aov(h, p, view, out);
+    if (rc != RT_OK) return rc;
+    const uint64_t N = h->tp.npix_local;
+    if (N == 0) return RT_OK;
+    auto wall0 = std::chrono::steady_clock::now();
+    HANDLE_PROLOGUE(h);
+    DeviceCtx* ctx = h->ctx;
+    for (auto& e : ctx->query_ev) if (!e) CU(cudaEventCreate(&e));
+    // device image: counters (kStatBytes; the guard counters at stat[30..31]), then the outputs
+    const AovOut o = aov_out(*out);
+    HostStage io;
+    for (int k = 0; k < 5; ++k) io.add_out(o.ptr[k], o.ptr[k] ? N * kAovBytes[k] : 0);
+    if ((rc = io.place(ctx, kStatBytes)) != RT_OK) return rc;
+    unsigned long long* stat = (unsigned long long*)ctx->query.p;
+    AovOut dout = o;
+    for (int k = 0; k < 5; ++k) dout.ptr[k] = io.a[k].dev;
+    cudaStream_t st;
+    CU(scene_stream(h, nullptr, &st));
+    cudaEvent_t* ev = ctx->query_ev;
+    CU(cudaEventRecord(ev[0], st));
+    CU(cudaMemsetAsync(stat, 0, kStatBytes, st));
+    CU(cudaEventRecord(ev[1], st));
+    if ((rc = aov_enqueue(h, *p, view, dout, stat, stat + 30, st)) != RT_OK) return rc;
+    CU(cudaEventRecord(ev[2], st));
+    if ((rc = io.copy(st, true)) != RT_OK) return rc;
+    unsigned long long hstat[kStatBytes / 8];
+    CU(cudaMemcpyAsync(hstat, stat, kStatBytes, cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(ev[3], st));
+    CU(cudaStreamSynchronize(st));
+    if (hstat[31] != 0) return fail(RT_ERR_CUDA, "internal error: the traversal guard tripped; the aov results are not valid");
+    if (!stats) return RT_OK;
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, ev[0], ev[3])); stats->device_ms = ms;
+    CU(cudaEventElapsedTime(&ms, ev[1], ev[2])); stats->trace_ms = ms;
+    stats->rays = hstat[0]; stats->samples = hstat[3]; stats->candidates = hstat[1]; stats->clusters = hstat[4]; stats->nodes = hstat[6];
+    stats->kernel_launches = 1; stats->batches = 1; stats->frames = 1; stats->gpus_used = 1;
+    stats->d2h_bytes = kStatBytes + io.d2h;
+    stats->wall_ms = ms_since(wall0);
+    return RT_OK;
+  });
+}

@@ -234,6 +234,18 @@ struct OcclusionParams {
     uint32_t n;
 };
 
+// Auxiliary buffers of the camera samples [sample0, sample0 + samples) of every pixel of the handle's rows (rtb200_aov.cu,
+// DESIGN.md §4.14). `p` is the handle's TraceParams with the view's camera and key in cam / key0 / key1: closest_hit reads its
+// scene fields, err (guard trips) and stat (the counters; null: not counted). Outputs are compact, per local pixel; each may be null.
+struct AovParams {
+    TraceParams p;
+    float* albedo; float* normal;     // [n][3] the means of the samples' albedo and f32 normal
+    uint32_t* hits;                   // [n] samples with a hit
+    uint32_t* sphere; double* point;  // [n], [n][3] the hit of sample sample0
+    uint32_t samples, sample0;
+    uint32_t n;                       // local pixels = npix_local
+};
+
 struct KernelInfo { int registers, max_threads, const_bytes, local_bytes; char name[96]; };
 
 // `queue` (TraceQueue): Q_FRAMES is the multi-frame kernel (work ids span p.ftab's frames), Q_LIST the adaptive round's,
@@ -248,6 +260,10 @@ cudaError_t launch_resolve(const ResolveParams& p, cudaStream_t st);
 int query_max_ctas_per_sm(uint32_t mode, bool any);
 cudaError_t launch_query(const QueryParams& q, uint32_t mode, int max_grid, cudaStream_t st);
 cudaError_t launch_occluded(const OcclusionParams& q, uint32_t mode, int max_grid, cudaStream_t st);
+// the auxiliary buffers: resident CTAs per SM of the kernel of `mode` (0 when it cannot run on the current device), and a launch
+// of at most `max_grid` CTAs
+int aov_max_ctas_per_sm(uint32_t mode);
+cudaError_t launch_aov(const AovParams& q, uint32_t mode, int max_grid, cudaStream_t st);
 // adaptive rendering (rtb200_adaptive.cu): the round's accumulate-and-test, the list compaction (cub::DeviceSelect::Flagged,
 // keep[0, npix_local) over list_in, the count to *list_n_out), and the resolve
 cudaError_t launch_adaptive_list(uint32_t* list, uint32_t* list_n, uint32_t npix_local, cudaStream_t st);   // list = 0, 1, .., npix_local - 1

@@ -13,23 +13,12 @@
 // and slots: it calls the any-hit kind of the same stage, closest_hit<MODE, true>, under each ray's own bound
 // T = min(t_max, f64::MAX), which prunes boxes beyond T and stops at the first sphere that accepts a root below T. A ray with
 // !(T > 0.001) cannot be occluded (an accepted root is > 0.001 and < T) and does not enter the stage.
-#include <algorithm>
-
-#include "rtb200_trace.cuh"
+#include "rtb200_query.cuh"
 
 namespace rtk {
 
 namespace {
 
-constexpr int kQueryBlock = 128;
-constexpr uint32_t kQueryWarps = kQueryBlock / 32;
-constexpr uint32_t kQuerySlotBytes = 7 * 8 + 2 * 4;   // Pool.ox .. Pool.bt, Pool.bi, Pool.src
-
-// shared memory of one warp: its traversal context (MODE_TREE), then its 32 pool slots
-__host__ __device__ constexpr uint32_t query_warp_bytes(uint32_t mode) {
-    return (mode == MODE_TREE ? kWarpCtxBytes : 0u) + 32u * kQuerySlotBytes;
-}
-constexpr size_t query_smem_bytes(uint32_t mode) { return (size_t)kQueryWarps * query_warp_bytes(mode); }
 // occlusion queries: the traversal context is followed by the 32 rays' f32 bounds T~ (MODE_TREE), then the slots
 constexpr uint32_t kTcapBytes = 32u * 4u;
 __host__ __device__ constexpr uint32_t occluded_warp_bytes(uint32_t mode) {
@@ -44,14 +33,8 @@ __global__ void __launch_bounds__(kQueryBlock) rt_query_kernel(const __grid_cons
     const uint32_t warp = threadIdx.x >> 5;
     unsigned char* base = smem_raw + warp * query_warp_bytes(MODE);
     const WarpCtx W = warpctx_at(base);   // read by MODE_TREE only
-    double* dbl = reinterpret_cast<double*>(base + (MODE == MODE_TREE ? kWarpCtxBytes : 0u));
-    uint32_t* u32 = reinterpret_cast<uint32_t*>(dbl + 7 * 32);
-    Pool P{};   // closest_hit touches the ray, the best root and index, and the source sphere of a slot
-    P.ox = dbl; P.oy = dbl + 32; P.oz = dbl + 64; P.dx = dbl + 96; P.dy = dbl + 128; P.dz = dbl + 160; P.bt = dbl + 192;
-    P.bi = u32; P.src = u32 + 32;
-    P.n_slots = 32u;
-    SceneRefs sc;
-    sc.nodes = q.p.nodes; sc.leaf_rec = q.p.leaf_rec; sc.leaf_id = q.p.leaf_id; sc.filt = q.p.filt; sc.geo = q.p.geo; sc.mat = q.p.mat;
+    const Pool P = query_pool_at(base + (MODE == MODE_TREE ? kWarpCtxBytes : 0u));
+    const SceneRefs sc = scene_refs(q.p);
     Stats st;
     const uint64_t chunks = ((uint64_t)q.n + 31u) / 32u;
     for (uint64_t c = (uint64_t)blockIdx.x * kQueryWarps + warp; c < chunks; c += (uint64_t)gridDim.x * kQueryWarps) {
@@ -101,14 +84,8 @@ __global__ void __launch_bounds__(kQueryBlock) rt_occluded_kernel(const __grid_c
     unsigned char* base = smem_raw + warp * occluded_warp_bytes(MODE);
     const WarpCtx W = warpctx_at(base);   // read by MODE_TREE only
     float* tcap = reinterpret_cast<float*>(base + kWarpCtxBytes);   // MODE_TREE only
-    double* dbl = reinterpret_cast<double*>(base + (MODE == MODE_TREE ? kWarpCtxBytes + kTcapBytes : 0u));
-    uint32_t* u32 = reinterpret_cast<uint32_t*>(dbl + 7 * 32);
-    Pool P{};   // the slots of rt_query_kernel
-    P.ox = dbl; P.oy = dbl + 32; P.oz = dbl + 64; P.dx = dbl + 96; P.dy = dbl + 128; P.dz = dbl + 160; P.bt = dbl + 192;
-    P.bi = u32; P.src = u32 + 32;
-    P.n_slots = 32u;
-    SceneRefs sc;
-    sc.nodes = q.p.nodes; sc.leaf_rec = q.p.leaf_rec; sc.leaf_id = q.p.leaf_id; sc.filt = q.p.filt; sc.geo = q.p.geo; sc.mat = q.p.mat;
+    const Pool P = query_pool_at(base + (MODE == MODE_TREE ? kWarpCtxBytes + kTcapBytes : 0u));
+    const SceneRefs sc = scene_refs(q.p);
     Stats st;
     const uint64_t chunks = ((uint64_t)q.n + 31u) / 32u;
     for (uint64_t c = (uint64_t)blockIdx.x * kQueryWarps + warp; c < chunks; c += (uint64_t)gridDim.x * kQueryWarps) {
@@ -153,37 +130,18 @@ static auto dispatch_kind(bool any, uint32_t mode, F&& f) {
     return dispatch_query(mode, [&](auto kern) { return f(kern, query_smem_bytes(mode)); });
 }
 
-template <typename K>
-static int max_ctas_per_sm(K kern, size_t smem) {
-    int nb = 0;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { cudaGetLastError(); return 0; }
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, kern, kQueryBlock, smem) != cudaSuccess) { cudaGetLastError(); return 0; }
-    return nb;
-}
-
-template <typename K, typename Q>
-static cudaError_t launch(K kern, size_t smem, const Q& q, int max_grid, cudaStream_t st) {
-    if (q.n == 0) return cudaSuccess;
-    const uint64_t ctas = ((uint64_t)q.n + 32u * kQueryWarps - 1u) / (32u * kQueryWarps);
-    const int grid = (int)std::min<uint64_t>(ctas, (uint64_t)std::max(max_grid, 1));
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    kern<<<grid, kQueryBlock, smem, st>>>(q);
-    return cudaGetLastError();
-}
-
 }  // namespace
 
 int query_max_ctas_per_sm(uint32_t mode, bool any) {
-    return dispatch_kind(any, mode, [&](auto kern, size_t smem) -> int { return max_ctas_per_sm(kern, smem); });
+    return dispatch_kind(any, mode, [&](auto kern, size_t smem) -> int { return query_ctas_per_sm(kern, smem); });
 }
 
 cudaError_t launch_query(const QueryParams& q, uint32_t mode, int max_grid, cudaStream_t st) {
-    return dispatch_query(mode, [&](auto kern) { return launch(kern, query_smem_bytes(mode), q, max_grid, st); });
+    return dispatch_query(mode, [&](auto kern) { return query_launch(kern, query_smem_bytes(mode), q, max_grid, st); });
 }
 
 cudaError_t launch_occluded(const OcclusionParams& q, uint32_t mode, int max_grid, cudaStream_t st) {
-    return dispatch_occluded(mode, [&](auto kern) { return launch(kern, occluded_smem_bytes(mode), q, max_grid, st); });
+    return dispatch_occluded(mode, [&](auto kern) { return query_launch(kern, occluded_smem_bytes(mode), q, max_grid, st); });
 }
 
 }  // namespace rtk

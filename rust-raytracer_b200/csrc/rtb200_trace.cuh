@@ -8,8 +8,8 @@
 //   shade_slot<LIGHTS>  ray_color's body for one path vertex (raytracer.rs:71-165): Material::scatter of all five
 //                       materials, the sky, the stochastic light test with its shadow-frame stack, and - when the path
 //                       ends - the backwards unwinding of the albedo stack that reproduces the recursion's f32 products;
-//   regenerate_slot     render_line's per-sample set-up (raytracer.rs:199-201) + Camera::get_ray (camera.rs:79-84), or a
-//                       caller-supplied primary ray (Q_RAYS).
+//   regenerate_slot     render_line's per-sample set-up (raytracer.rs:199-201) + Camera::get_ray (camera.rs:79-84) through
+//                       primary_ray, or a caller-supplied primary ray (Q_RAYS).
 //
 // Ray state lives in shared memory, SoA over the slots of a CTA's pool (struct Pool).
 #pragma once
@@ -501,6 +501,26 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
 }
 
 // =====================================================================================================================
+// The render's primary ray of local pixel (x, y_local) of the launch's rows and sample s0 + s_local, under camera `cam` and the
+// Philox key (k0, k1): the pixel's image row (row band y_local / band_rows is the shard's, raytracer.rs:254-262), the two
+// jitter draws of raytracer.rs:199-200 from the stream of (pixel, sample), then Camera::get_ray (camera.rs:79-84). `rng` is
+// left after the two draws. The trace kernel (regenerate_slot) and the auxiliary buffers (rtb200_aov.cu) both make their
+// camera rays here.
+// =====================================================================================================================
+RT_DEV void primary_ray(const TraceParams& p, const rt_camera& cam, uint32_t k0, uint32_t k1, uint32_t x, uint32_t y_local,
+                        uint32_t s0, uint32_t s_local, Rng& rng, D3& o, D3& d) {
+    const uint32_t band_rows = p.band_rows, width = p.width, height = p.height;
+    uint32_t band = y_local / band_rows;
+    uint32_t y = (band * (uint32_t)p.world + (uint32_t)p.rank) * band_rows + (y_local - band * band_rows);
+    rng_init(rng, y * width + x, s0 + s_local);
+    double xi1 = rng_f64(rng, k0, k1);
+    double u = __ddiv_rn(__dadd_rn((double)x, xi1), __dsub_rn((double)width, 1.0));
+    double xi2 = rng_f64(rng, k0, k1);
+    double v = __ddiv_rn(__dsub_rn((double)height, __dadd_rn((double)y, xi2)), __dsub_rn((double)height, 1.0));
+    get_ray(cam, u, v, o, d);
+}
+
+// =====================================================================================================================
 // Regenerate pool slot `s` from the global (pixel,sample) queue. Warp-synchronous: every lane of the warp calls it,
 // `want` says whether this lane's slot needs a new path; `exhausted` is the warp's (uniform) knowledge that the queue is
 // dry. Returns true when the slot received a new primary ray. raytracer.rs:199-201 + camera.rs:79-84.
@@ -565,15 +585,8 @@ RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint
             y_local = p.rows_local - 1u - rr;
             lp = y_local * p.width + x;
         }
-        uint32_t band = y_local / p.band_rows;
-        uint32_t y = (band * (uint32_t)p.world + (uint32_t)p.rank) * p.band_rows + (y_local - band * p.band_rows);
-        rng_init(rng, y * p.width + x, p.s0 + s_local);
-        double xi1 = rng_f64(rng, k0, k1);
-        double u = __ddiv_rn(__dadd_rn((double)x, xi1), __dsub_rn((double)p.width, 1.0));
-        double xi2 = rng_f64(rng, k0, k1);
-        double v = __ddiv_rn(__dsub_rn((double)p.height, __dadd_rn((double)y, xi2)), __dsub_rn((double)p.height, 1.0));
-        if constexpr (FRAMES) get_ray(p.ftab[f].cam, u, v, o, d);
-        else get_ray(p.cam, u, v, o, d);
+        if constexpr (FRAMES) primary_ray(p, p.ftab[f].cam, k0, k1, x, y_local, p.s0, s_local, rng, o, d);
+        else primary_ray(p, p.cam, k0, k1, x, y_local, p.s0, s_local, rng, o, d);
     }
     P.ox[s] = o.x; P.oy[s] = o.y; P.oz[s] = o.z; P.dx[s] = d.x; P.dy[s] = d.y; P.dz[s] = d.z;
     // samplebuf index [sample][pixel], [frame][sample][pixel], [sample][list position] (Q_LIST) or [sample][ray] (Q_RAYS)

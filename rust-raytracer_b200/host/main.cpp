@@ -11,7 +11,12 @@
 // 0, 8, 16) with max_samples = the scene's samples_per_pixel: a pixel stops once its standard error is within
 // abs_tol + rel_tol * mean in every channel (DESIGN.md §4.9). Same two stdout lines; RTB200_STATS also prints the samples
 // traced out of samples_per_pixel * width * height.
+// RTB200_AOV=<samples>[,<sample0>] also writes the auxiliary buffers of those camera samples of the frame (rtb200_scene_aov,
+// DESIGN.md §4.14) next to <output_file>: <stem>_albedo.png, the mean first-hit albedo in the beauty image's encoding, and
+// <stem>_normal.png, the mean normal n as 0.5 * n + 0.5 (no square root), where <stem> is <output_file> without its extension.
 #include <chrono>
+#include <cmath>
+#include <cstring>
 #include <cstdio>
 #include <cstdlib>
 #include <fstream>
@@ -79,6 +84,49 @@ static int render_adaptive(const rt_scene& s, const char* spec, const rt_options
     return 0;
 }
 
+// palette's f32 -> u8 (raytracer.rs:207-213 after its square root): min(x * 255, 255) plus 2^23, whose low mantissa bits
+// are the value rounded half to even; 0 below 0 and 255 for NaN, like the kernel's quantise_u8
+static uint8_t to_u8(float x) {
+    const float scaled = std::fmin(x * 255.0f, 255.0f);
+    const float f = scaled + 8388608.0f;
+    uint32_t bits;
+    memcpy(&bits, &f, 4);
+    return bits >= 0x4B000000u ? (uint8_t)(bits - 0x4B000000u) : (uint8_t)0;
+}
+
+// RTB200_AOV: the albedo and normal buffers of samples [sample0, sample0 + samples) of every pixel of `s`, written beside `out`
+static int write_aov(const rt_scene& s, const char* spec, const rt_options& opts, const std::string& out) {
+    char* end = nullptr;
+    const unsigned long long samples = strtoull(spec, &end, 10);
+    unsigned long long sample0 = 0;
+    bool ok = end != spec && (*end == 0 || *end == ',');
+    if (ok && *end == ',') { const char* c = end + 1; sample0 = strtoull(c, &end, 10); ok = end != c && *end == 0; }
+    if (!ok || samples < 1 || samples > 4294967295ull || sample0 > 4294967295ull) {
+        fprintf(stderr, "RTB200_AOV: expected <samples>[,<sample0>] with samples >= 1, got \"%s\"\n", spec);
+        return 101;
+    }
+    const size_t npix = (size_t)s.width * s.height;
+    std::vector<float> albedo(npix * 3), normal(npix * 3);
+    rt_aov_params p{(uint32_t)samples, (uint32_t)sample0, {0u, 0u}};
+    rt_aov_out o{albedo.data(), normal.data(), nullptr, nullptr, nullptr};
+    rtb200_scene_handle h = nullptr;
+    int rc = rtb200_scene_upload(&s, &opts, &h);
+    if (rc == 0) rc = rtb200_scene_aov(h, &p, nullptr, &o, nullptr);
+    if (h) rtb200_scene_release(h);
+    if (rc != 0) { fprintf(stderr, "aov failed (%d): %s\n", rc, rtb200_last_error()); return 101; }
+    std::vector<uint8_t> a8(npix * 3), n8(npix * 3);
+    for (size_t i = 0; i < npix * 3; ++i) {
+        a8[i] = to_u8(std::sqrt(albedo[i]));
+        n8[i] = to_u8(0.5f * normal[i] + 0.5f);
+    }
+    const size_t slash = out.find_last_of('/'), dot = out.find_last_of('.');
+    const std::string stem = dot != std::string::npos && (slash == std::string::npos || dot > slash) ? out.substr(0, dot) : out;
+    std::string err;
+    for (const auto& img : {std::make_pair(stem + "_albedo.png", &a8), std::make_pair(stem + "_normal.png", &n8)})
+        if (!rthost::write_png_rgb8(img.first.c_str(), img.second->data(), s.width, s.height, &err)) { fprintf(stderr, "error writing image: %s\n", err.c_str()); return 101; }
+    return 0;
+}
+
 int main(int argc, char** argv) {
     if (argc != 3) {                                                       // main.rs:9-12
         printf("Usage: %s <config_file> <output_file>\n", argc > 0 ? argv[0] : "raytracer");
@@ -97,6 +145,11 @@ int main(int argc, char** argv) {
     const char* adaptive = getenv("RTB200_ADAPTIVE");
     if (adaptive && (getenv("RTB200_GPUS") || getenv("RTB200_FRAMES"))) {
         fprintf(stderr, "RTB200_ADAPTIVE with RTB200_GPUS or RTB200_FRAMES is not supported: adaptive renders are one frame on one GPU\n");
+        return 101;
+    }
+    const char* aov = getenv("RTB200_AOV");
+    if (aov && (getenv("RTB200_GPUS") || getenv("RTB200_FRAMES") || adaptive)) {
+        fprintf(stderr, "RTB200_AOV with RTB200_GPUS, RTB200_FRAMES or RTB200_ADAPTIVE is not supported: the buffers are of one frame's camera samples on one GPU\n");
         return 101;
     }
     if (const char* fp = getenv("RTB200_FRAMES")) return render_animation(holder.scene, fp, argv[2]);
@@ -129,5 +182,6 @@ int main(int argc, char** argv) {
     }
     std::string err;
     if (!rthost::write_png_rgb8(argv[2], pixels.data(), s.width, s.height, &err)) { fprintf(stderr, "error writing image: %s\n", err.c_str()); return 101; }   // raytracer.rs:265
+    if (aov) return write_aov(s, aov, opts, argv[2]);
     return 0;
 }

@@ -127,11 +127,26 @@ class rt_trace_params(C.Structure):
                 ("max_depth", C.c_uint32), ("reserved", C.c_uint32 * 2)]
 
 
+class rt_aov_params(C.Structure):
+    """Auxiliary buffers of a resident scene's camera samples (rtb200_scene_aov[_device]): the samples per pixel and the index
+    of the first."""
+    _fields_ = [("samples", C.c_uint32), ("sample0", C.c_uint32), ("reserved", C.c_uint32 * 2)]
+
+
+class rt_aov_out(C.Structure):
+    """Outputs of rtb200_scene_aov[_device], each NULL or rows * width (hits, sphere) or rows * width * 3 (albedo, normal, point)
+    elements."""
+    _fields_ = [("albedo", C.c_void_p), ("normal", C.c_void_p), ("hits", C.c_void_p), ("sphere", C.c_void_p), ("point", C.c_void_p)]
+
+
 HIT_FIELDS = (("t", 1, np.float64), ("sphere", 1, np.int32), ("point", 3, np.float64), ("normal", 3, np.float64),
               ("uv", 2, np.float64), ("front_face", 1, np.uint8))   # rt_hits: name, values per ray, dtype (sphere -1 = 0xffffffff)
 
 assert C.sizeof(rt_sphere) == 64 and C.sizeof(rt_frame) == 112 and C.sizeof(rt_adaptive_params) == 24
 assert C.sizeof(rt_rays) == 24 and C.sizeof(rt_hits) == 48 and C.sizeof(rt_trace_params) == 32
+assert C.sizeof(rt_aov_params) == 16 and C.sizeof(rt_aov_out) == 40
+AOV_FIELDS = (("albedo", 3, np.float32), ("normal", 3, np.float32), ("hits", 1, np.uint32), ("sphere", 1, np.int32),
+              ("point", 3, np.float64))   # rt_aov_out: name, values per pixel, dtype (sphere -1 = 0xffffffff)
 
 # every symbol include/rtb200.h declares (tests check that the library exports all of them)
 ABI_SYMBOLS = [
@@ -149,6 +164,7 @@ ABI_SYMBOLS = [
     "rtb200_scene_occluded_device", "rtb200_scene_occluded",
     "rtb200_scene_trace_rays_device", "rtb200_scene_trace_rays",
     "rtb200_scene_edit_spheres",
+    "rtb200_scene_aov_device", "rtb200_scene_aov",
 ]
 
 _lib = None
@@ -216,6 +232,8 @@ def lib() -> C.CDLL:
     L.rtb200_scene_trace_rays.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.POINTER(rt_trace_params), C.c_void_p,
                                           C.c_void_p, C.POINTER(rt_stats)]
     L.rtb200_scene_edit_spheres.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
+    L.rtb200_scene_aov_device.argtypes = [C.c_void_p, C.POINTER(rt_aov_params), C.POINTER(rt_frame), C.POINTER(rt_aov_out), C.c_void_p]
+    L.rtb200_scene_aov.argtypes = [C.c_void_p, C.POINTER(rt_aov_params), C.POINTER(rt_frame), C.POINTER(rt_aov_out), C.POINTER(rt_stats)]
     _lib = L
     return L
 
@@ -798,6 +816,44 @@ class ResidentScene:
             _check(lib().rtb200_scene_trace_rays_device(self.h, C.byref(rays), n, C.byref(p), lin_p, rgb_p,
                                                         C.c_void_p(self._stream(stream, origin.device) or None), C.byref(st)))
         out["stats"] = st.as_dict()
+        return out
+
+    def aov(self, samples: int = 1, *, sample0: int = 0, view: Optional[rt_frame] = None, outputs=None, on_device: bool = False,
+            stream=None) -> dict:
+        """Auxiliary buffers of the render's camera samples [sample0, sample0 + samples) of every pixel of the handle's rows, as
+        include/rtb200.h states them: for each sample the render's primary ray and its first hit on the current spheres, then
+        per pixel the mean albedo at the hit (the sky on a miss) and the mean normal (0 on a miss; not renormalised), the
+        samples that hit, and the sphere and hit point of sample sample0. `view` (an rt_frame) replaces the handle's camera
+        and seed, like a frame of :meth:`render_frames`.
+
+        With on_device=False the blocking host form (rtb200_scene_aov) returns numpy arrays and "stats"; with on_device=True
+        the device form (rtb200_scene_aov_device) returns CUDA tensors on `stream` (as in :meth:`update_geometry`, by default
+        torch's current stream) without waiting. Returns one entry per name of `outputs` (default: all): "albedo" and
+        "normal" float32 [rows, w, 3], "hits" uint32 [rows, w], "sphere" int32 [rows, w] (-1: miss, the bits of 0xffffffff),
+        "point" float64 [rows, w, 3]."""
+        names = [f[0] for f in AOV_FIELDS] if outputs is None else list(outputs)
+        if not names or any(k not in [f[0] for f in AOV_FIELDS] for k in names):
+            raise ValueError(f"aov outputs are a non-empty subset of {[f[0] for f in AOV_FIELDS]}, got {names}")
+        shape = (self.rows, int(self.scene.c.width))
+        p = rt_aov_params(int(samples), int(sample0))
+        vp = C.byref(view) if view is not None else None
+        if not on_device:
+            out = {k: np.empty(shape + ((c,) if c > 1 else ()), dtype=ty) for k, c, ty in AOV_FIELDS if k in names}
+            o = rt_aov_out(*(out[k].ctypes.data if k in out else None for k, _, _ in AOV_FIELDS))
+            st = rt_stats()
+            _check(lib().rtb200_scene_aov(self.h, C.byref(p), vp, C.byref(o), C.byref(st)))
+            out["stats"] = st.as_dict()
+            return out
+        import torch
+        device = torch.device("cuda", self.device if self.device is not None else torch.cuda.current_device())
+        dt = {np.float64: torch.float64, np.float32: torch.float32, np.int32: torch.int32, np.uint32: torch.uint32}
+        # the outputs belong to the call's stream when it is a torch stream (the caching allocator orders their reuse after it)
+        with torch.cuda.stream(stream) if isinstance(stream, torch.cuda.Stream) else torch.cuda.device(device):
+            out = {k: torch.empty(shape + ((c,) if c > 1 else ()), dtype=dt[ty], device=device) for k, c, ty in AOV_FIELDS if k in names}
+        if self.rows == 0:   # a shard with no rows (the library's no-op)
+            return out
+        o = rt_aov_out(*(out[k].data_ptr() if k in out else None for k, _, _ in AOV_FIELDS))
+        _check(lib().rtb200_scene_aov_device(self.h, C.byref(p), vp, C.byref(o), C.c_void_p(self._stream(stream, device) or None)))
         return out
 
     def _query_device_args(self, what, origin, direction, t_max, stream, fields):

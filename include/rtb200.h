@@ -465,6 +465,50 @@ int rtb200_scene_aov_device(rtb200_scene_handle h, const rt_aov_params* p, const
  * traversal-guard trip fails the call with RT_ERR_CUDA. */
 int rtb200_scene_aov(rtb200_scene_handle h, const rt_aov_params* p, const rt_frame* view, const rt_aov_out* out, rt_stats* stats);
 
+/* ---- denoising a frame with its auxiliary buffers (DESIGN.md §4.15) -------------------------------------------------------
+ * The edge-avoiding à-trous wavelet filter (Dammertz et al. 2010) with rational edge-stopping weights, every f32 operation
+ * rounded to nearest and never contracted. Inputs, width x height pixels of 3 x f32, row-major, top row first: color (normally a
+ * render's linear mean) and the optional guides albedo and normal (normally rtb200_scene_aov's). A guide is on when it is given
+ * and its weight is not 0. Iteration i = 0 .. L-1 reads image c (color for i = 0, else the previous output) with step h = 2^i.
+ * Pixel p keeps c_p if any value of p (its colour, and every guide given) is not finite. Otherwise num_k = den = 0 and for
+ * dy = -2..2 (outer), dx = -2..2 (inner), q = p + h * (dx, dy), skipping q outside the image or with a non-finite value:
+ *   k = B[dx] * B[dy] with B = {1/16, 1/4, 3/8, 1/4, 1/16};
+ *   d_g = ((q0 - p0)^2 + (q1 - p1)^2) + (q2 - p2)^2 for each guide on (colour from c, albedo and normal as given);
+ *   w = k / ((1 + lc_i * d_c) * (1 + la * d_a) * (1 + ln * d_n)), lc_i = color_weight * 4^i, factors left to right, an off
+ *       guide's left out (an overflowing factor gives w = 0);
+ *   num_k += w * c_q,k, then den += w.
+ * The output is num_k / den (the centre tap alone gives den >= 9/64). Whole frames only: gather a sharded render first.
+ * Outputs: out_linear (3 x f32) and/or out_rgb8, the render's quantisation of sqrt(linear) (rtb200_probe_quantise). */
+typedef struct {
+    uint32_t width, height;
+    uint32_t iterations;          /* L, in [1, 10] */
+    uint32_t reserved;            /* must be 0 */
+    float    color_weight, albedo_weight, normal_weight;   /* finite, >= 0; 0 turns that guide off */
+    float    reserved2;           /* must be 0 */
+} rt_denoise_params;              /* 32 bytes */
+/* Defaults of the Python binding and the CLI (DESIGN.md §4.15: chosen on the 2-spp cover render at 64 x 48) */
+#define RTB200_DENOISE_DEFAULT_ITERATIONS    3
+#define RTB200_DENOISE_DEFAULT_COLOR_WEIGHT  16.0f
+#define RTB200_DENOISE_DEFAULT_ALBEDO_WEIGHT 4.0f
+#define RTB200_DENOISE_DEFAULT_NORMAL_WEIGHT 1.0f
+/* Bytes of device scratch rtb200_denoise_device needs for width x height pixels (the library owns its layout). */
+uint64_t rtb200_denoise_scratch_bytes(uint32_t width, uint32_t height);
+/* Device buffers of `device` (-1: the current device) or managed memory; scratch holds rtb200_denoise_scratch_bytes and is
+ * 16-byte aligned. Stream-ordered, without waiting for the GPU: runs on `stream` (NULL: the library's stream of that device);
+ * the caller keeps every buffer valid until it has run. It touches no scene handle and no work set, so any number of calls
+ * with separate scratch may overlap on different streams.
+ * RT_ERR_INVALID, before any device work, for a NULL params, color or scratch, both outputs NULL, a nonzero reserved or
+ * reserved2, iterations outside [1, 10], a weight that is NaN, negative or infinite, color_weight * 4^(iterations - 1) not
+ * finite, a nonzero weight for a NULL guide, width * height >= 2^31, an output or the scratch overlapping an input or each
+ * other, or a pointer that is not device memory of `device` nor managed memory. A 0-pixel image is a no-op. */
+int rtb200_denoise_device(int32_t device, const rt_denoise_params* p, const float* color, const float* albedo, const float* normal,
+                          void* scratch, float* out_linear, uint8_t* out_rgb8, void* stream);
+/* Host buffers, blocking: the same through the same kernels on the library's stream, with the inputs copied in and the outputs
+ * copied out. stats (may be NULL): device_ms (copies and kernels), trace_ms (the kernels), wall_ms, h2d_bytes, d2h_bytes and
+ * kernel_launches (iterations + 1). Same checks, bar the scratch and the memory kind. */
+int rtb200_denoise(int32_t device, const rt_denoise_params* p, const float* color, const float* albedo, const float* normal,
+                   float* out_linear, uint8_t* out_rgb8, rt_stats* stats);
+
 /* load_texture_image — materials.rs:213-219, config.rs:36-47: decode a baseline JPEG file to RGB8 (host-side scene staging
  * helper for hosts without their own decoder; the reference uses the jpeg-decoder crate). *out_rgb8 is released with rtb200_free(). */
 int  rtb200_decode_jpeg_file(const char* path, uint8_t** out_rgb8, uint64_t* width, uint64_t* height);

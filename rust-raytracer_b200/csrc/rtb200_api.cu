@@ -70,15 +70,18 @@ cudaError_t rtk::scene_stream(rtb200_scene_handle h, void* stream_in, cudaStream
     return h->updated ? cudaStreamWaitEvent(st, h->updated, 0) : cudaSuccess;
 }
 
-int rtk::check_device_ptrs(rtb200_scene_handle h, const std::vector<std::pair<const void*, const char*>>& ptrs) {
+int rtk::check_device_ptrs(int device, const std::vector<std::pair<const void*, const char*>>& ptrs) {
     for (const auto& q : ptrs) {
         if (!q.first) continue;
         cudaPointerAttributes a{};
         if (cudaPointerGetAttributes(&a, q.first) != cudaSuccess) { cudaGetLastError(); a.type = cudaMemoryTypeUnregistered; }
-        if (!((a.type == cudaMemoryTypeDevice && a.device == h->device) || a.type == cudaMemoryTypeManaged))
-            return fail(RT_ERR_INVALID, std::string(q.second) + " is not device or managed memory of device " + std::to_string(h->device));
+        if (!((a.type == cudaMemoryTypeDevice && a.device == device) || a.type == cudaMemoryTypeManaged))
+            return fail(RT_ERR_INVALID, std::string(q.second) + " is not device or managed memory of device " + std::to_string(device));
     }
     return RT_OK;
+}
+int rtk::check_device_ptrs(rtb200_scene_handle h, const std::vector<std::pair<const void*, const char*>>& ptrs) {
+    return check_device_ptrs(h->device, ptrs);
 }
 
 struct V3 { double x, y, z; };

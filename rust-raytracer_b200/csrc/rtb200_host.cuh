@@ -1,6 +1,6 @@
 // rtb200_host.cuh — what the host translation units of the C ABI share (rtb200_api.cu, rtb200_api_render.cu,
-// rtb200_api_scene.cu, rtb200_api_query.cu): error reporting, the per-device contexts, the scene handle and the helpers more
-// than one of them calls. Not installed.
+// rtb200_api_scene.cu, rtb200_api_query.cu, rtb200_api_denoise.cu): error reporting, the per-device contexts, the scene
+// handle and the helpers more than one of them calls. Not installed.
 #pragma once
 #include <algorithm>
 #include <chrono>
@@ -102,7 +102,7 @@ struct DeviceCtx {
     std::vector<OccKey> occ_cache;        // cudaOccupancyMaxActiveBlocksPerMultiprocessor answers
     PinnedBuf staging;                    // host image of the arena being uploaded
     cudaEvent_t staging_free = nullptr;   // the last H2D copy out of `staging` has finished
-    // the host forms of rtb200_scene_intersect, _occluded, _trace_rays and _aov: rays, outputs and counters on the device
+    // the host forms of rtb200_scene_intersect, _occluded, _trace_rays, _aov and rtb200_denoise: their arrays on the device
     // (HostStage), the query's timing events (created at its first call), and the resident CTAs per SM of the query kernel of
     // each kind and mode (0: not asked yet)
     GrowBuf query;
@@ -238,8 +238,10 @@ int scene_upload_records(const rt_scene* s, const rt_options& opts, uint32_t n_l
 // The stream of a call on h, `stream_in` (NULL: the context's stream), made to wait for what last wrote the scene arrays:
 // the upload, which ran on the context's stream, and the last update or rebuild, on whichever stream it ran.
 cudaError_t scene_stream(rtb200_scene_t* h, void* stream_in, cudaStream_t* out);
-// RT_ERR_INVALID unless every non-null pointer of `ptrs` (pointer, name) is device memory of h's device or managed memory.
-// The caller has made h's device current.
+// RT_ERR_INVALID unless every non-null pointer of `ptrs` (pointer, name) is device memory of `device` or managed memory.
+// The caller has made that device current.
+int check_device_ptrs(int device, const std::vector<std::pair<const void*, const char*>>& ptrs);
+// the same for h's device
 int check_device_ptrs(rtb200_scene_t* h, const std::vector<std::pair<const void*, const char*>>& ptrs);
 
 // ---- rtb200_api_render.cu ----

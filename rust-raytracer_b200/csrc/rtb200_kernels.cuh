@@ -146,6 +146,16 @@ struct AdaptiveResolveParams {
     float* out_linear; uint8_t* out_rgb8; uint32_t* out_count;   // each may be null
 };
 
+// The edge-avoiding à-trous filter (rtb200_denoise.cu, DESIGN.md §4.15) of a width x height image: the caller's buffers and
+// the scratch of denoise_scratch_bytes, which the library lays out (denoise_carve).
+struct DenoiseArgs {
+    uint32_t width, height, iterations;
+    float color_weight, albedo_weight, normal_weight;
+    const float* color; const float* albedo; const float* normal;   // [npix][3]; a guide may be null (its weight is then 0)
+    void* scratch;
+    float* out_linear; uint8_t* out_rgb8;                            // [npix][3]; either may be null, not both
+};
+
 struct ResolveParams {
     const float4* samplebuf;
     float*   accum;        // [npix_local][3] running f32 sums in sample order
@@ -272,6 +282,10 @@ size_t adaptive_compact_bytes(uint32_t npix_local);   // cub's temporary storage
 cudaError_t launch_adaptive_compact(void* temp, size_t temp_bytes, const uint32_t* list_in, const uint32_t* keep, uint32_t* list_out,
                                     uint32_t* list_n_out, uint32_t npix_local, cudaStream_t st);
 cudaError_t launch_adaptive_resolve(const AdaptiveResolveParams& p, cudaStream_t st);
+// the denoise (rtb200_denoise.cu): its scratch for npix pixels, and its iterations + 1 launches (the guides' packing, then one
+// per iteration)
+uint64_t denoise_scratch_bytes(uint64_t npix);
+cudaError_t launch_denoise(const DenoiseArgs& a, cudaStream_t st);
 // geo[idx[k]] = geo_in[k], mat[idx[k]] = mat_in[k] for k < n (idx has no repeats)
 cudaError_t launch_update_scatter(const uint32_t* idx, const double4* geo_in, const DevMat* mat_in, uint32_t n, double4* geo, DevMat* mat,
                                   cudaStream_t st);

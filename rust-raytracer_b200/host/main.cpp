@@ -14,6 +14,10 @@
 // RTB200_AOV=<samples>[,<sample0>] also writes the auxiliary buffers of those camera samples of the frame (rtb200_scene_aov,
 // DESIGN.md §4.14) next to <output_file>: <stem>_albedo.png, the mean first-hit albedo in the beauty image's encoding, and
 // <stem>_normal.png, the mean normal n as 0.5 * n + 0.5 (no square root), where <stem> is <output_file> without its extension.
+// RTB200_DENOISE=<iterations>[,<color_weight>[,<albedo_weight>[,<normal_weight>]]] also writes <stem>_denoised.png: the frame's
+// linear image denoised (rtb200_denoise, DESIGN.md §4.15; omitted weights are the header's RTB200_DENOISE_DEFAULT_*) with the
+// albedo and normal of the frame's own samples (samples_per_pixel samples from sample 0) as guides. The frame is rendered once,
+// in linear f32, and out.png is its quantisation; the AOV pass uploads the scene once more.
 #include <chrono>
 #include <cmath>
 #include <cstring>
@@ -94,6 +98,24 @@ static uint8_t to_u8(float x) {
     return bits >= 0x4B000000u ? (uint8_t)(bits - 0x4B000000u) : (uint8_t)0;
 }
 
+// <output_file> without its extension
+static std::string stem_of(const std::string& out) {
+    const size_t slash = out.find_last_of('/'), dot = out.find_last_of('.');
+    return dot != std::string::npos && (slash == std::string::npos || dot > slash) ? out.substr(0, dot) : out;
+}
+
+// the mean albedo and normal of samples [sample0, sample0 + samples) of every pixel of `s` (rtb200_scene_aov)
+static int aov_of(const rt_scene& s, const rt_options& opts, uint32_t samples, uint32_t sample0, float* albedo, float* normal) {
+    rt_aov_params p{samples, sample0, {0u, 0u}};
+    rt_aov_out o{albedo, normal, nullptr, nullptr, nullptr};
+    rtb200_scene_handle h = nullptr;
+    int rc = rtb200_scene_upload(&s, &opts, &h);
+    if (rc == 0) rc = rtb200_scene_aov(h, &p, nullptr, &o, nullptr);
+    if (h) rtb200_scene_release(h);
+    if (rc != 0) fprintf(stderr, "aov failed (%d): %s\n", rc, rtb200_last_error());
+    return rc;
+}
+
 // RTB200_AOV: the albedo and normal buffers of samples [sample0, sample0 + samples) of every pixel of `s`, written beside `out`
 static int write_aov(const rt_scene& s, const char* spec, const rt_options& opts, const std::string& out) {
     char* end = nullptr;
@@ -107,23 +129,52 @@ static int write_aov(const rt_scene& s, const char* spec, const rt_options& opts
     }
     const size_t npix = (size_t)s.width * s.height;
     std::vector<float> albedo(npix * 3), normal(npix * 3);
-    rt_aov_params p{(uint32_t)samples, (uint32_t)sample0, {0u, 0u}};
-    rt_aov_out o{albedo.data(), normal.data(), nullptr, nullptr, nullptr};
-    rtb200_scene_handle h = nullptr;
-    int rc = rtb200_scene_upload(&s, &opts, &h);
-    if (rc == 0) rc = rtb200_scene_aov(h, &p, nullptr, &o, nullptr);
-    if (h) rtb200_scene_release(h);
-    if (rc != 0) { fprintf(stderr, "aov failed (%d): %s\n", rc, rtb200_last_error()); return 101; }
+    if (aov_of(s, opts, (uint32_t)samples, (uint32_t)sample0, albedo.data(), normal.data()) != 0) return 101;
     std::vector<uint8_t> a8(npix * 3), n8(npix * 3);
     for (size_t i = 0; i < npix * 3; ++i) {
         a8[i] = to_u8(std::sqrt(albedo[i]));
         n8[i] = to_u8(0.5f * normal[i] + 0.5f);
     }
-    const size_t slash = out.find_last_of('/'), dot = out.find_last_of('.');
-    const std::string stem = dot != std::string::npos && (slash == std::string::npos || dot > slash) ? out.substr(0, dot) : out;
+    const std::string stem = stem_of(out);
     std::string err;
     for (const auto& img : {std::make_pair(stem + "_albedo.png", &a8), std::make_pair(stem + "_normal.png", &n8)})
         if (!rthost::write_png_rgb8(img.first.c_str(), img.second->data(), s.width, s.height, &err)) { fprintf(stderr, "error writing image: %s\n", err.c_str()); return 101; }
+    return 0;
+}
+
+// RTB200_DENOISE: the parameters of `spec` for the frame of `s` (101 and a message when it is malformed)
+static int parse_denoise(const rt_scene& s, const char* spec, rt_denoise_params* p) {
+    double v[4] = {RTB200_DENOISE_DEFAULT_ITERATIONS, RTB200_DENOISE_DEFAULT_COLOR_WEIGHT, RTB200_DENOISE_DEFAULT_ALBEDO_WEIGHT,
+                   RTB200_DENOISE_DEFAULT_NORMAL_WEIGHT};
+    int k = 0;
+    for (const char* c = spec; k < 4; ++k) {
+        char* end = nullptr;
+        v[k] = strtod(c, &end);
+        if (end == c || (*end != ',' && *end != 0)) {
+            fprintf(stderr, "RTB200_DENOISE: expected <iterations>[,<color_weight>[,<albedo_weight>[,<normal_weight>]]], got \"%s\"\n", spec);
+            return 101;
+        }
+        if (*end == 0) break;
+        c = end + 1;
+    }
+    if (!(v[0] >= 1 && v[0] <= 10 && v[0] == std::floor(v[0]))) { fprintf(stderr, "RTB200_DENOISE: iterations must be an integer in [1, 10]\n"); return 101; }
+    if ((uint64_t)s.width * s.height >= (1ull << 31)) { fprintf(stderr, "RTB200_DENOISE: the frame must have fewer than 2^31 pixels\n"); return 101; }
+    *p = rt_denoise_params{s.width, s.height, (uint32_t)v[0], 0u, (float)v[1], (float)v[2], (float)v[3], 0.0f};
+    return 0;
+}
+
+// RTB200_DENOISE: `linear`, the frame of `s`, denoised with the AOVs of its own samples, written to <stem>_denoised.png
+static int write_denoised(const rt_scene& s, const rt_denoise_params& p, const rt_options& opts, const float* linear, const std::string& out) {
+    const size_t npix = (size_t)s.width * s.height;
+    std::vector<float> albedo(npix * 3), normal(npix * 3);
+    std::vector<uint8_t> rgb8(npix * 3);
+    if (aov_of(s, opts, s.samples_per_pixel, 0u, albedo.data(), normal.data()) != 0) return 101;
+    if (rtb200_denoise(opts.device, &p, linear, albedo.data(), normal.data(), nullptr, rgb8.data(), nullptr) != 0) {
+        fprintf(stderr, "denoise failed: %s\n", rtb200_last_error());
+        return 101;
+    }
+    std::string err;
+    if (!rthost::write_png_rgb8((stem_of(out) + "_denoised.png").c_str(), rgb8.data(), s.width, s.height, &err)) { fprintf(stderr, "error writing image: %s\n", err.c_str()); return 101; }
     return 0;
 }
 
@@ -152,6 +203,13 @@ int main(int argc, char** argv) {
         fprintf(stderr, "RTB200_AOV with RTB200_GPUS, RTB200_FRAMES or RTB200_ADAPTIVE is not supported: the buffers are of one frame's camera samples on one GPU\n");
         return 101;
     }
+    const char* denoise = getenv("RTB200_DENOISE");
+    if (denoise && (getenv("RTB200_GPUS") || getenv("RTB200_FRAMES") || adaptive)) {
+        fprintf(stderr, "RTB200_DENOISE with RTB200_GPUS, RTB200_FRAMES or RTB200_ADAPTIVE is not supported: it denoises one frame on one GPU\n");
+        return 101;
+    }
+    rt_denoise_params denoise_p{};
+    if (denoise && parse_denoise(holder.scene, denoise, &denoise_p) != 0) return 101;
     if (const char* fp = getenv("RTB200_FRAMES")) return render_animation(holder.scene, fp, argv[2]);
     printf("\nRendering %s\n", argv[2]);                                  // main.rs:18
     fflush(stdout);
@@ -162,10 +220,17 @@ int main(int argc, char** argv) {
     rt_stats st{};
     auto t0 = std::chrono::steady_clock::now();                           // raytracer.rs:259
     const char* gpus = getenv("RTB200_GPUS");
+    std::vector<float> linear;
     int rc = 0;
     if (adaptive) {
         rc = render_adaptive(s, adaptive, opts, pixels.data(), &st);
         if (rc == 101) return rc;
+    } else if (denoise) {
+        // the denoise needs the linear image: one render gives it, and out.png is its quantisation by the render's own routine
+        // (rtb200_probe_quantise), byte for byte the RGB8 render's
+        linear.resize(pixels.size());
+        rc = rtb200_render_linear_f32(&s, &opts, linear.data(), &st);
+        if (rc == 0) rc = rtb200_probe_quantise(linear.data(), (uint32_t)linear.size(), pixels.data());
     } else {
         rc = gpus ? rtb200_render_rgb8_multi(&s, &opts, atoi(gpus), pixels.data(), &st)   // replaces raytracer.rs:260-262
                   : rtb200_render_rgb8(&s, &opts, pixels.data(), &st);
@@ -182,6 +247,7 @@ int main(int argc, char** argv) {
     }
     std::string err;
     if (!rthost::write_png_rgb8(argv[2], pixels.data(), s.width, s.height, &err)) { fprintf(stderr, "error writing image: %s\n", err.c_str()); return 101; }   // raytracer.rs:265
-    if (aov) return write_aov(s, aov, opts, argv[2]);
+    if (aov && (rc = write_aov(s, aov, opts, argv[2])) != 0) return rc;
+    if (denoise) return write_denoised(s, denoise_p, opts, linear.data(), argv[2]);
     return 0;
 }

@@ -139,12 +139,19 @@ class rt_aov_out(C.Structure):
     _fields_ = [("albedo", C.c_void_p), ("normal", C.c_void_p), ("hits", C.c_void_p), ("sphere", C.c_void_p), ("point", C.c_void_p)]
 
 
+class rt_denoise_params(C.Structure):
+    """The edge-avoiding à-trous filter of rtb200_denoise[_device]: image size, iterations L in [1, 10], and the finite,
+    non-negative weights of the colour, albedo and normal guides (0 turns a guide off)."""
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("iterations", C.c_uint32), ("reserved", C.c_uint32),
+                ("color_weight", C.c_float), ("albedo_weight", C.c_float), ("normal_weight", C.c_float), ("reserved2", C.c_float)]
+
+
 HIT_FIELDS = (("t", 1, np.float64), ("sphere", 1, np.int32), ("point", 3, np.float64), ("normal", 3, np.float64),
               ("uv", 2, np.float64), ("front_face", 1, np.uint8))   # rt_hits: name, values per ray, dtype (sphere -1 = 0xffffffff)
 
 assert C.sizeof(rt_sphere) == 64 and C.sizeof(rt_frame) == 112 and C.sizeof(rt_adaptive_params) == 24
 assert C.sizeof(rt_rays) == 24 and C.sizeof(rt_hits) == 48 and C.sizeof(rt_trace_params) == 32
-assert C.sizeof(rt_aov_params) == 16 and C.sizeof(rt_aov_out) == 40
+assert C.sizeof(rt_aov_params) == 16 and C.sizeof(rt_aov_out) == 40 and C.sizeof(rt_denoise_params) == 32
 AOV_FIELDS = (("albedo", 3, np.float32), ("normal", 3, np.float32), ("hits", 1, np.uint32), ("sphere", 1, np.int32),
               ("point", 3, np.float64))   # rt_aov_out: name, values per pixel, dtype (sphere -1 = 0xffffffff)
 
@@ -165,6 +172,7 @@ ABI_SYMBOLS = [
     "rtb200_scene_trace_rays_device", "rtb200_scene_trace_rays",
     "rtb200_scene_edit_spheres",
     "rtb200_scene_aov_device", "rtb200_scene_aov",
+    "rtb200_denoise_scratch_bytes", "rtb200_denoise_device", "rtb200_denoise",
 ]
 
 _lib = None
@@ -234,6 +242,12 @@ def lib() -> C.CDLL:
     L.rtb200_scene_edit_spheres.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
     L.rtb200_scene_aov_device.argtypes = [C.c_void_p, C.POINTER(rt_aov_params), C.POINTER(rt_frame), C.POINTER(rt_aov_out), C.c_void_p]
     L.rtb200_scene_aov.argtypes = [C.c_void_p, C.POINTER(rt_aov_params), C.POINTER(rt_frame), C.POINTER(rt_aov_out), C.POINTER(rt_stats)]
+    L.rtb200_denoise_scratch_bytes.restype = C.c_uint64
+    L.rtb200_denoise_scratch_bytes.argtypes = [C.c_uint32, C.c_uint32]
+    L.rtb200_denoise_device.argtypes = [C.c_int32, C.POINTER(rt_denoise_params), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                        C.c_void_p, C.c_void_p, C.c_void_p]
+    L.rtb200_denoise.argtypes = [C.c_int32, C.POINTER(rt_denoise_params), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                 C.POINTER(rt_stats)]
     _lib = L
     return L
 
@@ -935,6 +949,77 @@ class ResidentScene:
             self.release()
         except Exception:
             pass
+
+
+# the denoise's defaults, include/rtb200.h's RTB200_DENOISE_DEFAULT_* (DESIGN.md §4.15: chosen on the oracle's 2-spp cover render at
+# 64x48 with its AOV guides)
+DENOISE_ITERATIONS, DENOISE_COLOR_WEIGHT, DENOISE_ALBEDO_WEIGHT, DENOISE_NORMAL_WEIGHT = 3, 16.0, 4.0, 1.0
+
+
+def denoise(color, albedo=None, normal=None, *, iterations: int = DENOISE_ITERATIONS, color_weight: float = DENOISE_COLOR_WEIGHT,
+            albedo_weight: Optional[float] = None, normal_weight: Optional[float] = None, linear: bool = True, rgb8: bool = False,
+            stream=None) -> dict:
+    """Denoise a [h, w, 3] float32 image (normally a render's linear mean) with the edge-avoiding à-trous filter of
+    include/rtb200.h, guided by the optional albedo and normal of :meth:`ResidentScene.aov`. A guide's weight defaults to
+    DENOISE_ALBEDO_WEIGHT / DENOISE_NORMAL_WEIGHT when the guide is given and to 0 (off) when it is not.
+
+    numpy arrays use the blocking host form (rtb200_denoise) and the result also holds "stats". CUDA tensors (contiguous, on one
+    device) use the device form (rtb200_denoise_device) on `stream` without waiting: a torch.cuda.Stream, a nonzero
+    cudaStream_t handle (CUDA_STREAM_LEGACY is torch's default stream), or by default torch's current stream. The scratch and
+    the outputs are allocated by torch on that stream, so the caching allocator hands the scratch to no other stream's
+    allocation before the call has run; the library's own stream (handle 0) is refused for that reason. Returns
+    {"linear": float32 [h, w, 3]} and/or {"rgb8": uint8 [h, w, 3]}, whichever is asked for."""
+    if not (linear or rgb8):
+        raise ValueError("denoise: ask for linear, rgb8 or both")
+    if albedo_weight is None:
+        albedo_weight = DENOISE_ALBEDO_WEIGHT if albedo is not None else 0.0
+    if normal_weight is None:
+        normal_weight = DENOISE_NORMAL_WEIGHT if normal is not None else 0.0
+    host = isinstance(color, np.ndarray)
+    shape = tuple(color.shape)
+    if len(shape) != 3 or shape[2] != 3:
+        raise ValueError(f"denoise: color must have shape [h, w, 3], got {shape}")
+    for name, g in (("color", color), ("albedo", albedo), ("normal", normal)):
+        if g is None:
+            continue
+        if host:
+            ok = isinstance(g, np.ndarray) and g.dtype == np.float32 and g.flags.c_contiguous
+        else:
+            import torch
+            ok = isinstance(g, torch.Tensor) and g.is_cuda and g.dtype == torch.float32 and g.is_contiguous() and g.device == color.device
+        if not ok or tuple(g.shape) != shape:
+            kind = "C-contiguous float32 numpy arrays" if host else "contiguous float32 CUDA tensors on one device"
+            raise ValueError(f"denoise takes {kind} of shape {list(shape)}: {name} is not one")
+    p = rt_denoise_params(shape[1], shape[0], int(iterations), 0, float(color_weight), float(albedo_weight), float(normal_weight), 0.0)
+    if host:
+        out = {k: np.empty(shape, dtype=ty) for k, ty, want in (("linear", np.float32, linear), ("rgb8", np.uint8, rgb8)) if want}
+        st = rt_stats()
+        ptr = lambda a: a.ctypes.data if a is not None else None  # noqa: E731
+        _check(lib().rtb200_denoise(-1, C.byref(p), ptr(color), ptr(albedo), ptr(normal), ptr(out.get("linear")), ptr(out.get("rgb8")),
+                                    C.byref(st)))
+        out["stats"] = st.as_dict()
+        return out
+    import torch
+    device = color.device
+    if stream is None:
+        stream = torch.cuda.current_stream(device)
+    elif not isinstance(stream, torch.cuda.Stream):
+        if int(stream) == 0:
+            raise ValueError("denoise on CUDA tensors takes a torch stream or a nonzero cudaStream_t: the library's own stream "
+                             "(0) cannot order the reuse of the scratch torch allocates")
+        stream = torch.cuda.default_stream(device) if int(stream) == CUDA_STREAM_LEGACY else torch.cuda.ExternalStream(int(stream), device=device)
+    handle = stream.cuda_stream or CUDA_STREAM_LEGACY
+    # the scratch and the outputs belong to the call's stream: the caching allocator reuses the scratch, freed when this
+    # function returns, only for later work on that stream, which runs after the call
+    with torch.cuda.stream(stream):
+        scratch = torch.empty(int(lib().rtb200_denoise_scratch_bytes(shape[1], shape[0])), dtype=torch.uint8, device=device)
+        out = {k: torch.empty(shape, dtype=ty, device=device) for k, ty, want in (("linear", torch.float32, linear), ("rgb8", torch.uint8, rgb8)) if want}
+    if color.numel() == 0:   # a 0-pixel image (the library's no-op)
+        return out
+    ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+    _check(lib().rtb200_denoise_device(device.index, C.byref(p), ptr(color), ptr(albedo), ptr(normal), ptr(scratch),
+                                       ptr(out.get("linear")), ptr(out.get("rgb8")), C.c_void_p(handle)))
+    return out
 
 
 def write_png(path: str, rgb8: np.ndarray):

@@ -509,6 +509,65 @@ int rtb200_denoise_device(int32_t device, const rt_denoise_params* p, const floa
 int rtb200_denoise(int32_t device, const rt_denoise_params* p, const float* color, const float* albedo, const float* normal,
                    float* out_linear, uint8_t* out_rgb8, rt_stats* stats);
 
+/* ---- temporal accumulation of animation frames (DESIGN.md §4.16) ----------------------------------------------------------
+ * Blends each pixel of a frame with the history of the previous frame where its first hit was, the reprojection and blend of
+ * SVGF's first stage. Every f64 and f32 operation is rounded to nearest and never contracted; sums and products run in the
+ * order written. Whole frames only (width x height pixels, row-major, top row first): a shard's compact rows are not image
+ * neighbours. Inputs of this frame (rt_temporal_frame): color 3 x f32 (normally a render's linear mean), sphere u32 and
+ * point 3 x f64 (rtb200_scene_aov's sphere and point of the same camera; 0xffffffff is a miss), camera = p->camera. The previous
+ * frame (rt_temporal_history, or NULL for none): the previous call's output color and length, the previous frame's AOV sphere
+ * and point, and p->prev_camera. motion (may be NULL when n_motion is 0): n_motion x 3 f64, the displacement of sphere j since
+ * the previous frame (its current centre minus its previous one); spheres j >= n_motion did not move. N = p->max_history.
+ * Per pixel p = (x, y), with c = color[p]:
+ *  1. if c has a non-finite value or there is no previous frame: the output is c, length 1. Otherwise:
+ *  2. a hit (j = sphere[p] != 0xffffffff): P = point[p], P' = P - motion[j] (P when j >= n_motion), D_cur = P - camera.origin,
+ *     D_prev = P' - prev_camera.origin. A miss: D_cur = D_prev = Camera::get_ray's direction under camera at the pixel centre,
+ *     u = (x + 0.5) / (W - 1), v = (H - (y + 0.5)) / (H - 1) (camera.rs:79-84, raytracer.rs:199-200 with both draws 0.5).
+ *  3. the projection of D into a camera {origin, llc, h, vt}: a = llc - origin; cn = h x vt, cu = vt x a, cv = a x h (cross
+ *     products (y1 z2 - z1 y2, z1 x2 - x1 z2, x1 y2 - y1 x2), dot products (x + y) + z); den = cn . D; u = (cu . D) / den,
+ *     v = (cv . D) / den. It is valid when den != 0, (cn . a) / den > 0 (in front of the camera), and u and v are finite.
+ *  4. (u_c, v_c) of D_cur under camera, (u_p, v_p) of D_prev under prev_camera; fx = x + (u_p - u_c) * (W - 1),
+ *     fy = y - (v_p - v_c) * (H - 1). No history if a projection is invalid or fx or fy is not finite. A static camera with no
+ *     motion gives fx = x, fy = y exactly: the motion is measured at the sample's own point and applied to the pixel centre.
+ *  5. x0 = floor(fx), y0 = floor(fy), ax = f32(fx - x0), ay = f32(fy - y0); taps (x0, y0), (x0+1, y0), (x0, y0+1),
+ *     (x0+1, y0+1) in that order with f32 weights (1-ax)(1-ay), ax(1-ay), (1-ax)ay, ax ay. Tap q is valid when its weight is
+ *     > 0, it is inside the image, length[q] >= 1, the history colour of q is finite, the previous sphere of q is sphere[p] and,
+ *     for a hit, |prev_point[q] - P'|^2 <= (depth_tol * depth_tol) * |D_prev|^2 (|v|^2 = v . v, f64).
+ *  6. s = the f32 sum of the valid taps' weights in tap order; s = 0 is no history. Else h_k = (sum of w * hist_k in tap
+ *     order) / s, L = the least length of the valid taps, n = min(L, N - 1) + 1 (no overflow at L = 2^32 - 1), and for n >= 2
+ *     the output is h_k + (1.0f / f32(n)) * (c_k - h_k) with length n. No history (or n = 1) is c with length 1.
+ * A history must ping-pong between two buffers: an output may not overlap any input. After an edit that renumbers spheres
+ * (rtb200_scene_edit_spheres), pass no previous frame. */
+typedef struct {
+    uint32_t  width, height;
+    uint32_t  max_history;        /* N >= 1: a pixel's history is the mean of at most its last N frames */
+    uint32_t  n_motion;           /* rows of motion */
+    rt_camera camera, prev_camera;   /* this frame's and the previous frame's (prev_camera is ignored without a previous frame) */
+    double    depth_tol;          /* finite, >= 0: a relative depth tolerance */
+    uint32_t  reserved[2];        /* must be 0 */
+} rt_temporal_params;             /* 224 bytes */
+typedef struct { const float* color; const uint32_t* sphere; const double* point; } rt_temporal_frame;   /* 24 bytes */
+typedef struct { const float* color; const uint32_t* length; const uint32_t* sphere; const double* point; } rt_temporal_history;   /* 32 bytes */
+typedef struct { float* color; uint32_t* length; } rt_temporal_out;   /* 16 bytes: the new history */
+/* Defaults of the Python binding and the CLI (DESIGN.md §4.16: chosen on an orbit of the 2-spp cover render at 64 x 48) */
+#define RTB200_TEMPORAL_DEFAULT_MAX_HISTORY 2
+#define RTB200_TEMPORAL_DEFAULT_DEPTH_TOL   0.03
+/* Device buffers of `device` (-1: the current device) or managed memory. Stream-ordered, without waiting for the GPU: runs on
+ * `stream` (NULL: the library's stream of that device); the caller keeps every buffer valid until it has run. It needs no
+ * scratch and touches no scene handle and no work set.
+ * RT_ERR_INVALID, before any device work, for a NULL params, cur, cur->color, cur->sphere, cur->point, out, out->color or
+ * out->length, a prev with a NULL member, a nonzero reserved, max_history 0, a depth_tol that is NaN, negative or infinite, a
+ * NULL motion with n_motion > 0, width * height >= 2^31, a misaligned pointer (4 bytes for f32 and u32 arrays, 8 for f64), an
+ * output overlapping an input or the other output, or a pointer that is not device memory of `device` nor managed memory.
+ * A 0-pixel image is a no-op. */
+int rtb200_temporal_device(int32_t device, const rt_temporal_params* p, const rt_temporal_frame* cur, const rt_temporal_history* prev,
+                           const double* motion, const rt_temporal_out* out, void* stream);
+/* Host buffers, blocking: the same through the same kernel on the library's stream, with the inputs copied in and the outputs
+ * copied out. stats (may be NULL): device_ms (copies and kernel), trace_ms (the kernel), wall_ms, h2d_bytes, d2h_bytes and
+ * kernel_launches (1). Same checks, bar the alignment and the memory kind. */
+int rtb200_temporal(int32_t device, const rt_temporal_params* p, const rt_temporal_frame* cur, const rt_temporal_history* prev,
+                    const double* motion, const rt_temporal_out* out, rt_stats* stats);
+
 /* load_texture_image — materials.rs:213-219, config.rs:36-47: decode a baseline JPEG file to RGB8 (host-side scene staging
  * helper for hosts without their own decoder; the reference uses the jpeg-decoder crate). *out_rgb8 is released with rtb200_free(). */
 int  rtb200_decode_jpeg_file(const char* path, uint8_t** out_rgb8, uint64_t* width, uint64_t* height);

@@ -1,0 +1,130 @@
+// rtb200_api_temporal.cu — the temporal accumulation of animation frames through the C ABI (DESIGN.md §4.16), in both forms:
+// device buffers on the caller's stream, or host buffers staged through the context's query block (HostStage). The kernel is
+// in rtb200_temporal.cu.
+
+#include "rtb200_host.cuh"
+
+using namespace rtk;
+
+namespace {
+
+struct Range { const void* p; uint64_t bytes; const char* name; uintptr_t align; };
+
+bool overlap(const Range& a, const Range& b) {
+    if (!a.p || !b.p || !a.bytes || !b.bytes) return false;
+    const uintptr_t a0 = (uintptr_t)a.p, b0 = (uintptr_t)b.p;
+    return a0 < b0 + b.bytes && b0 < a0 + a.bytes;
+}
+
+// The argument checks of both forms (no device is touched); the alignment is checked in the device form only.
+int check_temporal(const rt_temporal_params* p, const rt_temporal_frame* cur, const rt_temporal_history* prev, const double* motion,
+                   const rt_temporal_out* out, bool device_form) {
+    if (!p) return fail(RT_ERR_INVALID, "params is null");
+    if (!cur || !cur->color || !cur->sphere || !cur->point) return fail(RT_ERR_INVALID, "cur or one of its arrays is null");
+    if (!out || !out->color || !out->length) return fail(RT_ERR_INVALID, "out or one of its arrays is null");
+    if (prev && !(prev->color && prev->length && prev->sphere && prev->point))
+        return fail(RT_ERR_INVALID, "prev is a partial previous frame: give all four arrays or no prev");
+    if (p->reserved[0] != 0 || p->reserved[1] != 0) return fail(RT_ERR_INVALID, "rt_temporal_params.reserved must be 0");
+    if (p->max_history == 0) return fail(RT_ERR_INVALID, "rt_temporal_params.max_history must be >= 1");
+    if (!(std::isfinite(p->depth_tol) && p->depth_tol >= 0.0)) return fail(RT_ERR_INVALID, "rt_temporal_params.depth_tol must be finite and >= 0");
+    if (!motion && p->n_motion > 0) return fail(RT_ERR_INVALID, "motion is null but n_motion > 0");
+    const uint64_t n = (uint64_t)p->width * p->height;
+    if (n >= (1ull << 31)) return fail(RT_ERR_INVALID, "width * height must be below 2^31");
+    const Range in[8] = {{cur->color, n * 12, "cur.color", 4}, {cur->sphere, n * 4, "cur.sphere", 4}, {cur->point, n * 24, "cur.point", 8},
+                         {prev ? prev->color : nullptr, n * 12, "prev.color", 4}, {prev ? prev->length : nullptr, n * 4, "prev.length", 4},
+                         {prev ? prev->sphere : nullptr, n * 4, "prev.sphere", 4}, {prev ? prev->point : nullptr, n * 24, "prev.point", 8},
+                         {motion, (uint64_t)p->n_motion * 24, "motion", 8}};
+    const Range outs[2] = {{out->color, n * 12, "out.color", 4}, {out->length, n * 4, "out.length", 4}};
+    if (device_form) {
+        for (const Range* g : {in, outs})
+            for (int k = 0; k < (g == in ? 8 : 2); ++k)
+                if ((uintptr_t)g[k].p % g[k].align) return fail(RT_ERR_INVALID, std::string(g[k].name) + " is not " + std::to_string(g[k].align) + "-byte aligned");
+    }
+    // an output must not overlap an input or the other output
+    for (int i = 0; i < 2; ++i) {
+        for (const Range& r : in)
+            if (overlap(outs[i], r)) return fail(RT_ERR_INVALID, std::string(outs[i].name) + " overlaps " + r.name);
+        if (i == 1 && overlap(outs[1], outs[0])) return fail(RT_ERR_INVALID, "out.length overlaps out.color");
+    }
+    return RT_OK;
+}
+
+TemporalArgs temporal_args(const rt_temporal_params& p, const float* color, const uint32_t* sphere, const double* point, const float* h_color,
+                           const uint32_t* h_length, const uint32_t* h_sphere, const double* h_point, const double* motion,
+                           float* out_color, uint32_t* out_length) {
+    return TemporalArgs{p.width, p.height, p.max_history, p.n_motion, p.camera, p.prev_camera, p.depth_tol, color, sphere, point,
+                        h_color, h_length, h_sphere, h_point, p.n_motion ? motion : nullptr, out_color, out_length};
+}
+
+}  // namespace
+
+int rtb200_temporal_device(int32_t device, const rt_temporal_params* p, const rt_temporal_frame* cur, const rt_temporal_history* prev,
+                           const double* motion, const rt_temporal_out* out, void* stream_in) {
+  return guarded([&]() -> int {
+    int rc = check_temporal(p, cur, prev, motion, out, true);
+    if (rc != RT_OK) return rc;
+    if ((uint64_t)p->width * p->height == 0) return RT_OK;
+    DeviceRestore restore_;
+    DeviceCtx* ctx = nullptr;
+    if ((rc = get_ctx(device, &ctx)) != RT_OK) return rc;
+    std::lock_guard<std::recursive_mutex> lock_(ctx->mu);
+    const rt_temporal_history none{};
+    const rt_temporal_history& h = prev ? *prev : none;
+    if ((rc = check_device_ptrs(ctx->device, {{cur->color, "cur.color"}, {cur->sphere, "cur.sphere"}, {cur->point, "cur.point"},
+                                              {h.color, "prev.color"}, {h.length, "prev.length"}, {h.sphere, "prev.sphere"},
+                                              {h.point, "prev.point"}, {p->n_motion ? motion : nullptr, "motion"},
+                                              {out->color, "out.color"}, {out->length, "out.length"}})) != RT_OK)
+        return rc;
+    const cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
+    CU(launch_temporal(temporal_args(*p, cur->color, cur->sphere, cur->point, h.color, h.length, h.sphere, h.point, motion, out->color,
+                                     out->length), st));
+    return RT_OK;
+  });
+}
+
+int rtb200_temporal(int32_t device, const rt_temporal_params* p, const rt_temporal_frame* cur, const rt_temporal_history* prev,
+                    const double* motion, const rt_temporal_out* out, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (stats) memset(stats, 0, sizeof *stats);
+    int rc = check_temporal(p, cur, prev, motion, out, false);
+    if (rc != RT_OK) return rc;
+    const uint64_t N = (uint64_t)p->width * p->height;
+    if (N == 0) return RT_OK;
+    auto wall0 = std::chrono::steady_clock::now();
+    DeviceRestore restore_;
+    DeviceCtx* ctx = nullptr;
+    if ((rc = get_ctx(device, &ctx)) != RT_OK) return rc;
+    std::lock_guard<std::recursive_mutex> lock_(ctx->mu);
+    for (auto& e : ctx->query_ev) if (!e) CU(cudaEventCreate(&e));
+    // device image: this frame, the previous frame (absent: 0 bytes, a null dev), the motion, the outputs
+    const uint64_t hb = prev ? N : 0;
+    HostStage io;
+    io.add_in(cur->color, N * 12); io.add_in(cur->sphere, N * 4); io.add_in(cur->point, N * 24);
+    io.add_in(prev ? prev->color : nullptr, hb * 12); io.add_in(prev ? prev->length : nullptr, hb * 4);
+    io.add_in(prev ? prev->sphere : nullptr, hb * 4); io.add_in(prev ? prev->point : nullptr, hb * 24);
+    io.add_in(motion, (uint64_t)p->n_motion * 24);
+    io.add_out(out->color, N * 12); io.add_out(out->length, N * 4);
+    if ((rc = io.place(ctx, 0)) != RT_OK) return rc;
+    const cudaStream_t st = ctx->stream;
+    cudaEvent_t* ev = ctx->query_ev;
+    CU(cudaEventRecord(ev[0], st));
+    if ((rc = io.copy(st, false)) != RT_OK) return rc;
+    CU(cudaEventRecord(ev[1], st));
+    auto dev = [&](int k) { return (const void*)io.a[k].dev; };
+    CU(launch_temporal(temporal_args(*p, (const float*)dev(0), (const uint32_t*)dev(1), (const double*)dev(2), (const float*)dev(3),
+                                     (const uint32_t*)dev(4), (const uint32_t*)dev(5), (const double*)dev(6), (const double*)dev(7),
+                                     (float*)io.a[8].dev, (uint32_t*)io.a[9].dev), st));
+    CU(cudaEventRecord(ev[2], st));
+    if ((rc = io.copy(st, true)) != RT_OK) return rc;
+    CU(cudaEventRecord(ev[3], st));
+    CU(cudaStreamSynchronize(st));
+    if (!stats) return RT_OK;
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, ev[0], ev[3])); stats->device_ms = ms;
+    CU(cudaEventElapsedTime(&ms, ev[1], ev[2])); stats->trace_ms = ms;
+    stats->kernel_launches = 1;
+    stats->h2d_bytes = io.h2d; stats->d2h_bytes = io.d2h;
+    stats->wall_ms = ms_since(wall0);
+    return RT_OK;
+  });
+}

@@ -1,5 +1,5 @@
 // rtb200_host.cuh — what the host translation units of the C ABI share (rtb200_api.cu, rtb200_api_render.cu,
-// rtb200_api_scene.cu, rtb200_api_query.cu, rtb200_api_denoise.cu): error reporting, the per-device contexts, the scene
+// rtb200_api_scene.cu, rtb200_api_query.cu, rtb200_api_denoise.cu, rtb200_api_temporal.cu): error reporting, the per-device contexts, the scene
 // handle and the helpers more than one of them calls. Not installed.
 #pragma once
 #include <algorithm>
@@ -102,7 +102,7 @@ struct DeviceCtx {
     std::vector<OccKey> occ_cache;        // cudaOccupancyMaxActiveBlocksPerMultiprocessor answers
     PinnedBuf staging;                    // host image of the arena being uploaded
     cudaEvent_t staging_free = nullptr;   // the last H2D copy out of `staging` has finished
-    // the host forms of rtb200_scene_intersect, _occluded, _trace_rays, _aov and rtb200_denoise: their arrays on the device
+    // the host forms of rtb200_scene_intersect, _occluded, _trace_rays, _aov, rtb200_denoise and rtb200_temporal: their arrays on the device
     // (HostStage), the query's timing events (created at its first call), and the resident CTAs per SM of the query kernel of
     // each kind and mode (0: not asked yet)
     GrowBuf query;
@@ -258,7 +258,7 @@ int render_collect(rtb200_scene_t* h, rt_stats* stats);
 // block is free. copy enqueues the inputs' copies to the device, or with `back` the outputs' to the host; h2d and d2h count them.
 struct HostStage {
     struct Array { const void* in; void* out; uint64_t bytes; char* dev; };
-    Array a[9];
+    Array a[10];
     int n = 0;
     uint64_t h2d = 0, d2h = 0;
     void add_in(const void* host, uint64_t bytes) { a[n++] = Array{host, nullptr, bytes, nullptr}; }

@@ -156,6 +156,17 @@ struct DenoiseArgs {
     float* out_linear; uint8_t* out_rgb8;                            // [npix][3]; either may be null, not both
 };
 
+// The temporal accumulation (rtb200_temporal.cu, DESIGN.md §4.16) of a width x height frame: the caller's buffers.
+struct TemporalArgs {
+    uint32_t width, height, max_history, n_motion;
+    rt_camera cam, prev_cam;
+    double depth_tol;
+    const float* color; const uint32_t* sphere; const double* point;                  // this frame
+    const float* h_color; const uint32_t* h_length; const uint32_t* h_sphere; const double* h_point;   // all null: no history
+    const double* motion;                                                             // [n_motion][3], null when n_motion is 0
+    float* out_color; uint32_t* out_length;
+};
+
 struct ResolveParams {
     const float4* samplebuf;
     float*   accum;        // [npix_local][3] running f32 sums in sample order
@@ -286,6 +297,8 @@ cudaError_t launch_adaptive_resolve(const AdaptiveResolveParams& p, cudaStream_t
 // per iteration)
 uint64_t denoise_scratch_bytes(uint64_t npix);
 cudaError_t launch_denoise(const DenoiseArgs& a, cudaStream_t st);
+// the temporal accumulation (rtb200_temporal.cu): one launch, one thread per pixel
+cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t st);
 // geo[idx[k]] = geo_in[k], mat[idx[k]] = mat_in[k] for k < n (idx has no repeats)
 cudaError_t launch_update_scatter(const uint32_t* idx, const double4* geo_in, const DevMat* mat_in, uint32_t n, double4* geo, DevMat* mat,
                                   cudaStream_t st);

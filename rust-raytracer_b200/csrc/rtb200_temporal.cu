@@ -1,0 +1,122 @@
+// rtb200_temporal.cu — the temporal accumulation of rtb200_temporal[_device] (DESIGN.md §4.16): each pixel of a frame is
+// reprojected into the previous frame through its first hit and blended with the history found there, as include/rtb200.h
+// states it and tests/temporal_restatement.py restates it in numpy. Every f64 and f32 operation goes through the __d*_rn /
+// __f*_rn intrinsics, so nothing is contracted or reordered.
+//
+// rt_temporal_kernel   one thread per pixel: the pixel's two projections in f64, then a 2x2 gather of the previous frame's
+//                      history colour and length, sphere and point around the reprojected position, in the contract's tap
+//                      order. Memory-bound: about 40 B of the pixel's own inputs, up to 4 x 44 B of neighbours (mostly the
+//                      pixel's own neighbourhood, so L1/L2 hits) and 16 B of output.
+#include "rtb200_kernels.cuh"
+
+using namespace rtd;
+
+namespace rtk {
+
+constexpr int kTemporalBlock = 256;
+
+namespace {
+
+// (y1 z2 - z1 y2, z1 x2 - x1 z2, x1 y2 - y1 x2)
+RT_DEV D3 cross(D3 a, D3 b) {
+    return mk(__dsub_rn(__dmul_rn(a.y, b.z), __dmul_rn(a.z, b.y)), __dsub_rn(__dmul_rn(a.z, b.x), __dmul_rn(a.x, b.z)),
+              __dsub_rn(__dmul_rn(a.x, b.y), __dmul_rn(a.y, b.x)));
+}
+
+// The image coordinates (u, v) of direction d under camera c; false when d does not project (behind the camera, parallel to
+// the image plane, or u or v not finite).
+RT_DEV bool project(const rt_camera& c, D3 d, double& u, double& v) {
+    const D3 a = sub(from(c.lower_left_corner), from(c.origin)), h = from(c.horizontal), vt = from(c.vertical);
+    const D3 cn = cross(h, vt);
+    const double den = dot(cn, d);
+    const double front = __ddiv_rn(dot(cn, a), den);
+    u = __ddiv_rn(dot(cross(vt, a), d), den);
+    v = __ddiv_rn(dot(cross(a, h), d), den);
+    return den != 0.0 && front > 0.0 && isfinite(u) && isfinite(v);
+}
+
+RT_DEV bool finite3(float a, float b, float c) { return isfinite(a) && isfinite(b) && isfinite(c); }
+
+}  // namespace
+
+__global__ void __launch_bounds__(kTemporalBlock) rt_temporal_kernel(const TemporalArgs a) {
+    const uint64_t W = a.width, H = a.height;
+    const uint64_t p = (uint64_t)blockIdx.x * kTemporalBlock + threadIdx.x;
+    if (p >= W * H) return;
+    const uint32_t x = (uint32_t)(p % W), y = (uint32_t)(p / W);
+    const float c0 = a.color[3 * p], c1 = a.color[3 * p + 1], c2 = a.color[3 * p + 2];
+    float o0 = c0, o1 = c1, o2 = c2;
+    uint32_t len = 1;
+    if (a.h_color && finite3(c0, c1, c2)) {
+        const uint32_t j = a.sphere[p];
+        const bool hit = j != 0xffffffffu;
+        D3 pp = mk(0.0, 0.0, 0.0), dc, dp;
+        if (hit) {
+            const D3 P = mk(a.point[3 * p], a.point[3 * p + 1], a.point[3 * p + 2]);
+            pp = j < a.n_motion ? sub(P, mk(a.motion[3 * (uint64_t)j], a.motion[3 * (uint64_t)j + 1], a.motion[3 * (uint64_t)j + 2])) : P;
+            dc = sub(P, from(a.cam.origin));
+            dp = sub(pp, from(a.prev_cam.origin));
+        } else {
+            const double u = __ddiv_rn(__dadd_rn((double)x, 0.5), __dsub_rn((double)W, 1.0));
+            const double v = __ddiv_rn(__dsub_rn((double)H, __dadd_rn((double)y, 0.5)), __dsub_rn((double)H, 1.0));
+            D3 o;
+            get_ray(a.cam, u, v, o, dc);
+            dp = dc;
+        }
+        double uc, vc, up, vp;
+        if (project(a.cam, dc, uc, vc) && project(a.prev_cam, dp, up, vp)) {
+            const double fx = __dadd_rn((double)x, __dmul_rn(__dsub_rn(up, uc), __dsub_rn((double)W, 1.0)));
+            const double fy = __dsub_rn((double)y, __dmul_rn(__dsub_rn(vp, vc), __dsub_rn((double)H, 1.0)));
+            if (isfinite(fx) && isfinite(fy)) {
+                const double x0 = floor(fx), y0 = floor(fy);
+                const float ax = __double2float_rn(__dsub_rn(fx, x0)), ay = __double2float_rn(__dsub_rn(fy, y0));
+                const float bx = __fsub_rn(1.0f, ax), by = __fsub_rn(1.0f, ay);
+                const float w[4] = {__fmul_rn(bx, by), __fmul_rn(ax, by), __fmul_rn(bx, ay), __fmul_rn(ax, ay)};
+                const double tol2 = __dmul_rn(a.depth_tol, a.depth_tol);
+                const double lim = hit ? __dmul_rn(tol2, dot(dp, dp)) : 0.0;
+                float s = 0.0f, n0 = 0.0f, n1 = 0.0f, n2 = 0.0f;
+                uint32_t L = 0xffffffffu;
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const double tx = __dadd_rn(x0, (double)(k & 1)), ty = __dadd_rn(y0, (double)(k >> 1));
+                    if (!(w[k] > 0.0f && tx >= 0.0 && tx < (double)W && ty >= 0.0 && ty < (double)H)) continue;
+                    const uint64_t q = (uint64_t)ty * W + (uint64_t)tx;
+                    const uint32_t lq = a.h_length[q];
+                    if (lq < 1 || a.h_sphere[q] != j) continue;
+                    const float h0 = a.h_color[3 * q], h1 = a.h_color[3 * q + 1], h2 = a.h_color[3 * q + 2];
+                    if (!finite3(h0, h1, h2)) continue;
+                    if (hit) {
+                        const D3 e = sub(mk(a.h_point[3 * q], a.h_point[3 * q + 1], a.h_point[3 * q + 2]), pp);
+                        if (!(dot(e, e) <= lim)) continue;
+                    }
+                    s = __fadd_rn(s, w[k]);
+                    n0 = __fadd_rn(n0, __fmul_rn(w[k], h0));
+                    n1 = __fadd_rn(n1, __fmul_rn(w[k], h1));
+                    n2 = __fadd_rn(n2, __fmul_rn(w[k], h2));
+                    L = min(L, lq);
+                }
+                if (s != 0.0f) {
+                    const uint32_t n = min(L, a.max_history - 1) + 1;
+                    if (n >= 2) {
+                        const float g0 = __fdiv_rn(n0, s), g1 = __fdiv_rn(n1, s), g2 = __fdiv_rn(n2, s);
+                        const float alpha = __fdiv_rn(1.0f, __uint2float_rn(n));
+                        o0 = __fadd_rn(g0, __fmul_rn(alpha, __fsub_rn(c0, g0)));
+                        o1 = __fadd_rn(g1, __fmul_rn(alpha, __fsub_rn(c1, g1)));
+                        o2 = __fadd_rn(g2, __fmul_rn(alpha, __fsub_rn(c2, g2)));
+                        len = n;
+                    }
+                }
+            }
+        }
+    }
+    a.out_color[3 * p] = o0; a.out_color[3 * p + 1] = o1; a.out_color[3 * p + 2] = o2;
+    a.out_length[p] = len;
+}
+
+cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t st) {
+    const uint64_t npix = (uint64_t)a.width * a.height;
+    rt_temporal_kernel<<<(unsigned)((npix + kTemporalBlock - 1) / kTemporalBlock), kTemporalBlock, 0, st>>>(a);
+    return cudaGetLastError();
+}
+
+}  // namespace rtk

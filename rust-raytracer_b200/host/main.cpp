@@ -18,6 +18,14 @@
 // linear image denoised (rtb200_denoise, DESIGN.md §4.15; omitted weights are the header's RTB200_DENOISE_DEFAULT_*) with the
 // albedo and normal of the frame's own samples (samples_per_pixel samples from sample 0) as guides. The frame is rendered once,
 // in linear f32, and out.png is its quantisation; the AOV pass uploads the scene once more.
+// RTB200_TEMPORAL=<max_history>[,<iterations>[,<color_weight>[,<albedo_weight>[,<normal_weight>]]]], with RTB200_FRAMES only,
+// also writes <prefix>_{i:03}_denoised.png per frame: the AOV pass of the frame's own samples (samples_per_pixel samples from
+// sample 0, the frame's camera and seed), the temporal accumulation of its linear image over the frames before it
+// (rtb200_temporal, DESIGN.md §4.16, without sphere motion: the frames move only the camera; depth_tol is the header's default),
+// then the denoise with the frame's albedo and normal (iterations 0: the accumulated image alone; omitted values are the
+// header's RTB200_DENOISE_DEFAULT_*). The frames are rendered once, in linear f32, and <prefix>_{i:03}.png is each one's
+// quantisation, byte for byte the run's without the variable. Accumulation averages noise only across frames whose seeds
+// differ: a frames file that omits "seed" renders every frame with the scene's seed, and the same noise accumulates.
 #include <chrono>
 #include <cmath>
 #include <cstring>
@@ -34,7 +42,33 @@
 #include "scene_json.hpp"
 
 // RTB200_FRAMES: every frame of frames_path over `s`, written to <prefix>_000.png, <prefix>_001.png, ...
-static int render_animation(const rt_scene& s, const char* frames_path, const std::string& prefix) {
+static int write_temporal(const rt_scene& s, const std::vector<rt_frame>& frames, const rt_options& opts, const float* linear,
+                          const std::vector<std::string>& files, uint32_t max_history, const rt_denoise_params& dp);
+
+// RTB200_TEMPORAL: the parameters of `spec` (101 and a message when it is malformed)
+static int parse_temporal(const rt_scene& s, const char* spec, uint32_t* max_history, rt_denoise_params* p) {
+    double v[5] = {0.0, RTB200_DENOISE_DEFAULT_ITERATIONS, RTB200_DENOISE_DEFAULT_COLOR_WEIGHT, RTB200_DENOISE_DEFAULT_ALBEDO_WEIGHT,
+                   RTB200_DENOISE_DEFAULT_NORMAL_WEIGHT};
+    int k = 0;
+    for (const char* c = spec; k < 5; ++k) {
+        char* end = nullptr;
+        v[k] = strtod(c, &end);
+        if (end == c || (*end != ',' && *end != 0)) {
+            fprintf(stderr, "RTB200_TEMPORAL: expected <max_history>[,<iterations>[,<color_weight>[,<albedo_weight>[,<normal_weight>]]]], got \"%s\"\n", spec);
+            return 101;
+        }
+        if (*end == 0) break;
+        c = end + 1;
+    }
+    if (!(v[0] >= 1 && v[0] <= 4294967295.0 && v[0] == std::floor(v[0]))) { fprintf(stderr, "RTB200_TEMPORAL: max_history must be an integer >= 1\n"); return 101; }
+    if (!(v[1] >= 0 && v[1] <= 10 && v[1] == std::floor(v[1]))) { fprintf(stderr, "RTB200_TEMPORAL: iterations must be an integer in [0, 10]\n"); return 101; }
+    if ((uint64_t)s.width * s.height >= (1ull << 31)) { fprintf(stderr, "RTB200_TEMPORAL: the frame must have fewer than 2^31 pixels\n"); return 101; }
+    *max_history = (uint32_t)v[0];
+    *p = rt_denoise_params{s.width, s.height, (uint32_t)v[1], 0u, (float)v[2], (float)v[3], (float)v[4], 0.0f};
+    return 0;
+}
+
+static int render_animation(const rt_scene& s, const char* frames_path, const std::string& prefix, const char* temporal) {
     if (getenv("RTB200_GPUS")) { fprintf(stderr, "RTB200_FRAMES with RTB200_GPUS is not supported: animations render on one GPU\n"); return 101; }
     std::ifstream f(frames_path, std::ios::binary);
     if (!f) { fprintf(stderr, "Unable to read frames file.: %s\n", frames_path); return 101; }
@@ -50,13 +84,22 @@ static int render_animation(const rt_scene& s, const char* frames_path, const st
         printf("\nRendering %s\n", files[i].c_str());
     }
     fflush(stdout);
+    uint32_t max_history = 0;
+    rt_denoise_params dp{};
+    if (temporal && parse_temporal(s, temporal, &max_history, &dp) != 0) return 101;
     const size_t frame_bytes = (size_t)s.width * s.height * 3;
     std::vector<uint8_t> pixels(frame_bytes * frames.size());
+    std::vector<float> linear(temporal ? frame_bytes * frames.size() : 0);
     rt_options opts{};
     opts.device = getenv("RTB200_DEVICE") ? atoi(getenv("RTB200_DEVICE")) : -1; opts.rank = 0; opts.world = 1; opts.band_rows = 1;
     rt_stats st{};
     auto t0 = std::chrono::steady_clock::now();
-    int rc = rtb200_render_frames(&s, &opts, frames.data(), (uint32_t)frames.size(), pixels.data(), nullptr, &st);
+    // the accumulation needs the linear frames: one render gives them, and each PNG is its frame's quantisation by the render's
+    // own routine (rtb200_probe_quantise), byte for byte the RGB8 render's
+    int rc = temporal ? rtb200_render_frames(&s, &opts, frames.data(), (uint32_t)frames.size(), nullptr, linear.data(), &st)
+                      : rtb200_render_frames(&s, &opts, frames.data(), (uint32_t)frames.size(), pixels.data(), nullptr, &st);
+    for (size_t i = 0; rc == 0 && temporal && i < frames.size(); ++i)
+        rc = rtb200_probe_quantise(linear.data() + i * frame_bytes, (uint32_t)frame_bytes, pixels.data() + i * frame_bytes);
     if (rc != 0) { fprintf(stderr, "render failed (%d): %s\n", rc, rtb200_last_error()); return 101; }
     long long ms = std::chrono::duration_cast<std::chrono::milliseconds>(std::chrono::steady_clock::now() - t0).count();
     printf("Frames time: %lldms for %zu frames\n", ms, frames.size());
@@ -67,6 +110,46 @@ static int render_animation(const rt_scene& s, const char* frames_path, const st
         std::string err;
         if (!rthost::write_png_rgb8(files[i].c_str(), pixels.data() + i * frame_bytes, s.width, s.height, &err)) { fprintf(stderr, "error writing image: %s\n", err.c_str()); return 101; }
     }
+    return temporal ? write_temporal(s, frames, opts, linear.data(), files, max_history, dp) : 0;
+}
+
+// RTB200_TEMPORAL: frame i's AOVs, its accumulation over frames 0 .. i (the history ping-pongs between two buffers) and its
+// denoise, written to <prefix>_{i:03}_denoised.png
+static int write_temporal(const rt_scene& s, const std::vector<rt_frame>& frames, const rt_options& opts, const float* linear,
+                          const std::vector<std::string>& files, uint32_t max_history, const rt_denoise_params& dp) {
+    const size_t npix = (size_t)s.width * s.height;
+    std::vector<float> albedo(npix * 3), normal(npix * 3), color[2] = {std::vector<float>(npix * 3), std::vector<float>(npix * 3)};
+    std::vector<uint32_t> sphere[2] = {std::vector<uint32_t>(npix), std::vector<uint32_t>(npix)}, length[2] = {std::vector<uint32_t>(npix), std::vector<uint32_t>(npix)};
+    std::vector<double> point[2] = {std::vector<double>(npix * 3), std::vector<double>(npix * 3)};
+    std::vector<uint8_t> rgb8(npix * 3);
+    rtb200_scene_handle h = nullptr;
+    int rc = rtb200_scene_upload(&s, &opts, &h);
+    for (size_t i = 0, k = 0; rc == 0 && i < frames.size(); ++i, k ^= 1) {
+        const rt_aov_params ap{s.samples_per_pixel, 0u, {0u, 0u}};
+        const rt_aov_out ao{albedo.data(), normal.data(), nullptr, sphere[k].data(), point[k].data()};
+        if ((rc = rtb200_scene_aov(h, &ap, &frames[i], &ao, nullptr)) != 0) break;
+        rt_temporal_params tp{};
+        tp.width = s.width; tp.height = s.height; tp.max_history = max_history; tp.n_motion = 0;
+        tp.camera = frames[i].camera;
+        if (i > 0) tp.prev_camera = frames[i - 1].camera;
+        tp.depth_tol = RTB200_TEMPORAL_DEFAULT_DEPTH_TOL;
+        const rt_temporal_frame cur{linear + i * npix * 3, sphere[k].data(), point[k].data()};
+        const rt_temporal_history prev{color[k ^ 1].data(), length[k ^ 1].data(), sphere[k ^ 1].data(), point[k ^ 1].data()};
+        const rt_temporal_out out{color[k].data(), length[k].data()};
+        if ((rc = rtb200_temporal(opts.device, &tp, &cur, i > 0 ? &prev : nullptr, nullptr, &out, nullptr)) != 0) break;
+        rc = dp.iterations ? rtb200_denoise(opts.device, &dp, color[k].data(), albedo.data(), normal.data(), nullptr, rgb8.data(), nullptr)
+                           : rtb200_probe_quantise(color[k].data(), (uint32_t)(npix * 3), rgb8.data());
+        if (rc != 0) break;
+        const std::string path = files[i].substr(0, files[i].size() - 4) + "_denoised.png";
+        std::string err;
+        if (!rthost::write_png_rgb8(path.c_str(), rgb8.data(), s.width, s.height, &err)) {
+            fprintf(stderr, "error writing image: %s\n", err.c_str());
+            if (h) rtb200_scene_release(h);
+            return 101;
+        }
+    }
+    if (h) rtb200_scene_release(h);
+    if (rc != 0) { fprintf(stderr, "temporal accumulation failed (%d): %s\n", rc, rtb200_last_error()); return 101; }
     return 0;
 }
 
@@ -193,6 +276,12 @@ int main(int argc, char** argv) {
         rthost::load_scene_json(ss.str(), slash == std::string::npos ? std::string(".") : path.substr(0, slash), &holder);
     } catch (const std::exception& e) { fprintf(stderr, "Unable to parse config json: %s\n", e.what()); return 101; }   // main.rs:15
     if (const char* sd = getenv("RTB200_SEED")) holder.scene.seed = strtoull(sd, nullptr, 0);
+    const char* temporal = getenv("RTB200_TEMPORAL");
+    if (temporal && (!getenv("RTB200_FRAMES") || getenv("RTB200_GPUS") || getenv("RTB200_ADAPTIVE") || getenv("RTB200_AOV") || getenv("RTB200_DENOISE"))) {
+        fprintf(stderr, "RTB200_TEMPORAL needs RTB200_FRAMES, without RTB200_GPUS, RTB200_ADAPTIVE, RTB200_AOV or RTB200_DENOISE: it accumulates "
+                        "the frames of one animation on one GPU and denoises them itself\n");
+        return 101;
+    }
     const char* adaptive = getenv("RTB200_ADAPTIVE");
     if (adaptive && (getenv("RTB200_GPUS") || getenv("RTB200_FRAMES"))) {
         fprintf(stderr, "RTB200_ADAPTIVE with RTB200_GPUS or RTB200_FRAMES is not supported: adaptive renders are one frame on one GPU\n");
@@ -210,7 +299,7 @@ int main(int argc, char** argv) {
     }
     rt_denoise_params denoise_p{};
     if (denoise && parse_denoise(holder.scene, denoise, &denoise_p) != 0) return 101;
-    if (const char* fp = getenv("RTB200_FRAMES")) return render_animation(holder.scene, fp, argv[2]);
+    if (const char* fp = getenv("RTB200_FRAMES")) return render_animation(holder.scene, fp, argv[2], temporal);
     printf("\nRendering %s\n", argv[2]);                                  // main.rs:18
     fflush(stdout);
     const rt_scene& s = holder.scene;

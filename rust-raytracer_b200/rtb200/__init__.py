@@ -146,12 +146,33 @@ class rt_denoise_params(C.Structure):
                 ("color_weight", C.c_float), ("albedo_weight", C.c_float), ("normal_weight", C.c_float), ("reserved2", C.c_float)]
 
 
+class rt_temporal_params(C.Structure):
+    """The temporal accumulation of rtb200_temporal[_device]: image size, max_history N >= 1, the rows of motion, this frame's
+    and the previous frame's cameras, and the finite, non-negative relative depth tolerance."""
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("max_history", C.c_uint32), ("n_motion", C.c_uint32),
+                ("camera", rt_camera), ("prev_camera", rt_camera), ("depth_tol", C.c_double), ("reserved", C.c_uint32 * 2)]
+
+
+class rt_temporal_frame(C.Structure):
+    _fields_ = [("color", C.c_void_p), ("sphere", C.c_void_p), ("point", C.c_void_p)]
+
+
+class rt_temporal_history(C.Structure):
+    _fields_ = [("color", C.c_void_p), ("length", C.c_void_p), ("sphere", C.c_void_p), ("point", C.c_void_p)]
+
+
+class rt_temporal_out(C.Structure):
+    _fields_ = [("color", C.c_void_p), ("length", C.c_void_p)]
+
+
 HIT_FIELDS = (("t", 1, np.float64), ("sphere", 1, np.int32), ("point", 3, np.float64), ("normal", 3, np.float64),
               ("uv", 2, np.float64), ("front_face", 1, np.uint8))   # rt_hits: name, values per ray, dtype (sphere -1 = 0xffffffff)
 
 assert C.sizeof(rt_sphere) == 64 and C.sizeof(rt_frame) == 112 and C.sizeof(rt_adaptive_params) == 24
 assert C.sizeof(rt_rays) == 24 and C.sizeof(rt_hits) == 48 and C.sizeof(rt_trace_params) == 32
 assert C.sizeof(rt_aov_params) == 16 and C.sizeof(rt_aov_out) == 40 and C.sizeof(rt_denoise_params) == 32
+assert C.sizeof(rt_temporal_params) == 224 and C.sizeof(rt_temporal_frame) == 24 and C.sizeof(rt_temporal_history) == 32
+assert C.sizeof(rt_temporal_out) == 16
 AOV_FIELDS = (("albedo", 3, np.float32), ("normal", 3, np.float32), ("hits", 1, np.uint32), ("sphere", 1, np.int32),
               ("point", 3, np.float64))   # rt_aov_out: name, values per pixel, dtype (sphere -1 = 0xffffffff)
 
@@ -173,6 +194,7 @@ ABI_SYMBOLS = [
     "rtb200_scene_edit_spheres",
     "rtb200_scene_aov_device", "rtb200_scene_aov",
     "rtb200_denoise_scratch_bytes", "rtb200_denoise_device", "rtb200_denoise",
+    "rtb200_temporal_device", "rtb200_temporal",
 ]
 
 _lib = None
@@ -248,6 +270,10 @@ def lib() -> C.CDLL:
                                         C.c_void_p, C.c_void_p, C.c_void_p]
     L.rtb200_denoise.argtypes = [C.c_int32, C.POINTER(rt_denoise_params), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.POINTER(rt_stats)]
+    L.rtb200_temporal_device.argtypes = [C.c_int32, C.POINTER(rt_temporal_params), C.POINTER(rt_temporal_frame),
+                                         C.POINTER(rt_temporal_history), C.c_void_p, C.POINTER(rt_temporal_out), C.c_void_p]
+    L.rtb200_temporal.argtypes = [C.c_int32, C.POINTER(rt_temporal_params), C.POINTER(rt_temporal_frame), C.POINTER(rt_temporal_history),
+                                  C.c_void_p, C.POINTER(rt_temporal_out), C.POINTER(rt_stats)]
     _lib = L
     return L
 
@@ -951,6 +977,21 @@ class ResidentScene:
             pass
 
 
+def _call_stream(stream, device, what: str, buffers: str):
+    """The torch stream and the cudaStream_t handle a device-form call on `device` runs on: `stream` (a torch.cuda.Stream, a
+    nonzero handle, CUDA_STREAM_LEGACY for torch's default stream) or by default torch's current stream. The library's own
+    stream (0) is refused: torch could not order the reuse of `buffers` it allocates for the call after the call."""
+    import torch
+    if stream is None:
+        stream = torch.cuda.current_stream(device)
+    elif not isinstance(stream, torch.cuda.Stream):
+        if int(stream) == 0:
+            raise ValueError(f"{what} on CUDA tensors takes a torch stream or a nonzero cudaStream_t: the library's own stream "
+                             f"(0) cannot order the reuse of {buffers} torch allocates")
+        stream = torch.cuda.default_stream(device) if int(stream) == CUDA_STREAM_LEGACY else torch.cuda.ExternalStream(int(stream), device=device)
+    return stream, stream.cuda_stream or CUDA_STREAM_LEGACY
+
+
 # the denoise's defaults, include/rtb200.h's RTB200_DENOISE_DEFAULT_* (DESIGN.md §4.15: chosen on the oracle's 2-spp cover render at
 # 64x48 with its AOV guides)
 DENOISE_ITERATIONS, DENOISE_COLOR_WEIGHT, DENOISE_ALBEDO_WEIGHT, DENOISE_NORMAL_WEIGHT = 3, 16.0, 4.0, 1.0
@@ -1001,14 +1042,7 @@ def denoise(color, albedo=None, normal=None, *, iterations: int = DENOISE_ITERAT
         return out
     import torch
     device = color.device
-    if stream is None:
-        stream = torch.cuda.current_stream(device)
-    elif not isinstance(stream, torch.cuda.Stream):
-        if int(stream) == 0:
-            raise ValueError("denoise on CUDA tensors takes a torch stream or a nonzero cudaStream_t: the library's own stream "
-                             "(0) cannot order the reuse of the scratch torch allocates")
-        stream = torch.cuda.default_stream(device) if int(stream) == CUDA_STREAM_LEGACY else torch.cuda.ExternalStream(int(stream), device=device)
-    handle = stream.cuda_stream or CUDA_STREAM_LEGACY
+    stream, handle = _call_stream(stream, device, "denoise", "the scratch")
     # the scratch and the outputs belong to the call's stream: the caching allocator reuses the scratch, freed when this
     # function returns, only for later work on that stream, which runs after the call
     with torch.cuda.stream(stream):
@@ -1020,6 +1054,158 @@ def denoise(color, albedo=None, normal=None, *, iterations: int = DENOISE_ITERAT
     _check(lib().rtb200_denoise_device(device.index, C.byref(p), ptr(color), ptr(albedo), ptr(normal), ptr(scratch),
                                        ptr(out.get("linear")), ptr(out.get("rgb8")), C.c_void_p(handle)))
     return out
+
+
+# the temporal accumulation's defaults, include/rtb200.h's RTB200_TEMPORAL_DEFAULT_* (DESIGN.md §4.16: chosen on an orbit of the
+# oracle's 2-spp cover render at 64x48)
+TEMPORAL_MAX_HISTORY, TEMPORAL_DEPTH_TOL = 2, 0.03
+
+
+def _camera_of(c) -> rt_camera:
+    """An rt_camera, or the camera of an rt_frame."""
+    c = c.camera if isinstance(c, rt_frame) else c
+    if not isinstance(c, rt_camera):
+        raise ValueError(f"a camera is an rt_camera or an rt_frame, got {type(c).__name__}")
+    return c
+
+
+def temporal(color, sphere, point, camera, prev: Optional[dict] = None, *, motion=None, max_history: int = TEMPORAL_MAX_HISTORY,
+             depth_tol: float = TEMPORAL_DEPTH_TOL, stream=None) -> dict:
+    """Accumulate a frame over time (include/rtb200.h, rtb200_temporal[_device]): each pixel of `color` ([h, w, 3] float32,
+    normally a render's linear mean) is reprojected into the previous frame through its first hit (`sphere` [h, w] int32 or
+    uint32 with -1 / 0xffffffff for a miss, `point` [h, w, 3] float64: :meth:`ResidentScene.aov`'s, of the same camera) and
+    blended with the history there where it shows the same surface. `camera` is this frame's rt_camera (or rt_frame).
+    `prev` is None for the first frame, else a dict of the previous call's "color" and "length" and the previous frame's
+    "sphere", "point" and "camera". `motion` ([n, 3] float64, may be None) is the displacement of sphere j since the previous
+    frame; spheres j >= n did not move.
+
+    numpy arrays use the blocking host form (rtb200_temporal) and the result also holds "stats". CUDA tensors (contiguous, on one
+    device) use the device form (rtb200_temporal_device) on `stream` without waiting, with the stream rules of :func:`denoise`:
+    the outputs are allocated by torch on the call's stream, and handle 0 is refused. Returns {"color": float32 [h, w, 3],
+    "length": uint32 [h, w]}, the new history: pass it back as prev's "color" and "length" with the next frame."""
+    return _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol, stream, None)
+
+
+def _max_history(n) -> int:
+    """max_history as the u32 of rt_temporal_params; a value outside [0, 2^32 - 1] would wrap, and is refused here (0 is the
+    library's refusal)."""
+    n = int(n)
+    if not 0 <= n <= 0xFFFFFFFF:
+        raise ValueError(f"max_history must be an integer in [1, 2^32 - 1], got {n}")
+    return n
+
+
+def _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol, stream, out):
+    """temporal(), writing into `out` ({"color", "length"} CUDA tensors of the right shapes) when it is given."""
+    host = isinstance(color, np.ndarray)
+    shape = tuple(color.shape)
+    if len(shape) != 3 or shape[2] != 3:
+        raise ValueError(f"temporal: color must have shape [h, w, 3], got {shape}")
+    hw = shape[:2]
+    prev = dict(prev) if prev is not None else None
+    if prev is not None and not {"color", "length", "sphere", "point", "camera"} <= set(prev):
+        raise ValueError("temporal: prev holds the previous frame's color, length, sphere, point and camera")
+    args = [("color", color, (np.float32,), shape), ("sphere", sphere, (np.int32, np.uint32), hw), ("point", point, (np.float64,), shape)]
+    if prev is not None:
+        args += [("prev color", prev["color"], (np.float32,), shape), ("prev length", prev["length"], (np.uint32,), hw),
+                 ("prev sphere", prev["sphere"], (np.int32, np.uint32), hw), ("prev point", prev["point"], (np.float64,), shape)]
+    if motion is not None:
+        args.append(("motion", motion, (np.float64,), (int(motion.shape[0]), 3) if len(motion.shape) == 2 else None))
+    if host:
+        for name, a, dts, shp in args:
+            if not (isinstance(a, np.ndarray) and a.dtype in dts and a.flags.c_contiguous and a.shape == shp):
+                raise ValueError(f"temporal takes C-contiguous numpy arrays: {name} must be {'/'.join(np.dtype(d).name for d in dts)} {shp}")
+    else:
+        import torch
+        tdt = {np.float32: torch.float32, np.float64: torch.float64, np.int32: torch.int32, np.uint32: torch.uint32}
+        for name, a, dts, shp in args:
+            if not (isinstance(a, torch.Tensor) and a.is_cuda and a.device == color.device and a.dtype in [tdt[d] for d in dts]
+                    and a.is_contiguous() and tuple(a.shape) == shp):
+                raise ValueError(f"temporal takes contiguous CUDA tensors on one device: {name} must be "
+                                 f"{'/'.join(np.dtype(d).name for d in dts)} {shp}")
+    p = rt_temporal_params(hw[1], hw[0], _max_history(max_history), 0 if motion is None else int(motion.shape[0]), _camera_of(camera),
+                           _camera_of(prev["camera"]) if prev is not None else rt_camera(), float(depth_tol))
+    if host:
+        ptr = lambda a: a.ctypes.data if a is not None else None  # noqa: E731
+    else:
+        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
+    cur = rt_temporal_frame(ptr(color), ptr(sphere), ptr(point))
+    hist = rt_temporal_history(*(ptr(prev[k]) for k in ("color", "length", "sphere", "point"))) if prev is not None else None
+    hp = C.byref(hist) if hist is not None else None
+    if host:
+        out = {"color": np.empty(shape, np.float32), "length": np.empty(hw, np.uint32)}
+        st = rt_stats()
+        _check(lib().rtb200_temporal(-1, C.byref(p), C.byref(cur), hp, ptr(motion), C.byref(rt_temporal_out(ptr(out["color"]), ptr(out["length"]))),
+                                     C.byref(st)))
+        out["stats"] = st.as_dict()
+        return out
+    import torch
+    device = color.device
+    stream, handle = _call_stream(stream, device, "temporal", "the outputs")
+    if out is None:
+        with torch.cuda.stream(stream):
+            out = {"color": torch.empty(shape, dtype=torch.float32, device=device), "length": torch.empty(hw, dtype=torch.uint32, device=device)}
+    if color.numel() == 0:   # a 0-pixel image (the library's no-op)
+        return out
+    _check(lib().rtb200_temporal_device(device.index, C.byref(p), C.byref(cur), hp, ptr(motion),
+                                        C.byref(rt_temporal_out(ptr(out["color"]), ptr(out["length"]))), C.c_void_p(handle)))
+    return out
+
+
+class TemporalDenoiser:
+    """An animation's low-sample frames made stable and clean on the GPU: each :meth:`push` accumulates the frame over time
+    (:func:`temporal`) and denoises the result (:func:`denoise`, guided by the frame's albedo and normal). It owns two history
+    buffers, which its pushes ping-pong between, and copies of the previous frame's sphere and point, on the device;
+    :meth:`reset` forgets the history (after an edit that renumbers spheres, or a cut)."""
+
+    def __init__(self, *, max_history: int = TEMPORAL_MAX_HISTORY, depth_tol: float = TEMPORAL_DEPTH_TOL,
+                 iterations: int = DENOISE_ITERATIONS, color_weight: float = DENOISE_COLOR_WEIGHT,
+                 albedo_weight: float = DENOISE_ALBEDO_WEIGHT, normal_weight: float = DENOISE_NORMAL_WEIGHT):
+        self.max_history, self.depth_tol = _max_history(max_history), float(depth_tol)
+        if self.max_history < 1:
+            raise ValueError("max_history must be >= 1")
+        self.denoise_kw = dict(iterations=iterations, color_weight=color_weight, albedo_weight=albedo_weight, normal_weight=normal_weight)
+        self._hist = None      # two {"color", "length"} buffers; push k writes _hist[k % 2] and reads the other as the history
+        self._k = 0
+        self._sphere = self._point = self._camera = self._stream = None
+        self._has_prev = False
+
+    def reset(self):
+        self._has_prev = False
+
+    def push(self, linear, aov: dict, camera, motion=None, stream=None) -> dict:
+        """One frame: `linear` [h, w, 3] float32 CUDA tensor, `aov` the frame's :meth:`ResidentScene.aov` on the device with
+        albedo, normal, sphere and point, `camera` its rt_camera or rt_frame, `motion` the spheres' displacement since the
+        previous push. Runs on `stream` (by default torch's current stream) after the previous push, on whichever stream it ran.
+        Returns {"color": the accumulated image, "length": its history lengths, "denoised": the accumulated image denoised}.
+        "color" and "length" are the denoiser's own history buffer: the next push reads it as its history and the push after
+        that overwrites it, so do not write to them, and clone them to keep them."""
+        import torch
+        stream, _ = _call_stream(stream, linear.device, "TemporalDenoiser.push", "the history")
+        shape = tuple(linear.shape)
+        hw = shape[:2]
+        if self._stream is not None and self._stream != stream:
+            stream.wait_stream(self._stream)   # the previous push's reads and writes of the buffers come first
+        if self._hist is None or tuple(self._hist[0]["color"].shape) != shape or self._hist[0]["color"].device != linear.device:
+            with torch.cuda.stream(stream):
+                self._hist = [{"color": torch.empty(shape, dtype=torch.float32, device=linear.device),
+                               "length": torch.empty(hw, dtype=torch.uint32, device=linear.device)} for _ in range(2)]
+                self._sphere = torch.empty(hw, dtype=torch.int32, device=linear.device)
+                self._point = torch.empty(shape, dtype=torch.float64, device=linear.device)
+            self._has_prev = False
+        out = self._hist[self._k]
+        prev = None
+        if self._has_prev:
+            h = self._hist[self._k ^ 1]
+            prev = {"color": h["color"], "length": h["length"], "sphere": self._sphere, "point": self._point, "camera": self._camera}
+        _temporal(linear, aov["sphere"], aov["point"], camera, prev, motion, self.max_history, self.depth_tol, stream, out)
+        with torch.cuda.stream(stream):   # the next push's previous frame, after this push has read the current one
+            self._sphere.view(aov["sphere"].dtype).copy_(aov["sphere"])
+            self._point.copy_(aov["point"])
+        self._camera = rt_camera.from_buffer_copy(_camera_of(camera))
+        self._has_prev, self._k, self._stream = True, self._k ^ 1, stream
+        den = denoise(out["color"], aov["albedo"], aov["normal"], stream=stream, **self.denoise_kw)
+        return {"color": out["color"], "length": out["length"], "denoised": den["linear"]}
 
 
 def write_png(path: str, rgb8: np.ndarray):

@@ -225,6 +225,47 @@ int rtb200_render_frames(const rt_scene* scene, const rt_options* opts, const rt
 int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, uint32_t n_frames,
                                 void* dev_rgb8, void* dev_linear_f32, void* stream, rt_stats* stats);
 
+/* ---- depth of field: a thin-lens camera (DESIGN.md §4.17) ---------------------------------------------------------------
+ * The reference's camera is a pinhole. This is the lens of Ray Tracing in One Weekend's camera (random_in_unit_disk), with this
+ * library's own contract; every f64 operation is rounded to nearest, never contracted, and runs in the order written.
+ * Camera: rtb200_camera_from_params_lens takes p, aperture >= 0 and focus_dist fd > 0 (both finite), computes half_height,
+ * half_width, w, u and v as rtb200_camera_from_params (Camera::new, camera.rs:52-58), then
+ *     origin = look_from    lower_left_corner = ((origin - u*(half_width*fd)) - v*(half_height*fd)) - w*fd
+ *     horizontal = ((u*2.0)*half_width)*fd    vertical = ((v*2.0)*half_height)*fd    lens = {u, v, radius = aperture / 2}.
+ * At fd = 1.0 every product by fd is exact: the camera is rtb200_camera_from_params' bit for bit.
+ * Lens draws, a separate RNG domain: trial k = 0, 1, .. of sample (pixel, sample) reads Philox block (k, sample, pixel, 1) under
+ * the frame's key (the path's draws are blocks (b, sample, pixel, 0)); x = gen_range(-1.0..1.0) of the u64 (w1 << 32) | w0 and
+ * y of (w3 << 32) | w2 (the mapping of rtb200_probe_rng kind 1). The first trial with x*x + y*y < 1.0 is accepted; the loop is
+ * unbounded, like random_in_unit_sphere. The two jitter draws and every path draw therefore stay where the pinhole render has
+ * them, and a lens render equals rtb200_scene_trace_rays of its own lens primary rays, sample by sample.
+ * Ray: (o0, d0) = Camera::get_ray(camera, u, v) of the pixel's jittered (u, v) (raytracer.rs:199-201); with radius r > 0
+ *     rdx = r*x   rdy = r*y   offset = lens.u*rdx + lens.v*rdy (per component)   origin = o0 + offset   direction = d0 - offset.
+ * With r == 0 no lens block is drawn and the ray is (o0, d0): a pinhole render is bit for bit today's. */
+typedef struct {
+    rt_vec3  u, v;        /* the camera's unit right and up vectors */
+    double   radius;      /* aperture / 2; 0 = pinhole */
+    uint64_t reserved;    /* must be 0 */
+} rt_lens;                /* 64 bytes */
+
+/* RT_ERR_INVALID for a NULL p / out / lens, a negative or non-finite aperture, or a focus_dist that is not finite and > 0. */
+int rtb200_camera_from_params_lens(const rt_camera_params* p, double aperture, double focus_dist, rt_camera* out, rt_lens* lens);
+/* The lens of a resident scene (NULL or radius 0: pinhole, as uploaded). Host-side handle state, copied: it applies to every call
+ * enqueued after this returns that makes camera rays from a view without its own lens - rtb200_render_device[_async],
+ * rtb200_render_frames[_device] (every frame), the adaptive rounds and rtb200_scene_aov[_device] with or without a view.
+ * rtb200_scene_trace_rays and the queries take the caller's rays and ignore it. It counts as an update for adaptive rendering
+ * (rtb200_adaptive_step refuses until the next begin); updates, rebuilds and edits keep it. RT_ERR_INVALID for a NULL handle,
+ * a non-finite u, v or radius, a negative radius or a nonzero reserved (the handle's lens is then unchanged). */
+int rtb200_scene_set_lens(rtb200_scene_handle h, const rt_lens* lens);
+/* rtb200_render_frames[_device] with a lens per frame: frame i is rendered with lenses[i] (radius 0: pinhole) instead of the
+ * handle's lens. The lens table of the frames that share a launch is a separate device array, uploaded on `stream` and counted in
+ * h2d_bytes. lenses == NULL: exactly rtb200_render_frames[_device]. The host form with n_frames = 1 is the one-shot render of a
+ * lens camera. RT_ERR_INVALID, before any device is touched, for a lens that rtb200_scene_set_lens would refuse, and for every
+ * reason rtb200_render_frames[_device] refuses. rtb200_render_rgb8_multi takes no lens. */
+int rtb200_render_frames_lens(const rt_scene* scene, const rt_options* opts, const rt_frame* frames, const rt_lens* lenses,
+                              uint32_t n_frames, uint8_t* out_rgb8, float* out_linear_f32, rt_stats* stats);
+int rtb200_render_frames_lens_device(rtb200_scene_handle h, const rt_frame* frames, const rt_lens* lenses, uint32_t n_frames,
+                                     void* dev_rgb8, void* dev_linear_f32, void* stream, rt_stats* stats);
+
 /* ---- moving spheres of a resident scene ---------------------------------------------------------------------------------
  * The hierarchy is refitted on the GPU (its topology and recentring stay as uploaded, DESIGN.md §4.7) instead of rebuilt.
  * Contract: after an update every render of h is bit-identical, in linear f32, RGB8 and ray count, to the same render of a
@@ -593,6 +634,10 @@ int rtb200_probe_refract(const rt_vec3* uv, const rt_vec3* n, double etai_over_e
 int rtb200_probe_reflectance(double cosine, double ref_idx, double* out);
 int rtb200_probe_sky(const rt_vec3* dir, uint32_t sky_mode, float out_rgb[3]);
 int rtb200_probe_get_ray(const rt_camera* cam, double u, double v, rt_vec3* origin, rt_vec3* dir);
+/* The lens ray of (pixel, sample) under `seed` at the jittered (u, v) (DESIGN.md §4.17), by the kernel's own lens routine;
+ * *trials (may be NULL) = lens trials drawn (0 for a pinhole lens). lens NULL: pinhole. Same lens checks as rtb200_scene_set_lens. */
+int rtb200_probe_lens_ray(const rt_camera* cam, const rt_lens* lens, uint64_t seed, uint32_t pixel, uint32_t sample, double u,
+                          double v, rt_vec3* origin, rt_vec3* dir, uint32_t* trials);
 /* n uniform draws of the per-(pixel,sample) stream: kind 0 = gen::<f64>() in [0,1), 1 = gen_range(-1.0..1.0) */
 int rtb200_probe_rng(uint64_t seed, uint32_t pixel, uint32_t sample, uint32_t kind, uint32_t n, double* out);
 /* u_v_from_sphere_hit_point (sphere.rs:35-43) of n vectors hp = hit point - centre (3 doubles each); out = n {u, v} pairs */

@@ -5,15 +5,16 @@
 // in grid-stride order, so that neighbouring lanes trace neighbouring camera rays. For each sample in order every lane writes
 // its pixel's primary ray into its slot - the render's own, made by primary_ray (rtb200_trace.cuh) - and the warp runs
 // closest_hit<MODE> unchanged; each lane then adds the sample's albedo and normal to its f32 sums in registers. Nothing goes
-// through a sample buffer and no random number is drawn beyond the render's two jitter draws.
+// through a sample buffer and no random number is drawn beyond the render's two jitter draws (and, on a lens handle, the
+// lens draws of primary_ray<true>, in a domain of their own: rt_aov_lens_kernel, DESIGN.md §4.17).
 #include "rtb200_query.cuh"
 
 namespace rtk {
 
 namespace {
 
-template <uint32_t MODE>
-__global__ void __launch_bounds__(kQueryBlock) rt_aov_kernel(const __grid_constant__ AovParams q) {
+template <uint32_t MODE, bool LENS>
+__device__ __forceinline__ void aov_body(const AovParams& q) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = threadIdx.x & 31;
     const uint32_t warp = threadIdx.x >> 5;
@@ -35,7 +36,7 @@ __global__ void __launch_bounds__(kQueryBlock) rt_aov_kernel(const __grid_consta
             D3 o = mk(0, 0, 0), d = mk(0, 0, 0);
             if (alive) {
                 Rng rng;
-                primary_ray(q.p, q.p.cam, q.p.key0, q.p.key1, x, y_local, q.sample0, k, rng, o, d);
+                primary_ray<LENS>(q.p, q.p.cam, q.p.lens, q.p.key0, q.p.key1, x, y_local, q.sample0, k, rng, o, d);
                 P.ox[lane] = o.x; P.oy[lane] = o.y; P.oz[lane] = o.z; P.dx[lane] = d.x; P.dy[lane] = d.y; P.dz[lane] = d.z;
                 P.src[lane] = kNoSphere;   // a camera ray starts on no sphere
                 ++st.samples;
@@ -84,8 +85,19 @@ __global__ void __launch_bounds__(kQueryBlock) rt_aov_kernel(const __grid_consta
     if (q.p.stat) flush_stats(q.p, st, lane);
 }
 
+template <uint32_t MODE>
+__global__ void __launch_bounds__(kQueryBlock) rt_aov_kernel(const __grid_constant__ AovParams q) { aov_body<MODE, false>(q); }
+// the camera rays through the handle's lens, q.p.lens (its radius is not 0)
+template <uint32_t MODE>
+__global__ void __launch_bounds__(kQueryBlock) rt_aov_lens_kernel(const __grid_constant__ AovParams q) { aov_body<MODE, true>(q); }
+
 template <typename F>
-static auto dispatch_aov(uint32_t mode, F&& f) {
+static auto dispatch_aov(uint32_t mode, bool lens, F&& f) {
+    if (lens) {
+        if (mode == MODE_EXACT) return f(rt_aov_lens_kernel<MODE_EXACT>);
+        if (mode == MODE_BRUTE) return f(rt_aov_lens_kernel<MODE_BRUTE>);
+        return f(rt_aov_lens_kernel<MODE_TREE>);
+    }
     if (mode == MODE_EXACT) return f(rt_aov_kernel<MODE_EXACT>);
     if (mode == MODE_BRUTE) return f(rt_aov_kernel<MODE_BRUTE>);
     return f(rt_aov_kernel<MODE_TREE>);
@@ -93,12 +105,12 @@ static auto dispatch_aov(uint32_t mode, F&& f) {
 
 }  // namespace
 
-int aov_max_ctas_per_sm(uint32_t mode) {
-    return dispatch_aov(mode, [&](auto kern) { return query_ctas_per_sm(kern, query_smem_bytes(mode)); });
+int aov_max_ctas_per_sm(uint32_t mode, bool lens) {
+    return dispatch_aov(mode, lens, [&](auto kern) { return query_ctas_per_sm(kern, query_smem_bytes(mode)); });
 }
 
 cudaError_t launch_aov(const AovParams& q, uint32_t mode, int max_grid, cudaStream_t st) {
-    return dispatch_aov(mode, [&](auto kern) { return query_launch(kern, query_smem_bytes(mode), q, max_grid, st); });
+    return dispatch_aov(mode, q.p.lens.radius != 0.0, [&](auto kern) { return query_launch(kern, query_smem_bytes(mode), q, max_grid, st); });
 }
 
 }  // namespace rtk

@@ -122,6 +122,50 @@ int rtb200_camera_from_params(const rt_camera_params* p, rt_camera* out) {
     return RT_OK;
 }
 
+// The thin-lens camera (include/rtb200.h, DESIGN.md §4.17): Camera::new's basis, then the image plane at focus_dist.
+int rtb200_camera_from_params_lens(const rt_camera_params* p, double aperture, double focus_dist, rt_camera* out, rt_lens* lens) {
+    if (!p || !out || !lens) return fail(RT_ERR_INVALID, "null argument");
+    if (!std::isfinite(aperture) || aperture < 0.0) return fail(RT_ERR_INVALID, "aperture must be finite and >= 0");
+    if (!std::isfinite(focus_dist) || !(focus_dist > 0.0)) return fail(RT_ERR_INVALID, "focus_dist must be finite and > 0");
+    const double PI = 3.14159265358979323846264338327950288, fd = focus_dist;
+    double theta = p->vfov_deg * (PI / 180.0);
+    double half_height = std::tan(theta / 2.0);
+    double half_width = p->aspect * half_height;
+    V3 look_from = v3(p->look_from), look_at = v3(p->look_at), vup = v3(p->vup);
+    V3 w = vunit(look_from - look_at);
+    V3 u = vunit(vcross(vup, w));
+    V3 v = vcross(w, u);
+    V3 origin = look_from;
+    V3 llc = origin - (u * (half_width * fd)) - (v * (half_height * fd)) - w * fd;
+    V3 horizontal = u * 2.0 * half_width * fd;
+    V3 vertical = v * 2.0 * half_height * fd;
+    out->origin = rv(origin); out->lower_left_corner = rv(llc); out->horizontal = rv(horizontal); out->vertical = rv(vertical);
+    *lens = rt_lens{rv(u), rv(v), aperture / 2.0, 0};
+    return RT_OK;
+}
+
+int rtk::check_lens(const rt_lens& L, const char* what) {
+    const double f[7] = {L.u.x, L.u.y, L.u.z, L.v.x, L.v.y, L.v.z, L.radius};
+    for (double x : f) if (!std::isfinite(x)) return fail(RT_ERR_INVALID, std::string(what) + ": u, v and radius must be finite");
+    if (L.radius < 0.0) return fail(RT_ERR_INVALID, std::string(what) + ": radius must be >= 0");
+    if (L.reserved != 0) return fail(RT_ERR_INVALID, std::string(what) + ": reserved must be 0");
+    return RT_OK;
+}
+
+int rtb200_scene_set_lens(rtb200_scene_handle h, const rt_lens* lens) {
+  return guarded([&]() -> int {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    const rt_lens L = lens ? *lens : rt_lens{};
+    int rc = check_lens(L, "lens");
+    if (rc != RT_OK) return rc;
+    HANDLE_PROLOGUE(h);
+    if (L.radius == 0.0) h->tp.lens = rt_lens{};   // one pinhole: the lens of a fresh upload
+    else h->tp.lens = L;
+    ++h->updates;   // an adaptive render's sums would mix two cameras
+    return RT_OK;
+  });
+}
+
 uint32_t rtb200_shard_rows(uint32_t height, int32_t rank, int32_t world, uint32_t band_rows) {
     if (world <= 1) return height;
     if (band_rows == 0) band_rows = 1;
@@ -515,6 +559,24 @@ int rtb200_probe_get_ray(const rt_camera* cam, double u, double v, rt_vec3* orig
     });
     if (rc != RT_OK) return rc;
     *origin = rt_vec3{out[0], out[1], out[2]}; *dir = rt_vec3{out[3], out[4], out[5]};
+    return RT_OK;
+}
+int rtb200_probe_lens_ray(const rt_camera* cam, const rt_lens* lens, uint64_t seed, uint32_t pixel, uint32_t sample, double u,
+                          double v, rt_vec3* origin, rt_vec3* dir, uint32_t* trials) {
+    if (!cam || !origin || !dir) return fail(RT_ERR_INVALID, "null argument");
+    struct { rt_camera cam; rt_lens lens; double uv[2]; } in;
+    in.cam = *cam; in.lens = lens ? *lens : rt_lens{}; in.uv[0] = u; in.uv[1] = v;
+    int rc = check_lens(in.lens, "lens");
+    if (rc != RT_OK) return rc;
+    double out[7];
+    rc = probe_run(&in, sizeof in, out, sizeof out, [&](void* din, void* dout, cudaStream_t st) {
+        char* b = (char*)din;
+        return probe_lens_ray((const rt_camera*)b, (const rt_lens*)(b + sizeof(rt_camera)), (const double*)(b + sizeof(rt_camera) + sizeof(rt_lens)),
+                              seed, pixel, sample, (double*)dout, st);
+    });
+    if (rc != RT_OK) return rc;
+    *origin = rt_vec3{out[0], out[1], out[2]}; *dir = rt_vec3{out[3], out[4], out[5]};
+    if (trials) *trials = (uint32_t)out[6];
     return RT_OK;
 }
 int rtb200_probe_rng(uint64_t seed, uint32_t pixel, uint32_t sample, uint32_t kind, uint32_t n, double* o) {

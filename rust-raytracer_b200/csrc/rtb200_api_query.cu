@@ -234,8 +234,9 @@ static int check_aov(rtb200_scene_handle h, const rt_aov_params* p, const rt_fra
 // has ordered after the scene's last writer (scene_stream). Guard trips go to err[1], the counters to stat (null: not counted).
 static int aov_enqueue(rtb200_scene_handle h, const rt_aov_params& prm, const rt_frame* view, const AovOut& out,
                        unsigned long long* stat, unsigned long long* err, cudaStream_t st) {
-    int& occ = h->ctx->query_occ[2][h->mode];
-    if (occ == 0) occ = aov_max_ctas_per_sm(h->mode);
+    const bool lens = h->tp.lens.radius != 0.0;   // the handle's lens (rtb200_scene_set_lens)
+    int& occ = h->ctx->query_occ[lens ? 3 : 2][h->mode];
+    if (occ == 0) occ = aov_max_ctas_per_sm(h->mode, lens);
     if (occ <= 0) { occ = 0; return fail(RT_ERR_UNSUPPORTED, "no launch configuration of the aov kernel fits shared memory"); }
     AovParams q{};
     q.p = h->tp; q.p.stat = stat; q.p.err = err;

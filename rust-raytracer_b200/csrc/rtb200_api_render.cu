@@ -18,7 +18,7 @@ int rtk::launch_geometry(rtb200_scene_handle h, uint32_t queue, bool lights, Lau
     static const char* const kernel[4] = {"", " of the multi-frame trace kernel", " of the list trace kernel", " of the rays trace kernel"};
     g->smem = wavefront_smem_bytes(h->tp, h->mode, h->tp.scene_in_smem, queue);
     g->ctas_per_sm = occupancy(h->ctx, h->mode, lights, queue, g->smem);
-    if (g->ctas_per_sm <= 0) return fail(RT_ERR_UNSUPPORTED, std::string("no launch configuration") + kernel[queue] + " fits shared memory");
+    if (g->ctas_per_sm <= 0) return fail(RT_ERR_UNSUPPORTED, std::string("no launch configuration") + kernel[base_queue(queue)] + " fits shared memory");
     g->grid = h->ctx->sm_count * g->ctas_per_sm;
     return RT_OK;
 }
@@ -77,10 +77,10 @@ static int submission_open(rtb200_scene_handle h, void* stream_in, uint32_t fram
 
 // The opened submission s in `batches` batches, whose widest trace launch has `grid` CTAs, for paths up to max_depth deep that
 // stage up to samplebuf_bytes of samples; points tp at the set's buffers. The multi-frame kernel reads each frame's camera and
-// key from the n_ftab records of `ftab`, copied here because the copy has to come after the wait for the set's last user
-// and before the stat block is cleared.
+// key from the n_ftab records of `ftab` (and, when ltab is not null, its lens from n_ftab lenses of `ltab`), copied here
+// because the copy has to come after the wait for the set's last user and before the stat block is cleared.
 static int submission_begin(rtb200_scene_handle h, int set, uint32_t batches, int grid, TraceParams& tp, uint32_t max_depth,
-                            size_t samplebuf_bytes, const FrameRec* ftab, uint32_t n_ftab, Submit* s) {
+                            size_t samplebuf_bytes, const FrameRec* ftab, uint32_t n_ftab, Submit* s, const rt_lens* ltab = nullptr) {
     DeviceCtx* ctx = h->ctx;
     DeviceCtx::WorkSet& W = ctx->ws[set];
     rtb200_scene_t::Submission& sub = s->sub;
@@ -96,6 +96,12 @@ static int submission_begin(rtb200_scene_handle h, int set, uint32_t batches, in
         sub.ftab_bytes = (uint64_t)n_ftab * sizeof(FrameRec);
         CU(W.ftab.ensure(sub.ftab_bytes, W.done));
         CU(cudaMemcpyAsync(W.ftab.p, ftab, sub.ftab_bytes, cudaMemcpyHostToDevice, st));
+        if (ltab) {
+            const uint64_t lbytes = (uint64_t)n_ftab * sizeof(rt_lens);
+            CU(W.ltab.ensure(lbytes, W.done));
+            CU(cudaMemcpyAsync(W.ltab.p, ltab, lbytes, cudaMemcpyHostToDevice, st));
+            sub.ftab_bytes += lbytes;
+        }
     }
     sub.n_ev = 2 + 2 * batches;
     while (h->ev.size() < (size_t)sub.ev0 + sub.n_ev) {
@@ -157,14 +163,19 @@ static std::vector<FrameGroup> frame_groups(const rt_frame* frames, uint32_t n, 
     return groups;
 }
 
-// rt_frame checks shared by both frames entry points (no device is touched)
-static int check_frames(const rt_frame* frames, uint32_t n, uint64_t rows, uint64_t width) {
+// rt_frame checks (and of the per-frame lenses, when not null) shared by the frames entry points (no device is touched)
+static int check_frames(const rt_frame* frames, uint32_t n, uint64_t rows, uint64_t width, const rt_lens* lenses = nullptr) {
     if (n == 0) return fail(RT_ERR_INVALID, "n_frames must be > 0");
     if (!frames) return fail(RT_ERR_INVALID, "frames is null");
     const uint64_t per_frame = rows * width * 3ull;   // < 2^33: width * height < 2^31 (validate_scene)
     if (per_frame != 0 && (uint64_t)n > ~0ull / per_frame) return fail(RT_ERR_INVALID, "n_frames * rows * width * 3 overflows 64 bits");
     for (uint32_t i = 0; i < n; ++i)
         if (frames[i].reserved != 0) return fail(RT_ERR_INVALID, "rt_frame.reserved must be 0 (frame " + std::to_string(i) + ")");
+    if (lenses)
+        for (uint32_t i = 0; i < n; ++i) {
+            const int rc = check_lens(lenses[i], ("lens of frame " + std::to_string(i)).c_str());
+            if (rc != RT_OK) return rc;
+        }
     return RT_OK;
 }
 
@@ -173,9 +184,11 @@ static rt_frame own_frame(rtb200_scene_handle h) { return rt_frame{h->tp.cam, h-
 
 // Enqueue frames[0, n) of h on `stream_in` (NULL: the context's stream) with work set `set`, without waiting, and append the
 // submission to h->pending; the caller holds the context's lock and has made h's device current. Frame i goes to output
-// slice i (rows * width * 3 elements).
+// slice i (rows * width * 3 elements). Frame i's lens is lenses[i], or the handle's (h->tp.lens) when lenses is null. When no
+// frame has a lens the launches are the pinhole ones; else every group, one frame or many, runs the multi-frame kernel with
+// the lens (Q_FRAMES_LENS), which reads each frame's camera, key and lens from the frame and lens tables.
 static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_t n, void* dev_rgb8, void* dev_linear_f32,
-                          void* stream_in, int set) {
+                          void* stream_in, int set, const rt_lens* lenses = nullptr) {
     Submit s;
     int rc = submission_open(h, stream_in, n, &s);
     if (rc != RT_OK) return rc;
@@ -189,6 +202,14 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
     // it only when 2 * spp * npl * 16 bytes fit the cap and 2 * spp * npl < 2^31, and with these samples_per_batch gave
     // spp_batch == spp.
     auto batches_of = [&](const FrameGroup& g) { return g.count > 1 ? 1u : n_batches; };
+    std::vector<rt_lens> ltab;   // each frame's lens, when one of them has a lens
+    for (uint32_t i = 0; i < n && ltab.empty(); ++i)
+        if ((lenses ? lenses[i] : tp.lens).radius != 0.0) ltab.resize(n);
+    for (uint32_t i = 0; i < ltab.size(); ++i) {
+        const rt_lens& L = lenses ? lenses[i] : tp.lens;
+        ltab[i] = L.radius != 0.0 ? L : rt_lens{};
+    }
+    const bool lensed = !ltab.empty();
 
     // trace launches, work buffer sizes and the launch geometry of the multi-frame kernel (its pool also holds the slots' frames)
     const LaunchGeom single{h->smem, h->ctas_per_sm, h->grid};
@@ -199,32 +220,39 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
         all_batches += batches_of(g);   // trace launches (or black memsets)
         sbuf = std::max(sbuf, (size_t)g.count * spb * npl * 16);
         max_depth = std::max(max_depth, frames[g.first].max_depth);
-        if (g.count > 1 && multi.grid == 0 && (rc = launch_geometry(h, Q_FRAMES, tp.n_lights > 0, &multi)) != RT_OK) return rc;
+        if ((g.count > 1 || lensed) && multi.grid == 0 && (rc = launch_geometry(h, lensed ? Q_FRAMES_LENS : Q_FRAMES, tp.n_lights > 0, &multi)) != RT_OK)
+            return rc;
     }
     std::vector<FrameRec> tab(multi.grid ? n : 0);
     for (uint32_t i = 0; i < tab.size(); ++i) {
         tab[i].cam = frames[i].camera; tab[i].key0 = (uint32_t)frames[i].seed; tab[i].key1 = (uint32_t)(frames[i].seed >> 32);
     }
     if ((rc = submission_begin(h, set, all_batches, std::max(h->grid, multi.grid), tp, max_depth, sbuf, tab.data(),
-                               (uint32_t)tab.size(), &s)) != RT_OK)
+                               (uint32_t)tab.size(), &s, lensed ? ltab.data() : nullptr)) != RT_OK)
         return rc;
 
     uint32_t b = 0;   // trace launch (or black memset) index: its queue counter and its event pair
     for (const FrameGroup& g : groups) {
         const rt_frame& f0 = frames[g.first];
-        const bool is_multi = g.count > 1;   // the multi-frame trace kernel, which reads each frame's camera and key from ftab
+        const bool is_multi = g.count > 1 || lensed;   // the multi-frame trace kernel, which reads each frame's camera and key from ftab
         const uint32_t batches = batches_of(g);
         uint8_t* o8 = dev_rgb8 ? (uint8_t*)dev_rgb8 + (size_t)g.first * npl * 3 : nullptr;
         float* ol = dev_linear_f32 ? (float*)dev_linear_f32 + (size_t)g.first * npl * 3 : nullptr;
         TraceParams q = tp;
         q.max_depth = f0.max_depth;
-        if (is_multi) { q.ftab = (const FrameRec*)s.W->ftab.p + g.first; q.frame_work = (uint32_t)frame_work; }
-        else { q.cam = f0.camera; q.key0 = (uint32_t)f0.seed; q.key1 = (uint32_t)(f0.seed >> 32); }
+        if (is_multi) {
+            q.ftab = (const FrameRec*)s.W->ftab.p + g.first;
+            if (lensed) q.ltab = (const rt_lens*)s.W->ltab.p + g.first;
+        } else {
+            q.cam = f0.camera; q.key0 = (uint32_t)f0.seed; q.key1 = (uint32_t)(f0.seed >> 32);
+        }
         for (uint32_t k = 0; k < batches; ++k, ++b) {
             q.s0 = k * spb;
             q.s_count = std::min(spb, spp - q.s0);
             q.total_work = g.count * q.s_count * q.npix_local;
-            if ((rc = trace_step(h, s, b, q, is_multi ? Q_FRAMES : Q_SINGLE, is_multi ? multi : single, (size_t)q.total_work * 16)) != RT_OK) return rc;
+            if (is_multi) q.frame_work = q.s_count * q.npix_local;   // frame_work of a group of several frames (one batch of spp)
+            const uint32_t queue = !is_multi ? Q_SINGLE : lensed ? Q_FRAMES_LENS : Q_FRAMES;
+            if ((rc = trace_step(h, s, b, q, queue, is_multi ? multi : single, (size_t)q.total_work * 16)) != RT_OK) return rc;
             for (uint32_t j = 0; j < g.count; ++j) {   // samplebuf [frame][sample][pixel]
                 ResolveParams r{};
                 r.samplebuf = q.samplebuf + (size_t)j * q.s_count * npl; r.accum = (float*)s.W->accum.p; r.npix_local = q.npix_local;
@@ -309,9 +337,9 @@ static int blocking(rtb200_scene_handle h, rt_stats* stats, Enqueue&& enqueue) {
 }
 
 static int render_blocking(rtb200_scene_handle h, const rt_frame* frames, uint32_t n, void* dev_rgb8, void* dev_linear_f32,
-                           void* stream_in, rt_stats* stats) {
+                           void* stream_in, rt_stats* stats, const rt_lens* lenses = nullptr) {
     HANDLE_PROLOGUE(h);
-    return blocking(h, stats, [&] { return render_enqueue(h, frames, n, dev_rgb8, dev_linear_f32, stream_in, 0); });
+    return blocking(h, stats, [&] { return render_enqueue(h, frames, n, dev_rgb8, dev_linear_f32, stream_in, 0, lenses); });
 }
 
 // Releases a scene handle on scope exit; the error that made the scope return early survives the release.
@@ -353,16 +381,16 @@ static int one_shot(const rt_scene* s, const rt_options& opts, uint64_t frames, 
 
 // Host buffers: render `frames` of s. The single-frame calls pass the scene's own view as one frame.
 static int render_host(const rt_scene* s, const rt_options* opts_in, const rt_frame* frames, uint32_t n_frames, uint8_t* out_rgb8,
-                       float* out_lin, rt_stats* stats) {
+                       float* out_lin, rt_stats* stats, const rt_lens* lenses = nullptr) {
     rt_options opts;
     int rc = normalise_options(opts_in, &opts);
     if (rc != RT_OK) return rc;
     uint32_t n_lights = 0;
     if ((rc = validate_scene(s, &n_lights)) != RT_OK) return rc;
-    if ((rc = check_frames(frames, n_frames, rtb200_shard_rows(s->height, opts.rank, opts.world, opts.band_rows), s->width)) != RT_OK) return rc;
+    if ((rc = check_frames(frames, n_frames, rtb200_shard_rows(s->height, opts.rank, opts.world, opts.band_rows), s->width, lenses)) != RT_OK) return rc;
     void* const out[3] = {out_rgb8, out_lin, nullptr};
     return one_shot(s, opts, n_frames, out, 128 + 16, stats, [&](rtb200_scene_handle h, void* const* dev, rt_stats* st) {
-        return render_blocking(h, frames, n_frames, dev[0], dev[1], nullptr, st);
+        return render_blocking(h, frames, n_frames, dev[0], dev[1], nullptr, st, lenses);
     });
 }
 
@@ -400,6 +428,17 @@ int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, u
   });
 }
 
+int rtb200_render_frames_lens_device(rtb200_scene_handle h, const rt_frame* frames, const rt_lens* lenses, uint32_t n_frames,
+                                     void* dev_rgb8, void* dev_linear_f32, void* stream_in, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    int rc = check_frames(frames, n_frames, h->tp.rows_local, h->tp.width, lenses);
+    if (rc != RT_OK) return rc;
+    if (!dev_rgb8 && !dev_linear_f32) return fail(RT_ERR_INVALID, "dev_rgb8 and dev_linear_f32 are both null");
+    return render_blocking(h, frames, n_frames, dev_rgb8, dev_linear_f32, stream_in, stats, lenses);
+  });
+}
+
 int rtb200_render_rgb8(const rt_scene* scene, const rt_options* opts, uint8_t* out_rgb8, rt_stats* stats) {
     if (!scene || !out_rgb8) return fail(RT_ERR_INVALID, "null argument");
     const rt_frame f{scene->camera, scene->seed, scene->max_depth, 0};
@@ -417,6 +456,15 @@ int rtb200_render_frames(const rt_scene* s, const rt_options* opts_in, const rt_
     if (!s) return fail(RT_ERR_INVALID, "null argument");
     if (!out_rgb8 && !out_lin) return fail(RT_ERR_INVALID, "out_rgb8 and out_linear_f32 are both null");
     return render_host(s, opts_in, frames, n_frames, out_rgb8, out_lin, stats);
+  });
+}
+
+int rtb200_render_frames_lens(const rt_scene* s, const rt_options* opts_in, const rt_frame* frames, const rt_lens* lenses,
+                              uint32_t n_frames, uint8_t* out_rgb8, float* out_lin, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (!s) return fail(RT_ERR_INVALID, "null argument");
+    if (!out_rgb8 && !out_lin) return fail(RT_ERR_INVALID, "out_rgb8 and out_linear_f32 are both null");
+    return render_host(s, opts_in, frames, n_frames, out_rgb8, out_lin, stats, lenses);
   });
 }
 
@@ -611,7 +659,8 @@ int rtb200_adaptive_step(rtb200_scene_handle h, uint32_t rounds, void* stream_in
         TraceParams tp = h->tp;
         const uint32_t npl = tp.npix_local;
         LaunchGeom g;
-        if ((rcs = launch_geometry(h, Q_LIST, tp.n_lights > 0, &g)) != RT_OK) return rcs;
+        const uint32_t queue = tp.lens.radius != 0.0 ? Q_LIST_LENS : Q_LIST;   // the handle's lens (rtb200_scene_set_lens)
+        if ((rcs = launch_geometry(h, queue, tp.n_lights > 0, &g)) != RT_OK) return rcs;
         if ((rcs = submission_begin(h, 0, rounds, g.grid, tp, tp.max_depth, (size_t)m * npl * 16, nullptr, 0, &s)) != RT_OK) return rcs;
         const bool black = tp.max_depth == 0;
         A.begun = false;   // until the rounds are enqueued: a step that fails part-way leaves the state unusable
@@ -621,7 +670,7 @@ int rtb200_adaptive_step(rtb200_scene_handle h, uint32_t rounds, void* stream_in
             q.s_count = std::min(m, A.N - A.n);
             q.total_work = 0;   // Q_LIST: n_list * s_count, n_list read on the device
             q.list = A.list[A.cur]; q.list_n = A.list_n + A.cur;
-            if ((rcs = trace_step(h, s, r, q, Q_LIST, g, (size_t)q.s_count * npl * 16)) != RT_OK) return rcs;
+            if ((rcs = trace_step(h, s, r, q, queue, g, (size_t)q.s_count * npl * 16)) != RT_OK) return rcs;
             AdaptiveParams a{};
             a.samplebuf = q.samplebuf; a.list = q.list; a.list_n = q.list_n;
             a.sum = A.sum; a.sq = A.sq; a.count = A.count; a.keep = A.keep;

@@ -116,6 +116,36 @@ RT_DEV bool random_in_unit_sphere_ilp(Rng& g, uint32_t k0, uint32_t k1, D3& out)
     return false;
 }
 
+// ---- the thin lens (DESIGN.md §4.17) --------------------------------------------------------------
+// The lens disk of sample (pixel, sample): trial k reads Philox block (k, sample, pixel, 1) - counter word 1, a domain of its
+// own, so the path's stream is untouched - x from its first u64, y from its second, both gen_range(-1.0..1.0); the first
+// trial with x*x + y*y < 1 is accepted. Two trials per loop trip, their blocks computed together (as random_in_unit_sphere_ilp).
+// Returns the trials drawn (k + 1 of the accepted one).
+RT_DEV uint32_t lens_disk(uint32_t pixel, uint32_t sample, uint32_t k0, uint32_t k1, double& x, double& y) {
+#pragma unroll 1
+    for (uint32_t k = 0;; k += 2u) {
+        uint32_t A[4], B[4];
+        philox4x32_10(k, sample, pixel, 1u, k0, k1, A);
+        philox4x32_10(k + 1u, sample, pixel, 1u, k0, k1, B);
+        const double x1 = u64_to_m1_1(A[0], A[1]), y1 = u64_to_m1_1(A[2], A[3]);
+        const double x2 = u64_to_m1_1(B[0], B[1]), y2 = u64_to_m1_1(B[2], B[3]);
+        if (__dadd_rn(__dmul_rn(x1, x1), __dmul_rn(y1, y1)) < 1.0) { x = x1; y = y1; return k + 1u; }
+        if (__dadd_rn(__dmul_rn(x2, x2), __dmul_rn(y2, y2)) < 1.0) { x = x2; y = y2; return k + 2u; }
+    }
+}
+// The pinhole ray (o, d) of (pixel, sample) moved onto the lens `L` of radius > 0: o + offset, d - offset with
+// offset = L.u * (r x) + L.v * (r y). Out of line: it runs only for a lens camera, and inlined into the trace kernel's
+// regeneration it would hold its registers across every path of a pinhole render too. Returns the trials drawn.
+RT_DEV uint32_t lens_apply(const rt_lens& L, uint32_t pixel, uint32_t sample, uint32_t k0, uint32_t k1, D3& o, D3& d) {
+    double x, y;
+    const uint32_t trials = lens_disk(pixel, sample, k0, k1, x, y);
+    const double rdx = __dmul_rn(L.radius, x), rdy = __dmul_rn(L.radius, y);
+    const D3 off = add(mul(from(L.u), rdx), mul(from(L.v), rdy));
+    o = add(o, off);
+    d = sub(d, off);
+    return trials;
+}
+
 // ---- Camera::get_ray (camera.rs:79-84) -------------------------------------------------------------
 RT_DEV void get_ray(const rt_camera& c, double u, double v, D3& origin, D3& dir) {
     origin = from(c.origin);

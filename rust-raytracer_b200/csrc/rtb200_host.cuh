@@ -90,7 +90,7 @@ struct DeviceCtx {
     // submission's stream; the next submission's stream waits for it, so submissions that share a set run one after the other
     // whatever their streams and handles.
     struct WorkSet {
-        GrowBuf samplebuf, accum, stack, small, frames, lterm, ftab;   // ftab: the multi-frame kernel's frame table
+        GrowBuf samplebuf, accum, stack, small, frames, lterm, ftab, ltab;   // ftab / ltab: the multi-frame kernel's frame and lens tables
         cudaEvent_t done = nullptr;
     } ws[2];
     GrowBuf out_rgb8, out_lin, out_cnt, probe, frame;
@@ -107,7 +107,7 @@ struct DeviceCtx {
     // each kind and mode (0: not asked yet)
     GrowBuf query;
     cudaEvent_t query_ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    int query_occ[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}};   // [closest-hit, occlusion, auxiliary buffers][mode]
+    int query_occ[4][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}};   // [closest-hit, occlusion, auxiliary buffers, lens ones][mode]
 };
 // the context of a device ordinal below 64, created at its first use
 int get_ctx(int device, DeviceCtx** out);
@@ -228,6 +228,8 @@ inline uint64_t sample_buffer_cap(const rt_options& o) { return o.sample_buffer_
 // bytes) holds, and fewer than 2^31 work ids in a batch.
 uint32_t samples_per_batch(uint64_t cap, uint64_t items, uint32_t samples);
 int normalise_options(const rt_options* opts_in, rt_options* o);
+// RT_ERR_INVALID (message prefixed by `what`) unless the lens's u, v and radius are finite, radius >= 0 and reserved is 0
+int check_lens(const rt_lens& L, const char* what);
 int validate_scene(const rt_scene* s, uint32_t* n_lights_out);
 uint32_t mode_of(uint32_t variant);
 bool albedo_nonfinite(const rt_sphere& sp);

@@ -79,6 +79,15 @@ __global__ void k_probe_get_ray(const rt_camera* cam, const double* in, double* 
     get_ray(*cam, in[0], in[1], o, d);
     out[0] = o.x; out[1] = o.y; out[2] = o.z; out[3] = d.x; out[4] = d.y; out[5] = d.z;
 }
+// the pinhole ray moved onto the lens, as primary_ray makes it; out[6] = the lens trials drawn
+__global__ void k_probe_lens_ray(const rt_camera* cam, const rt_lens* lens, const double* in, uint32_t k0, uint32_t k1, uint32_t pixel,
+                                 uint32_t sample, double* out) {
+    D3 o, d;
+    get_ray(*cam, in[0], in[1], o, d);
+    uint32_t trials = 0;
+    if (lens->radius != 0.0) trials = lens_apply(*lens, pixel, sample, k0, k1, o, d);
+    out[0] = o.x; out[1] = o.y; out[2] = o.z; out[3] = d.x; out[4] = d.y; out[5] = d.z; out[6] = (double)trials;
+}
 __global__ void k_probe_rng(uint32_t k0, uint32_t k1, uint32_t pixel, uint32_t sample, uint32_t kind, uint32_t n, double* out) {
     Rng g; rng_init(g, pixel, sample);
     for (uint32_t i = 0; i < n; ++i) out[i] = kind == 0 ? rng_f64(g, k0, k1) : rng_m1_1(g, k0, k1);
@@ -102,6 +111,11 @@ cudaError_t probe_refract(const double* in, double* out, cudaStream_t st) { k_pr
 cudaError_t probe_reflectance(const double* in, double* out, cudaStream_t st) { k_probe_reflectance<<<1, 1, 0, st>>>(in, out); return cudaGetLastError(); }
 cudaError_t probe_sky(const double* in, uint32_t mode, float* out, cudaStream_t st) { k_probe_sky<<<1, 1, 0, st>>>(in, mode, out); return cudaGetLastError(); }
 cudaError_t probe_get_ray(const rt_camera* cam, const double* in, double* out, cudaStream_t st) { k_probe_get_ray<<<1, 1, 0, st>>>(cam, in, out); return cudaGetLastError(); }
+cudaError_t probe_lens_ray(const rt_camera* cam, const rt_lens* lens, const double* in, uint64_t seed, uint32_t pixel, uint32_t sample,
+                           double* out, cudaStream_t st) {
+    k_probe_lens_ray<<<1, 1, 0, st>>>(cam, lens, in, (uint32_t)seed, (uint32_t)(seed >> 32), pixel, sample, out);
+    return cudaGetLastError();
+}
 cudaError_t probe_rng(uint64_t seed, uint32_t pixel, uint32_t sample, uint32_t kind, uint32_t n, double* out, cudaStream_t st) {
     k_probe_rng<<<1, 1, 0, st>>>((uint32_t)seed, (uint32_t)(seed >> 32), pixel, sample, kind, n, out);
     return cudaGetLastError();

@@ -57,7 +57,10 @@ enum TraceMode : uint32_t { MODE_TREE = 0, MODE_BRUTE = 1, MODE_EXACT = 2 };
 // The work queue of a trace launch: every pixel of one frame, every pixel of several frames (TraceParams::ftab), the
 // pixels of an adaptive render's list (TraceParams::list, DESIGN.md §4.9), or caller-supplied primary rays
 // (TraceParams::ray_o / ray_d, rtb200_scene_trace_rays, DESIGN.md §4.12)
-enum TraceQueue : uint32_t { Q_SINGLE = 0, Q_FRAMES = 1, Q_LIST = 2, Q_RAYS = 3 };
+// Q_FRAMES_LENS and Q_LIST_LENS are Q_FRAMES and Q_LIST with a thin lens (DESIGN.md §4.17): the lens is a compile-time choice,
+// so that the pinhole kernels carry no lens code.
+enum TraceQueue : uint32_t { Q_SINGLE = 0, Q_FRAMES = 1, Q_LIST = 2, Q_RAYS = 3, Q_FRAMES_LENS = 4, Q_LIST_LENS = 5 };
+__host__ __device__ constexpr uint32_t base_queue(uint32_t q) { return q == Q_FRAMES_LENS ? Q_FRAMES : q == Q_LIST_LENS ? Q_LIST : q; }
 
 // One frame of a multi-frame launch (rt_wavefront_kernel<.., Q_FRAMES>): the view and the Philox key that replace
 // TraceParams::cam / key0 / key1 for the work ids of that frame.
@@ -123,6 +126,9 @@ struct TraceParams {
         const uint32_t* list_n;  // Q_LIST: device: n_list, read once at kernel start; total_work = n_list * s_count
         const double* ray_d;     // Q_RAYS: [n][3] ray directions
     };
+    // ---- the thin lens (DESIGN.md §4.17), appended after the Q_LIST fields ----
+    rt_lens lens;                // the handle's lens (radius 0: pinhole); read by Q_LIST_LENS and the lens AOV kernel only
+    const rt_lens* ltab;         // Q_FRAMES_LENS: [frames of the launch] each frame's lens (radius 0: pinhole)
 };
 
 // An adaptive round's accumulate-and-test (rtb200_adaptive.cu, DESIGN.md §4.9): one thread per list position.
@@ -282,8 +288,8 @@ int query_max_ctas_per_sm(uint32_t mode, bool any);
 cudaError_t launch_query(const QueryParams& q, uint32_t mode, int max_grid, cudaStream_t st);
 cudaError_t launch_occluded(const OcclusionParams& q, uint32_t mode, int max_grid, cudaStream_t st);
 // the auxiliary buffers: resident CTAs per SM of the kernel of `mode` (0 when it cannot run on the current device), and a launch
-// of at most `max_grid` CTAs
-int aov_max_ctas_per_sm(uint32_t mode);
+// of at most `max_grid` CTAs (through the lens kernel when q.p.lens.radius is not 0)
+int aov_max_ctas_per_sm(uint32_t mode, bool lens);   // lens: the kernel whose camera rays go through p.lens
 cudaError_t launch_aov(const AovParams& q, uint32_t mode, int max_grid, cudaStream_t st);
 // adaptive rendering (rtb200_adaptive.cu): the round's accumulate-and-test, the list compaction (cub::DeviceSelect::Flagged,
 // keep[0, npix_local) over list_in, the count to *list_n_out), and the resolve
@@ -332,6 +338,8 @@ cudaError_t probe_refract(const double* in /*7*/, double* out /*3*/, cudaStream_
 cudaError_t probe_reflectance(const double* in /*2*/, double* out /*1*/, cudaStream_t st);
 cudaError_t probe_sky(const double* in /*3*/, uint32_t mode, float* out /*3*/, cudaStream_t st);
 cudaError_t probe_get_ray(const rt_camera* cam_dev, const double* in /*2*/, double* out /*6*/, cudaStream_t st);
+cudaError_t probe_lens_ray(const rt_camera* cam_dev, const rt_lens* lens_dev, const double* in /*2*/, uint64_t seed, uint32_t pixel,
+                           uint32_t sample, double* out /*7*/, cudaStream_t st);
 cudaError_t probe_rng(uint64_t seed, uint32_t pixel, uint32_t sample, uint32_t kind, uint32_t n, double* out, cudaStream_t st);
 cudaError_t probe_quantise(const float* in, uint32_t n, uint8_t* out, cudaStream_t st);
 cudaError_t probe_sphere_uv(const double* in /*3n*/, uint32_t n, double* out /*2n*/, cudaStream_t st);

@@ -503,12 +503,15 @@ RT_DEV uint32_t closest_hit(const TraceParams& p, const SceneRefs& sc, const Poo
 // =====================================================================================================================
 // The render's primary ray of local pixel (x, y_local) of the launch's rows and sample s0 + s_local, under camera `cam` and the
 // Philox key (k0, k1): the pixel's image row (row band y_local / band_rows is the shard's, raytracer.rs:254-262), the two
-// jitter draws of raytracer.rs:199-200 from the stream of (pixel, sample), then Camera::get_ray (camera.rs:79-84). `rng` is
-// left after the two draws. The trace kernel (regenerate_slot) and the auxiliary buffers (rtb200_aov.cu) both make their
-// camera rays here.
+// jitter draws of raytracer.rs:199-200 from the stream of (pixel, sample), then Camera::get_ray (camera.rs:79-84), moved onto
+// the lens `lens` when LENS and its radius is not 0 (lens_apply, whose draws are a domain of their own, DESIGN.md §4.17). `rng`
+// is left after the two draws. The trace kernel (regenerate_slot) and the auxiliary buffers (rtb200_aov.cu) both make their
+// camera rays here. The lens is a compile-time choice of the launch: a pinhole launch (LENS false) carries no lens code, so the
+// kernels of pinhole renders are the ones they were before the lens existed.
 // =====================================================================================================================
-RT_DEV void primary_ray(const TraceParams& p, const rt_camera& cam, uint32_t k0, uint32_t k1, uint32_t x, uint32_t y_local,
-                        uint32_t s0, uint32_t s_local, Rng& rng, D3& o, D3& d) {
+template <bool LENS = false>
+RT_DEV void primary_ray(const TraceParams& p, const rt_camera& cam, const rt_lens& lens, uint32_t k0, uint32_t k1, uint32_t x,
+                        uint32_t y_local, uint32_t s0, uint32_t s_local, Rng& rng, D3& o, D3& d) {
     const uint32_t band_rows = p.band_rows, width = p.width, height = p.height;
     uint32_t band = y_local / band_rows;
     uint32_t y = (band * (uint32_t)p.world + (uint32_t)p.rank) * band_rows + (y_local - band * band_rows);
@@ -518,6 +521,9 @@ RT_DEV void primary_ray(const TraceParams& p, const rt_camera& cam, uint32_t k0,
     double xi2 = rng_f64(rng, k0, k1);
     double v = __ddiv_rn(__dsub_rn((double)height, __dadd_rn((double)y, xi2)), __dsub_rn((double)height, 1.0));
     get_ray(cam, u, v, o, d);
+    if constexpr (LENS) {
+        if (lens.radius != 0.0) lens_apply(lens, rng.pixel, rng.sample, k0, k1, o, d);
+    }
 }
 
 // =====================================================================================================================
@@ -530,8 +536,9 @@ RT_DEV void primary_ray(const TraceParams& p, const rt_camera& cam, uint32_t k0,
 // §4.9); n_list is read from p.list_n once per launch by the caller.
 // Q_RAYS: the queue spans samples [s0, s0 + s_count) of the n = p.npix_local caller-supplied rays p.ray_o / p.ray_d (DESIGN.md
 // §4.12); the slot gets the ray itself instead of a camera ray.
+// LENS (FRAMES or Q_LIST only): the camera rays go through the lens, a frame's from p.ltab, an adaptive round's p.lens.
 // =====================================================================================================================
-template <bool LIGHTS, uint32_t QUEUE>
+template <bool LIGHTS, uint32_t QUEUE, bool LENS = false>
 RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint32_t s, int lane, bool& exhausted, Stats& st,
                             uint32_t n_list = 0u) {
     constexpr bool FRAMES = QUEUE == Q_FRAMES;
@@ -585,8 +592,8 @@ RT_DEV bool regenerate_slot(const TraceParams& p, const Pool& P, bool want, uint
             y_local = p.rows_local - 1u - rr;
             lp = y_local * p.width + x;
         }
-        if constexpr (FRAMES) primary_ray(p, p.ftab[f].cam, k0, k1, x, y_local, p.s0, s_local, rng, o, d);
-        else primary_ray(p, p.cam, k0, k1, x, y_local, p.s0, s_local, rng, o, d);
+        if constexpr (FRAMES) primary_ray<LENS>(p, p.ftab[f].cam, LENS ? p.ltab[f] : p.lens, k0, k1, x, y_local, p.s0, s_local, rng, o, d);
+        else primary_ray<LENS>(p, p.cam, p.lens, k0, k1, x, y_local, p.s0, s_local, rng, o, d);
     }
     P.ox[s] = o.x; P.oy[s] = o.y; P.oz[s] = o.z; P.dx[s] = d.x; P.dy[s] = d.y; P.dz[s] = d.z;
     // samplebuf index [sample][pixel], [frame][sample][pixel], [sample][list position] (Q_LIST) or [sample][ray] (Q_RAYS)

@@ -65,7 +65,7 @@ __host__ __device__ constexpr WfSmem wf_layout(uint32_t n, uint32_t n_pairs, uin
 }  // namespace
 
 size_t wavefront_smem_bytes(const TraceParams& p, uint32_t mode, uint32_t smem_mask, uint32_t queue) {
-    return wf_layout(p.n, p.n_pairs, p.n_nodes, p.n_leaves, mode, smem_mask, queue == Q_FRAMES).total;
+    return wf_layout(p.n, p.n_pairs, p.n_nodes, p.n_leaves, mode, smem_mask, base_queue(queue) == Q_FRAMES).total;
 }
 
 // CTAs per SM each kernel's register budget is built for: 3 of 256 threads for the BVH path (80 registers), 2 for the
@@ -111,8 +111,11 @@ static cudaError_t set_carveout(K kern, uint32_t mode, size_t smem) {
 // Q_FRAMES: one launch renders several frames of the scene (TraceParams::ftab / frame_work, rtb200_render_frames)
 // Q_LIST: one launch traces a round of an adaptive render (TraceParams::list / list_n, rtb200_adaptive_step)
 // Q_RAYS: one launch traces a batch of samples of caller-supplied rays (TraceParams::ray_o / ray_d, rtb200_scene_trace_rays)
-template <uint32_t MODE, bool LIGHTS, uint32_t QUEUE>
+// Q_FRAMES_LENS / Q_LIST_LENS: Q_FRAMES / Q_LIST whose camera rays go through a thin lens (TraceParams::ltab / lens, DESIGN.md §4.17)
+template <uint32_t MODE, bool LIGHTS, uint32_t QUEUE_>
 __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kernel(const __grid_constant__ TraceParams p) {
+    constexpr uint32_t QUEUE = base_queue(QUEUE_);
+    constexpr bool LENS = QUEUE != QUEUE_;
     constexpr bool FRAMES = QUEUE == Q_FRAMES;
     extern __shared__ __align__(128) unsigned char smem_raw[];
     const WfSmem L = wf_layout(p.n, p.n_pairs, p.n_nodes, p.n_leaves, MODE, p.scene_in_smem, FRAMES);
@@ -163,7 +166,7 @@ __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kern
     uint32_t dry_iters = 0;   // iterations of this CTA after it first found the global queue dry
     uint32_t n_list = 0u;   // Q_LIST: the pixels on the list, fixed for the launch
     if constexpr (QUEUE == Q_LIST) n_list = *p.list_n;
-    regenerate_slot<LIGHTS, QUEUE>(p, P, true, (uint32_t)tid, lane, exhausted, st, n_list);   // initial fill of the pool
+    regenerate_slot<LIGHTS, QUEUE, LENS>(p, P, true, (uint32_t)tid, lane, exhausted, st, n_list);   // initial fill of the pool
     __syncthreads();
 
 #if RT_PHASE_CLOCKS
@@ -224,7 +227,7 @@ __global__ void __launch_bounds__(kBlock, wf_min_blocks(MODE)) rt_wavefront_kern
             if (lane == 0) { ph[PH_ITERS] += 1ull; ph[PH_SCATTERS] += (unsigned)__popc(sm); ph[PH_DEFERRED] += (unsigned)__popc(dm); }
         }
 #endif
-        regenerate_slot<LIGHTS, QUEUE>(p, P, active && done, s, lane, exhausted, st, n_list);
+        regenerate_slot<LIGHTS, QUEUE, LENS>(p, P, active && done, s, lane, exhausted, st, n_list);
         if (exhausted && !stamped) { stamped = true; if (lane == 0) atomicMin(&p.stat[9], now_ns()); }
         if (stamped) ++dry_iters;
         const bool still_alive = active && (P.lvl[s] != kDeadLevel);
@@ -255,6 +258,8 @@ template <typename F>
 static auto dispatch(uint32_t mode, bool lights, uint32_t queue, F&& f) {
     if (queue == Q_RAYS) return dispatch_mode<Q_RAYS>(mode, lights, f);
     if (queue == Q_LIST) return dispatch_mode<Q_LIST>(mode, lights, f);
+    if (queue == Q_FRAMES_LENS) return dispatch_mode<Q_FRAMES_LENS>(mode, lights, f);
+    if (queue == Q_LIST_LENS) return dispatch_mode<Q_LIST_LENS>(mode, lights, f);
     return queue == Q_FRAMES ? dispatch_mode<Q_FRAMES>(mode, lights, f) : dispatch_mode<Q_SINGLE>(mode, lights, f);
 }
 
@@ -284,9 +289,10 @@ cudaError_t wavefront_info(uint32_t mode, bool lights, uint32_t queue, KernelInf
         cudaError_t e = cudaFuncGetAttributes(&a, kern);
         if (e != cudaSuccess) return e;
         out->registers = a.numRegs; out->max_threads = a.maxThreadsPerBlock; out->const_bytes = (int)a.constSizeBytes; out->local_bytes = (int)a.localSizeBytes;
-        snprintf(out->name, sizeof out->name, "rt_wavefront_kernel<%s,%s%s>",
+        const uint32_t bq = base_queue(queue);
+        snprintf(out->name, sizeof out->name, "rt_wavefront_kernel<%s,%s%s%s>",
                  mode == MODE_TREE ? "MODE_TREE" : mode == MODE_BRUTE ? "MODE_BRUTE" : "MODE_EXACT", lights ? "LIGHTS" : "NO_LIGHTS",
-                 queue == Q_FRAMES ? ",FRAMES" : queue == Q_LIST ? ",LIST" : queue == Q_RAYS ? ",RAYS" : "");
+                 bq == Q_FRAMES ? ",FRAMES" : bq == Q_LIST ? ",LIST" : bq == Q_RAYS ? ",RAYS" : "", bq != queue ? ",LENS" : "");
         return cudaSuccess;
     });
 }

@@ -26,6 +26,10 @@
 // header's RTB200_DENOISE_DEFAULT_*). The frames are rendered once, in linear f32, and <prefix>_{i:03}.png is each one's
 // quantisation, byte for byte the run's without the variable. Accumulation averages noise only across frames whose seeds
 // differ: a frames file that omits "seed" renders every frame with the scene's seed, and the same noise accumulates.
+// A camera (of the config or of a frame) may carry "aperture" and "focus_dist": the thin lens of DESIGN.md §4.17 (absent or 0
+// aperture: the reference's pinhole camera; absent focus_dist: |look_from - look_at|, or the scene's for a frame). Plain renders
+// and RTB200_FRAMES render lens cameras (rtb200_render_frames_lens). RTB200_GPUS, RTB200_ADAPTIVE, RTB200_AOV, RTB200_DENOISE
+// and RTB200_TEMPORAL refuse a lens camera with status 101: none of them renders it as a pinhole.
 #include <chrono>
 #include <cmath>
 #include <cstring>
@@ -68,14 +72,34 @@ static int parse_temporal(const rt_scene& s, const char* spec, uint32_t* max_his
     return 0;
 }
 
-static int render_animation(const rt_scene& s, const char* frames_path, const std::string& prefix, const char* temporal) {
+// The camera and lens of `spec` (rtb200_camera_from_params_lens) in place of Camera::new's `cam`; no lens: both unchanged.
+static int apply_lens(const rthost::LensSpec& spec, rt_camera* cam, rt_lens* lens) {
+    *lens = rt_lens{};
+    if (spec.aperture == 0.0) return 0;
+    if (rtb200_camera_from_params_lens(&spec.params, spec.aperture, spec.focus_dist, cam, lens) != 0) {
+        fprintf(stderr, "invalid lens camera: %s\n", rtb200_last_error());
+        return 101;
+    }
+    return 0;
+}
+
+static int render_animation(const rthost::SceneHolder& holder, const char* frames_path, const std::string& prefix, const char* temporal) {
+    const rt_scene& s = holder.scene;
     if (getenv("RTB200_GPUS")) { fprintf(stderr, "RTB200_FRAMES with RTB200_GPUS is not supported: animations render on one GPU\n"); return 101; }
     std::ifstream f(frames_path, std::ios::binary);
     if (!f) { fprintf(stderr, "Unable to read frames file.: %s\n", frames_path); return 101; }
     std::stringstream ss; ss << f.rdbuf();
     std::vector<rt_frame> frames;
-    try { frames = rthost::load_frames_json(ss.str(), s); }
+    std::vector<rthost::LensSpec> specs;
+    try { frames = rthost::load_frames_json(ss.str(), holder, &specs); }
     catch (const std::exception& e) { fprintf(stderr, "Unable to parse frames json: %s\n", e.what()); return 101; }
+    std::vector<rt_lens> lenses(frames.size());
+    bool lensed = false;
+    for (size_t i = 0; i < frames.size(); ++i) {
+        if (apply_lens(specs[i], &frames[i].camera, &lenses[i]) != 0) return 101;
+        lensed = lensed || lenses[i].radius != 0.0;
+    }
+    if (lensed && temporal) { fprintf(stderr, "RTB200_TEMPORAL with a lens camera (aperture > 0) is not supported\n"); return 101; }
     std::vector<std::string> files(frames.size());
     for (size_t i = 0; i < frames.size(); ++i) {
         char num[32];
@@ -97,6 +121,7 @@ static int render_animation(const rt_scene& s, const char* frames_path, const st
     // the accumulation needs the linear frames: one render gives them, and each PNG is its frame's quantisation by the render's
     // own routine (rtb200_probe_quantise), byte for byte the RGB8 render's
     int rc = temporal ? rtb200_render_frames(&s, &opts, frames.data(), (uint32_t)frames.size(), nullptr, linear.data(), &st)
+           : lensed   ? rtb200_render_frames_lens(&s, &opts, frames.data(), lenses.data(), (uint32_t)frames.size(), pixels.data(), nullptr, &st)
                       : rtb200_render_frames(&s, &opts, frames.data(), (uint32_t)frames.size(), pixels.data(), nullptr, &st);
     for (size_t i = 0; rc == 0 && temporal && i < frames.size(); ++i)
         rc = rtb200_probe_quantise(linear.data() + i * frame_bytes, (uint32_t)frame_bytes, pixels.data() + i * frame_bytes);
@@ -297,9 +322,17 @@ int main(int argc, char** argv) {
         fprintf(stderr, "RTB200_DENOISE with RTB200_GPUS, RTB200_FRAMES or RTB200_ADAPTIVE is not supported: it denoises one frame on one GPU\n");
         return 101;
     }
+    rt_lens scene_lens{};
+    if (apply_lens(holder.lens_spec, &holder.scene.camera, &scene_lens) != 0) return 101;
+    const bool lens = scene_lens.radius != 0.0;
+    if (lens && (getenv("RTB200_GPUS") || adaptive || aov || denoise || temporal)) {
+        fprintf(stderr, "a lens camera (aperture > 0) with RTB200_GPUS, RTB200_ADAPTIVE, RTB200_AOV, RTB200_DENOISE or RTB200_TEMPORAL is not "
+                        "supported: render it without them\n");
+        return 101;
+    }
     rt_denoise_params denoise_p{};
     if (denoise && parse_denoise(holder.scene, denoise, &denoise_p) != 0) return 101;
-    if (const char* fp = getenv("RTB200_FRAMES")) return render_animation(holder.scene, fp, argv[2], temporal);
+    if (const char* fp = getenv("RTB200_FRAMES")) return render_animation(holder, fp, argv[2], temporal);
     printf("\nRendering %s\n", argv[2]);                                  // main.rs:18
     fflush(stdout);
     const rt_scene& s = holder.scene;
@@ -320,6 +353,9 @@ int main(int argc, char** argv) {
         linear.resize(pixels.size());
         rc = rtb200_render_linear_f32(&s, &opts, linear.data(), &st);
         if (rc == 0) rc = rtb200_probe_quantise(linear.data(), (uint32_t)linear.size(), pixels.data());
+    } else if (lens) {
+        const rt_frame f{s.camera, s.seed, s.max_depth, 0};   // one frame of the lens camera
+        rc = rtb200_render_frames_lens(&s, &opts, &f, &scene_lens, 1, pixels.data(), nullptr, &st);
     } else {
         rc = gpus ? rtb200_render_rgb8_multi(&s, &opts, atoi(gpus), pixels.data(), &st)   // replaces raytracer.rs:260-262
                   : rtb200_render_rgb8(&s, &opts, pixels.data(), &st);

@@ -28,6 +28,19 @@ uint64_t uint_field(const Json& j, const char* name, double max_value) {
     if (!(v >= 0.0) || v > max_value || v != (double)(uint64_t)v) throw std::runtime_error(std::string(name) + ": non-negative integer expected");
     return (uint64_t)v;
 }
+// |look_from - look_at| (camera.rs:68, the reference's unused focal_length): the focus distance when none is given
+double focal_length(const rt_camera_params& p) {
+    const double dx = p.look_from.x - p.look_at.x, dy = p.look_from.y - p.look_at.y, dz = p.look_from.z - p.look_at.z;
+    return std::sqrt(dx * dx + dy * dy + dz * dz);
+}
+// The lens of a camera: aperture finite and >= 0 (0: none); with a lens, focus_dist (has_focus false: focal_length) finite, > 0
+LensSpec lens_spec(const rt_camera_params& p, double aperture, bool has_focus, double focus_dist, const std::string& what) {
+    if (!std::isfinite(aperture) || aperture < 0.0) throw std::runtime_error(what + ": aperture must be finite and >= 0");
+    LensSpec l{p, aperture, has_focus ? focus_dist : focal_length(p)};
+    if (aperture != 0.0 && !(std::isfinite(l.focus_dist) && l.focus_dist > 0.0))
+        throw std::runtime_error(what + ": focus_dist must be finite and > 0");
+    return l;
+}
 bool load_image(const std::string& path, const std::string& base_dir, Image* img) {
     std::string err;
     if (decode_jpeg_file(path, img, &err)) return true;
@@ -47,7 +60,12 @@ void load_scene_json(const std::string& text, const std::string& base_dir, Scene
     // camera: CameraParams -> Camera::new (camera.rs:29-42)
     const Json& cam = root.at("camera");
     rt_camera_params cp{vec3(cam.at("look_from")), vec3(cam.at("look_at")), vec3(cam.at("vup")), cam.at("vfov").number(), cam.at("aspect").number()};
+    // the optional thin lens (DESIGN.md §4.17): "aperture" (absent or 0: Camera::new, no lens) and "focus_dist"
     if (rtb200_camera_from_params(&cp, &s.camera) != 0) throw std::runtime_error(rtb200_last_error());
+    const Json* ap = cam.find("aperture");
+    const Json* fd = cam.find("focus_dist");
+    out->has_focus = fd != nullptr;
+    out->lens_spec = lens_spec(cp, ap ? ap->number() : 0.0, fd != nullptr, fd ? fd->number() : 0.0, "camera");
     // sky: missing or null -> None (black); {"texture": ""} -> gradient; path -> texture (config.rs:49-64)
     s.sky.mode = RT_SKY_NONE;
     if (const Json* sky = root.find("sky")) {
@@ -96,11 +114,20 @@ void load_scene_json(const std::string& text, const std::string& base_dir, Scene
 }
 
 std::vector<rt_frame> load_frames_json(const std::string& text, const rt_scene& scene) {
+    SceneHolder h;
+    h.scene = scene;
+    std::vector<LensSpec> lenses;
+    return load_frames_json(text, h, &lenses);
+}
+
+std::vector<rt_frame> load_frames_json(const std::string& text, const SceneHolder& holder, std::vector<LensSpec>* lenses) {
+    const rt_scene& scene = holder.scene;
     Json root = JsonParser::parse(text);
     if (root.kind != Json::Arr) throw std::runtime_error("frames: array expected");
     if (root.arr.empty()) throw std::runtime_error("frames: at least one frame expected");
     if (root.arr.size() > 0xffffffffull) throw std::runtime_error("frames: too many frames");
     std::vector<rt_frame> frames(root.arr.size());
+    lenses->assign(root.arr.size(), LensSpec{});
     for (size_t i = 0; i < root.arr.size(); ++i) {
         const Json& f = root.arr[i];
         if (f.kind != Json::Obj) throw std::runtime_error("frame " + std::to_string(i) + ": object expected");
@@ -109,6 +136,10 @@ std::vector<rt_frame> load_frames_json(const std::string& text, const rt_scene& 
         const Json& cam = f.at("camera");   // the config's camera schema (camera.rs:29-36)
         rt_camera_params cp{vec3(cam.at("look_from")), vec3(cam.at("look_at")), vec3(cam.at("vup")), cam.at("vfov").number(), cam.at("aspect").number()};
         if (rtb200_camera_from_params(&cp, &fr.camera) != 0) throw std::runtime_error("frame " + std::to_string(i) + ": invalid camera");
+        const Json* a = cam.find("aperture");
+        const Json* fd = cam.find("focus_dist");
+        (*lenses)[i] = lens_spec(cp, a ? a->number() : holder.lens_spec.aperture, fd || holder.has_focus,
+                                 fd ? fd->number() : holder.lens_spec.focus_dist, "frame " + std::to_string(i) + ": invalid camera");
         const Json* seed = f.find("seed");
         fr.seed = seed ? uint_field(*seed, "seed", 9007199254740992.0) : scene.seed;
         const Json* depth = f.find("max_depth");

@@ -11,6 +11,7 @@ from __future__ import annotations
 
 import ctypes as C
 import json
+import math
 import os
 from typing import Optional, Sequence
 
@@ -102,6 +103,11 @@ class rt_frame(C.Structure):
     _fields_ = [("camera", rt_camera), ("seed", C.c_uint64), ("max_depth", C.c_uint32), ("reserved", C.c_uint32)]
 
 
+class rt_lens(C.Structure):
+    """A thin lens (rtb200_camera_from_params_lens): the camera's unit right and up vectors and radius = aperture / 2 (0: pinhole)."""
+    _fields_ = [("u", rt_vec3), ("v", rt_vec3), ("radius", C.c_double), ("reserved", C.c_uint64)]
+
+
 class rt_adaptive_params(C.Structure):
     """Adaptive rendering (rtb200_adaptive_*): samples per round, the sample budget (0: the scene's samples_per_pixel), the
     samples before a pixel may stop, and the f32 tolerances of the stopping rule err_c <= abs_tol + rel_tol * mean_c."""
@@ -172,7 +178,7 @@ assert C.sizeof(rt_sphere) == 64 and C.sizeof(rt_frame) == 112 and C.sizeof(rt_a
 assert C.sizeof(rt_rays) == 24 and C.sizeof(rt_hits) == 48 and C.sizeof(rt_trace_params) == 32
 assert C.sizeof(rt_aov_params) == 16 and C.sizeof(rt_aov_out) == 40 and C.sizeof(rt_denoise_params) == 32
 assert C.sizeof(rt_temporal_params) == 224 and C.sizeof(rt_temporal_frame) == 24 and C.sizeof(rt_temporal_history) == 32
-assert C.sizeof(rt_temporal_out) == 16
+assert C.sizeof(rt_temporal_out) == 16 and C.sizeof(rt_lens) == 64
 AOV_FIELDS = (("albedo", 3, np.float32), ("normal", 3, np.float32), ("hits", 1, np.uint32), ("sphere", 1, np.int32),
               ("point", 3, np.float64))   # rt_aov_out: name, values per pixel, dtype (sphere -1 = 0xffffffff)
 
@@ -195,6 +201,8 @@ ABI_SYMBOLS = [
     "rtb200_scene_aov_device", "rtb200_scene_aov",
     "rtb200_denoise_scratch_bytes", "rtb200_denoise_device", "rtb200_denoise",
     "rtb200_temporal_device", "rtb200_temporal",
+    "rtb200_camera_from_params_lens", "rtb200_scene_set_lens", "rtb200_render_frames_lens", "rtb200_render_frames_lens_device",
+    "rtb200_probe_lens_ray",
 ]
 
 _lib = None
@@ -274,6 +282,14 @@ def lib() -> C.CDLL:
                                          C.POINTER(rt_temporal_history), C.c_void_p, C.POINTER(rt_temporal_out), C.c_void_p]
     L.rtb200_temporal.argtypes = [C.c_int32, C.POINTER(rt_temporal_params), C.POINTER(rt_temporal_frame), C.POINTER(rt_temporal_history),
                                   C.c_void_p, C.POINTER(rt_temporal_out), C.POINTER(rt_stats)]
+    L.rtb200_camera_from_params_lens.argtypes = [C.POINTER(rt_camera_params), C.c_double, C.c_double, C.POINTER(rt_camera), C.POINTER(rt_lens)]
+    L.rtb200_scene_set_lens.argtypes = [C.c_void_p, C.POINTER(rt_lens)]
+    L.rtb200_render_frames_lens.argtypes = [C.POINTER(rt_scene), C.POINTER(rt_options), C.POINTER(rt_frame), C.POINTER(rt_lens), C.c_uint32,
+                                            C.c_void_p, C.c_void_p, C.POINTER(rt_stats)]
+    L.rtb200_render_frames_lens_device.argtypes = [C.c_void_p, C.POINTER(rt_frame), C.POINTER(rt_lens), C.c_uint32, C.c_void_p, C.c_void_p,
+                                                   C.c_void_p, C.POINTER(rt_stats)]
+    L.rtb200_probe_lens_ray.argtypes = [C.POINTER(rt_camera), C.POINTER(rt_lens), C.c_uint64, C.c_uint32, C.c_uint32, C.c_double, C.c_double,
+                                        C.POINTER(rt_vec3), C.POINTER(rt_vec3), C.POINTER(C.c_uint32)]
     _lib = L
     return L
 
@@ -309,6 +325,49 @@ def camera_from_params(look_from, look_at, vup, vfov: float, aspect: float) -> r
         return out
     _check(lib().rtb200_camera_from_params(C.byref(p), C.byref(out)))
     return out
+
+
+_lens_backend = None   # the lens twin of _camera_backend: fn(rt_camera_params*, double, double, rt_camera*, rt_lens*) -> int
+
+
+def set_lens_backend(fn):
+    """fn(rt_camera_params*, aperture, focus_dist, rt_camera*, rt_lens*) -> int replacing rtb200_camera_from_params_lens (None
+    restores the library), so that CPU-only callers can build lens cameras without mapping librtb200.so."""
+    global _lens_backend
+    _lens_backend = fn
+
+
+def camera_from_params_lens(look_from, look_at, vup, vfov: float, aspect: float, aperture: float, focus_dist: float):
+    """The thin-lens camera (include/rtb200.h, DESIGN.md §4.17): (rt_camera, rt_lens). At focus_dist 1.0 the camera is
+    camera_from_params' bit for bit; aperture 0 gives a lens of radius 0 (a pinhole)."""
+    p = rt_camera_params(vec3(look_from), vec3(look_at), vec3(vup), float(vfov), float(aspect))
+    cam, lens = rt_camera(), rt_lens()
+    fn = _lens_backend if _lens_backend is not None else lib().rtb200_camera_from_params_lens
+    rc = fn(C.byref(p), float(aperture), float(focus_dist), C.byref(cam), C.byref(lens))
+    if rc != 0:
+        if _lens_backend is not None:
+            raise RtError(rc, "camera_from_params_lens: aperture must be finite and >= 0, focus_dist finite and > 0")
+        _check(rc)
+    return cam, lens
+
+
+def focal_length(look_from, look_at) -> float:
+    """|look_from - look_at| (camera.rs:68): a lens camera's focus distance when none is given."""
+    a, b = vec3(look_from), vec3(look_at)
+    d = (a.x - b.x, a.y - b.y, a.z - b.z)
+    return math.sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2])
+
+
+def lens_from_params(p: dict):
+    """(rt_camera, rt_lens or None) of a camera dict with optional "aperture" and "focus_dist" (None: no lens, the camera is
+    camera_from_params'). focus_dist defaults to focal_length(look_from, look_at)."""
+    aperture = float(p.get("aperture") or 0.0)
+    if aperture == 0.0:
+        return camera_from_params(p["look_from"], p["look_at"], p["vup"], p["vfov"], p["aspect"]), None
+    fd = p.get("focus_dist")
+    fd = focal_length(p["look_from"], p["look_at"]) if fd is None else float(fd)
+    cam, lens = camera_from_params_lens(p["look_from"], p["look_at"], p["vup"], p["vfov"], p["aspect"], aperture, fd)
+    return cam, (lens if lens.radius != 0.0 else None)
 
 
 def shard_rows(height: int, rank: int, world: int, band_rows: int = 1) -> int:
@@ -384,6 +443,7 @@ class Scene:
         self._tex_structs = None
         self._sky_array = None
         self.camera_params: Optional[dict] = None
+        self.lens: Optional[rt_lens] = None   # the thin lens of the camera (None: pinhole, DESIGN.md §4.17)
         self.source = None
 
     # -- construction ---------------------------------------------------------------------------------
@@ -395,7 +455,11 @@ class Scene:
         sc.c.samples_per_pixel = int(cfg["samples_per_pixel"]); sc.c.max_depth = int(cfg["max_depth"])
         cam = cfg["camera"]
         sc.camera_params = dict(look_from=cam["look_from"], look_at=cam["look_at"], vup=cam["vup"], vfov=cam["vfov"], aspect=cam["aspect"])
-        sc.c.camera = camera_from_params(cam["look_from"], cam["look_at"], cam["vup"], cam["vfov"], cam["aspect"])
+        if cam.get("aperture") is not None:
+            sc.camera_params["aperture"] = float(cam["aperture"])
+        if cam.get("focus_dist") is not None:
+            sc.camera_params["focus_dist"] = float(cam["focus_dist"])
+        sc.c.camera, sc.lens = lens_from_params(sc.camera_params)
         # sky: missing/null -> None (black); {"texture": ""} -> gradient; path -> equirect texture (config.rs:49-64, raytracer.rs:137-161)
         sky = cfg.get("sky", None)
         sc.c.sky.mode = RT_SKY_NONE
@@ -445,9 +509,13 @@ class Scene:
         return sc
 
     def set_camera(self, **kw):
+        """Change camera fields (look_from, look_at, vup, vfov, aspect, and the lens's aperture and focus_dist; None removes
+        aperture or focus_dist)."""
         self.camera_params.update(kw)
-        p = self.camera_params
-        self.c.camera = camera_from_params(p["look_from"], p["look_at"], p["vup"], p["vfov"], p["aspect"])
+        for k in ("aperture", "focus_dist"):
+            if k in self.camera_params and self.camera_params[k] is None:
+                del self.camera_params[k]
+        self.c.camera, self.lens = lens_from_params(self.camera_params)
 
     def resize(self, width: int, height: int, spp: Optional[int] = None, max_depth: Optional[int] = None, fix_aspect: bool = False):
         self.c.width, self.c.height = int(width), int(height)
@@ -500,6 +568,7 @@ class Scene:
         C.memmove(C.byref(sc.c), C.byref(self.c), C.sizeof(rt_scene))
         sc._tex_arrays, sc._tex_structs, sc._sky_array = self._tex_arrays, self._tex_structs, self._sky_array
         sc.camera_params = dict(self.camera_params) if self.camera_params is not None else None
+        sc.lens = rt_lens.from_buffer_copy(self.lens) if self.lens is not None else None
         sc._spheres = (rt_sphere * max(len(spheres), 1))(*spheres)
         sc.c.spheres = C.cast(sc._spheres, C.POINTER(rt_sphere)); sc.c.n_spheres = len(spheres)
         return sc
@@ -573,6 +642,8 @@ def render_rgb8(scene: Scene, opts: Optional[rt_options] = None, out: Optional[n
     rows = scene.c.height if (opts is None or opts.world <= 1) else shard_rows(scene.c.height, opts.rank, opts.world, opts.band_rows)
     if out is None:
         out = np.empty((rows, scene.c.width, 3), dtype=np.uint8)
+    if scene.lens is not None:   # the one-shot render of a lens camera: one frame of rtb200_render_frames_lens
+        return _render_lens_once(scene, opts, out, False)
     st = rt_stats()
     _check(lib().rtb200_render_rgb8(C.byref(scene.c), C.byref(opts) if opts is not None else None, out.ctypes.data, C.byref(st)))
     return out, st.as_dict()
@@ -582,9 +653,24 @@ def render_linear(scene: Scene, opts: Optional[rt_options] = None):
     """Per-pixel mean radiance before sqrt/quantisation (float32 [rows,w,3]) and stats."""
     rows = scene.c.height if (opts is None or opts.world <= 1) else shard_rows(scene.c.height, opts.rank, opts.world, opts.band_rows)
     out = np.empty((rows, scene.c.width, 3), dtype=np.float32)
+    if scene.lens is not None:
+        return _render_lens_once(scene, opts, out, True)
     st = rt_stats()
     _check(lib().rtb200_render_linear_f32(C.byref(scene.c), C.byref(opts) if opts is not None else None, out.ctypes.data, C.byref(st)))
     return out, st.as_dict()
+
+
+def _render_lens_once(scene: Scene, opts: Optional[rt_options], out: np.ndarray, linear: bool):
+    f = rt_frame(scene.c.camera, scene.seed, scene.c.max_depth, 0)
+    st = rt_stats()
+    _check(lib().rtb200_render_frames_lens(C.byref(scene.c), C.byref(opts) if opts is not None else None, C.byref(f), C.byref(scene.lens), 1,
+                                           None if linear else out.ctypes.data, out.ctypes.data if linear else None, C.byref(st)))
+    return out, st.as_dict()
+
+
+def _refuse_lens(scene: Scene, what: str):
+    if scene.lens is not None:
+        raise RtError(-1, f"{what} takes no lens: render a lens scene with render_rgb8 / render_frames or a ResidentScene")
 
 
 def device_count() -> int:
@@ -593,6 +679,7 @@ def device_count() -> int:
 
 def render_rgb8_multi(scene: Scene, n_gpus: int = 0, opts: Optional[rt_options] = None, out: Optional[np.ndarray] = None):
     """One process, n_gpus devices (0 = all): rtb200_render_rgb8_multi. Returns (uint8 [h,w,3], stats dict)."""
+    _refuse_lens(scene, "render_rgb8_multi")
     if out is None:
         out = np.empty((scene.c.height, scene.c.width, 3), dtype=np.uint8)
     st = rt_stats()
@@ -602,13 +689,37 @@ def render_rgb8_multi(scene: Scene, n_gpus: int = 0, opts: Optional[rt_options] 
 
 def make_frame(scene: Scene, look_from=None, look_at=None, vup=None, vfov: Optional[float] = None, aspect: Optional[float] = None,
                seed: Optional[int] = None, max_depth: Optional[int] = None) -> rt_frame:
-    """One frame of an animation over `scene`: camera fields, seed and max_depth that are not given are the scene's own."""
+    """One frame of an animation over `scene`: camera fields, seed and max_depth that are not given are the scene's own. On a
+    lens scene the camera is the lens camera's, focused like the scene's (make_frame_lens also returns the frame's lens)."""
     p = dict(scene.camera_params)
     for k, v in (("look_from", look_from), ("look_at", look_at), ("vup", vup), ("vfov", vfov), ("aspect", aspect)):
         if v is not None:
             p[k] = v
-    cam = camera_from_params(p["look_from"], p["look_at"], p["vup"], p["vfov"], p["aspect"])
+    cam, _ = lens_from_params(p)
     return rt_frame(cam, scene.seed if seed is None else int(seed), scene.c.max_depth if max_depth is None else int(max_depth), 0)
+
+
+def make_frame_lens(scene: Scene, look_from=None, look_at=None, vup=None, vfov: Optional[float] = None, aspect: Optional[float] = None,
+                    seed: Optional[int] = None, max_depth: Optional[int] = None, aperture: Optional[float] = None,
+                    focus_dist: Optional[float] = None):
+    """make_frame with a lens: (rt_frame, rt_lens). Omitted aperture and focus_dist are the scene's; with no focus_dist
+    anywhere it is the frame's own |look_from - look_at|. An aperture of 0 gives a lens of radius 0 (a pinhole frame)."""
+    p = dict(scene.camera_params)
+    for k, v in (("look_from", look_from), ("look_at", look_at), ("vup", vup), ("vfov", vfov), ("aspect", aspect),
+                 ("aperture", aperture), ("focus_dist", focus_dist)):
+        if v is not None:
+            p[k] = v
+    cam, lens = lens_from_params(p)
+    f = rt_frame(cam, scene.seed if seed is None else int(seed), scene.c.max_depth if max_depth is None else int(max_depth), 0)
+    return f, (lens if lens is not None else rt_lens())
+
+
+def _lens_array(lenses: Optional[Sequence[rt_lens]], n: int):
+    if lenses is None:
+        return None
+    if len(lenses) != n:
+        raise ValueError(f"{len(lenses)} lenses for {n} frames")
+    return (rt_lens * max(n, 1))(*[l if l is not None else rt_lens() for l in lenses])
 
 
 def _frame_array(frames: Sequence[rt_frame]):
@@ -616,16 +727,24 @@ def _frame_array(frames: Sequence[rt_frame]):
     return arr, len(frames)
 
 
-def render_frames(scene: Scene, frames: Sequence[rt_frame], opts: Optional[rt_options] = None, linear: bool = False):
+def render_frames(scene: Scene, frames: Sequence[rt_frame], opts: Optional[rt_options] = None, linear: bool = False,
+                  lenses: Optional[Sequence[rt_lens]] = None):
     """Render len(frames) frames of one scene in as few trace launches as the sample buffer allows (rtb200_render_frames).
-    Frame i equals render_rgb8 / render_linear of the scene with frames[i]'s camera, seed and max_depth. Returns
-    (uint8 [n,rows,w,3], or float32 with linear=True, stats dict)."""
+    Frame i equals render_rgb8 / render_linear of the scene with frames[i]'s camera, seed and max_depth. lenses: frame i's
+    lens (None or radius 0: pinhole; rtb200_render_frames_lens); without it a lens scene renders every frame with its own lens.
+    Returns (uint8 [n,rows,w,3], or float32 with linear=True, stats dict)."""
     rows = scene.c.height if (opts is None or opts.world <= 1) else shard_rows(scene.c.height, opts.rank, opts.world, opts.band_rows)
     arr, n = _frame_array(frames)
+    if lenses is None and scene.lens is not None:
+        lenses = [scene.lens] * n
     out = np.empty((n, rows, scene.c.width, 3), dtype=np.float32 if linear else np.uint8)
     st = rt_stats()
-    _check(lib().rtb200_render_frames(C.byref(scene.c), C.byref(opts) if opts is not None else None, arr, n,
-                                      None if linear else out.ctypes.data, out.ctypes.data if linear else None, C.byref(st)))
+    o = C.byref(opts) if opts is not None else None
+    o8, ol = (None, out.ctypes.data) if linear else (out.ctypes.data, None)
+    if lenses is None:
+        _check(lib().rtb200_render_frames(C.byref(scene.c), o, arr, n, o8, ol, C.byref(st)))
+    else:
+        _check(lib().rtb200_render_frames_lens(C.byref(scene.c), o, arr, _lens_array(lenses, n), n, o8, ol, C.byref(st)))
     return out, st.as_dict()
 
 
@@ -637,7 +756,9 @@ def make_adaptive(rel_tol: float, abs_tol: float = 0.0, samples_per_round: int =
 def render_adaptive(scene: Scene, params: rt_adaptive_params, opts: Optional[rt_options] = None):
     """Render adaptively (rtb200_render_adaptive): rounds of params.samples_per_round samples of the pixels that have not
     converged, until none is left. A pixel that received n samples equals the one-shot render at samples_per_pixel = n.
-    Returns (uint8 [rows,w,3], float32 linear [rows,w,3], uint32 counts [rows,w], stats dict)."""
+    Returns (uint8 [rows,w,3], float32 linear [rows,w,3], uint32 counts [rows,w], stats dict). A lens scene is refused:
+    render it adaptively through ResidentScene.adaptive_*."""
+    _refuse_lens(scene, "render_adaptive")
     rows = scene.c.height if (opts is None or opts.world <= 1) else shard_rows(scene.c.height, opts.rank, opts.world, opts.band_rows)
     img = np.empty((rows, scene.c.width, 3), dtype=np.uint8)
     lin = np.empty((rows, scene.c.width, 3), dtype=np.float32)
@@ -668,6 +789,15 @@ class ResidentScene:
         self.rows = scene.c.height if (opts is None or opts.world <= 1) else shard_rows(scene.c.height, opts.rank, opts.world, opts.band_rows)
         self.n = scene.n_spheres
         self.device = opts.device if opts is not None and opts.device >= 0 else _current_device()   # None: unknown without torch
+        self.lens = None
+        if scene.lens is not None:
+            self.set_lens(scene.lens)
+
+    def set_lens(self, lens: Optional[rt_lens]):
+        """The lens of every later camera ray of this handle (rtb200_scene_set_lens; None: pinhole). An adaptive render has
+        to begin again after it."""
+        _check(lib().rtb200_scene_set_lens(self.h, C.byref(lens) if lens is not None else None))
+        self.lens = rt_lens.from_buffer_copy(lens) if lens is not None and lens.radius != 0.0 else None
 
     def render(self, dev_rgb8_ptr: int = 0, dev_linear_ptr: int = 0, stream: int = 0) -> dict:
         st = rt_stats()
@@ -684,12 +814,13 @@ class ResidentScene:
         _check(lib().rtb200_render_device_wait(self.h, C.byref(st)))
         return st.as_dict()
 
-    def render_frames(self, frames: Sequence[rt_frame], dev_rgb8_ptr: int = 0, dev_linear_ptr: int = 0, stream: int = 0) -> dict:
+    def render_frames(self, frames: Sequence[rt_frame], dev_rgb8_ptr: int = 0, dev_linear_ptr: int = 0, stream: int = 0,
+                      lenses: Optional[Sequence[rt_lens]] = None) -> dict:
         """Render len(frames) frames into device buffers of n * rows * w * 3 elements (blocking; the handle's own camera,
-        seed and max_depth stay as uploaded)."""
+        seed and max_depth stay as uploaded). lenses: frame i's lens (rtb200_render_frames_lens_device); None: the handle's."""
         arr, n = _frame_array(frames)
         st = rt_stats()
-        _check(lib().rtb200_render_frames_device(self.h, arr, n, C.c_void_p(dev_rgb8_ptr or None), C.c_void_p(dev_linear_ptr or None),
+        _check(lib().rtb200_render_frames_lens_device(self.h, arr, _lens_array(lenses, n), n, C.c_void_p(dev_rgb8_ptr or None), C.c_void_p(dev_linear_ptr or None),
                                                  C.c_void_p(stream or None), C.byref(st)))
         return st.as_dict()
 

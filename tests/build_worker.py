@@ -52,9 +52,36 @@ def _unmoved_scene():
     return _light_scene(1, 6, seed=46)
 
 
+SEED64 = 0x9E3779B97F4A7C15   # a 64-bit key whose high word is nonzero and differs from its low word
+
+
+def lens_room_frames(sc):
+    """Frames and lenses of the room: two lens views, a pinhole view and a focus pull, each with its own 64-bit seed."""
+    fl = [R.make_frame_lens(sc, aperture=0.3, focus_dist=8.0, seed=SEED64),
+          R.make_frame_lens(sc, look_from=[-9.0, 3.0, 7.0], aperture=0.0, seed=SEED64 + 0x100000001),
+          R.make_frame_lens(sc, look_from=[4.0, 8.0, -12.0], look_at=[0.0, 1.0, 0.0], aperture=0.6, seed=SEED64 ^ (5 << 40)),
+          R.make_frame_lens(sc, aperture=0.3, focus_dist=20.0, seed=SEED64 + 7)]
+    return [f for f, _ in fl], [L for _, L in fl]
+
+
+def _with_lens(mk, aperture, focus_dist=None):
+    def make():
+        sc = mk()
+        sc.seed = SEED64
+        sc.set_camera(aperture=aperture, focus_dist=focus_dist)
+        return sc
+    return make
+
+
+def lens_adaptive_params():
+    return _params()
+
+
 # case -> (kind, scene maker, variant, RTB200_WF_SMEM mask). Kinds: "one_shot" (render_linear and render_rgb8), "rebuilt" (a
 # resident handle after rebuild()), "update" (a resident handle after update_spheres), "frames" (render_frames of
-# _room_frames), "adaptive" (render_adaptive with test_gpu_adaptive's parameters), "topology" (see the module docstring).
+# _room_frames), "adaptive" (render_adaptive with test_gpu_adaptive's parameters), "topology" (see the module docstring), and
+# for a lens scene "lens_one_shot" (one_shot through its lens), "lens_frames" (render_frames of lens_room_frames, with their
+# lenses) and "lens_adaptive" (the adaptive rounds of a resident handle with the scene's lens, run to the end).
 CASES = {
     **{f"golden_{name}": ("one_shot", mk, FILTERED, 0) for name, mk in GOLDEN},
     "room_3_lights_depth_50": ("one_shot", lambda: R.Scene.from_config(_room_cfg(3, 50)), FILTERED, 0),
@@ -71,6 +98,11 @@ CASES = {
     "room_frames": ("frames", lambda: R.Scene.from_config(_room_cfg(3, 50)), FILTERED, 0),
     "adaptive_mixed_2_lights": ("adaptive", ADAPTIVE_SCENES["mixed_2_lights"], FILTERED, 0),
     "room_exact_f64": ("one_shot", lambda: R.Scene.from_config(_room_cfg(3, 50)), EXACT, 0),
+    # the lens kernels (DESIGN.md §4.17): Q_FRAMES_LENS at deep albedo stacks, over the dense candidate lists of the
+    # coincident spheres, and Q_LIST_LENS, under 64-bit keys
+    "lens_room_frames": ("lens_frames", lambda: R.Scene.from_config(_room_cfg(3, 50, w=48, h=36, spp=4)), FILTERED, 0),
+    "lens_coincident_10k": ("lens_one_shot", _with_lens(lambda: _coincident(1), 0.4), FILTERED, 0),
+    "lens_adaptive_mixed_2_lights": ("lens_adaptive", _with_lens(ADAPTIVE_SCENES["mixed_2_lights"], 0.3, 12.0), FILTERED, 0),
 }
 
 # Scene staging (RTB200_WF_SMEM) on every build: every mask in both modes that stage bit 0, on scenes whose hierarchy has an
@@ -86,7 +118,7 @@ for _base in STAGE_SCENES:
             _name = f"staged_{_base}_{_mode}_m{_mask}"
             CASES[_name] = ("one_shot", CASES[_base][1], _variant, _mask)
             BASE[_name] = _base
-for _base in ("room_frames", "adaptive_mixed_2_lights"):
+for _base in ("room_frames", "adaptive_mixed_2_lights", "lens_room_frames"):
     CASES[f"staged_{_base}_m7"] = CASES[_base][:3] + (7,)
     BASE[f"staged_{_base}_m7"] = _base
 
@@ -178,6 +210,32 @@ def render_case(name, kind, sc, opts, out, meta):
         img, lin, cnt, st = R.render_adaptive(sc, _params(), opts)
         out[name + ".counts"] = cnt
         meta[name] = _stats(st)
+    elif kind == "lens_one_shot":
+        lin, st = R.render_linear(sc, opts)
+        img, st8 = R.render_rgb8(sc, opts)
+        meta[name] = dict(_stats(st), rays_rgb8=int(st8["rays"]))
+    elif kind == "lens_frames":
+        frames, lenses = lens_room_frames(sc)
+        img, st = R.render_frames(sc, frames, opts, lenses=lenses)
+        lin, st2 = R.render_frames(sc, frames, opts, linear=True, lenses=lenses)
+        meta[name] = dict(_stats(st), rays_linear=int(st2["rays"]), batches=int(st["batches"]))
+    elif kind == "lens_adaptive":
+        import torch
+        rs = R.ResidentScene(sc, opts)
+        try:
+            rs.adaptive_begin(lens_adaptive_params())
+            active, st = rs.adaptive_step(1000)
+            n = rs.rows * int(sc.c.width)
+            o8 = torch.zeros(3 * n, dtype=torch.uint8, device="cuda")
+            ol = torch.zeros(3 * n, dtype=torch.float32, device="cuda")
+            oc = torch.zeros(n, dtype=torch.int32, device="cuda")
+            rs.adaptive_resolve(o8, ol, oc)
+            sh = (rs.rows, int(sc.c.width))
+            img, lin = o8.cpu().numpy().reshape(*sh, 3), ol.cpu().numpy().reshape(*sh, 3)
+            out[name + ".counts"] = oc.cpu().numpy().view(np.uint32).reshape(sh)
+            meta[name] = dict(_stats(st), active=active)
+        finally:
+            rs.release()
     else:
         raise ValueError(kind)
     out[name + ".linear"] = lin

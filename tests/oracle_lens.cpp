@@ -130,6 +130,26 @@ int oracle_lens_render(const rt_scene* s, const rt_lens* lens, float* out_linear
     return 0;
 }
 
+// Samples [s0, s1) of every pixel through the lens, each alone (oracle_sample's, with the lens ray): radiance
+// [s1 - s0][npix][3] and the hit_world calls of each sample [s1 - s0][npix], for the adaptive rule's restatement.
+int oracle_lens_samples(const rt_scene* s, const rt_lens* lens, uint32_t s0, uint32_t s1, float* out_rgb, uint64_t* rays) {
+    const Scene sc(s);
+    if (sc.lights.size() >= 10) return -4;
+    const int64_t npix = (int64_t)s->width * s->height, n = npix * (int64_t)(s1 - s0);
+#pragma omp parallel for schedule(dynamic, 16)
+    for (int64_t i = 0; i < n; ++i) {
+        const int64_t k = i % npix;
+        const uint32_t smp = s0 + (uint32_t)(i / npix), x = (uint32_t)(k % s->width), y = (uint32_t)(k / s->width);
+        Stats st;
+        SampleRng rng(s->seed, y * s->width + x, smp);
+        const Ray r = primary(*s, *lens, x, y, smp, rng);
+        const Rgb c = ray_color(sc, r, s->max_depth, s->max_depth, rng, st, nullptr, nullptr);
+        out_rgb[3 * i] = c.r; out_rgb[3 * i + 1] = c.g; out_rgb[3 * i + 2] = c.b;
+        rays[i] = st.rays;
+    }
+    return 0;
+}
+
 // The first hit of sample sample0's lens ray and the count of samples in [sample0, sample0 + samples) that hit: sphere
 // (0xffffffff on a miss), point [npix][3] (0 on a miss), hits [npix].
 int oracle_lens_hits(const rt_scene* s, const rt_lens* lens, uint32_t samples, uint32_t sample0, uint32_t* sphere, double* point,

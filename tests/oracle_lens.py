@@ -45,6 +45,7 @@ def lib() -> C.CDLL:
                                       C.c_double, C.c_void_p, C.POINTER(C.c_uint32)]
         L.oracle_lens_primary.argtypes = [C.c_void_p, C.POINTER(R.rt_lens), C.c_uint32, C.c_void_p, C.c_void_p]
         L.oracle_lens_render.argtypes = [C.c_void_p, C.POINTER(R.rt_lens), C.c_void_p, C.c_void_p, C.POINTER(C.c_uint64)]
+        L.oracle_lens_samples.argtypes = [C.c_void_p, C.POINTER(R.rt_lens), C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]
         L.oracle_lens_hits.argtypes = [C.c_void_p, C.POINTER(R.rt_lens), C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
         L.oracle_lens_aov.argtypes = [C.c_void_p, C.POINTER(R.rt_lens), C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p]
         _lib = L
@@ -85,6 +86,31 @@ def render(scene, lens) -> dict:
     if rc != 0:
         raise RuntimeError(f"oracle_lens_render failed: {rc}")
     return {"linear": lin, "rgb8": rgb, "rays": int(rays.value)}
+
+
+def render_samples(scene, lens, s0: int, s1: int):
+    """Samples [s0, s1) of every pixel through `lens`, each alone: adaptive_restatement.render_samples with the lens.
+    Returns (float32 radiance [s1-s0, h, w, 3], uint32 rays [s1-s0, h, w])."""
+    w, h = int(scene.c.width), int(scene.c.height)
+    out, rays = np.empty((s1 - s0, h, w, 3), np.float32), np.empty((s1 - s0, h, w), np.uint64)
+    rc = lib().oracle_lens_samples(C.addressof(scene.c), C.byref(_lens(lens)), int(s0), int(s1), out.ctypes.data, rays.ctypes.data)
+    if rc != 0:
+        raise RuntimeError(f"oracle_lens_samples failed: {rc}")
+    return out, rays.astype(np.uint32)
+
+
+def adaptive(scene, lens, params, N=None):
+    """adaptive_restatement.run on the oracle's lens samples of `scene` with rt_adaptive_params `params` (N: the resolved
+    max_samples): counts, linear, rgb8, rays and samples of the adaptive render of a lens handle."""
+    import adaptive_restatement as A
+    N = N or params.max_samples or scene.c.samples_per_pixel
+    x, rays = render_samples(scene, lens, 0, N)
+    return A.run(x, rays, params.samples_per_round, N, params.min_samples, params.abs_tol, params.rel_tol)
+
+
+def aov_all(scene, lens, samples: int = 1, sample0: int = 0) -> dict:
+    """Every output of rt_aov_out for a lens handle: aov()'s albedo and normal with hits()'s hits, sphere and point."""
+    return {**aov(scene, lens, samples, sample0), **hits(scene, lens, samples, sample0)}
 
 
 def hits(scene, lens, samples: int = 1, sample0: int = 0) -> dict:

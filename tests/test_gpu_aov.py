@@ -322,10 +322,16 @@ def test_cli_writes_the_albedo_and_normal_pngs(tmp_path):
 # ---- the stress builds ---------------------------------------------------------------------------------------------------
 
 def test_stress_builds_match_the_oracle(tmp_path):
-    """Every stress build gives the oracle's outputs on the worker's sets."""
+    """Every stress build gives the oracle's outputs on the worker's sets, and the lens oracle's on its lens sets."""
     import aov_worker as AW
+    import oracle_lens as OL
     manifest = json.load(open(os.path.join(STRESS, "manifest.json")))
-    wants = {name: OA.aov(mk(), samples, sample0) for name, (mk, samples, sample0, _) in AW.SETS.items()}
+
+    def want(mk, samples, sample0):
+        sc = mk()
+        return OA.aov(sc, samples, sample0) if sc.lens is None else OL.aov_all(sc, sc.lens, samples, sample0)
+    wants = {name: want(mk, samples, sample0) for name, (mk, samples, sample0, _) in AW.SETS.items()}
+    assert sum(AW.SETS[name][0]().lens is not None for name in AW.SETS) == 2
     for build in manifest:
         out = tmp_path / f"{build}.npz"
         env = dict(os.environ, RTB200_LIB=os.path.join(STRESS, f"librtb200_{build}.so"))

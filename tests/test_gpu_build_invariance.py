@@ -21,6 +21,7 @@ import pytest
 
 import adaptive_restatement as A
 import build_worker as BW
+import oracle_lens as OL
 import oracle_py as O
 from test_gpu_adaptive import M, MIN, N, _samples
 from test_gpu_scene_staging import staged_bytes
@@ -90,6 +91,20 @@ def reference(name):
         p = BW._params()
         want = A.run(x, rays, M, N, MIN, p.abs_tol, p.rel_tol)
         ref = dict(linear=want["linear"], rgb8=want["rgb8"], counts=want["counts"], rays=want["rays"], samples=want["samples"])
+    elif kind == "lens_one_shot":
+        sc = mk()
+        want = OL.render(sc, sc.lens)
+        ref = dict(linear=want["linear"], rgb8=want["rgb8"], rays=want["rays"], samples=sc.c.width * sc.c.height * sc.c.samples_per_pixel)
+    elif kind == "lens_frames":
+        sc = mk()
+        frames, lenses = BW.lens_room_frames(sc)
+        outs = [OL.render(_view(sc, f), L) for f, L in zip(frames, lenses)]
+        ref = dict(linear=np.stack([o["linear"] for o in outs]), rgb8=np.stack([o["rgb8"] for o in outs]),
+                   rays=sum(o["rays"] for o in outs), samples=len(frames) * sc.c.width * sc.c.height * sc.c.samples_per_pixel)
+    elif kind == "lens_adaptive":
+        sc = mk()
+        want = OL.adaptive(sc, sc.lens, BW.lens_adaptive_params())
+        ref = dict(linear=want["linear"], rgb8=want["rgb8"], counts=want["counts"], rays=want["rays"], samples=want["samples"])
     else:
         raise ValueError(kind)
     _REF[name] = ref
@@ -105,7 +120,7 @@ def test_the_room_reaches_deep_albedo_levels():
 def compare(name, z, meta):
     ref = reference(name)
     lin, img = z[name + ".linear"], z[name + ".rgb8"]
-    if BW.CASES[name][0] == "frames":
+    if BW.CASES[name][0] in ("frames", "lens_frames"):
         assert lin.shape == ref["linear"].shape, (name, lin.shape)
         for i in range(len(lin)):
             assert_frames_match((lin[i], img[i]), (ref["linear"][i], ref["rgb8"][i]), f"{name} frame {i}")

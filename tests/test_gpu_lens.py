@@ -1,6 +1,8 @@
 """The thin-lens camera on the GPU (DESIGN.md §4.17), bit for bit against the oracle's lens (tests/oracle_lens.cpp) in linear
 f32, RGB8 and rays: every variant, shard and staged handles, the device's lens routine, pinhole invariance, trace_rays of the
 lens rays, lens frames, adaptive rounds, auxiliary buffers and a lens handle after updates, rebuilds and edits."""
+import math
+
 import numpy as np
 import pytest
 
@@ -12,6 +14,7 @@ from test_gpu_intersect import BRUTE, EXACT, FILTERED, _torch
 
 pytestmark = pytest.mark.gpu
 VARIANTS = [FILTERED, EXACT, BRUTE]
+SEED64 = 0x9E3779B97F4A7C15   # a 64-bit key whose high word is nonzero and differs from its low word
 
 
 def bits(a):
@@ -87,6 +90,15 @@ def test_probe_equals_the_oracle_lens_ray():
         R._check(L.rtb200_probe_lens_ray(R.C.byref(cam), R.C.byref(lens), 42 + k, pixel, sample, u, v, R.C.byref(o), R.C.byref(d), R.C.byref(t)))
         wo, wd, wt = OL.lens_ray(cam, lens, 42 + k, pixel, sample, u, v)
         assert bits(np.array([o.x, o.y, o.z, d.x, d.y, d.z])) == bits(np.concatenate([wo, wd])) and t.value == wt
+    # a 64-bit key: the high word keys the disk too, so these rays are not the rays of the low word alone
+    for k in range(64):
+        pixel, sample = int(rng.integers(0, 1 << 31)), int(rng.integers(0, 4096))
+        o, d, t = R.rt_vec3(), R.rt_vec3(), R.C.c_uint32()
+        R._check(L.rtb200_probe_lens_ray(R.C.byref(cam), R.C.byref(lens), SEED64 + k, pixel, sample, 0.25, 0.75, R.C.byref(o), R.C.byref(d), R.C.byref(t)))
+        wo, wd, wt = OL.lens_ray(cam, lens, SEED64 + k, pixel, sample, 0.25, 0.75)
+        assert bits(np.array([o.x, o.y, o.z, d.x, d.y, d.z])) == bits(np.concatenate([wo, wd])) and t.value == wt
+        lo, _, _ = OL.lens_ray(cam, lens, (SEED64 + k) & 0xFFFFFFFF, pixel, sample, 0.25, 0.75)
+        assert bits(lo) != bits(wo), k
 
 
 def test_pinhole_stays_pinhole():
@@ -286,3 +298,213 @@ def test_cli_lens_config_and_frames_give_the_python_path(tmp_path):
     imgs, _ = R.render_frames(sc, [f for f, _ in fl], lenses=[l for _, l in fl])
     for i in range(3):
         assert np.array_equal(pixels(tmp_path / f"anim_{i:03d}.png"), imgs[i]), i
+
+
+# ---- every lens kernel, 64-bit keys, launch groups and stream order (DESIGN.md §3, "The thin lens at its edges") ----------
+
+def seed64(sc, seed=SEED64):
+    """sc under a 64-bit key, after checking that its lens render under the key's low word alone is another render."""
+    sc.seed = seed & 0xFFFFFFFF
+    low = OL.render(sc, sc.lens)["linear"]
+    sc.seed = seed
+    assert bits(low) != bits(OL.render(sc, sc.lens)["linear"])
+    return sc
+
+
+def adaptive_scenes():
+    return {"mixed_lit": lambda: seed64(lensed(mixed_lit_scene(24, 18, 4), 0.4, 0.6)),          # lit: Q_LIST_LENS with lights
+            "cover": lambda: seed64(lensed(scenes.cover_scene(24, 18, 4, depth=8), 0.3, fd=10.0))}   # unlit
+
+
+ADAPTIVE = R.make_adaptive(0.05, abs_tol=0.002, samples_per_round=1, min_samples=2, max_samples=5)
+
+
+def adaptive_resolve(rs):
+    torch = _torch()
+    n = rs.rows * int(rs.scene.c.width)
+    o8 = torch.zeros(3 * n, dtype=torch.uint8, device="cuda:0")
+    ol = torch.zeros(3 * n, dtype=torch.float32, device="cuda:0")
+    oc = torch.zeros(n, dtype=torch.int32, device="cuda:0")
+    rs.adaptive_resolve(o8, ol, oc)
+    sh = (rs.rows, int(rs.scene.c.width))
+    return o8.cpu().numpy().reshape(*sh, 3), ol.cpu().numpy().reshape(*sh, 3), oc.cpu().numpy().view(np.uint32).reshape(sh)
+
+
+def assert_adaptive(rs, want, what, rows=None):
+    """An adaptive render of the handle run to the end equals the restatement on the oracle's lens samples (its rows)."""
+    rs.adaptive_begin(ADAPTIVE)
+    active, st = rs.adaptive_step(100)
+    img, lin, cnt = adaptive_resolve(rs)
+    sl = slice(None) if rows is None else rows
+    assert active == 0, what
+    assert np.array_equal(cnt, want["counts"][sl]), f"{what}: counts differ in {int((cnt != want['counts'][sl]).sum())} pixels"
+    assert bits(lin) == bits(want["linear"][sl]) and np.array_equal(img, want["rgb8"][sl]), what
+    if rows is None:
+        assert (st["rays"], st["samples"]) == (want["rays"], want["samples"]), (what, st["rays"], want["rays"])
+    return cnt
+
+
+@pytest.mark.parametrize("scene", ["mixed_lit", "cover"])
+@pytest.mark.parametrize("variant", VARIANTS)
+def test_adaptive_rounds_of_every_lens_kernel(variant, scene):
+    """Q_LIST_LENS of every mode, with and without lights, over rounds that start past sample 0, under a 64-bit key."""
+    sc = adaptive_scenes()[scene]()
+    want = OL.adaptive(sc, sc.lens, ADAPTIVE)
+    u = np.unique(want["counts"])
+    assert len(u) >= 3 and u[0] == ADAPTIVE.min_samples and u[-1] == ADAPTIVE.max_samples, u   # the rule's edges, s0 > 0
+    rs = R.ResidentScene(sc, R.make_options(device=0, variant=variant))
+    try:
+        assert_adaptive(rs, want, f"{scene}/{variant}")
+    finally:
+        rs.release()
+
+
+def test_adaptive_lens_shards_and_max_depth_0():
+    sc = adaptive_scenes()["mixed_lit"]()
+    want = OL.adaptive(sc, sc.lens, ADAPTIVE)
+    h = int(sc.c.height)
+    for rank in range(3):
+        rs = R.ResidentScene(sc, R.make_options(device=0, rank=rank, world=3, band_rows=7))
+        try:
+            assert_adaptive(rs, want, f"rank {rank}", R.shard_row_indices(h, rank, 3, 7))
+        finally:
+            rs.release()
+    sc.c.max_depth = 0   # black samples: a memset per round, no ray
+    want = OL.adaptive(sc, sc.lens, ADAPTIVE)
+    assert (want["counts"] == ADAPTIVE.min_samples).all() and want["rays"] == 0 and not want["linear"].any()
+    rs = R.ResidentScene(sc, R.make_options(device=0))
+    try:
+        assert_adaptive(rs, want, "max_depth 0")
+    finally:
+        rs.release()
+
+
+@pytest.mark.parametrize("variant", VARIANTS)
+def test_aov_of_every_lens_kernel(variant):
+    """rt_aov_lens_kernel of every mode, past sample 0, under a 64-bit key, on the whole frame and on shard handles."""
+    from test_gpu_aov import assert_aov_equal
+    sc = seed64(scene_set()["mixed_lit"])
+    want = OL.aov_all(sc, sc.lens, samples=3, sample0=2)
+    rs = R.ResidentScene(sc, R.make_options(device=0, variant=variant))
+    try:
+        got = rs.aov(3, sample0=2)
+        assert_aov_equal(got, want, f"aov/{variant}")
+        assert got["stats"]["rays"] == int(sc.c.width) * int(sc.c.height) * 3
+    finally:
+        rs.release()
+    for rank in range(3):
+        rs = R.ResidentScene(sc, R.make_options(device=0, variant=variant, rank=rank, world=3, band_rows=7))
+        try:
+            assert_aov_equal(rs.aov(3, sample0=2), want, f"aov/{variant}/rank {rank}", R.shard_row_indices(int(sc.c.height), rank, 3, 7))
+        finally:
+            rs.release()
+
+
+def lens_frame_table(sc, specs):
+    """Frames and lenses of sc from (aperture, focus_dist, max_depth) specs, each with its own 64-bit seed; an aperture of
+    -0.0 gives the camera's lens with radius -0.0."""
+    frames, lenses = [], []
+    for k, (ap, fd, depth) in enumerate(specs):
+        f, L = R.make_frame_lens(sc, aperture=abs(ap) if ap else 0.3, focus_dist=fd, seed=SEED64 + k * 0x0000000100000003,
+                                 max_depth=depth)
+        if ap == 0.0:
+            L = R.rt_lens(L.u, L.v, ap, 0)   # radius 0.0 or -0.0: a pinhole frame
+        frames.append(f); lenses.append(L)
+    return frames, lenses
+
+
+def assert_frames_equal_the_oracle(sc, frames, lenses, lin, rows=None):
+    for k, (f, L) in enumerate(zip(frames, lenses)):
+        one = R.Scene.edited(sc)
+        one.c.camera = f.camera; one.seed = f.seed; one.c.max_depth = f.max_depth
+        want = OL.render(one, L)["linear"]
+        assert bits(lin[k]) == bits(want if rows is None else want[rows]), k
+
+
+def group_counts(frames, cap, frame_work):
+    """The launch groups of rtb200_api_render.cu's frame_groups: runs of equal max_depth (never 0) of at most
+    cap / (16 * frame_work) frames."""
+    out, i = [], 0
+    while i < len(frames):
+        F = 1
+        if frames[i].max_depth != 0:
+            while i + F < len(frames) and frames[i + F].max_depth == frames[i].max_depth and (F + 1) * frame_work * 16 <= cap:
+                F += 1
+        out.append(F)
+        i += F
+    return out
+
+
+def test_lens_frames_across_launch_groups_and_batches():
+    """Seven lens frames in groups of 2, 2, 1 (another max_depth) and 1 (max_depth 0), each with its own lens and 64-bit key,
+    so that each group reads the lens table from its own offset; then the same frames with a cap below one frame's samples,
+    so that every frame is a group of its own over several sample batches."""
+    sc = scene_set()["textured_sky"]
+    spp, npix = int(sc.c.samples_per_pixel), int(sc.c.width) * int(sc.c.height)
+    frames, lenses = lens_frame_table(sc, [(0.3, 1.0, 6), (0.0, None, 6), (-0.0, 2.0, 6), (0.5, 0.7, 6), (0.2, 3.0, 4), (0.4, None, 0),
+                                           (0.1, 0.9, 6)])
+    assert math.copysign(1.0, lenses[2].radius) < 0 and lenses[1].radius == 0.0
+    cap = 2 * spp * npix * 16
+    groups = group_counts(frames, cap, spp * npix)
+    assert groups == [2, 2, 1, 1, 1], groups
+    lin, st = R.render_frames(sc, frames, R.make_options(device=0, sample_buffer_bytes=cap), linear=True, lenses=lenses)
+    assert st["batches"] == len(groups) and st["kernel_launches"] == sum(1 + g for g in groups), st
+    assert_frames_equal_the_oracle(sc, frames, lenses, lin)
+    # a cap of two samples of one frame: spp 3 takes batches of 2 and 1, every frame alone
+    sc.c.samples_per_pixel = spp = 3
+    cap = 2 * npix * 16
+    assert group_counts(frames, cap, spp * npix) == [1] * len(frames)
+    lin, st = R.render_frames(sc, frames, R.make_options(device=0, sample_buffer_bytes=cap), linear=True, lenses=lenses)
+    # every frame is a group of one frame in two batches, each a trace launch (a black memset at max_depth 0) and a resolve
+    assert st["batches"] == 2 * len(frames) and st["kernel_launches"] == 4 * len(frames), st
+    assert_frames_equal_the_oracle(sc, frames, lenses, lin)
+
+
+def test_lens_frames_on_a_shard_handle():
+    torch = _torch()
+    sc = scene_set()["mixed_lit"]
+    frames, lenses = lens_frame_table(sc, [(0.3, 1.0, 12), (0.0, None, 12), (0.6, 0.5, 12)])
+    w, h = int(sc.c.width), int(sc.c.height)
+    for rank in range(3):
+        rs = R.ResidentScene(sc, R.make_options(device=0, rank=rank, world=3, band_rows=2))
+        try:
+            rows = R.shard_row_indices(h, rank, 3, 2)
+            out = torch.empty((3, len(rows), w, 3), dtype=torch.float32, device="cuda:0")
+            rs.render_frames(frames, dev_linear_ptr=out.data_ptr(), lenses=lenses)
+            assert_frames_equal_the_oracle(sc, frames, lenses, out.cpu().numpy(), rows)
+        finally:
+            rs.release()
+
+
+def test_set_lens_orders_against_asynchronous_renders():
+    """The handle's lens applies to the renders enqueued after set_lens returns: L1, then L2, then the pinhole, on two
+    streams, while a second handle's blocking lens frames put a larger lens table into the work sets the first one uses."""
+    torch = _torch()
+    sc = scene_set()["mixed_lit"]
+    l1 = sc.lens
+    l2 = R.make_frame_lens(sc, aperture=0.7, focus_dist=2.0)[1]
+    wants = [OL.render(sc, l1)["linear"], OL.render(sc, l2)["linear"], OL.render(sc, None)["linear"]]
+    other = scene_set()["cover"]
+    frames, lenses = lens_frame_table(other, [(0.2, 8.0, 8), (0.3, 10.0, 8), (0.0, None, 8), (0.1, 12.0, 8), (0.4, 9.0, 8)])
+    a = R.ResidentScene(sc, R.make_options(device=0))
+    b = R.ResidentScene(other, R.make_options(device=0))
+    s1, s2 = torch.cuda.Stream(), torch.cuda.Stream()
+    outs = [torch.zeros((18, 24, 3), dtype=torch.float32, device="cuda:0") for _ in range(3)]
+    fo = torch.zeros((5, int(other.c.height), int(other.c.width), 3), dtype=torch.float32, device="cuda:0")
+    try:
+        with torch.cuda.stream(s1):
+            torch.cuda._sleep(50_000_000)   # hold the first render back behind the later host calls
+        a.render_async(0, outs[0].data_ptr(), s1.cuda_stream)
+        a.set_lens(l2)
+        a.render_async(0, outs[1].data_ptr(), s2.cuda_stream)
+        b.render_frames(frames, dev_linear_ptr=fo.data_ptr(), lenses=lenses)
+        a.set_lens(None)
+        a.render_async(0, outs[2].data_ptr(), s1.cuda_stream)
+        a.wait()
+        torch.cuda.synchronize()
+        for k in range(3):
+            assert bits(outs[k].cpu().numpy()) == bits(wants[k]), k
+        assert_frames_equal_the_oracle(other, frames, lenses, fo.cpu().numpy())
+    finally:
+        torch.cuda.synchronize()
+        a.release(); b.release()

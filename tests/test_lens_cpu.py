@@ -57,13 +57,29 @@ def test_focus_one_is_camera_new_bit_for_bit(aperture):
     assert abs(np.linalg.norm(vec(lens.u)) - 1.0) < 1e-15 and abs(np.linalg.norm(vec(lens.v)) - 1.0) < 1e-15
 
 
-@pytest.mark.parametrize("fd", [1.0, 10.0, 0.37, 1e5])
+@pytest.mark.parametrize("fd", [1.0, 10.0, 0.37, 1e5, 1e-300, 1e308])
 def test_library_camera_equals_the_oracle(fd):
     p = R.rt_camera_params(R.vec3(COVER["look_from"]), R.vec3(COVER["look_at"]), R.vec3(COVER["vup"]), COVER["vfov"], COVER["aspect"])
     cam_o, lens_o = R.rt_camera(), R.rt_lens()
     assert OL.lib().oracle_camera_lens(C.byref(p), 0.1, fd, C.byref(cam_o), C.byref(lens_o)) == 0
     cam, lens = R.camera_from_params_lens(**COVER, aperture=0.1, focus_dist=fd)
     assert bytes(cam) == bytes(cam_o) and bytes(lens) == bytes(lens_o)
+
+
+@pytest.mark.parametrize("fd,vfov", [(1e-300, 20.0), (1e-300, 120.0), (1e308, 120.0), (1e308, 170.0)])
+def test_library_camera_equals_the_oracle_at_extreme_focus(fd, vfov):
+    """focus_dist 1e-300, where the lower-left corner rounds to the origin, and 1e308 at wide fields of view, where
+    `horizontal` overflows: the library's camera is the oracle's bit for bit, infinities included."""
+    q = dict(COVER, vfov=vfov)
+    p = R.rt_camera_params(R.vec3(q["look_from"]), R.vec3(q["look_at"]), R.vec3(q["vup"]), q["vfov"], q["aspect"])
+    cam_o, lens_o = R.rt_camera(), R.rt_lens()
+    assert OL.lib().oracle_camera_lens(C.byref(p), 0.4, fd, C.byref(cam_o), C.byref(lens_o)) == 0
+    cam, lens = R.camera_from_params_lens(**q, aperture=0.4, focus_dist=fd)
+    assert bytes(cam) == bytes(cam_o) and bytes(lens) == bytes(lens_o)
+    if fd < 1.0:
+        assert bytes(cam.lower_left_corner) == bytes(cam.origin)   # the pinhole direction is 0 wherever u and v are small
+    else:
+        assert not np.isfinite(vec(cam.horizontal)).all()
 
 
 @pytest.mark.parametrize("aperture,fd", [(-0.1, 10.0), (math.nan, 10.0), (math.inf, 10.0), (0.1, 0.0), (0.1, -1.0),

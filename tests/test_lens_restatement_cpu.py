@@ -84,3 +84,42 @@ def test_the_oracle_reproduces_the_golden_fixture():
     want = json.load(open(make_lens.OUT))
     got = {name: make_lens.pins(sc) for name, sc in make_lens.cases().items()}
     assert got == want
+
+
+# The degenerate lenses of tests/lens_edges.py (E1, E3, E4, E7) under a 64-bit key: radius, u and v as the case sets them
+# (None: the camera's own), and the camera's aperture, focus distance and field of view.
+SEED64 = 0x9E3779B97F4A7C15
+EDGES = {
+    "tiny": dict(aperture=2.0 ** -1073, fd=9.0),
+    "zero_uv": dict(u=(0.0, 0.0, 0.0), v=(0.0, 0.0, 0.0), radius=0.3),
+    "u_zero": dict(u=(0.0, 0.0, 0.0), radius=0.3),
+    "u_eq_v": dict(v="u", radius=0.3),
+    "u_1e3": dict(u=1e3, radius=3e-4),
+    "huge": dict(radius=1e300),
+    "fd_tiny": dict(aperture=0.4, fd=1e-300),
+    "fd_huge": dict(aperture=0.4, fd=1e308, vfov=120.0),
+}
+
+
+@pytest.mark.parametrize("name", list(EDGES))
+def test_degenerate_lenses_under_a_64_bit_key(name):
+    e = dict(dict(aperture=0.6, fd=9.0, vfov=20.0), **EDGES[name])
+    cfg = mixed_config(6, 4, 2, 6, seed=31, n=10)
+    cfg["objects"].insert(2, {"center": _v(0.0, 6.0, 0.0), "radius": 1.0, "material": {"Light": {}}})
+    cfg["camera"]["vfov"] = e["vfov"]
+    cfg = _with_lens(cfg, e["aperture"], e["fd"])
+    sc = R.Scene.from_config(cfg, scenes.SCENES_DIR)
+    sc.seed = SEED64
+    w = LensWorld(cfg, e["aperture"], e["fd"], seed=SEED64)
+    lc = w.lens_camera
+    u, v = np.array(lc.u, float), np.array(lc.v, float)
+    u = u * e["u"] if isinstance(e.get("u"), float) else np.array(e.get("u", u), float)
+    v = u if e.get("v") == "u" else np.array(e.get("v", v), float)
+    lc.u, lc.v, lc.radius = tuple(u.tolist()), tuple(v.tolist()), float(e.get("radius", lc.radius))
+    lens = R.rt_lens(R.vec3(lc.u), R.vec3(lc.v), lc.radius, 0)
+    want = OL.render(sc, lens)
+    lin, img, rays = w.render()
+    assert rays == want["rays"], (rays, want["rays"])
+    assert np.array_equal(np.isnan(lin), np.isnan(want["linear"]))
+    assert np.array_equal(np.nan_to_num(lin).view(np.uint32), np.nan_to_num(want["linear"]).view(np.uint32)), name
+    assert np.array_equal(img, want["rgb8"]), name

@@ -73,18 +73,25 @@ def resolve(n, S):
 def run(samples, rays, m, N, min_samples, abs_tol, rel_tol, rounds=None):
     """Adaptive render of the per-sample radiances samples[s] ([>= N, h, w, 3] float32) with rays[s] ([>= N, h, w]).
     `rounds`: stop after that many rounds (None: until no pixel is active). Returns a dict: counts [h, w] (uint32), S, Q,
-    linear, rgb8, rays (the rays of every sample taken), samples (taken), active (pixels still on the list), rounds (run)."""
+    linear, rgb8, rays (the rays of every sample taken), samples (taken), active (pixels still on the list), rounds (run),
+    and per round run: list_sizes (the pixels on its list), list_runs (the runs of consecutive pixels, in raster order, that
+    its list is made of) and list_samples (the samples it took of each of them)."""
     h, w = samples.shape[1:3]
     n = np.zeros((h, w), dtype=np.uint32)
     S = np.zeros((h, w, 3), dtype=F); Q = np.zeros((h, w, 3), dtype=F)
     active = np.ones((h, w), dtype=bool)
     taken_rays = 0
     r = 0
+    sizes, runs, counts = [], [], []
     with np.errstate(all="ignore"):
         while active.any() and (rounds is None or r < rounds):
+            listed = np.flatnonzero(active)
+            sizes.append(len(listed))
+            runs.append(1 + int((np.diff(listed) != 1).sum()))
             s0 = int(n[active][0])
             assert (n[active] == s0).all(), "every listed pixel has the same n"
             s1 = min(s0 + m, N)
+            counts.append(s1 - s0)
             for s in range(s0, s1):
                 x = samples[s][active]
                 S[active] = S[active] + x
@@ -95,7 +102,7 @@ def run(samples, rays, m, N, min_samples, abs_tol, rel_tol, rounds=None):
             r += 1
     lin, img = resolve(n, S)
     return {"counts": n, "S": S, "Q": Q, "linear": lin, "rgb8": img, "rays": taken_rays, "samples": int(n.astype(np.uint64).sum()),
-            "active": int(active.sum()), "rounds": r}
+            "active": int(active.sum()), "rounds": r, "list_sizes": sizes, "list_runs": runs, "list_samples": counts}
 
 
 def of_scene(scene, params, N=None, rounds=None):

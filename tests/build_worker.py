@@ -25,6 +25,7 @@ import numpy as np  # noqa: E402
 
 import rtb200 as R  # noqa: E402
 from rtb200 import scenes  # noqa: E402
+from test_full_frames_cpu import lit_scene as full_frame_lit_scene, params as full_frame_params  # noqa: E402
 from test_gpu_adaptive import SCENES as ADAPTIVE_SCENES, _params  # noqa: E402
 from test_gpu_parity import GOLDEN  # noqa: E402
 from test_gpu_rebuild_restatement import _coincident, _deep_dense, _drifted, _geometry, _render_stats, _scene, rebuilt  # noqa: E402
@@ -77,10 +78,14 @@ def lens_adaptive_params():
     return _params()
 
 
+# the parameters of an "adaptive" case other than test_gpu_adaptive's
+ADAPTIVE_PARAMS = {"adaptive_full_frame_lit": lambda: full_frame_params(8)}
+
+
 # case -> (kind, scene maker, variant, RTB200_WF_SMEM mask). Kinds: "one_shot" (render_linear and render_rgb8), "rebuilt" (a
 # resident handle after rebuild()), "update" (a resident handle after update_spheres), "frames" (render_frames of
-# _room_frames), "adaptive" (render_adaptive with test_gpu_adaptive's parameters), "topology" (see the module docstring), and
-# for a lens scene "lens_one_shot" (one_shot through its lens), "lens_frames" (render_frames of lens_room_frames, with their
+# _room_frames), "adaptive" (render_adaptive with test_gpu_adaptive's parameters, or the case's ADAPTIVE_PARAMS), "topology"
+# (see the module docstring), and for a lens scene "lens_one_shot" (one_shot through its lens), "lens_frames" (render_frames of lens_room_frames, with their
 # lenses) and "lens_adaptive" (the adaptive rounds of a resident handle with the scene's lens, run to the end).
 CASES = {
     **{f"golden_{name}": ("one_shot", mk, FILTERED, 0) for name, mk in GOLDEN},
@@ -97,6 +102,9 @@ CASES = {
     "resident_update": ("update", _unmoved_scene, FILTERED, 0),
     "room_frames": ("frames", lambda: R.Scene.from_config(_room_cfg(3, 50)), FILTERED, 0),
     "adaptive_mixed_2_lights": ("adaptive", ADAPTIVE_SCENES["mixed_2_lights"], FILTERED, 0),
+    # the full-frame adaptive case (tests/test_gpu_full_frames.py): 640 x 360 at 8 samples a round, whose rounds refill the
+    # trace kernel's slots many times over and compact lists of hundreds of thousands of pixels
+    "adaptive_full_frame_lit": ("adaptive", full_frame_lit_scene, FILTERED, 0),
     "room_exact_f64": ("one_shot", lambda: R.Scene.from_config(_room_cfg(3, 50)), EXACT, 0),
     # the lens kernels (DESIGN.md §4.17): Q_FRAMES_LENS at deep albedo stacks, over the dense candidate lists of the
     # coincident spheres, and Q_LIST_LENS, under 64-bit keys
@@ -207,7 +215,7 @@ def render_case(name, kind, sc, opts, out, meta):
         lin, st2 = R.render_frames(sc, frames, opts, linear=True)
         meta[name] = dict(_stats(st), rays_linear=int(st2["rays"]), batches=int(st["batches"]))
     elif kind == "adaptive":
-        img, lin, cnt, st = R.render_adaptive(sc, _params(), opts)
+        img, lin, cnt, st = R.render_adaptive(sc, ADAPTIVE_PARAMS.get(name, _params)(), opts)
         out[name + ".counts"] = cnt
         meta[name] = _stats(st)
     elif kind == "lens_one_shot":

@@ -23,6 +23,7 @@ import adaptive_restatement as A
 import build_worker as BW
 import oracle_lens as OL
 import oracle_py as O
+import test_full_frames_cpu as FF
 from test_gpu_adaptive import M, MIN, N, _samples
 from test_gpu_scene_staging import staged_bytes
 from test_gpu_shading_edges import assert_frames_match
@@ -85,6 +86,12 @@ def reference(name):
         outs = [O.render(_view(sc, f)) for f in _room_frames(sc)]
         ref = dict(linear=np.stack([o[0] for o in outs]), rgb8=np.stack([o[1] for o in outs]),
                    rays=sum(o[2]["rays"] for o in outs), samples=sum(o[2]["samples"] for o in outs))
+    elif kind == "adaptive" and name in BW.ADAPTIVE_PARAMS:   # a full-frame case: the oracle's bulk route
+        sc = mk()
+        x, rays = FF.oracle_samples(name, sc)
+        p = BW.ADAPTIVE_PARAMS[name]()
+        want = A.run(x, rays, p.samples_per_round, sc.c.samples_per_pixel, p.min_samples, p.abs_tol, p.rel_tol)
+        ref = dict(linear=want["linear"], rgb8=want["rgb8"], counts=want["counts"], rays=want["rays"], samples=want["samples"])
     elif kind == "adaptive":
         sc = mk()
         x, rays = _samples("mixed_2_lights", sc)

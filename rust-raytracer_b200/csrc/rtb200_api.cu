@@ -64,7 +64,7 @@ uint32_t rtk::samples_per_batch(uint64_t cap, uint64_t items, uint32_t samples) 
 }
 
 cudaError_t rtk::scene_stream(rtb200_scene_handle h, void* stream_in, cudaStream_t* out) {
-    const cudaStream_t st = stream_in ? (cudaStream_t)stream_in : h->ctx->stream;
+    const cudaStream_t st = call_stream(h->ctx, stream_in);
     *out = st;
     if (st != h->ctx->stream) { cudaError_t e = cudaStreamWaitEvent(st, h->ctx->staging_free, 0); if (e != cudaSuccess) return e; }
     return h->updated ? cudaStreamWaitEvent(st, h->updated, 0) : cudaSuccess;

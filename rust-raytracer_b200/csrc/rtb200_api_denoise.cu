@@ -8,14 +8,6 @@ using namespace rtk;
 
 namespace {
 
-struct Range { const void* p; uint64_t bytes; const char* name; };
-
-bool overlap(const Range& a, const Range& b) {
-    if (!a.p || !b.p || !a.bytes || !b.bytes) return false;
-    const uintptr_t a0 = (uintptr_t)a.p, b0 = (uintptr_t)b.p;
-    return a0 < b0 + b.bytes && b0 < a0 + a.bytes;
-}
-
 // The argument checks of both forms (no device is touched); `scratch` is checked in the device form only.
 int check_denoise(const rt_denoise_params* p, const float* color, const float* albedo, const float* normal, const void* scratch,
                   bool device_form, const float* out_linear, const uint8_t* out_rgb8) {
@@ -37,15 +29,15 @@ int check_denoise(const rt_denoise_params* p, const float* color, const float* a
     if (!normal && p->normal_weight != 0.0f) return fail(RT_ERR_INVALID, "normal_weight is nonzero but normal is null");
     const uint64_t n = (uint64_t)p->width * p->height;
     if (n >= (1ull << 31)) return fail(RT_ERR_INVALID, "width * height must be below 2^31");
+    const Range in[3] = {{color, n * 12, "color", 4}, {albedo, n * 12, "albedo", 4}, {normal, n * 12, "normal", 4}};
+    const Range out[3] = {{out_linear, n * 12, "out_linear", 4}, {out_rgb8, n * 3, "out_rgb8", 1},
+                          {scratch, device_form ? denoise_scratch_bytes(n) : 0, "scratch", 16}};
     if (device_form) {
-        for (const Range& r : {Range{color, 0, "color"}, Range{albedo, 0, "albedo"}, Range{normal, 0, "normal"}, Range{out_linear, 0, "out_linear"}})
-            if ((uintptr_t)r.p % 4) return fail(RT_ERR_INVALID, std::string(r.name) + " is not 4-byte aligned");
-        if ((uintptr_t)scratch % 16) return fail(RT_ERR_INVALID, "scratch is not 16-byte aligned");
+        for (const Range* g : {in, out})
+            for (int k = 0; k < 3; ++k)
+                if ((uintptr_t)g[k].p % g[k].align) return fail(RT_ERR_INVALID, std::string(g[k].name) + " is not " + std::to_string(g[k].align) + "-byte aligned");
     }
     // an output or the scratch must not overlap an input or each other
-    const Range in[3] = {{color, n * 12, "color"}, {albedo, n * 12, "albedo"}, {normal, n * 12, "normal"}};
-    const Range out[3] = {{out_linear, n * 12, "out_linear"}, {out_rgb8, n * 3, "out_rgb8"},
-                          {scratch, device_form ? denoise_scratch_bytes(n) : 0, "scratch"}};
     for (int i = 0; i < 3; ++i) {
         for (const Range& r : in)
             if (overlap(out[i], r)) return fail(RT_ERR_INVALID, std::string(out[i].name) + " overlaps " + r.name);
@@ -71,15 +63,11 @@ int rtb200_denoise_device(int32_t device, const rt_denoise_params* p, const floa
     int rc = check_denoise(p, color, albedo, normal, scratch, true, out_linear, out_rgb8);
     if (rc != RT_OK) return rc;
     if ((uint64_t)p->width * p->height == 0) return RT_OK;
-    DeviceRestore restore_;
-    DeviceCtx* ctx = nullptr;
-    if ((rc = get_ctx(device, &ctx)) != RT_OK) return rc;
-    std::lock_guard<std::recursive_mutex> lock_(ctx->mu);
+    CTX_PROLOGUE(device, ctx);
     if ((rc = check_device_ptrs(ctx->device, {{color, "color"}, {albedo, "albedo"}, {normal, "normal"}, {scratch, "scratch"},
                                               {out_linear, "out_linear"}, {out_rgb8, "out_rgb8"}})) != RT_OK)
         return rc;
-    const cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
-    CU(launch_denoise(denoise_args(*p, color, albedo, normal, scratch, out_linear, out_rgb8), st));
+    CU(launch_denoise(denoise_args(*p, color, albedo, normal, scratch, out_linear, out_rgb8), call_stream(ctx, stream_in)));
     return RT_OK;
   });
 }
@@ -93,35 +81,19 @@ int rtb200_denoise(int32_t device, const rt_denoise_params* p, const float* colo
     const uint64_t N = (uint64_t)p->width * p->height;
     if (N == 0) return RT_OK;
     auto wall0 = std::chrono::steady_clock::now();
-    DeviceRestore restore_;
-    DeviceCtx* ctx = nullptr;
-    if ((rc = get_ctx(device, &ctx)) != RT_OK) return rc;
-    std::lock_guard<std::recursive_mutex> lock_(ctx->mu);
-    for (auto& e : ctx->query_ev) if (!e) CU(cudaEventCreate(&e));
+    CTX_PROLOGUE(device, ctx);
     // device image: the inputs, the scratch, the outputs
     HostStage io;
     io.add_in(color, N * 12); io.add_in(albedo, albedo ? N * 12 : 0); io.add_in(normal, normal ? N * 12 : 0);
     io.add_in(nullptr, denoise_scratch_bytes(N));
     io.add_out(out_linear, out_linear ? N * 12 : 0); io.add_out(out_rgb8, out_rgb8 ? N * 3 : 0);
-    if ((rc = io.place(ctx, 0)) != RT_OK) return rc;
-    const cudaStream_t st = ctx->stream;
-    cudaEvent_t* ev = ctx->query_ev;
-    CU(cudaEventRecord(ev[0], st));
-    if ((rc = io.copy(st, false)) != RT_OK) return rc;
-    CU(cudaEventRecord(ev[1], st));
-    CU(launch_denoise(denoise_args(*p, (const float*)io.a[0].dev, (const float*)io.a[1].dev, (const float*)io.a[2].dev, io.a[3].dev,
-                                   (float*)io.a[4].dev, (uint8_t*)io.a[5].dev), st));
-    CU(cudaEventRecord(ev[2], st));
-    if ((rc = io.copy(st, true)) != RT_OK) return rc;
-    CU(cudaEventRecord(ev[3], st));
-    CU(cudaStreamSynchronize(st));
-    if (!stats) return RT_OK;
-    float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, ev[0], ev[3])); stats->device_ms = ms;
-    CU(cudaEventElapsedTime(&ms, ev[1], ev[2])); stats->trace_ms = ms;
+    rc = host_call(ctx, ctx->stream, io, nullptr, nullptr, wall0, stats, [&](unsigned long long*) -> int {
+        CU(launch_denoise(denoise_args(*p, (const float*)io.a[0].dev, (const float*)io.a[1].dev, (const float*)io.a[2].dev, io.a[3].dev,
+                                       (float*)io.a[4].dev, (uint8_t*)io.a[5].dev), ctx->stream));
+        return RT_OK;
+    });
+    if (rc != RT_OK || !stats) return rc;
     stats->kernel_launches = p->iterations + 1;
-    stats->h2d_bytes = io.h2d; stats->d2h_bytes = io.d2h;
-    stats->wall_ms = ms_since(wall0);
     return RT_OK;
   });
 }

@@ -137,41 +137,24 @@ static int query_host(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, co
     if (n == 0) return RT_OK;
     auto wall0 = std::chrono::steady_clock::now();
     HANDLE_PROLOGUE(h);
-    DeviceCtx* ctx = h->ctx;
-    for (auto& e : ctx->query_ev) if (!e) CU(cudaEventCreate(&e));
-    // device image: counters (kStatBytes; the guard counters at stat[30..31]), then rays and outputs
+    // device image: counters, then rays and outputs
     const uint64_t N = n;
     HostStage io;
     io.add_in(rays->origin, N * 24); io.add_in(rays->direction, N * 24); io.add_in(rays->t_max, rays->t_max ? N * 8 : 0);
     for (int k = 0; k < out->count; ++k) io.add_out(out->ptr[k], out->ptr[k] ? N * out->bytes[k] : 0);
-    if ((rc = io.place(ctx, kStatBytes)) != RT_OK) return rc;
-    unsigned long long* stat = (unsigned long long*)ctx->query.p;
-    char* dout[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-    for (int k = 0; k < out->count; ++k) dout[k] = io.a[3 + k].dev;
     cudaStream_t st;
     CU(scene_stream(h, nullptr, &st));
-    cudaEvent_t* ev = ctx->query_ev;
-    CU(cudaEventRecord(ev[0], st));
-    CU(cudaMemsetAsync(stat, 0, kStatBytes, st));
-    if ((rc = io.copy(st, false)) != RT_OK) return rc;
-    const rt_rays drays{(const double*)io.a[0].dev, (const double*)io.a[1].dev, (const double*)io.a[2].dev};
-    CU(cudaEventRecord(ev[1], st));
-    if ((rc = query_enqueue(h, drays, n, with_ptrs(*out, dout), stat, stat + 30, st)) != RT_OK) return rc;
-    CU(cudaEventRecord(ev[2], st));
-    if ((rc = io.copy(st, true)) != RT_OK) return rc;
     unsigned long long hstat[kStatBytes / 8];
-    CU(cudaMemcpyAsync(hstat, stat, kStatBytes, cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(ev[3], st));
-    CU(cudaStreamSynchronize(st));
-    if (hstat[31] != 0) return fail(RT_ERR_CUDA, "internal error: the traversal guard tripped; the query results are not valid");
-    if (!stats) return RT_OK;
-    float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, ev[0], ev[3])); stats->device_ms = ms;
-    CU(cudaEventElapsedTime(&ms, ev[1], ev[2])); stats->trace_ms = ms;
+    rc = host_call(h->ctx, st, io, hstat, "internal error: the traversal guard tripped; the query results are not valid", wall0, stats,
+                   [&](unsigned long long* stat) {
+        char* dout[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
+        for (int k = 0; k < out->count; ++k) dout[k] = io.a[3 + k].dev;
+        const rt_rays drays{(const double*)io.a[0].dev, (const double*)io.a[1].dev, (const double*)io.a[2].dev};
+        return query_enqueue(h, drays, n, with_ptrs(*out, dout), stat, stat + 30, st);
+    });
+    if (rc != RT_OK || !stats) return rc;
     stats->rays = hstat[0]; stats->candidates = hstat[1]; stats->clusters = hstat[4]; stats->nodes = hstat[6];
     stats->kernel_launches = 1; stats->batches = 1; stats->gpus_used = 1;
-    stats->h2d_bytes = io.h2d; stats->d2h_bytes = kStatBytes + io.d2h;
-    stats->wall_ms = ms_since(wall0);
     return RT_OK;
 }
 
@@ -275,38 +258,22 @@ int rtb200_scene_aov(rtb200_scene_handle h, const rt_aov_params* p, const rt_fra
     if (N == 0) return RT_OK;
     auto wall0 = std::chrono::steady_clock::now();
     HANDLE_PROLOGUE(h);
-    DeviceCtx* ctx = h->ctx;
-    for (auto& e : ctx->query_ev) if (!e) CU(cudaEventCreate(&e));
-    // device image: counters (kStatBytes; the guard counters at stat[30..31]), then the outputs
+    // device image: counters, then the outputs
     const AovOut o = aov_out(*out);
     HostStage io;
     for (int k = 0; k < 5; ++k) io.add_out(o.ptr[k], o.ptr[k] ? N * kAovBytes[k] : 0);
-    if ((rc = io.place(ctx, kStatBytes)) != RT_OK) return rc;
-    unsigned long long* stat = (unsigned long long*)ctx->query.p;
-    AovOut dout = o;
-    for (int k = 0; k < 5; ++k) dout.ptr[k] = io.a[k].dev;
     cudaStream_t st;
     CU(scene_stream(h, nullptr, &st));
-    cudaEvent_t* ev = ctx->query_ev;
-    CU(cudaEventRecord(ev[0], st));
-    CU(cudaMemsetAsync(stat, 0, kStatBytes, st));
-    CU(cudaEventRecord(ev[1], st));
-    if ((rc = aov_enqueue(h, *p, view, dout, stat, stat + 30, st)) != RT_OK) return rc;
-    CU(cudaEventRecord(ev[2], st));
-    if ((rc = io.copy(st, true)) != RT_OK) return rc;
     unsigned long long hstat[kStatBytes / 8];
-    CU(cudaMemcpyAsync(hstat, stat, kStatBytes, cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(ev[3], st));
-    CU(cudaStreamSynchronize(st));
-    if (hstat[31] != 0) return fail(RT_ERR_CUDA, "internal error: the traversal guard tripped; the aov results are not valid");
-    if (!stats) return RT_OK;
-    float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, ev[0], ev[3])); stats->device_ms = ms;
-    CU(cudaEventElapsedTime(&ms, ev[1], ev[2])); stats->trace_ms = ms;
+    rc = host_call(h->ctx, st, io, hstat, "internal error: the traversal guard tripped; the aov results are not valid", wall0, stats,
+                   [&](unsigned long long* stat) {
+        AovOut dout = o;
+        for (int k = 0; k < 5; ++k) dout.ptr[k] = io.a[k].dev;
+        return aov_enqueue(h, *p, view, dout, stat, stat + 30, st);
+    });
+    if (rc != RT_OK || !stats) return rc;
     stats->rays = hstat[0]; stats->samples = hstat[3]; stats->candidates = hstat[1]; stats->clusters = hstat[4]; stats->nodes = hstat[6];
     stats->kernel_launches = 1; stats->batches = 1; stats->frames = 1; stats->gpus_used = 1;
-    stats->d2h_bytes = kStatBytes + io.d2h;
-    stats->wall_ms = ms_since(wall0);
     return RT_OK;
   });
 }

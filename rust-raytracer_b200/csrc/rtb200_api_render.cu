@@ -164,7 +164,7 @@ static std::vector<FrameGroup> frame_groups(const rt_frame* frames, uint32_t n, 
 }
 
 // rt_frame checks (and of the per-frame lenses, when not null) shared by the frames entry points (no device is touched)
-static int check_frames(const rt_frame* frames, uint32_t n, uint64_t rows, uint64_t width, const rt_lens* lenses = nullptr) {
+static int check_frames(const rt_frame* frames, uint32_t n, uint64_t rows, uint64_t width, const rt_lens* lenses) {
     if (n == 0) return fail(RT_ERR_INVALID, "n_frames must be > 0");
     if (!frames) return fail(RT_ERR_INVALID, "frames is null");
     const uint64_t per_frame = rows * width * 3ull;   // < 2^33: width * height < 2^31 (validate_scene)
@@ -417,17 +417,6 @@ int rtb200_render_device_wait(rtb200_scene_handle h, rt_stats* stats) {
     return render_collect(h, stats);
 }
 
-int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, uint32_t n_frames, void* dev_rgb8, void* dev_linear_f32,
-                                void* stream_in, rt_stats* stats) {
-  return guarded([&]() -> int {
-    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
-    int rc = check_frames(frames, n_frames, h->tp.rows_local, h->tp.width);
-    if (rc != RT_OK) return rc;
-    if (!dev_rgb8 && !dev_linear_f32) return fail(RT_ERR_INVALID, "dev_rgb8 and dev_linear_f32 are both null");
-    return render_blocking(h, frames, n_frames, dev_rgb8, dev_linear_f32, stream_in, stats);
-  });
-}
-
 int rtb200_render_frames_lens_device(rtb200_scene_handle h, const rt_frame* frames, const rt_lens* lenses, uint32_t n_frames,
                                      void* dev_rgb8, void* dev_linear_f32, void* stream_in, rt_stats* stats) {
   return guarded([&]() -> int {
@@ -437,6 +426,11 @@ int rtb200_render_frames_lens_device(rtb200_scene_handle h, const rt_frame* fram
     if (!dev_rgb8 && !dev_linear_f32) return fail(RT_ERR_INVALID, "dev_rgb8 and dev_linear_f32 are both null");
     return render_blocking(h, frames, n_frames, dev_rgb8, dev_linear_f32, stream_in, stats, lenses);
   });
+}
+
+int rtb200_render_frames_device(rtb200_scene_handle h, const rt_frame* frames, uint32_t n_frames, void* dev_rgb8, void* dev_linear_f32,
+                                void* stream_in, rt_stats* stats) {
+    return rtb200_render_frames_lens_device(h, frames, nullptr, n_frames, dev_rgb8, dev_linear_f32, stream_in, stats);
 }
 
 int rtb200_render_rgb8(const rt_scene* scene, const rt_options* opts, uint8_t* out_rgb8, rt_stats* stats) {
@@ -450,15 +444,6 @@ int rtb200_render_linear_f32(const rt_scene* scene, const rt_options* opts, floa
     return guarded([&]() -> int { return render_host(scene, opts, &f, 1, nullptr, out_rgb, stats); });
 }
 
-int rtb200_render_frames(const rt_scene* s, const rt_options* opts_in, const rt_frame* frames, uint32_t n_frames, uint8_t* out_rgb8,
-                         float* out_lin, rt_stats* stats) {
-  return guarded([&]() -> int {
-    if (!s) return fail(RT_ERR_INVALID, "null argument");
-    if (!out_rgb8 && !out_lin) return fail(RT_ERR_INVALID, "out_rgb8 and out_linear_f32 are both null");
-    return render_host(s, opts_in, frames, n_frames, out_rgb8, out_lin, stats);
-  });
-}
-
 int rtb200_render_frames_lens(const rt_scene* s, const rt_options* opts_in, const rt_frame* frames, const rt_lens* lenses,
                               uint32_t n_frames, uint8_t* out_rgb8, float* out_lin, rt_stats* stats) {
   return guarded([&]() -> int {
@@ -466,6 +451,11 @@ int rtb200_render_frames_lens(const rt_scene* s, const rt_options* opts_in, cons
     if (!out_rgb8 && !out_lin) return fail(RT_ERR_INVALID, "out_rgb8 and out_linear_f32 are both null");
     return render_host(s, opts_in, frames, n_frames, out_rgb8, out_lin, stats, lenses);
   });
+}
+
+int rtb200_render_frames(const rt_scene* s, const rt_options* opts_in, const rt_frame* frames, uint32_t n_frames, uint8_t* out_rgb8,
+                         float* out_lin, rt_stats* stats) {
+    return rtb200_render_frames_lens(s, opts_in, frames, nullptr, n_frames, out_rgb8, out_lin, stats);
 }
 
 // ---- radiance of caller-supplied primary rays on a resident scene (DESIGN.md §4.12) ----

@@ -8,14 +8,6 @@ using namespace rtk;
 
 namespace {
 
-struct Range { const void* p; uint64_t bytes; const char* name; uintptr_t align; };
-
-bool overlap(const Range& a, const Range& b) {
-    if (!a.p || !b.p || !a.bytes || !b.bytes) return false;
-    const uintptr_t a0 = (uintptr_t)a.p, b0 = (uintptr_t)b.p;
-    return a0 < b0 + b.bytes && b0 < a0 + a.bytes;
-}
-
 // The argument checks of both forms (no device is touched); the alignment is checked in the device form only.
 int check_temporal(const rt_temporal_params* p, const rt_temporal_frame* cur, const rt_temporal_history* prev, const double* motion,
                    const rt_temporal_out* out, bool device_form) {
@@ -64,10 +56,7 @@ int rtb200_temporal_device(int32_t device, const rt_temporal_params* p, const rt
     int rc = check_temporal(p, cur, prev, motion, out, true);
     if (rc != RT_OK) return rc;
     if ((uint64_t)p->width * p->height == 0) return RT_OK;
-    DeviceRestore restore_;
-    DeviceCtx* ctx = nullptr;
-    if ((rc = get_ctx(device, &ctx)) != RT_OK) return rc;
-    std::lock_guard<std::recursive_mutex> lock_(ctx->mu);
+    CTX_PROLOGUE(device, ctx);
     const rt_temporal_history none{};
     const rt_temporal_history& h = prev ? *prev : none;
     if ((rc = check_device_ptrs(ctx->device, {{cur->color, "cur.color"}, {cur->sphere, "cur.sphere"}, {cur->point, "cur.point"},
@@ -75,9 +64,8 @@ int rtb200_temporal_device(int32_t device, const rt_temporal_params* p, const rt
                                               {h.point, "prev.point"}, {p->n_motion ? motion : nullptr, "motion"},
                                               {out->color, "out.color"}, {out->length, "out.length"}})) != RT_OK)
         return rc;
-    const cudaStream_t st = stream_in ? (cudaStream_t)stream_in : ctx->stream;
     CU(launch_temporal(temporal_args(*p, cur->color, cur->sphere, cur->point, h.color, h.length, h.sphere, h.point, motion, out->color,
-                                     out->length), st));
+                                     out->length), call_stream(ctx, stream_in)));
     return RT_OK;
   });
 }
@@ -91,11 +79,7 @@ int rtb200_temporal(int32_t device, const rt_temporal_params* p, const rt_tempor
     const uint64_t N = (uint64_t)p->width * p->height;
     if (N == 0) return RT_OK;
     auto wall0 = std::chrono::steady_clock::now();
-    DeviceRestore restore_;
-    DeviceCtx* ctx = nullptr;
-    if ((rc = get_ctx(device, &ctx)) != RT_OK) return rc;
-    std::lock_guard<std::recursive_mutex> lock_(ctx->mu);
-    for (auto& e : ctx->query_ev) if (!e) CU(cudaEventCreate(&e));
+    CTX_PROLOGUE(device, ctx);
     // device image: this frame, the previous frame (absent: 0 bytes, a null dev), the motion, the outputs
     const uint64_t hb = prev ? N : 0;
     HostStage io;
@@ -104,27 +88,15 @@ int rtb200_temporal(int32_t device, const rt_temporal_params* p, const rt_tempor
     io.add_in(prev ? prev->sphere : nullptr, hb * 4); io.add_in(prev ? prev->point : nullptr, hb * 24);
     io.add_in(motion, (uint64_t)p->n_motion * 24);
     io.add_out(out->color, N * 12); io.add_out(out->length, N * 4);
-    if ((rc = io.place(ctx, 0)) != RT_OK) return rc;
-    const cudaStream_t st = ctx->stream;
-    cudaEvent_t* ev = ctx->query_ev;
-    CU(cudaEventRecord(ev[0], st));
-    if ((rc = io.copy(st, false)) != RT_OK) return rc;
-    CU(cudaEventRecord(ev[1], st));
-    auto dev = [&](int k) { return (const void*)io.a[k].dev; };
-    CU(launch_temporal(temporal_args(*p, (const float*)dev(0), (const uint32_t*)dev(1), (const double*)dev(2), (const float*)dev(3),
-                                     (const uint32_t*)dev(4), (const uint32_t*)dev(5), (const double*)dev(6), (const double*)dev(7),
-                                     (float*)io.a[8].dev, (uint32_t*)io.a[9].dev), st));
-    CU(cudaEventRecord(ev[2], st));
-    if ((rc = io.copy(st, true)) != RT_OK) return rc;
-    CU(cudaEventRecord(ev[3], st));
-    CU(cudaStreamSynchronize(st));
-    if (!stats) return RT_OK;
-    float ms = 0.f;
-    CU(cudaEventElapsedTime(&ms, ev[0], ev[3])); stats->device_ms = ms;
-    CU(cudaEventElapsedTime(&ms, ev[1], ev[2])); stats->trace_ms = ms;
+    rc = host_call(ctx, ctx->stream, io, nullptr, nullptr, wall0, stats, [&](unsigned long long*) -> int {
+        auto dev = [&](int k) { return (const void*)io.a[k].dev; };
+        CU(launch_temporal(temporal_args(*p, (const float*)dev(0), (const uint32_t*)dev(1), (const double*)dev(2), (const float*)dev(3),
+                                         (const uint32_t*)dev(4), (const uint32_t*)dev(5), (const double*)dev(6), (const double*)dev(7),
+                                         (float*)io.a[8].dev, (uint32_t*)io.a[9].dev), ctx->stream));
+        return RT_OK;
+    });
+    if (rc != RT_OK || !stats) return rc;
     stats->kernel_launches = 1;
-    stats->h2d_bytes = io.h2d; stats->d2h_bytes = io.d2h;
-    stats->wall_ms = ms_since(wall0);
     return RT_OK;
   });
 }

@@ -103,7 +103,7 @@ struct DeviceCtx {
     PinnedBuf staging;                    // host image of the arena being uploaded
     cudaEvent_t staging_free = nullptr;   // the last H2D copy out of `staging` has finished
     // the host forms of rtb200_scene_intersect, _occluded, _trace_rays, _aov, rtb200_denoise and rtb200_temporal: their arrays on the device
-    // (HostStage), the query's timing events (created at its first call), and the resident CTAs per SM of the query kernel of
+    // (HostStage), host_call's timing events (created at its first call), and the resident CTAs per SM of the query kernel of
     // each kind and mode (0: not asked yet)
     GrowBuf query;
     cudaEvent_t query_ev[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -125,6 +125,25 @@ struct DeviceRestore {
     DeviceRestore restore_;                                          \
     std::lock_guard<std::recursive_mutex> lock_((h)->ctx->mu);       \
     CU(cudaSetDevice(h->device))
+
+// The same for an entry point on a device ordinal (-1: the current device): declares `ctx`, the device's context, which
+// get_ctx has made current.
+#define CTX_PROLOGUE(device, ctx)                                    \
+    DeviceRestore restore_;                                          \
+    DeviceCtx* ctx = nullptr;                                        \
+    if (int rc_ = get_ctx(device, &ctx); rc_ != RT_OK) return rc_;   \
+    std::lock_guard<std::recursive_mutex> lock_(ctx->mu)
+
+// The stream of a call on ctx's device: `stream_in`, or the context's stream for NULL
+inline cudaStream_t call_stream(const DeviceCtx* ctx, void* stream_in) { return stream_in ? (cudaStream_t)stream_in : ctx->stream; }
+
+// A caller's array in an argument check: its bytes, its name in a refusal and the alignment the device form needs
+struct Range { const void* p; uint64_t bytes; const char* name; uintptr_t align; };
+inline bool overlap(const Range& a, const Range& b) {
+    if (!a.p || !b.p || !a.bytes || !b.bytes) return false;
+    const uintptr_t a0 = (uintptr_t)a.p, b0 = (uintptr_t)b.p;
+    return a0 < b0 + b.bytes && b0 < a0 + a.bytes;
+}
 
 inline double ms_since(std::chrono::steady_clock::time_point t0) {
     return std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
@@ -254,10 +273,11 @@ int launch_geometry(rtb200_scene_t* h, uint32_t queue, bool lights, LaunchGeom* 
 // Wait for the pending submissions of h and report them (stats may be NULL).
 int render_collect(rtb200_scene_t* h, rt_stats* stats);
 
-// The host form of a call on caller-supplied arrays (closest-hit, occlusion, trace_rays): the device images of the caller's
-// host arrays in the context's query block, after `head` bytes the call keeps for itself, in the order they were added, each
-// at a 256-byte boundary (an array of 0 bytes has none: a null dev). The last host-form call waited for its stream, so the
-// block is free. copy enqueues the inputs' copies to the device, or with `back` the outputs' to the host; h2d and d2h count them.
+// The host form of a call on caller-supplied arrays (closest-hit, occlusion, trace_rays, aov, denoise, temporal): the device
+// images of the caller's host arrays in the context's query block, after `head` bytes the call keeps for itself, in the order
+// they were added, each at a 256-byte boundary (an array of 0 bytes has none: a null dev). The last host-form call waited for
+// its stream, so the block is free. copy enqueues the inputs' copies to the device, or with `back` the outputs' to the host;
+// h2d and d2h count them.
 struct HostStage {
     struct Array { const void* in; void* out; uint64_t bytes; char* dev; };
     Array a[10];
@@ -268,5 +288,39 @@ struct HostStage {
     int place(DeviceCtx* ctx, size_t head);
     int copy(cudaStream_t st, bool back);
 };
+
+// The blocking host form of a call whose wall clock started at wall0, on `st` of ctx's device (made current, ctx->mu held): io's
+// arrays are staged through the query block, `launch(stat)` enqueues the call on their device images, the outputs are copied
+// back and the stream is waited for. With `hstat`, the image starts with a counter block (kStatBytes; the guard counters at
+// [30..31]), cleared before the inputs are copied in and read back into hstat after the outputs; `stat` is its device image
+// (else NULL), and a trip of the traversal guard refuses with `guard_trip`. Fills the times and byte counts of stats (may be
+// NULL); the caller adds its own counters.
+template <typename Launch>
+int host_call(DeviceCtx* ctx, cudaStream_t st, HostStage& io, unsigned long long* hstat, const char* guard_trip,
+              std::chrono::steady_clock::time_point wall0, rt_stats* stats, Launch&& launch) {
+    for (auto& e : ctx->query_ev) if (!e) CU(cudaEventCreate(&e));
+    int rc = io.place(ctx, hstat ? kStatBytes : 0);
+    if (rc != RT_OK) return rc;
+    unsigned long long* stat = hstat ? (unsigned long long*)ctx->query.p : nullptr;
+    cudaEvent_t* ev = ctx->query_ev;
+    CU(cudaEventRecord(ev[0], st));
+    if (stat) CU(cudaMemsetAsync(stat, 0, kStatBytes, st));
+    if ((rc = io.copy(st, false)) != RT_OK) return rc;
+    CU(cudaEventRecord(ev[1], st));
+    if ((rc = launch(stat)) != RT_OK) return rc;
+    CU(cudaEventRecord(ev[2], st));
+    if ((rc = io.copy(st, true)) != RT_OK) return rc;
+    if (stat) CU(cudaMemcpyAsync(hstat, stat, kStatBytes, cudaMemcpyDeviceToHost, st));
+    CU(cudaEventRecord(ev[3], st));
+    CU(cudaStreamSynchronize(st));
+    if (hstat && hstat[31] != 0) return fail(RT_ERR_CUDA, guard_trip);
+    if (!stats) return RT_OK;
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, ev[0], ev[3])); stats->device_ms = ms;
+    CU(cudaEventElapsedTime(&ms, ev[1], ev[2])); stats->trace_ms = ms;
+    stats->h2d_bytes = io.h2d; stats->d2h_bytes = (stat ? kStatBytes : 0) + io.d2h;
+    stats->wall_ms = ms_since(wall0);
+    return RT_OK;
+}
 
 }  // namespace rtk

@@ -10,6 +10,7 @@ library or an H100 is missing every render call raises :class:`RtError`.
 from __future__ import annotations
 
 import ctypes as C
+import functools
 import json
 import math
 import os
@@ -778,6 +779,69 @@ def _current_device() -> Optional[int]:
     return torch.cuda.current_device()
 
 
+@functools.cache   # np.dtype(...).name costs microseconds, and every array of a call asks
+def _torch_dtype(dtype):
+    """The torch dtype of a numpy type (float64, float32, int32, uint32, uint8: torch names them alike)."""
+    import torch
+    return getattr(torch, np.dtype(dtype).name)
+
+
+class _Arrays:
+    """The arrays of one call of an entry point that has a host form (C-contiguous numpy arrays; the library stages them and
+    waits) and a device form (contiguous CUDA tensors on one device, on a stream). Unless `host` fixes the form, the first
+    array checked picks it; in the device form that array's device is the call's, unless `device` (an ordinal) fixes it."""
+
+    def __init__(self, what: str, host: Optional[bool] = None, device: Optional[int] = None):
+        self.what, self.host, self.device = what, host, device
+
+    def ptr(self, a):
+        """The address of a numpy array or a tensor of the call's form; None for None."""
+        if a is None:
+            return None
+        return a.ctypes.data if self.host else a.data_ptr()
+
+    def arg(self, name: str, a, dtypes, shape, optional: bool = False):
+        """ptr(a) once `a` (None too when `optional`) is an array of the call's form and device with a dtype of `dtypes` (numpy
+        types) and `shape`: a tuple, where "n" stands for a length no array has, or an int, a number of elements in any shape.
+        Raises ValueError naming `name` otherwise."""
+        if a is None and optional:
+            return None
+        if self.host is None:
+            self.host = isinstance(a, np.ndarray)
+        if self.host:
+            ok = isinstance(a, np.ndarray) and a.dtype in dtypes and a.flags.c_contiguous
+        else:
+            import torch
+            ok = isinstance(a, torch.Tensor) and a.is_cuda and a.dtype in [_torch_dtype(d) for d in dtypes] and a.is_contiguous()
+            if ok and self.device is None:
+                self.device = a.device.index
+            ok = ok and a.device.index == self.device
+        if not ok or (math.prod(a.shape) != shape if isinstance(shape, int) else tuple(a.shape) != shape):
+            kind = "C-contiguous numpy array" if self.host else "contiguous CUDA tensor" + (f" on cuda:{self.device}" if self.device is not None else "")
+            want = f"{shape} elements" if isinstance(shape, int) else "shape [" + ", ".join(map(str, shape)) + "]"
+            raise ValueError(f"{self.what}: {name} must be a {kind} of {'/'.join(np.dtype(d).name for d in dtypes)} with {want}, got "
+                             f"{type(a).__name__} {getattr(a, 'dtype', '')} {tuple(getattr(a, 'shape', ()))} {getattr(a, 'device', '')}")
+        return self.ptr(a)
+
+    def empty(self, outs, stream=None) -> dict:
+        """{name: a new array} of the outputs `outs` (name, shape, numpy dtype): numpy arrays in the host form; in the device
+        form tensors on the call's device, allocated on `stream` when it is a torch stream (the caching allocator then orders
+        their reuse after the call), else on the device's current stream."""
+        if self.host:
+            return {k: np.empty(s, dtype=d) for k, s, d in outs}
+        import torch
+        device = torch.device("cuda", self.device)
+        with torch.cuda.stream(stream) if isinstance(stream, torch.cuda.Stream) else torch.cuda.device(device):
+            return {k: torch.empty(s, dtype=_torch_dtype(d), device=device) for k, s, d in outs}
+
+
+def _rays(A: _Arrays, origin, direction, t_max):
+    """rt_rays and n of a query's rays, checked by A: origin and direction float64 [n, 3], t_max float64 [n] or None."""
+    n = origin.shape[0] if getattr(origin, "ndim", 0) == 2 else "n"
+    f64 = (np.float64,)
+    return rt_rays(A.arg("origin", origin, f64, (n, 3)), A.arg("direction", direction, f64, (n, 3)), A.arg("t_max", t_max, f64, (n,), True)), n
+
+
 class ResidentScene:
     """Scene kept in HBM between frames (rtb200_scene_upload / rtb200_render_device)."""
 
@@ -838,27 +902,22 @@ class ResidentScene:
         {cx, cy, cz, radius} on the handle's device (rtb200_scene_update_geometry_device); materials stay. Runs on `stream`
         (a torch.cuda.Stream, or a cudaStream_t handle where 0 is the library's own stream, as in :meth:`render`), by default
         torch's current stream, so `t` may be computed on it just before and released just after."""
-        import torch
-        if not isinstance(t, torch.Tensor) or not t.is_cuda:
-            raise ValueError("update_geometry takes a CUDA tensor")
-        if t.dtype != torch.float64 or tuple(t.shape) != (self.n, 4) or not t.is_contiguous():
-            raise ValueError(f"update_geometry takes a contiguous float64 tensor of shape [{self.n}, 4], got {t.dtype} {tuple(t.shape)}")
-        if self.device is not None and t.device.index != self.device:
-            raise ValueError(f"the tensor is on cuda:{t.device.index}, the scene on cuda:{self.device}")
-        _check(lib().rtb200_scene_update_geometry_device(self.h, C.c_void_p(t.data_ptr()), C.c_void_p(self._stream(stream, t.device) or None)))
+        A = _Arrays("update_geometry", False, self.device)
+        _check(lib().rtb200_scene_update_geometry_device(self.h, A.arg("t", t, (np.float64,), (self.n, 4)), self._stream(stream, A.device)))
 
     def _stream(self, stream, device):
-        """The cudaStream_t handle of `stream` (see :meth:`update_geometry`); None: torch's current stream on `device`."""
+        """The cudaStream_t argument of `stream` (see :meth:`update_geometry`; handle 0 is NULL, the library's own stream);
+        None: torch's current stream on `device`."""
         if stream is None:
             import torch
             stream = torch.cuda.current_stream(device)
-        return (stream.cuda_stream or CUDA_STREAM_LEGACY) if hasattr(stream, "cuda_stream") else int(stream)
+        return C.c_void_p(((stream.cuda_stream or CUDA_STREAM_LEGACY) if hasattr(stream, "cuda_stream") else int(stream)) or None)
 
     def rebuild(self, stream=None):
         """Rebuild the hierarchy from the current spheres on the GPU (rtb200_scene_rebuild): a new topology for spheres that
         moved, ordered like an update on `stream` (as in :meth:`update_geometry`, by default torch's current stream). Returns
         when the new tree exists; later frames trace it and later updates refit it. A no-op without a hierarchy."""
-        _check(lib().rtb200_scene_rebuild(self.h, C.c_void_p(self._stream(stream, self.device) or None)))
+        _check(lib().rtb200_scene_rebuild(self.h, self._stream(stream, self.device)))
 
     def edit_spheres(self, remove: Sequence[int] = (), insert: Sequence[rt_sphere] = (), at: Optional[Sequence[int]] = None, stream=None):
         """Remove the spheres `remove` and place insert[k] just before old sphere at[k] (None: append every insert), on the GPU
@@ -871,37 +930,29 @@ class ResidentScene:
         arr = (rt_sphere * max(len(insert), 1))(*insert)
         _check(lib().rtb200_scene_edit_spheres(self.h, rem.ctypes.data if rem.size else None, rem.size,
                                                pos.ctypes.data if pos is not None and pos.size else None, arr, len(insert),
-                                               C.c_void_p(self._stream(stream, self.device) or None)))
+                                               self._stream(stream, self.device)))
         self.n += len(insert) - rem.size
 
     def adaptive_begin(self, params: rt_adaptive_params, stream=None):
         """(Re)start an adaptive render of the handle (rtb200_adaptive_begin): n = 0 everywhere, every pixel active. `stream`
         as in :meth:`update_geometry`."""
-        _check(lib().rtb200_adaptive_begin(self.h, C.byref(params), C.c_void_p(self._stream(stream, self.device) or None)))
+        _check(lib().rtb200_adaptive_begin(self.h, C.byref(params), self._stream(stream, self.device)))
 
     def adaptive_step(self, rounds: int = 1, stream=None):
         """Run up to `rounds` rounds and wait (rtb200_adaptive_step). Returns (pixels still active, stats summed over the
         rounds)."""
         active = C.c_uint32(); st = rt_stats()
-        _check(lib().rtb200_adaptive_step(self.h, int(rounds), C.c_void_p(self._stream(stream, self.device) or None), C.byref(active), C.byref(st)))
+        _check(lib().rtb200_adaptive_step(self.h, int(rounds), self._stream(stream, self.device), C.byref(active), C.byref(st)))
         return int(active.value), st.as_dict()
 
     def adaptive_resolve(self, rgb8=None, linear=None, counts=None, stream=None):
         """Write the current adaptive image into CUDA tensors (rtb200_adaptive_resolve), each optional: uint8 rgb8 and float32
         linear of rows * w * 3 elements, int32 or uint32-sized counts of rows * w elements, on the handle's device."""
-        import torch
         n = self.rows * self.scene.c.width
-        ptrs = []
-        for t, dt, size in ((rgb8, (torch.uint8,), 3 * n), (linear, (torch.float32,), 3 * n), (counts, (torch.int32,), n)):
-            if t is None:
-                ptrs.append(None)
-                continue
-            if not isinstance(t, torch.Tensor) or not t.is_cuda or t.dtype not in dt or t.numel() != size or not t.is_contiguous():
-                raise ValueError(f"adaptive_resolve takes contiguous CUDA tensors of {dt[0]} with {size} elements")
-            if self.device is not None and t.device.index != self.device:
-                raise ValueError(f"the tensor is on cuda:{t.device.index}, the scene on cuda:{self.device}")
-            ptrs.append(C.c_void_p(t.data_ptr()))
-        _check(lib().rtb200_adaptive_resolve(self.h, *ptrs, C.c_void_p(self._stream(stream, self.device) or None)))
+        A = _Arrays("adaptive_resolve", False, self.device)
+        ptrs = [A.arg("rgb8", rgb8, (np.uint8,), 3 * n, True), A.arg("linear", linear, (np.float32,), 3 * n, True),
+                A.arg("counts", counts, (np.int32,), n, True)]
+        _check(lib().rtb200_adaptive_resolve(self.h, *ptrs, self._stream(stream, self.device)))
 
     def intersect(self, origin, direction, t_max=None, stream=None, outputs=None) -> dict:
         """Closest hits of caller-supplied rays on the handle's current spheres: for ray i, hit_world(world, Ray{origin[i],
@@ -918,18 +969,16 @@ class ResidentScene:
         unknown = [k for k in names if k not in dict((f[0], f) for f in HIT_FIELDS)]
         if unknown or not names:
             raise ValueError(f"intersect outputs are a non-empty subset of {[f[0] for f in HIT_FIELDS]}, got {names}")
-        fields = [f for f in HIT_FIELDS if f[0] in names]
-        if isinstance(origin, np.ndarray):
-            out, rays, n = self._query_host_args("intersect", origin, direction, t_max, fields)
-            hits = rt_hits(*(out[k].ctypes.data if k in out else None for k, _, _ in HIT_FIELDS))
+        A = _Arrays("intersect", device=self.device)
+        rays, n = _rays(A, origin, direction, t_max)
+        out = A.empty([(k, (n, c) if c > 1 else (n,), ty) for k, c, ty in HIT_FIELDS if k in names], stream)
+        hits = rt_hits(*(A.ptr(out.get(k)) for k, _, _ in HIT_FIELDS))
+        if A.host:
             st = rt_stats()
             _check(lib().rtb200_scene_intersect(self.h, C.byref(rays), n, C.byref(hits), C.byref(st)))
             out["stats"] = st.as_dict()
-            return out
-        out, rays, n = self._query_device_args("intersect", origin, direction, t_max, stream, fields)
-        if n:
-            hits = rt_hits(*(out[k].data_ptr() if k in out else None for k, _, _ in HIT_FIELDS))
-            _check(lib().rtb200_scene_intersect_device(self.h, C.byref(rays), n, C.byref(hits), C.c_void_p(self._stream(stream, origin.device) or None)))
+        elif n:
+            _check(lib().rtb200_scene_intersect_device(self.h, C.byref(rays), n, C.byref(hits), self._stream(stream, A.device)))
         return out
 
     def occluded(self, origin, direction, t_max=None, stream=None) -> dict:
@@ -941,17 +990,15 @@ class ResidentScene:
         CUDA tensors use the device form (rtb200_scene_occluded_device) and numpy arrays the blocking host form
         (rtb200_scene_occluded), with the same arguments, checks and stream ordering as :meth:`intersect`. Returns
         {"occluded": uint8 [n]}, and with numpy arrays also "stats"."""
-        fields = [("occluded", 1, np.uint8)]
-        if isinstance(origin, np.ndarray):
-            out, rays, n = self._query_host_args("occluded", origin, direction, t_max, fields)
+        A = _Arrays("occluded", device=self.device)
+        rays, n = _rays(A, origin, direction, t_max)
+        out = A.empty([("occluded", (n,), np.uint8)], stream)
+        if A.host:
             st = rt_stats()
-            _check(lib().rtb200_scene_occluded(self.h, C.byref(rays), n, C.c_void_p(out["occluded"].ctypes.data), C.byref(st)))
+            _check(lib().rtb200_scene_occluded(self.h, C.byref(rays), n, A.ptr(out["occluded"]), C.byref(st)))
             out["stats"] = st.as_dict()
-            return out
-        out, rays, n = self._query_device_args("occluded", origin, direction, t_max, stream, fields)
-        if n:
-            _check(lib().rtb200_scene_occluded_device(self.h, C.byref(rays), n, C.c_void_p(out["occluded"].data_ptr()),
-                                                      C.c_void_p(self._stream(stream, origin.device) or None)))
+        elif n:
+            _check(lib().rtb200_scene_occluded_device(self.h, C.byref(rays), n, A.ptr(out["occluded"]), self._stream(stream, A.device)))
         return out
 
     def trace_rays(self, origin, direction, samples: int = 1, *, sample0: int = 0, stream0: int = 0, seed: Optional[int] = None,
@@ -967,25 +1014,20 @@ class ResidentScene:
         {"rgb8": uint8 [n, 3]}, whichever is asked for, and "stats"."""
         if not (linear or rgb8):
             raise ValueError("trace_rays: ask for linear, rgb8 or both")
-        fields = ([("linear", 3, np.float32)] if linear else []) + ([("rgb8", 3, np.uint8)] if rgb8 else [])
         p = rt_trace_params(self.scene.seed if seed is None else int(seed), int(samples), int(sample0), int(stream0),
                             self.scene.c.max_depth if max_depth is None else int(max_depth))
         st = rt_stats()
-        host = isinstance(origin, np.ndarray)
-        if host:
-            out, rays, n = self._query_host_args("trace_rays", origin, direction, None, fields)
-        else:
-            out, rays, n = self._query_device_args("trace_rays", origin, direction, None, stream, fields)
-        ptr = (lambda a: a.ctypes.data) if host else (lambda t: t.data_ptr())
-        lin_p = C.c_void_p(ptr(out["linear"])) if linear else None
-        rgb_p = C.c_void_p(ptr(out["rgb8"])) if rgb8 else None
+        A = _Arrays("trace_rays", device=self.device)
+        rays, n = _rays(A, origin, direction, None)
+        out = A.empty(([("linear", (n, 3), np.float32)] if linear else []) + ([("rgb8", (n, 3), np.uint8)] if rgb8 else []), stream)
+        lin_p, rgb_p = A.ptr(out.get("linear")), A.ptr(out.get("rgb8"))
         if n == 0:   # nothing to trace (the library's no-op)
             pass
-        elif host:
+        elif A.host:
             _check(lib().rtb200_scene_trace_rays(self.h, C.byref(rays), n, C.byref(p), lin_p, rgb_p, C.byref(st)))
         else:
             _check(lib().rtb200_scene_trace_rays_device(self.h, C.byref(rays), n, C.byref(p), lin_p, rgb_p,
-                                                        C.c_void_p(self._stream(stream, origin.device) or None), C.byref(st)))
+                                                        self._stream(stream, A.device), C.byref(st)))
         out["stats"] = st.as_dict()
         return out
 
@@ -1008,59 +1050,20 @@ class ResidentScene:
         shape = (self.rows, int(self.scene.c.width))
         p = rt_aov_params(int(samples), int(sample0))
         vp = C.byref(view) if view is not None else None
-        if not on_device:
-            out = {k: np.empty(shape + ((c,) if c > 1 else ()), dtype=ty) for k, c, ty in AOV_FIELDS if k in names}
-            o = rt_aov_out(*(out[k].ctypes.data if k in out else None for k, _, _ in AOV_FIELDS))
+        device = self.device
+        if on_device and device is None:
+            import torch
+            device = torch.cuda.current_device()
+        A = _Arrays("aov", not on_device, device)
+        out = A.empty([(k, shape + ((c,) if c > 1 else ()), ty) for k, c, ty in AOV_FIELDS if k in names], stream)
+        o = rt_aov_out(*(A.ptr(out.get(k)) for k, _, _ in AOV_FIELDS))
+        if A.host:
             st = rt_stats()
             _check(lib().rtb200_scene_aov(self.h, C.byref(p), vp, C.byref(o), C.byref(st)))
             out["stats"] = st.as_dict()
-            return out
-        import torch
-        device = torch.device("cuda", self.device if self.device is not None else torch.cuda.current_device())
-        dt = {np.float64: torch.float64, np.float32: torch.float32, np.int32: torch.int32, np.uint32: torch.uint32}
-        # the outputs belong to the call's stream when it is a torch stream (the caching allocator orders their reuse after it)
-        with torch.cuda.stream(stream) if isinstance(stream, torch.cuda.Stream) else torch.cuda.device(device):
-            out = {k: torch.empty(shape + ((c,) if c > 1 else ()), dtype=dt[ty], device=device) for k, c, ty in AOV_FIELDS if k in names}
-        if self.rows == 0:   # a shard with no rows (the library's no-op)
-            return out
-        o = rt_aov_out(*(out[k].data_ptr() if k in out else None for k, _, _ in AOV_FIELDS))
-        _check(lib().rtb200_scene_aov_device(self.h, C.byref(p), vp, C.byref(o), C.c_void_p(self._stream(stream, device) or None)))
+        elif self.rows:   # a shard with no rows is the library's no-op
+            _check(lib().rtb200_scene_aov_device(self.h, C.byref(p), vp, C.byref(o), self._stream(stream, device)))
         return out
-
-    def _query_device_args(self, what, origin, direction, t_max, stream, fields):
-        """Checks of a query's CUDA tensors; returns the outputs `fields` (name, values per ray, numpy dtype), rt_rays and n."""
-        import torch
-        args = [("origin", origin, 2), ("direction", direction, 2)] + ([("t_max", t_max, 1)] if t_max is not None else [])
-        n = origin.shape[0] if isinstance(origin, torch.Tensor) and origin.dim() == 2 else -1
-        for name, t, dim in args:
-            if not isinstance(t, torch.Tensor) or not t.is_cuda:
-                raise ValueError(f"{what} takes CUDA tensors (or numpy arrays): {name} is {type(t).__name__}")
-            shape = (n, 3) if dim == 2 else (n,)
-            if t.dtype != torch.float64 or tuple(t.shape) != shape or n < 0 or not t.is_contiguous():
-                raise ValueError(f"{what}: {name} must be a contiguous float64 tensor of shape {list(shape) if n >= 0 else '[n, 3]'}, got {t.dtype} {tuple(t.shape)}")
-            if self.device is not None and t.device.index != self.device:
-                raise ValueError(f"the tensor {name} is on cuda:{t.device.index}, the scene on cuda:{self.device}")
-            if t.device != origin.device:
-                raise ValueError(f"origin is on {origin.device}, {name} on {t.device}")
-        dt = {np.float64: torch.float64, np.float32: torch.float32, np.int32: torch.int32, np.uint8: torch.uint8}
-        # outputs belong to the query's stream when it is a torch stream (the caching allocator orders their reuse after it)
-        with torch.cuda.stream(stream) if isinstance(stream, torch.cuda.Stream) else torch.cuda.device(origin.device):
-            out = {k: torch.empty((n, c) if c > 1 else (n,), dtype=dt[ty], device=origin.device) for k, c, ty in fields}
-        rays = rt_rays(origin.data_ptr(), direction.data_ptr(), t_max.data_ptr() if t_max is not None else None)
-        return out, rays, n
-
-    def _query_host_args(self, what, origin, direction, t_max, fields):
-        """Checks of a query's numpy arrays; returns the outputs `fields`, rt_rays and n."""
-        n = origin.shape[0] if origin.ndim == 2 else -1
-        for name, a, shape in (("origin", origin, (n, 3)), ("direction", direction, (n, 3)), ("t_max", t_max, (n,))):
-            if name == "t_max" and a is None:
-                continue
-            if not isinstance(a, np.ndarray) or a.dtype != np.float64 or a.shape != shape or n < 0 or not a.flags.c_contiguous:
-                raise ValueError(f"{what}: {name} must be a C-contiguous float64 array of shape {list(shape) if n >= 0 else '[n, 3]'}, "
-                                 f"got {getattr(a, 'dtype', type(a).__name__)} {getattr(a, 'shape', '')}")
-        out = {k: np.empty((n, c) if c > 1 else (n,), dtype=ty) for k, c, ty in fields}
-        rays = rt_rays(origin.ctypes.data, direction.ctypes.data, t_max.ctypes.data if t_max is not None else None)
-        return out, rays, n
 
     def topology(self) -> dict:
         """The handle's current topology (rtb200_scene_debug_topology): recentre, leaf_id [n_leaves, k], always, skip_pos,
@@ -1147,43 +1150,28 @@ def denoise(color, albedo=None, normal=None, *, iterations: int = DENOISE_ITERAT
         albedo_weight = DENOISE_ALBEDO_WEIGHT if albedo is not None else 0.0
     if normal_weight is None:
         normal_weight = DENOISE_NORMAL_WEIGHT if normal is not None else 0.0
-    host = isinstance(color, np.ndarray)
     shape = tuple(color.shape)
     if len(shape) != 3 or shape[2] != 3:
         raise ValueError(f"denoise: color must have shape [h, w, 3], got {shape}")
-    for name, g in (("color", color), ("albedo", albedo), ("normal", normal)):
-        if g is None:
-            continue
-        if host:
-            ok = isinstance(g, np.ndarray) and g.dtype == np.float32 and g.flags.c_contiguous
-        else:
-            import torch
-            ok = isinstance(g, torch.Tensor) and g.is_cuda and g.dtype == torch.float32 and g.is_contiguous() and g.device == color.device
-        if not ok or tuple(g.shape) != shape:
-            kind = "C-contiguous float32 numpy arrays" if host else "contiguous float32 CUDA tensors on one device"
-            raise ValueError(f"denoise takes {kind} of shape {list(shape)}: {name} is not one")
+    A = _Arrays("denoise")
+    guides = [A.arg(name, g, (np.float32,), shape, name != "color") for name, g in (("color", color), ("albedo", albedo), ("normal", normal))]
     p = rt_denoise_params(shape[1], shape[0], int(iterations), 0, float(color_weight), float(albedo_weight), float(normal_weight), 0.0)
-    if host:
-        out = {k: np.empty(shape, dtype=ty) for k, ty, want in (("linear", np.float32, linear), ("rgb8", np.uint8, rgb8)) if want}
+    outs = [(k, shape, ty) for k, ty, want in (("linear", np.float32, linear), ("rgb8", np.uint8, rgb8)) if want]
+    if A.host:
+        out = A.empty(outs)
         st = rt_stats()
-        ptr = lambda a: a.ctypes.data if a is not None else None  # noqa: E731
-        _check(lib().rtb200_denoise(-1, C.byref(p), ptr(color), ptr(albedo), ptr(normal), ptr(out.get("linear")), ptr(out.get("rgb8")),
-                                    C.byref(st)))
+        _check(lib().rtb200_denoise(-1, C.byref(p), *guides, A.ptr(out.get("linear")), A.ptr(out.get("rgb8")), C.byref(st)))
         out["stats"] = st.as_dict()
         return out
-    import torch
-    device = color.device
-    stream, handle = _call_stream(stream, device, "denoise", "the scratch")
+    stream, handle = _call_stream(stream, A.device, "denoise", "the scratch")
     # the scratch and the outputs belong to the call's stream: the caching allocator reuses the scratch, freed when this
     # function returns, only for later work on that stream, which runs after the call
-    with torch.cuda.stream(stream):
-        scratch = torch.empty(int(lib().rtb200_denoise_scratch_bytes(shape[1], shape[0])), dtype=torch.uint8, device=device)
-        out = {k: torch.empty(shape, dtype=ty, device=device) for k, ty, want in (("linear", torch.float32, linear), ("rgb8", torch.uint8, rgb8)) if want}
+    out = A.empty(outs + [("scratch", (int(lib().rtb200_denoise_scratch_bytes(shape[1], shape[0])),), np.uint8)], stream)
+    scratch = out.pop("scratch")
     if color.numel() == 0:   # a 0-pixel image (the library's no-op)
         return out
-    ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
-    _check(lib().rtb200_denoise_device(device.index, C.byref(p), ptr(color), ptr(albedo), ptr(normal), ptr(scratch),
-                                       ptr(out.get("linear")), ptr(out.get("rgb8")), C.c_void_p(handle)))
+    _check(lib().rtb200_denoise_device(A.device, C.byref(p), *guides, A.ptr(scratch), A.ptr(out.get("linear")), A.ptr(out.get("rgb8")),
+                                       C.c_void_p(handle)))
     return out
 
 
@@ -1228,7 +1216,6 @@ def _max_history(n) -> int:
 
 def _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol, stream, out):
     """temporal(), writing into `out` ({"color", "length"} CUDA tensors of the right shapes) when it is given."""
-    host = isinstance(color, np.ndarray)
     shape = tuple(color.shape)
     if len(shape) != 3 or shape[2] != 3:
         raise ValueError(f"temporal: color must have shape [h, w, 3], got {shape}")
@@ -1236,50 +1223,32 @@ def _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol
     prev = dict(prev) if prev is not None else None
     if prev is not None and not {"color", "length", "sphere", "point", "camera"} <= set(prev):
         raise ValueError("temporal: prev holds the previous frame's color, length, sphere, point and camera")
-    args = [("color", color, (np.float32,), shape), ("sphere", sphere, (np.int32, np.uint32), hw), ("point", point, (np.float64,), shape)]
+    A = _Arrays("temporal")
+    f32, f64, u32, ids = (np.float32,), (np.float64,), (np.uint32,), (np.int32, np.uint32)
+    cur = rt_temporal_frame(A.arg("color", color, f32, shape), A.arg("sphere", sphere, ids, hw), A.arg("point", point, f64, shape))
+    hist = None
     if prev is not None:
-        args += [("prev color", prev["color"], (np.float32,), shape), ("prev length", prev["length"], (np.uint32,), hw),
-                 ("prev sphere", prev["sphere"], (np.int32, np.uint32), hw), ("prev point", prev["point"], (np.float64,), shape)]
-    if motion is not None:
-        args.append(("motion", motion, (np.float64,), (int(motion.shape[0]), 3) if len(motion.shape) == 2 else None))
-    if host:
-        for name, a, dts, shp in args:
-            if not (isinstance(a, np.ndarray) and a.dtype in dts and a.flags.c_contiguous and a.shape == shp):
-                raise ValueError(f"temporal takes C-contiguous numpy arrays: {name} must be {'/'.join(np.dtype(d).name for d in dts)} {shp}")
-    else:
-        import torch
-        tdt = {np.float32: torch.float32, np.float64: torch.float64, np.int32: torch.int32, np.uint32: torch.uint32}
-        for name, a, dts, shp in args:
-            if not (isinstance(a, torch.Tensor) and a.is_cuda and a.device == color.device and a.dtype in [tdt[d] for d in dts]
-                    and a.is_contiguous() and tuple(a.shape) == shp):
-                raise ValueError(f"temporal takes contiguous CUDA tensors on one device: {name} must be "
-                                 f"{'/'.join(np.dtype(d).name for d in dts)} {shp}")
+        hist = rt_temporal_history(A.arg("prev color", prev["color"], f32, shape), A.arg("prev length", prev["length"], u32, hw),
+                                   A.arg("prev sphere", prev["sphere"], ids, hw), A.arg("prev point", prev["point"], f64, shape))
+    mp = A.arg("motion", motion, f64, (motion.shape[0] if motion is not None and len(motion.shape) == 2 else "n", 3), True)
     p = rt_temporal_params(hw[1], hw[0], _max_history(max_history), 0 if motion is None else int(motion.shape[0]), _camera_of(camera),
                            _camera_of(prev["camera"]) if prev is not None else rt_camera(), float(depth_tol))
-    if host:
-        ptr = lambda a: a.ctypes.data if a is not None else None  # noqa: E731
-    else:
-        ptr = lambda t: t.data_ptr() if t is not None else None  # noqa: E731
-    cur = rt_temporal_frame(ptr(color), ptr(sphere), ptr(point))
-    hist = rt_temporal_history(*(ptr(prev[k]) for k in ("color", "length", "sphere", "point"))) if prev is not None else None
     hp = C.byref(hist) if hist is not None else None
-    if host:
-        out = {"color": np.empty(shape, np.float32), "length": np.empty(hw, np.uint32)}
+    outs = [("color", shape, np.float32), ("length", hw, np.uint32)]
+    if A.host:
+        out = A.empty(outs)
         st = rt_stats()
-        _check(lib().rtb200_temporal(-1, C.byref(p), C.byref(cur), hp, ptr(motion), C.byref(rt_temporal_out(ptr(out["color"]), ptr(out["length"]))),
+        _check(lib().rtb200_temporal(-1, C.byref(p), C.byref(cur), hp, mp, C.byref(rt_temporal_out(A.ptr(out["color"]), A.ptr(out["length"]))),
                                      C.byref(st)))
         out["stats"] = st.as_dict()
         return out
-    import torch
-    device = color.device
-    stream, handle = _call_stream(stream, device, "temporal", "the outputs")
+    stream, handle = _call_stream(stream, A.device, "temporal", "the outputs")
     if out is None:
-        with torch.cuda.stream(stream):
-            out = {"color": torch.empty(shape, dtype=torch.float32, device=device), "length": torch.empty(hw, dtype=torch.uint32, device=device)}
+        out = A.empty(outs, stream)
     if color.numel() == 0:   # a 0-pixel image (the library's no-op)
         return out
-    _check(lib().rtb200_temporal_device(device.index, C.byref(p), C.byref(cur), hp, ptr(motion),
-                                        C.byref(rt_temporal_out(ptr(out["color"]), ptr(out["length"]))), C.c_void_p(handle)))
+    _check(lib().rtb200_temporal_device(A.device, C.byref(p), C.byref(cur), hp, mp,
+                                        C.byref(rt_temporal_out(A.ptr(out["color"]), A.ptr(out["length"]))), C.c_void_p(handle)))
     return out
 
 

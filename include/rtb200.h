@@ -265,6 +265,18 @@ int rtb200_render_frames_lens(const rt_scene* scene, const rt_options* opts, con
                               uint32_t n_frames, uint8_t* out_rgb8, float* out_linear_f32, rt_stats* stats);
 int rtb200_render_frames_lens_device(rtb200_scene_handle h, const rt_frame* frames, const rt_lens* lenses, uint32_t n_frames,
                                      void* dev_rgb8, void* dev_linear_f32, void* stream, rt_stats* stats);
+/* The variance of the pixel means (DESIGN.md §4.18): rtb200_render_frames_lens[_device] plus dev_variance_f32 / out_variance
+ * (n_frames * rows * width * 3 floats, not NULL). Per pixel and channel, with S_c the f32 sum of the n = samples_per_pixel
+ * samples in sample order (the render's) and Q_c the f32 sum of x_c * x_c in the same order, every op rounded and never
+ * contracted: inv = 1.0f / n, mean_c = inv * S_c, d_c = inv * Q_c - mean_c * mean_c, var_c = (d_c < 0 ? 0 : d_c) * inv - the
+ * adaptive rule's err_c^2 without its max; a NaN d_c stays NaN; max_depth 0 gives 0. Q carries across sample batches in a
+ * second plane of the work set, grown only by these calls. lenses may be NULL; shards, every variant, multi-frame groups and
+ * batches work as in the frames call; the rgb8 and linear outputs (each may be NULL) equal that call's bit for bit. The resolve
+ * is a kernel of its own, so a render without a variance output launches exactly what it did. */
+int rtb200_render_frames_var_device(rtb200_scene_handle h, const rt_frame* frames, const rt_lens* lenses, uint32_t n_frames,
+                                    void* dev_rgb8, void* dev_linear_f32, float* dev_variance_f32, void* stream, rt_stats* stats);
+int rtb200_render_frames_var(const rt_scene* scene, const rt_options* opts, const rt_frame* frames, const rt_lens* lenses,
+                             uint32_t n_frames, uint8_t* out_rgb8, float* out_linear_f32, float* out_variance, rt_stats* stats);
 
 /* ---- moving spheres of a resident scene ---------------------------------------------------------------------------------
  * The hierarchy is refitted on the GPU (its topology and recentring stay as uploaded, DESIGN.md §4.7) instead of rebuilt.
@@ -376,10 +388,20 @@ typedef struct {
 int rtb200_adaptive_begin(rtb200_scene_handle h, const rt_adaptive_params* p, void* stream);
 int rtb200_adaptive_step(rtb200_scene_handle h, uint32_t rounds, void* stream, uint32_t* active_out, rt_stats* stats);
 int rtb200_adaptive_resolve(rtb200_scene_handle h, void* dev_rgb8, void* dev_linear_f32, void* dev_counts_u32, void* stream);
+/* rtb200_adaptive_resolve plus the variance of each pixel's mean (DESIGN.md §4.18) from the adaptive state's own sums S_c, Q_c
+ * and count n: inv = 1/n, mean_c = inv * S_c, d_c = inv * Q_c - mean_c * mean_c, var_c = (d_c < 0 ? 0 : d_c) * inv, every op
+ * rounded and never contracted (a NaN d_c stays NaN; n = 0 gives 0), into dev_variance_f32 (rows * width * 3 floats, not NULL).
+ * The other outputs equal rtb200_adaptive_resolve's bit for bit; it runs its own kernel, so that call launches what it did. */
+int rtb200_adaptive_resolve_var(rtb200_scene_handle h, void* dev_rgb8, void* dev_linear_f32, void* dev_counts_u32,
+                                float* dev_variance_f32, void* stream);
 /* Host form, like rtb200_render_frames: upload, run rounds until no pixel is active, copy back, release. Outputs are host
  * buffers of rows * width * 3 bytes / floats and rows * width counts; each may be NULL. Same checks as begin. */
 int rtb200_render_adaptive(const rt_scene* scene, const rt_options* opts, const rt_adaptive_params* p,
                            uint8_t* out_rgb8, float* out_linear_f32, uint32_t* out_counts, rt_stats* stats);
+/* rtb200_render_adaptive plus out_variance (rows * width * 3 floats, not NULL): rtb200_adaptive_resolve_var's variance of
+ * each pixel's mean; the other outputs equal rtb200_render_adaptive's bit for bit. */
+int rtb200_render_adaptive_var(const rt_scene* scene, const rt_options* opts, const rt_adaptive_params* p, uint8_t* out_rgb8,
+                               float* out_linear_f32, uint32_t* out_counts, float* out_variance, rt_stats* stats);
 
 /* ---- closest-hit queries on a resident scene (DESIGN.md §4.10) -----------------------------------------------------------
  * Contract: for ray i with origin o = origin[3i..3i+2], direction d = direction[3i..3i+2] (any f64 values, not necessarily
@@ -549,6 +571,61 @@ int rtb200_denoise_device(int32_t device, const rt_denoise_params* p, const floa
  * kernel_launches (iterations + 1). Same checks, bar the scratch and the memory kind. */
 int rtb200_denoise(int32_t device, const rt_denoise_params* p, const float* color, const float* albedo, const float* normal,
                    float* out_linear, uint8_t* out_rgb8, rt_stats* stats);
+
+/* ---- the variance-guided denoise (DESIGN.md §4.18) -------------------------------------------------------------------------
+ * The à-trous filter of rtb200_denoise with the colour distance divided by each pixel's prefiltered variance, which is filtered
+ * beside the colour (SVGF), every f32 operation rounded to nearest and never contracted. Inputs, width x height pixels of 3 x f32,
+ * row-major, top row first: color (normally a render's linear mean), variance (normally the variance of that mean) and the
+ * optional guides albedo and normal; a guide is on when it is given and its weight is not 0. eps = variance_floor.
+ * Pixel p is ok when its colour, its variance and every guide given are finite and its variance is >= 0 (-0 is). A pixel that
+ * is not ok keeps its colour and variance in every iteration. Iteration i = 0 .. L-1 reads colour c and variance var (the inputs
+ * for i = 0, else the previous outputs) with step h = 2^i. For each ok p:
+ *   v_q = (var_q0 + var_q1) + var_q2;
+ *   vbar_p = (sum of g[dx] * g[dy] * v_q) / (sum of g[dx] * g[dy]) over the ok q = p + (dx, dy) inside the image, dx, dy in
+ *       -1..1, dy outer, dx inner, g = {1/4, 1/2, 1/4} (step 1 in every iteration), each sum in that order;
+ *   num_k = den = nv_k = 0 and for dy = -2..2 (outer), dx = -2..2 (inner), q = p + h * (dx, dy), skipping q outside the image
+ *   or not ok:
+ *     k = B[dx] * B[dy] with B = {1/16, 1/4, 3/8, 1/4, 1/16};
+ *     d_g = ((q0 - p0)^2 + (q1 - p1)^2) + (q2 - p2)^2 for each guide on (colour from c, albedo and normal as given);
+ *     f = (1 + lc * (d_c / (eps + vbar_p))) * (1 + la * d_a) * (1 + ln * d_n), factors left to right, the colour factor left
+ *         out when lc = 0 and an off guide's left out (f = 1 when none is on); lc is not scaled by 4^i;
+ *     w = k / f; num_k += w * c_q,k; den += w; nv_k += (w * w) * var_q,k.
+ *   The outputs are num_k / den and nv_k / (den * den); p stays ok when all six are finite.
+ * Outputs (each may be NULL, not all three): out_linear (3 x f32), out_rgb8 (the render's quantisation of sqrt(linear), as
+ * rtb200_probe_quantise) and out_variance (3 x f32). Whole frames only: gather a sharded render first. */
+typedef struct {
+    uint32_t width, height;
+    uint32_t iterations;          /* L, in [1, 10] */
+    uint32_t reserved;            /* must be 0 */
+    float    color_weight, albedo_weight, normal_weight;   /* finite, >= 0; 0 turns that guide off */
+    float    variance_floor;      /* eps: finite, > 0 */
+} rt_denoise_var_params;          /* 32 bytes */
+/* Defaults of the Python binding and the CLI (DESIGN.md §4.18: chosen on the cover render at 64 x 48, 2 to 32 spp). On frames of
+ * 800 x 600 and 1920 x 1080 they lose to rtb200_denoise's defaults at 4 and 8 spp and win from 16 spp up. */
+#define RTB200_DENOISE_VAR_DEFAULT_ITERATIONS     3
+#define RTB200_DENOISE_VAR_DEFAULT_COLOR_WEIGHT   1.0f
+#define RTB200_DENOISE_VAR_DEFAULT_ALBEDO_WEIGHT  4.0f
+#define RTB200_DENOISE_VAR_DEFAULT_NORMAL_WEIGHT  1.0f
+#define RTB200_DENOISE_VAR_DEFAULT_VARIANCE_FLOOR 1e-4f
+/* Bytes of device scratch rtb200_denoise_var_device needs for width x height pixels (the library owns its layout). */
+uint64_t rtb200_denoise_var_scratch_bytes(uint32_t width, uint32_t height);
+/* Device buffers of `device` (-1: the current device) or managed memory; scratch holds rtb200_denoise_var_scratch_bytes and is
+ * 16-byte aligned. Stream-ordered as rtb200_denoise_device: runs on `stream` (NULL: the library's stream of that device)
+ * without waiting, touches no scene handle and no work set.
+ * RT_ERR_INVALID, before any device work, for a NULL params, color, variance or scratch, all three outputs NULL, a nonzero
+ * reserved, iterations outside [1, 10], a weight that is NaN, negative or infinite, a variance_floor that is not finite or not
+ * > 0, a nonzero weight for a NULL guide, width * height >= 2^31, a buffer that is not 4-byte aligned, an output or the scratch
+ * overlapping an input or each other, or a pointer that is not device memory of `device` nor managed memory. A 0-pixel image
+ * is a no-op. */
+int rtb200_denoise_var_device(int32_t device, const rt_denoise_var_params* p, const float* color, const float* variance,
+                              const float* albedo, const float* normal, void* scratch, float* out_linear, uint8_t* out_rgb8,
+                              float* out_variance, void* stream);
+/* Host buffers, blocking: the same through the same kernels on the library's stream, with the inputs copied in and the outputs
+ * copied out. stats (may be NULL): device_ms, trace_ms (the kernels), wall_ms, h2d_bytes, d2h_bytes and kernel_launches
+ * (2 * iterations + 1). Same checks, bar the scratch and the memory kind. */
+int rtb200_denoise_var(int32_t device, const rt_denoise_var_params* p, const float* color, const float* variance,
+                       const float* albedo, const float* normal, float* out_linear, uint8_t* out_rgb8, float* out_variance,
+                       rt_stats* stats);
 
 /* ---- temporal accumulation of animation frames (DESIGN.md §4.16) ----------------------------------------------------------
  * Blends each pixel of a frame with the history of the previous frame where its first hit was, the reprojection and blend of

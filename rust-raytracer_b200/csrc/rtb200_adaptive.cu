@@ -69,6 +69,30 @@ __global__ void __launch_bounds__(256) rt_adaptive_resolve_kernel(const Adaptive
     }
 }
 
+// rt_adaptive_resolve_kernel plus the variance of each pixel's mean from S, Q and n (0 where n = 0), as rt_resolve_var_kernel
+__global__ void __launch_bounds__(256) rt_adaptive_resolve_var_kernel(const AdaptiveResolveVarParams v) {
+    const AdaptiveResolveParams& q = v.r;
+    const uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
+    if (lp >= q.npix_local) return;
+    const uint32_t n = q.count[lp];
+    if (q.out_count) q.out_count[lp] = n;
+    float m[3] = {0.0f, 0.0f, 0.0f}, var[3] = {0.0f, 0.0f, 0.0f};
+    if (n) {
+        const float inv = __fdiv_rn(1.0f, (float)n);
+        for (int c = 0; c < 3; ++c) {
+            const float S = q.sum[3 * (size_t)lp + c], Q = v.sq[3 * (size_t)lp + c];
+            m[c] = __fmul_rn(inv, S);
+            const float d = __fsub_rn(__fmul_rn(inv, Q), __fmul_rn(m[c], m[c]));
+            var[c] = __fmul_rn(d < 0.0f ? 0.0f : d, inv);
+        }
+    }
+    for (int c = 0; c < 3; ++c) {
+        if (q.out_linear) q.out_linear[3 * (size_t)lp + c] = m[c];
+        if (q.out_rgb8) q.out_rgb8[3 * (size_t)lp + c] = quantise_u8(m[c]);
+        v.out_variance[3 * (size_t)lp + c] = var[c];
+    }
+}
+
 // begin: every pixel on the list, in increasing order
 __global__ void __launch_bounds__(256) rt_adaptive_list_kernel(uint32_t* list, uint32_t* list_n, uint32_t npix_local) {
     const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
@@ -100,6 +124,11 @@ cudaError_t launch_adaptive_compact(void* temp, size_t temp_bytes, const uint32_
 
 cudaError_t launch_adaptive_resolve(const AdaptiveResolveParams& q, cudaStream_t st) {
     rt_adaptive_resolve_kernel<<<(q.npix_local + 255u) / 256u, 256, 0, st>>>(q);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_adaptive_resolve_var(const AdaptiveResolveVarParams& v, cudaStream_t st) {
+    rt_adaptive_resolve_var_kernel<<<(v.r.npix_local + 255u) / 256u, 256, 0, st>>>(v);
     return cudaGetLastError();
 }
 

@@ -187,8 +187,10 @@ static rt_frame own_frame(rtb200_scene_handle h) { return rt_frame{h->tp.cam, h-
 // slice i (rows * width * 3 elements). Frame i's lens is lenses[i], or the handle's (h->tp.lens) when lenses is null. When no
 // frame has a lens the launches are the pinhole ones; else every group, one frame or many, runs the multi-frame kernel with
 // the lens (Q_FRAMES_LENS), which reads each frame's camera, key and lens from the frame and lens tables.
+// With dev_var (n * rows * width * 3 f32), the resolve is rt_resolve_var_kernel, which also writes each frame's variance of
+// the pixel means and carries the sums of squares across batches in the set's accum_sq.
 static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_t n, void* dev_rgb8, void* dev_linear_f32,
-                          void* stream_in, int set, const rt_lens* lenses = nullptr) {
+                          void* stream_in, int set, const rt_lens* lenses = nullptr, float* dev_var = nullptr) {
     Submit s;
     int rc = submission_open(h, stream_in, n, &s);
     if (rc != RT_OK) return rc;
@@ -227,6 +229,7 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
     for (uint32_t i = 0; i < tab.size(); ++i) {
         tab[i].cam = frames[i].camera; tab[i].key0 = (uint32_t)frames[i].seed; tab[i].key1 = (uint32_t)(frames[i].seed >> 32);
     }
+    if (dev_var) CU(h->ctx->ws[set].accum_sq.ensure((size_t)npl * 12, h->ctx->ws[set].done));
     if ((rc = submission_begin(h, set, all_batches, std::max(h->grid, multi.grid), tp, max_depth, sbuf, tab.data(),
                                (uint32_t)tab.size(), &s, lensed ? ltab.data() : nullptr)) != RT_OK)
         return rc;
@@ -258,7 +261,12 @@ static int render_enqueue(rtb200_scene_handle h, const rt_frame* frames, uint32_
                 r.samplebuf = q.samplebuf + (size_t)j * q.s_count * npl; r.accum = (float*)s.W->accum.p; r.npix_local = q.npix_local;
                 r.s_count = q.s_count; r.first = k == 0; r.last = k + 1 == batches; r.spp = spp;
                 r.out_linear = ol ? ol + (size_t)j * npl * 3 : nullptr; r.out_rgb8 = o8 ? o8 + (size_t)j * npl * 3 : nullptr;
-                CU(launch_resolve(r, s.st));
+                if (dev_var) {
+                    const ResolveVarParams v{r, (float*)s.W->accum_sq.p, dev_var + ((size_t)g.first + j) * npl * 3};
+                    CU(launch_resolve_var(v, s.st));
+                } else {
+                    CU(launch_resolve(r, s.st));
+                }
             }
         }
         s.sub.launches += batches * (1 + g.count);
@@ -337,9 +345,9 @@ static int blocking(rtb200_scene_handle h, rt_stats* stats, Enqueue&& enqueue) {
 }
 
 static int render_blocking(rtb200_scene_handle h, const rt_frame* frames, uint32_t n, void* dev_rgb8, void* dev_linear_f32,
-                           void* stream_in, rt_stats* stats, const rt_lens* lenses = nullptr) {
+                           void* stream_in, rt_stats* stats, const rt_lens* lenses = nullptr, float* dev_var = nullptr) {
     HANDLE_PROLOGUE(h);
-    return blocking(h, stats, [&] { return render_enqueue(h, frames, n, dev_rgb8, dev_linear_f32, stream_in, 0, lenses); });
+    return blocking(h, stats, [&] { return render_enqueue(h, frames, n, dev_rgb8, dev_linear_f32, stream_in, 0, lenses, dev_var); });
 }
 
 // Releases a scene handle on scope exit; the error that made the scope return early survives the release.
@@ -349,10 +357,11 @@ struct ReleaseGuard {
 };
 
 // A call on host buffers: upload s, run `body(h, dev, &stats)` with the context's output buffers dev[k] for `frames` frames
-// of the shard (rgb8, linear f32, u32 counts, each only when out[k] asks for it), copy them to out[k] and release the scene.
+// of the shard (rgb8, linear f32, u32 counts, f32 variance, each only when out[k] asks for it), copy them to out[k] and release
+// the scene.
 // The stats are body's with the upload's bytes, the copies' bytes plus `d2h` bytes the body read back, and the wall time.
 template <typename Body>
-static int one_shot(const rt_scene* s, const rt_options& opts, uint64_t frames, void* const out[3], uint64_t d2h, rt_stats* stats,
+static int one_shot(const rt_scene* s, const rt_options& opts, uint64_t frames, void* const out[4], uint64_t d2h, rt_stats* stats,
                     Body&& body) {
     const auto wall0 = std::chrono::steady_clock::now();
     rtb200_scene_handle h = nullptr;
@@ -361,13 +370,13 @@ static int one_shot(const rt_scene* s, const rt_options& opts, uint64_t frames, 
     ReleaseGuard rel{h};
     HANDLE_PROLOGUE(h);
     DeviceCtx* ctx = h->ctx;
-    GrowBuf* buf[3] = {&ctx->out_rgb8, &ctx->out_lin, &ctx->out_cnt};
-    const size_t pixels = frames * h->tp.npix_local, elem[3] = {3, 12, 4};
-    void* dev[3] = {nullptr, nullptr, nullptr};
-    for (int k = 0; k < 3; ++k) if (out[k]) { CU(buf[k]->ensure(pixels * elem[k] + 16)); dev[k] = buf[k]->p; }
+    GrowBuf* buf[4] = {&ctx->out_rgb8, &ctx->out_lin, &ctx->out_cnt, &ctx->out_var};
+    const size_t pixels = frames * h->tp.npix_local, elem[4] = {3, 12, 4, 12};
+    void* dev[4] = {nullptr, nullptr, nullptr, nullptr};
+    for (int k = 0; k < 4; ++k) if (out[k]) { CU(buf[k]->ensure(pixels * elem[k] + 16)); dev[k] = buf[k]->p; }
     rt_stats st{};
     if ((rc = body(h, dev, &st)) != RT_OK) return rc;
-    for (int k = 0; k < 3; ++k) {
+    for (int k = 0; k < 4; ++k) {
         if (out[k] && pixels) CU(cudaMemcpyAsync(out[k], dev[k], pixels * elem[k], cudaMemcpyDeviceToHost, ctx->stream));
         if (out[k]) d2h += pixels * elem[k];
     }
@@ -381,16 +390,16 @@ static int one_shot(const rt_scene* s, const rt_options& opts, uint64_t frames, 
 
 // Host buffers: render `frames` of s. The single-frame calls pass the scene's own view as one frame.
 static int render_host(const rt_scene* s, const rt_options* opts_in, const rt_frame* frames, uint32_t n_frames, uint8_t* out_rgb8,
-                       float* out_lin, rt_stats* stats, const rt_lens* lenses = nullptr) {
+                       float* out_lin, rt_stats* stats, const rt_lens* lenses = nullptr, float* out_var = nullptr) {
     rt_options opts;
     int rc = normalise_options(opts_in, &opts);
     if (rc != RT_OK) return rc;
     uint32_t n_lights = 0;
     if ((rc = validate_scene(s, &n_lights)) != RT_OK) return rc;
     if ((rc = check_frames(frames, n_frames, rtb200_shard_rows(s->height, opts.rank, opts.world, opts.band_rows), s->width, lenses)) != RT_OK) return rc;
-    void* const out[3] = {out_rgb8, out_lin, nullptr};
+    void* const out[4] = {out_rgb8, out_lin, nullptr, out_var};
     return one_shot(s, opts, n_frames, out, 128 + 16, stats, [&](rtb200_scene_handle h, void* const* dev, rt_stats* st) {
-        return render_blocking(h, frames, n_frames, dev[0], dev[1], nullptr, st, lenses);
+        return render_blocking(h, frames, n_frames, dev[0], dev[1], nullptr, st, lenses, (float*)dev[3]);
     });
 }
 
@@ -456,6 +465,27 @@ int rtb200_render_frames_lens(const rt_scene* s, const rt_options* opts_in, cons
 int rtb200_render_frames(const rt_scene* s, const rt_options* opts_in, const rt_frame* frames, uint32_t n_frames, uint8_t* out_rgb8,
                          float* out_lin, rt_stats* stats) {
     return rtb200_render_frames_lens(s, opts_in, frames, nullptr, n_frames, out_rgb8, out_lin, stats);
+}
+
+// ---- the variance of the pixel means (DESIGN.md §4.18) ----
+int rtb200_render_frames_var_device(rtb200_scene_handle h, const rt_frame* frames, const rt_lens* lenses, uint32_t n_frames,
+                                    void* dev_rgb8, void* dev_linear_f32, float* dev_variance_f32, void* stream_in, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    int rc = check_frames(frames, n_frames, h->tp.rows_local, h->tp.width, lenses);
+    if (rc != RT_OK) return rc;
+    if (!dev_variance_f32) return fail(RT_ERR_INVALID, "dev_variance_f32 is null");
+    return render_blocking(h, frames, n_frames, dev_rgb8, dev_linear_f32, stream_in, stats, lenses, dev_variance_f32);
+  });
+}
+
+int rtb200_render_frames_var(const rt_scene* s, const rt_options* opts_in, const rt_frame* frames, const rt_lens* lenses,
+                             uint32_t n_frames, uint8_t* out_rgb8, float* out_lin, float* out_variance, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (!s) return fail(RT_ERR_INVALID, "null argument");
+    if (!out_variance) return fail(RT_ERR_INVALID, "out_variance is null");
+    return render_host(s, opts_in, frames, n_frames, out_rgb8, out_lin, stats, lenses, out_variance);
+  });
 }
 
 // ---- radiance of caller-supplied primary rays on a resident scene (DESIGN.md §4.12) ----
@@ -684,6 +714,26 @@ int rtb200_adaptive_step(rtb200_scene_handle h, uint32_t rounds, void* stream_in
   });
 }
 
+int rtb200_adaptive_resolve_var(rtb200_scene_handle h, void* dev_rgb8, void* dev_linear_f32, void* dev_counts_u32,
+                                float* dev_variance_f32, void* stream_in) {
+  return guarded([&]() -> int {
+    if (!h) return fail(RT_ERR_INVALID, "null scene handle");
+    if (!h->ad.begun) return fail(RT_ERR_INVALID, "no adaptive render on this handle: call rtb200_adaptive_begin");
+    if (!dev_variance_f32) return fail(RT_ERR_INVALID, "dev_variance_f32 is null");
+    if (h->tp.npix_local == 0) return RT_OK;
+    HANDLE_PROLOGUE(h);
+    cudaStream_t st;
+    CU(scene_stream(h, stream_in, &st));
+    AdaptiveResolveVarParams v{};
+    v.r.sum = h->ad.sum; v.r.count = h->ad.count; v.r.npix_local = h->tp.npix_local;
+    v.r.out_linear = (float*)dev_linear_f32; v.r.out_rgb8 = (uint8_t*)dev_rgb8; v.r.out_count = (uint32_t*)dev_counts_u32;
+    v.sq = h->ad.sq; v.out_variance = dev_variance_f32;
+    CU(launch_adaptive_resolve_var(v, st));
+    CU(cudaStreamSynchronize(st));
+    return RT_OK;
+  });
+}
+
 int rtb200_adaptive_resolve(rtb200_scene_handle h, void* dev_rgb8, void* dev_linear_f32, void* dev_counts_u32, void* stream_in) {
   return guarded([&]() -> int {
     if (!h) return fail(RT_ERR_INVALID, "null scene handle");
@@ -701,9 +751,9 @@ int rtb200_adaptive_resolve(rtb200_scene_handle h, void* dev_rgb8, void* dev_lin
   });
 }
 
-int rtb200_render_adaptive(const rt_scene* s, const rt_options* opts_in, const rt_adaptive_params* p, uint8_t* out_rgb8,
-                           float* out_lin, uint32_t* out_counts, rt_stats* stats) {
-  return guarded([&]() -> int {
+// The host form of an adaptive render, with the variance of the pixel means when out_var is not null.
+static int render_adaptive_host(const rt_scene* s, const rt_options* opts_in, const rt_adaptive_params* p, uint8_t* out_rgb8,
+                                float* out_lin, uint32_t* out_counts, float* out_var, rt_stats* stats) {
     if (!s) return fail(RT_ERR_INVALID, "null argument");
     rt_options opts;
     int rc = normalise_options(opts_in, &opts);
@@ -712,15 +762,28 @@ int rtb200_render_adaptive(const rt_scene* s, const rt_options* opts_in, const r
     if ((rc = validate_scene(s, &n_lights)) != RT_OK) return rc;
     const uint64_t npl = (uint64_t)rtb200_shard_rows(s->height, opts.rank, opts.world, opts.band_rows) * s->width;
     if ((rc = check_adaptive(p, npl, sample_buffer_cap(opts))) != RT_OK) return rc;
-    void* const out[3] = {out_rgb8, out_lin, out_counts};
+    void* const out[4] = {out_rgb8, out_lin, out_counts, out_var};
     return one_shot(s, opts, 1, out, 128 + 16 + 4, stats, [&](rtb200_scene_handle h, void* const* dev, rt_stats* st) {
         uint32_t active = 0;
         int rcb = rtb200_adaptive_begin(h, p, nullptr);
         if (rcb == RT_OK) rcb = rtb200_adaptive_step(h, 0xffffffffu, nullptr, &active, st);
-        if (rcb == RT_OK) rcb = rtb200_adaptive_resolve(h, dev[0], dev[1], dev[2], nullptr);
+        if (rcb == RT_OK) rcb = out_var ? rtb200_adaptive_resolve_var(h, dev[0], dev[1], dev[2], (float*)dev[3], nullptr)
+                                        : rtb200_adaptive_resolve(h, dev[0], dev[1], dev[2], nullptr);
         st->frames = 1;
         return rcb;
     });
+}
+
+int rtb200_render_adaptive(const rt_scene* s, const rt_options* opts_in, const rt_adaptive_params* p, uint8_t* out_rgb8,
+                           float* out_lin, uint32_t* out_counts, rt_stats* stats) {
+    return guarded([&]() -> int { return render_adaptive_host(s, opts_in, p, out_rgb8, out_lin, out_counts, nullptr, stats); });
+}
+
+int rtb200_render_adaptive_var(const rt_scene* s, const rt_options* opts_in, const rt_adaptive_params* p, uint8_t* out_rgb8,
+                               float* out_lin, uint32_t* out_counts, float* out_variance, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (!out_variance) return fail(RT_ERR_INVALID, "out_variance is null");
+    return render_adaptive_host(s, opts_in, p, out_rgb8, out_lin, out_counts, out_variance, stats);
   });
 }
 

@@ -91,9 +91,10 @@ struct DeviceCtx {
     // whatever their streams and handles.
     struct WorkSet {
         GrowBuf samplebuf, accum, stack, small, frames, lterm, ftab, ltab;   // ftab / ltab: the multi-frame kernel's frame and lens tables
+        GrowBuf accum_sq;   // the resolve's sums of squares, grown only by a render with a variance output
         cudaEvent_t done = nullptr;
     } ws[2];
-    GrowBuf out_rgb8, out_lin, out_cnt, probe, frame;
+    GrowBuf out_rgb8, out_lin, out_cnt, out_var, probe, frame;
     // scene arenas of released handles, kept for the next upload (a per-frame upload costs no cudaMalloc / cudaFree)
     struct Arena { void* p; size_t cap; };
     std::vector<Arena> arena_cache;

@@ -34,6 +34,42 @@ __global__ void __launch_bounds__(256) rt_resolve_kernel(const ResolveParams q) 
     }
 }
 
+// The variance of a pixel's mean from its sums S_c and Q_c over n samples: inv = 1/n, mean_c = inv * S_c,
+// d_c = inv * Q_c - mean_c * mean_c, var_c = (d_c < 0 ? 0 : d_c) * inv (a NaN d_c stays NaN). n = 0 gives 0.
+static RT_DEV float mean_variance(float S, float Q, float inv) {
+    const float mean = __fmul_rn(inv, S);
+    const float d = __fsub_rn(__fmul_rn(inv, Q), __fmul_rn(mean, mean));
+    return __fmul_rn(d < 0.0f ? 0.0f : d, inv);
+}
+
+// rt_resolve_kernel with the running sums Q_c of x_c * x_c beside S_c and, on the last batch, the variance of the mean: the
+// linear and RGB8 outputs are rt_resolve_kernel's, operation for operation. A separate kernel, so that a render without a
+// variance output launches rt_resolve_kernel exactly as before.
+__global__ void __launch_bounds__(256) rt_resolve_var_kernel(const ResolveVarParams v) {
+    const ResolveParams& q = v.r;
+    uint32_t lp = blockIdx.x * blockDim.x + threadIdx.x;
+    if (lp >= q.npix_local) return;
+    float S[3] = {0.f, 0.f, 0.f}, Q[3] = {0.f, 0.f, 0.f};
+    if (!q.first)
+        for (int c = 0; c < 3; ++c) { S[c] = q.accum[3 * (size_t)lp + c]; Q[c] = v.accum_sq[3 * (size_t)lp + c]; }
+    for (uint32_t s = 0; s < q.s_count; ++s) {
+        const float4 x = q.samplebuf[(size_t)s * q.npix_local + lp];
+        S[0] = __fadd_rn(S[0], x.x); S[1] = __fadd_rn(S[1], x.y); S[2] = __fadd_rn(S[2], x.z);
+        Q[0] = __fadd_rn(Q[0], __fmul_rn(x.x, x.x)); Q[1] = __fadd_rn(Q[1], __fmul_rn(x.y, x.y)); Q[2] = __fadd_rn(Q[2], __fmul_rn(x.z, x.z));
+    }
+    if (!q.last) {
+        for (int c = 0; c < 3; ++c) { q.accum[3 * (size_t)lp + c] = S[c]; v.accum_sq[3 * (size_t)lp + c] = Q[c]; }
+        return;
+    }
+    const float scale = __fdiv_rn(1.0f, (float)q.spp);
+    for (int c = 0; c < 3; ++c) {
+        const float m = __fmul_rn(scale, S[c]);
+        if (q.out_linear) q.out_linear[3 * (size_t)lp + c] = m;
+        if (q.out_rgb8) q.out_rgb8[3 * (size_t)lp + c] = quantise_u8(m);
+        v.out_variance[3 * (size_t)lp + c] = mean_variance(S[c], Q[c], scale);
+    }
+}
+
 cudaError_t trace_configure(int device, int* sm_count, size_t* max_smem_optin) {
     cudaDeviceProp prop;
     cudaError_t e = cudaGetDeviceProperties(&prop, device);
@@ -46,6 +82,11 @@ cudaError_t trace_configure(int device, int* sm_count, size_t* max_smem_optin) {
 cudaError_t launch_resolve(const ResolveParams& q, cudaStream_t st) {
     int grid = (int)((q.npix_local + 255u) / 256u);
     rt_resolve_kernel<<<grid, 256, 0, st>>>(q);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_resolve_var(const ResolveVarParams& v, cudaStream_t st) {
+    rt_resolve_var_kernel<<<(v.r.npix_local + 255u) / 256u, 256, 0, st>>>(v);
     return cudaGetLastError();
 }
 

@@ -162,6 +162,16 @@ struct DenoiseArgs {
     float* out_linear; uint8_t* out_rgb8;                            // [npix][3]; either may be null, not both
 };
 
+// The variance-guided à-trous filter (rtb200_denoise_var.cu, DESIGN.md §4.18): the caller's buffers and the scratch of
+// denoise_var_scratch_bytes.
+struct DenoiseVarArgs {
+    uint32_t width, height, iterations;
+    float color_weight, albedo_weight, normal_weight, variance_floor;
+    const float* color; const float* variance; const float* albedo; const float* normal;   // [npix][3]; a guide may be null
+    void* scratch;
+    float* out_linear; uint8_t* out_rgb8; float* out_variance;                             // [npix][3]; each may be null, not all
+};
+
 // The temporal accumulation (rtb200_temporal.cu, DESIGN.md §4.16) of a width x height frame: the caller's buffers.
 struct TemporalArgs {
     uint32_t width, height, max_history, n_motion;
@@ -182,6 +192,19 @@ struct ResolveParams {
     float*   out_linear;   // [npix_local][3] or null
     uint8_t* out_rgb8;     // [npix_local][3] or null
 };
+// The resolve with the variance of each pixel's mean (rt_resolve_var_kernel, DESIGN.md §4.18): `r`'s sums and outputs, plus
+// the running f32 sums of x_c * x_c in sample order and the variance output.
+struct ResolveVarParams {
+    ResolveParams r;
+    float* accum_sq;       // [npix_local][3] Q_c, carried across batches like r.accum
+    float* out_variance;   // [npix_local][3]
+};
+struct AdaptiveResolveVarParams {
+    AdaptiveResolveParams r;
+    const float* sq;       // [npix_local][3] Q_c
+    float* out_variance;   // [npix_local][3]
+};
+
 
 // Refit of a resident scene after its spheres moved (rtb200_refit.cu, DESIGN.md §4.7): the records and f32 boxes are
 // recomputed from `geo` on the upload's topology and recentring offset. Exact boxes are {lo[3], hi[3]} f64.
@@ -282,6 +305,7 @@ cudaError_t launch_wavefront(const TraceParams& p, uint32_t mode, uint32_t queue
 int wavefront_max_ctas_per_sm(uint32_t mode, bool lights, uint32_t queue, size_t smem);   // 0 when the kernel cannot run on the current device
 cudaError_t wavefront_info(uint32_t mode, bool lights, uint32_t queue, KernelInfo* out);
 cudaError_t launch_resolve(const ResolveParams& p, cudaStream_t st);
+cudaError_t launch_resolve_var(const ResolveVarParams& p, cudaStream_t st);
 // closest-hit (any = false) and occlusion (any = true) queries: resident CTAs per SM of the query kernel of that kind and
 // `mode` (0 when it cannot run on the current device), and a launch of at most `max_grid` CTAs (no more than the rays need)
 int query_max_ctas_per_sm(uint32_t mode, bool any);
@@ -299,10 +323,15 @@ size_t adaptive_compact_bytes(uint32_t npix_local);   // cub's temporary storage
 cudaError_t launch_adaptive_compact(void* temp, size_t temp_bytes, const uint32_t* list_in, const uint32_t* keep, uint32_t* list_out,
                                     uint32_t* list_n_out, uint32_t npix_local, cudaStream_t st);
 cudaError_t launch_adaptive_resolve(const AdaptiveResolveParams& p, cudaStream_t st);
+cudaError_t launch_adaptive_resolve_var(const AdaptiveResolveVarParams& p, cudaStream_t st);
 // the denoise (rtb200_denoise.cu): its scratch for npix pixels, and its iterations + 1 launches (the guides' packing, then one
 // per iteration)
 uint64_t denoise_scratch_bytes(uint64_t npix);
 cudaError_t launch_denoise(const DenoiseArgs& a, cudaStream_t st);
+// the variance-guided denoise (rtb200_denoise_var.cu): its scratch, and its 2 * iterations + 1 launches (the packing, then a
+// prefilter and a step per iteration)
+uint64_t denoise_var_scratch_bytes(uint64_t npix);
+cudaError_t launch_denoise_var(const DenoiseVarArgs& a, cudaStream_t st);
 // the temporal accumulation (rtb200_temporal.cu): one launch, one thread per pixel
 cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t st);
 // geo[idx[k]] = geo_in[k], mat[idx[k]] = mat_in[k] for k < n (idx has no repeats)

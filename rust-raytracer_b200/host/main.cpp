@@ -30,6 +30,10 @@
 // aperture: the reference's pinhole camera; absent focus_dist: |look_from - look_at|, or the scene's for a frame). Plain renders
 // and RTB200_FRAMES render lens cameras (rtb200_render_frames_lens). RTB200_GPUS, RTB200_ADAPTIVE, RTB200_AOV, RTB200_DENOISE
 // and RTB200_TEMPORAL refuse a lens camera with status 101: none of them renders it as a pinhole.
+// RTB200_DENOISE_VAR=<iterations>[,<color_weight>[,<albedo_weight>[,<normal_weight>[,<variance_floor>]]]] renders the frame with
+// the variance of its pixel means (rtb200_render_frames_var) and writes <stem>_denoised.png: the variance-guided denoise
+// (rtb200_denoise_var, DESIGN.md §4.18; omitted values are the header's RTB200_DENOISE_VAR_DEFAULT_*) with the AOVs of the
+// frame's own samples. Not with RTB200_DENOISE, RTB200_GPUS, RTB200_FRAMES, RTB200_ADAPTIVE, RTB200_TEMPORAL or a lens camera.
 #include <chrono>
 #include <cmath>
 #include <cstring>
@@ -286,6 +290,48 @@ static int write_denoised(const rt_scene& s, const rt_denoise_params& p, const r
     return 0;
 }
 
+// RTB200_DENOISE_VAR: the parameters of `spec` for the frame of `s` (101 and a message when it is malformed); omitted values
+// are the header's RTB200_DENOISE_VAR_DEFAULT_*
+static int parse_denoise_var(const rt_scene& s, const char* spec, rt_denoise_var_params* p) {
+    double v[5] = {RTB200_DENOISE_VAR_DEFAULT_ITERATIONS, RTB200_DENOISE_VAR_DEFAULT_COLOR_WEIGHT, RTB200_DENOISE_VAR_DEFAULT_ALBEDO_WEIGHT,
+                   RTB200_DENOISE_VAR_DEFAULT_NORMAL_WEIGHT, RTB200_DENOISE_VAR_DEFAULT_VARIANCE_FLOOR};
+    int k = 0;
+    for (const char* c = spec; k < 5; ++k) {
+        char* end = nullptr;
+        v[k] = strtod(c, &end);
+        if (end == c || (*end != ',' && *end != 0) || (k == 4 && *end != 0)) {
+            fprintf(stderr, "RTB200_DENOISE_VAR: expected <iterations>[,<color_weight>[,<albedo_weight>[,<normal_weight>[,<variance_floor>]]]], got \"%s\"\n", spec);
+            return 101;
+        }
+        if (*end == 0) break;
+        c = end + 1;
+    }
+    if (!(v[0] >= 1 && v[0] <= 10 && v[0] == std::floor(v[0]))) { fprintf(stderr, "RTB200_DENOISE_VAR: iterations must be an integer in [1, 10]\n"); return 101; }
+    for (int i = 1; i < 4; ++i)
+        if (!(std::isfinite((float)v[i]) && v[i] >= 0)) { fprintf(stderr, "RTB200_DENOISE_VAR: the weights must be finite and >= 0\n"); return 101; }
+    if (!(std::isfinite((float)v[4]) && (float)v[4] > 0.0f)) { fprintf(stderr, "RTB200_DENOISE_VAR: variance_floor must be finite and > 0\n"); return 101; }
+    if ((uint64_t)s.width * s.height >= (1ull << 31)) { fprintf(stderr, "RTB200_DENOISE_VAR: the frame must have fewer than 2^31 pixels\n"); return 101; }
+    *p = rt_denoise_var_params{s.width, s.height, (uint32_t)v[0], 0u, (float)v[1], (float)v[2], (float)v[3], (float)v[4]};
+    return 0;
+}
+
+// RTB200_DENOISE_VAR: `linear` and `variance`, the frame of `s` and the variance of its pixel means, denoised with the AOVs of
+// its own samples, written to <stem>_denoised.png
+static int write_denoised_var(const rt_scene& s, const rt_denoise_var_params& p, const rt_options& opts, const float* linear,
+                              const float* variance, const std::string& out) {
+    const size_t npix = (size_t)s.width * s.height;
+    std::vector<float> albedo(npix * 3), normal(npix * 3);
+    std::vector<uint8_t> rgb8(npix * 3);
+    if (aov_of(s, opts, s.samples_per_pixel, 0u, albedo.data(), normal.data()) != 0) return 101;
+    if (rtb200_denoise_var(opts.device, &p, linear, variance, albedo.data(), normal.data(), nullptr, rgb8.data(), nullptr, nullptr) != 0) {
+        fprintf(stderr, "denoise failed: %s\n", rtb200_last_error());
+        return 101;
+    }
+    std::string err;
+    if (!rthost::write_png_rgb8((stem_of(out) + "_denoised.png").c_str(), rgb8.data(), s.width, s.height, &err)) { fprintf(stderr, "error writing image: %s\n", err.c_str()); return 101; }
+    return 0;
+}
+
 int main(int argc, char** argv) {
     if (argc != 3) {                                                       // main.rs:9-12
         printf("Usage: %s <config_file> <output_file>\n", argc > 0 ? argv[0] : "raytracer");
@@ -322,16 +368,24 @@ int main(int argc, char** argv) {
         fprintf(stderr, "RTB200_DENOISE with RTB200_GPUS, RTB200_FRAMES or RTB200_ADAPTIVE is not supported: it denoises one frame on one GPU\n");
         return 101;
     }
+    const char* denoise_var = getenv("RTB200_DENOISE_VAR");
+    if (denoise_var && (denoise || getenv("RTB200_GPUS") || getenv("RTB200_FRAMES") || adaptive || temporal)) {
+        fprintf(stderr, "RTB200_DENOISE_VAR with RTB200_DENOISE, RTB200_GPUS, RTB200_FRAMES, RTB200_ADAPTIVE or RTB200_TEMPORAL is not "
+                        "supported: it denoises one frame on one GPU with its own variance\n");
+        return 101;
+    }
     rt_lens scene_lens{};
     if (apply_lens(holder.lens_spec, &holder.scene.camera, &scene_lens) != 0) return 101;
     const bool lens = scene_lens.radius != 0.0;
-    if (lens && (getenv("RTB200_GPUS") || adaptive || aov || denoise || temporal)) {
-        fprintf(stderr, "a lens camera (aperture > 0) with RTB200_GPUS, RTB200_ADAPTIVE, RTB200_AOV, RTB200_DENOISE or RTB200_TEMPORAL is not "
+    if (lens && (getenv("RTB200_GPUS") || adaptive || aov || denoise || denoise_var || temporal)) {
+        fprintf(stderr, "a lens camera (aperture > 0) with RTB200_GPUS, RTB200_ADAPTIVE, RTB200_AOV, RTB200_DENOISE, RTB200_DENOISE_VAR or RTB200_TEMPORAL is not "
                         "supported: render it without them\n");
         return 101;
     }
     rt_denoise_params denoise_p{};
     if (denoise && parse_denoise(holder.scene, denoise, &denoise_p) != 0) return 101;
+    rt_denoise_var_params denoise_var_p{};
+    if (denoise_var && parse_denoise_var(holder.scene, denoise_var, &denoise_var_p) != 0) return 101;
     if (const char* fp = getenv("RTB200_FRAMES")) return render_animation(holder, fp, argv[2], temporal);
     printf("\nRendering %s\n", argv[2]);                                  // main.rs:18
     fflush(stdout);
@@ -342,7 +396,7 @@ int main(int argc, char** argv) {
     rt_stats st{};
     auto t0 = std::chrono::steady_clock::now();                           // raytracer.rs:259
     const char* gpus = getenv("RTB200_GPUS");
-    std::vector<float> linear;
+    std::vector<float> linear, variance;
     int rc = 0;
     if (adaptive) {
         rc = render_adaptive(s, adaptive, opts, pixels.data(), &st);
@@ -352,6 +406,13 @@ int main(int argc, char** argv) {
         // (rtb200_probe_quantise), byte for byte the RGB8 render's
         linear.resize(pixels.size());
         rc = rtb200_render_linear_f32(&s, &opts, linear.data(), &st);
+        if (rc == 0) rc = rtb200_probe_quantise(linear.data(), (uint32_t)linear.size(), pixels.data());
+    } else if (denoise_var) {
+        // the frame with the variance of its pixel means; out.png is the linear image's quantisation, as for RTB200_DENOISE
+        linear.resize(pixels.size());
+        variance.resize(pixels.size());
+        const rt_frame f{s.camera, s.seed, s.max_depth, 0};
+        rc = rtb200_render_frames_var(&s, &opts, &f, nullptr, 1, nullptr, linear.data(), variance.data(), &st);
         if (rc == 0) rc = rtb200_probe_quantise(linear.data(), (uint32_t)linear.size(), pixels.data());
     } else if (lens) {
         const rt_frame f{s.camera, s.seed, s.max_depth, 0};   // one frame of the lens camera
@@ -374,5 +435,6 @@ int main(int argc, char** argv) {
     if (!rthost::write_png_rgb8(argv[2], pixels.data(), s.width, s.height, &err)) { fprintf(stderr, "error writing image: %s\n", err.c_str()); return 101; }   // raytracer.rs:265
     if (aov && (rc = write_aov(s, aov, opts, argv[2])) != 0) return rc;
     if (denoise) return write_denoised(s, denoise_p, opts, linear.data(), argv[2]);
+    if (denoise_var) return write_denoised_var(s, denoise_var_p, opts, linear.data(), variance.data(), argv[2]);
     return 0;
 }

@@ -153,6 +153,13 @@ class rt_denoise_params(C.Structure):
                 ("color_weight", C.c_float), ("albedo_weight", C.c_float), ("normal_weight", C.c_float), ("reserved2", C.c_float)]
 
 
+class rt_denoise_var_params(C.Structure):
+    """The variance-guided à-trous filter of rtb200_denoise_var[_device]: image size, iterations L in [1, 10], the finite,
+    non-negative weights of the colour, albedo and normal guides (0 turns a guide off), and the finite, positive variance floor."""
+    _fields_ = [("width", C.c_uint32), ("height", C.c_uint32), ("iterations", C.c_uint32), ("reserved", C.c_uint32),
+                ("color_weight", C.c_float), ("albedo_weight", C.c_float), ("normal_weight", C.c_float), ("variance_floor", C.c_float)]
+
+
 class rt_temporal_params(C.Structure):
     """The temporal accumulation of rtb200_temporal[_device]: image size, max_history N >= 1, the rows of motion, this frame's
     and the previous frame's cameras, and the finite, non-negative relative depth tolerance."""
@@ -179,7 +186,7 @@ assert C.sizeof(rt_sphere) == 64 and C.sizeof(rt_frame) == 112 and C.sizeof(rt_a
 assert C.sizeof(rt_rays) == 24 and C.sizeof(rt_hits) == 48 and C.sizeof(rt_trace_params) == 32
 assert C.sizeof(rt_aov_params) == 16 and C.sizeof(rt_aov_out) == 40 and C.sizeof(rt_denoise_params) == 32
 assert C.sizeof(rt_temporal_params) == 224 and C.sizeof(rt_temporal_frame) == 24 and C.sizeof(rt_temporal_history) == 32
-assert C.sizeof(rt_temporal_out) == 16 and C.sizeof(rt_lens) == 64
+assert C.sizeof(rt_temporal_out) == 16 and C.sizeof(rt_lens) == 64 and C.sizeof(rt_denoise_var_params) == 32
 AOV_FIELDS = (("albedo", 3, np.float32), ("normal", 3, np.float32), ("hits", 1, np.uint32), ("sphere", 1, np.int32),
               ("point", 3, np.float64))   # rt_aov_out: name, values per pixel, dtype (sphere -1 = 0xffffffff)
 
@@ -204,6 +211,8 @@ ABI_SYMBOLS = [
     "rtb200_temporal_device", "rtb200_temporal",
     "rtb200_camera_from_params_lens", "rtb200_scene_set_lens", "rtb200_render_frames_lens", "rtb200_render_frames_lens_device",
     "rtb200_probe_lens_ray",
+    "rtb200_denoise_var_scratch_bytes", "rtb200_denoise_var_device", "rtb200_denoise_var",
+    "rtb200_render_frames_var_device", "rtb200_render_frames_var", "rtb200_adaptive_resolve_var", "rtb200_render_adaptive_var",
 ]
 
 _lib = None
@@ -279,6 +288,17 @@ def lib() -> C.CDLL:
                                         C.c_void_p, C.c_void_p, C.c_void_p]
     L.rtb200_denoise.argtypes = [C.c_int32, C.POINTER(rt_denoise_params), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.POINTER(rt_stats)]
+    L.rtb200_render_frames_var_device.argtypes = [C.c_void_p, C.POINTER(rt_frame), C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p,
+                                                  C.c_void_p, C.c_void_p, C.POINTER(rt_stats)]
+    L.rtb200_render_frames_var.argtypes = [C.POINTER(rt_scene), C.POINTER(rt_options), C.POINTER(rt_frame), C.c_void_p, C.c_uint32,
+                                           C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(rt_stats)]
+    L.rtb200_adaptive_resolve_var.argtypes = [C.c_void_p] + [C.c_void_p] * 5
+    L.rtb200_render_adaptive_var.argtypes = [C.POINTER(rt_scene), C.POINTER(rt_options), C.POINTER(rt_adaptive_params), C.c_void_p,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(rt_stats)]
+    L.rtb200_denoise_var_scratch_bytes.restype = C.c_uint64
+    L.rtb200_denoise_var_scratch_bytes.argtypes = [C.c_uint32, C.c_uint32]
+    L.rtb200_denoise_var_device.argtypes = [C.c_int32, C.POINTER(rt_denoise_var_params)] + [C.c_void_p] * 9
+    L.rtb200_denoise_var.argtypes = [C.c_int32, C.POINTER(rt_denoise_var_params)] + [C.c_void_p] * 7 + [C.POINTER(rt_stats)]
     L.rtb200_temporal_device.argtypes = [C.c_int32, C.POINTER(rt_temporal_params), C.POINTER(rt_temporal_frame),
                                          C.POINTER(rt_temporal_history), C.c_void_p, C.POINTER(rt_temporal_out), C.c_void_p]
     L.rtb200_temporal.argtypes = [C.c_int32, C.POINTER(rt_temporal_params), C.POINTER(rt_temporal_frame), C.POINTER(rt_temporal_history),
@@ -729,11 +749,12 @@ def _frame_array(frames: Sequence[rt_frame]):
 
 
 def render_frames(scene: Scene, frames: Sequence[rt_frame], opts: Optional[rt_options] = None, linear: bool = False,
-                  lenses: Optional[Sequence[rt_lens]] = None):
+                  lenses: Optional[Sequence[rt_lens]] = None, variance: bool = False):
     """Render len(frames) frames of one scene in as few trace launches as the sample buffer allows (rtb200_render_frames).
     Frame i equals render_rgb8 / render_linear of the scene with frames[i]'s camera, seed and max_depth. lenses: frame i's
     lens (None or radius 0: pinhole; rtb200_render_frames_lens); without it a lens scene renders every frame with its own lens.
-    Returns (uint8 [n,rows,w,3], or float32 with linear=True, stats dict)."""
+    Returns (uint8 [n,rows,w,3], or float32 with linear=True, stats dict); with variance=True (rtb200_render_frames_var)
+    (image, variance float32 [n,rows,w,3] of each pixel's mean, stats dict)."""
     rows = scene.c.height if (opts is None or opts.world <= 1) else shard_rows(scene.c.height, opts.rank, opts.world, opts.band_rows)
     arr, n = _frame_array(frames)
     if lenses is None and scene.lens is not None:
@@ -742,6 +763,11 @@ def render_frames(scene: Scene, frames: Sequence[rt_frame], opts: Optional[rt_op
     st = rt_stats()
     o = C.byref(opts) if opts is not None else None
     o8, ol = (None, out.ctypes.data) if linear else (out.ctypes.data, None)
+    if variance:
+        var = np.empty((n, rows, scene.c.width, 3), dtype=np.float32)
+        _check(lib().rtb200_render_frames_var(C.byref(scene.c), o, arr, _lens_array(lenses, n) if lenses is not None else None, n,
+                                              o8, ol, var.ctypes.data, C.byref(st)))
+        return out, var, st.as_dict()
     if lenses is None:
         _check(lib().rtb200_render_frames(C.byref(scene.c), o, arr, n, o8, ol, C.byref(st)))
     else:
@@ -754,10 +780,11 @@ def make_adaptive(rel_tol: float, abs_tol: float = 0.0, samples_per_round: int =
     return rt_adaptive_params(int(samples_per_round), int(max_samples), int(min_samples), 0, float(abs_tol), float(rel_tol))
 
 
-def render_adaptive(scene: Scene, params: rt_adaptive_params, opts: Optional[rt_options] = None):
+def render_adaptive(scene: Scene, params: rt_adaptive_params, opts: Optional[rt_options] = None, variance: bool = False):
     """Render adaptively (rtb200_render_adaptive): rounds of params.samples_per_round samples of the pixels that have not
     converged, until none is left. A pixel that received n samples equals the one-shot render at samples_per_pixel = n.
-    Returns (uint8 [rows,w,3], float32 linear [rows,w,3], uint32 counts [rows,w], stats dict). A lens scene is refused:
+    Returns (uint8 [rows,w,3], float32 linear [rows,w,3], uint32 counts [rows,w], stats dict); with variance=True
+    (rtb200_render_adaptive_var) the variance of each pixel's mean, float32 [rows,w,3], comes before the stats. A lens scene is refused:
     render it adaptively through ResidentScene.adaptive_*."""
     _refuse_lens(scene, "render_adaptive")
     rows = scene.c.height if (opts is None or opts.world <= 1) else shard_rows(scene.c.height, opts.rank, opts.world, opts.band_rows)
@@ -765,8 +792,14 @@ def render_adaptive(scene: Scene, params: rt_adaptive_params, opts: Optional[rt_
     lin = np.empty((rows, scene.c.width, 3), dtype=np.float32)
     cnt = np.empty((rows, scene.c.width), dtype=np.uint32)
     st = rt_stats()
-    _check(lib().rtb200_render_adaptive(C.byref(scene.c), C.byref(opts) if opts is not None else None, C.byref(params),
-                                        img.ctypes.data, lin.ctypes.data, cnt.ctypes.data, C.byref(st)))
+    o = C.byref(opts) if opts is not None else None
+    if variance:
+        var = np.empty((rows, scene.c.width, 3), dtype=np.float32)
+        _check(lib().rtb200_render_adaptive_var(C.byref(scene.c), o, C.byref(params), img.ctypes.data, lin.ctypes.data,
+                                                cnt.ctypes.data, var.ctypes.data, C.byref(st)))
+        return img, lin, cnt, var, st.as_dict()
+    _check(lib().rtb200_render_adaptive(C.byref(scene.c), o, C.byref(params), img.ctypes.data, lin.ctypes.data, cnt.ctypes.data,
+                                        C.byref(st)))
     return img, lin, cnt, st.as_dict()
 
 
@@ -879,11 +912,18 @@ class ResidentScene:
         return st.as_dict()
 
     def render_frames(self, frames: Sequence[rt_frame], dev_rgb8_ptr: int = 0, dev_linear_ptr: int = 0, stream: int = 0,
-                      lenses: Optional[Sequence[rt_lens]] = None) -> dict:
+                      lenses: Optional[Sequence[rt_lens]] = None, variance: int = 0) -> dict:
         """Render len(frames) frames into device buffers of n * rows * w * 3 elements (blocking; the handle's own camera,
-        seed and max_depth stay as uploaded). lenses: frame i's lens (rtb200_render_frames_lens_device); None: the handle's."""
+        seed and max_depth stay as uploaded). lenses: frame i's lens (rtb200_render_frames_lens_device); None: the handle's.
+        variance: the address of a float32 device buffer of n * rows * w * 3 elements for the variance of each pixel's mean
+        (rtb200_render_frames_var_device); 0: none."""
         arr, n = _frame_array(frames)
         st = rt_stats()
+        if variance:
+            _check(lib().rtb200_render_frames_var_device(self.h, arr, _lens_array(lenses, n), n, C.c_void_p(dev_rgb8_ptr or None),
+                                                         C.c_void_p(dev_linear_ptr or None), C.c_void_p(int(variance)),
+                                                         C.c_void_p(stream or None), C.byref(st)))
+            return st.as_dict()
         _check(lib().rtb200_render_frames_lens_device(self.h, arr, _lens_array(lenses, n), n, C.c_void_p(dev_rgb8_ptr or None), C.c_void_p(dev_linear_ptr or None),
                                                  C.c_void_p(stream or None), C.byref(st)))
         return st.as_dict()
@@ -945,13 +985,18 @@ class ResidentScene:
         _check(lib().rtb200_adaptive_step(self.h, int(rounds), self._stream(stream, self.device), C.byref(active), C.byref(st)))
         return int(active.value), st.as_dict()
 
-    def adaptive_resolve(self, rgb8=None, linear=None, counts=None, stream=None):
+    def adaptive_resolve(self, rgb8=None, linear=None, counts=None, stream=None, variance=None):
         """Write the current adaptive image into CUDA tensors (rtb200_adaptive_resolve), each optional: uint8 rgb8 and float32
-        linear of rows * w * 3 elements, int32 or uint32-sized counts of rows * w elements, on the handle's device."""
+        linear of rows * w * 3 elements, int32 or uint32-sized counts of rows * w elements, on the handle's device. variance: a
+        float32 tensor of rows * w * 3 elements for the variance of each pixel's mean (rtb200_adaptive_resolve_var)."""
         n = self.rows * self.scene.c.width
         A = _Arrays("adaptive_resolve", False, self.device)
         ptrs = [A.arg("rgb8", rgb8, (np.uint8,), 3 * n, True), A.arg("linear", linear, (np.float32,), 3 * n, True),
                 A.arg("counts", counts, (np.int32,), n, True)]
+        if variance is not None:
+            pv = A.arg("variance", variance, (np.float32,), 3 * n)
+            _check(lib().rtb200_adaptive_resolve_var(self.h, *ptrs, pv, self._stream(stream, self.device)))
+            return
         _check(lib().rtb200_adaptive_resolve(self.h, *ptrs, self._stream(stream, self.device)))
 
     def intersect(self, origin, direction, t_max=None, stream=None, outputs=None) -> dict:
@@ -1172,6 +1217,56 @@ def denoise(color, albedo=None, normal=None, *, iterations: int = DENOISE_ITERAT
         return out
     _check(lib().rtb200_denoise_device(A.device, C.byref(p), *guides, A.ptr(scratch), A.ptr(out.get("linear")), A.ptr(out.get("rgb8")),
                                        C.c_void_p(handle)))
+    return out
+
+
+# the variance-guided denoise's defaults, include/rtb200.h's RTB200_DENOISE_VAR_DEFAULT_* (DESIGN.md §4.18: chosen on the oracle's
+# cover render at 64x48 from 2 to 32 spp with its AOV guides)
+DENOISE_VAR_ITERATIONS, DENOISE_VAR_COLOR_WEIGHT, DENOISE_VAR_ALBEDO_WEIGHT, DENOISE_VAR_NORMAL_WEIGHT = 3, 1.0, 4.0, 1.0
+DENOISE_VAR_VARIANCE_FLOOR = 1e-4
+
+
+def denoise_var(color, variance, albedo=None, normal=None, *, iterations: int = DENOISE_VAR_ITERATIONS,
+                color_weight: float = DENOISE_VAR_COLOR_WEIGHT, albedo_weight: Optional[float] = None,
+                normal_weight: Optional[float] = None, variance_floor: float = DENOISE_VAR_VARIANCE_FLOOR, linear: bool = True,
+                rgb8: bool = False, out_variance: bool = False, stream=None) -> dict:
+    """Denoise a [h, w, 3] float32 image with its per-pixel variance (normally a render's linear mean and the variance of that
+    mean) by the variance-guided à-trous filter of include/rtb200.h, guided by the optional albedo and normal of
+    :meth:`ResidentScene.aov`. A guide's weight defaults to DENOISE_VAR_ALBEDO_WEIGHT / DENOISE_VAR_NORMAL_WEIGHT when the guide
+    is given and to 0 (off) when it is not. numpy arrays use the blocking host form (rtb200_denoise_var) and the result also holds
+    "stats"; CUDA tensors use the device form on `stream` with the stream rules of :func:`denoise`. Returns {"linear": float32
+    [h, w, 3]}, {"rgb8": uint8 [h, w, 3]} and/or {"variance": float32 [h, w, 3]} (out_variance), whichever is asked for."""
+    if not (linear or rgb8 or out_variance):
+        raise ValueError("denoise_var: ask for linear, rgb8, out_variance or several")
+    if albedo_weight is None:
+        albedo_weight = DENOISE_VAR_ALBEDO_WEIGHT if albedo is not None else 0.0
+    if normal_weight is None:
+        normal_weight = DENOISE_VAR_NORMAL_WEIGHT if normal is not None else 0.0
+    shape = tuple(color.shape)
+    if len(shape) != 3 or shape[2] != 3:
+        raise ValueError(f"denoise_var: color must have shape [h, w, 3], got {shape}")
+    A = _Arrays("denoise_var")
+    ins = [A.arg(name, g, (np.float32,), shape, name in ("albedo", "normal"))
+           for name, g in (("color", color), ("variance", variance), ("albedo", albedo), ("normal", normal))]
+    p = rt_denoise_var_params(shape[1], shape[0], int(iterations), 0, float(color_weight), float(albedo_weight), float(normal_weight),
+                              float(variance_floor))
+    outs = [(k, shape, ty) for k, ty, want in (("linear", np.float32, linear), ("rgb8", np.uint8, rgb8),
+                                               ("variance", np.float32, out_variance)) if want]
+    if A.host:
+        out = A.empty(outs)
+        st = rt_stats()
+        _check(lib().rtb200_denoise_var(-1, C.byref(p), *ins, A.ptr(out.get("linear")), A.ptr(out.get("rgb8")),
+                                        A.ptr(out.get("variance")), C.byref(st)))
+        out["stats"] = st.as_dict()
+        return out
+    stream, handle = _call_stream(stream, A.device, "denoise_var", "the scratch")
+    # the scratch and the outputs belong to the call's stream, as in denoise
+    out = A.empty(outs + [("scratch", (int(lib().rtb200_denoise_var_scratch_bytes(shape[1], shape[0])),), np.uint8)], stream)
+    scratch = out.pop("scratch")
+    if color.numel() == 0:   # a 0-pixel image (the library's no-op)
+        return out
+    _check(lib().rtb200_denoise_var_device(A.device, C.byref(p), *ins, A.ptr(scratch), A.ptr(out.get("linear")),
+                                           A.ptr(out.get("rgb8")), A.ptr(out.get("variance")), C.c_void_p(handle)))
     return out
 
 

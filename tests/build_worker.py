@@ -25,6 +25,7 @@ import numpy as np  # noqa: E402
 
 import rtb200 as R  # noqa: E402
 from rtb200 import scenes  # noqa: E402
+import test_full_frames_cpu as FF  # noqa: E402
 from test_full_frames_cpu import lit_scene as full_frame_lit_scene, params as full_frame_params  # noqa: E402
 from test_gpu_adaptive import SCENES as ADAPTIVE_SCENES, _params  # noqa: E402
 from test_gpu_parity import GOLDEN  # noqa: E402
@@ -85,7 +86,8 @@ ADAPTIVE_PARAMS = {"adaptive_full_frame_lit": lambda: full_frame_params(8)}
 # case -> (kind, scene maker, variant, RTB200_WF_SMEM mask). Kinds: "one_shot" (render_linear and render_rgb8), "rebuilt" (a
 # resident handle after rebuild()), "update" (a resident handle after update_spheres), "frames" (render_frames of
 # _room_frames), "adaptive" (render_adaptive with test_gpu_adaptive's parameters, or the case's ADAPTIVE_PARAMS), "topology"
-# (see the module docstring), and for a lens scene "lens_one_shot" (one_shot through its lens), "lens_frames" (render_frames of lens_room_frames, with their
+# (see the module docstring), "full_frames" (render_frames of test_full_frames_cpu.full_frames), "full_rays" (trace_rays of
+# test_full_frames_cpu.full_rays), and for a lens scene "lens_one_shot" (one_shot through its lens), "lens_frames" (render_frames of lens_room_frames, with their
 # lenses) and "lens_adaptive" (the adaptive rounds of a resident handle with the scene's lens, run to the end).
 CASES = {
     **{f"golden_{name}": ("one_shot", mk, FILTERED, 0) for name, mk in GOLDEN},
@@ -111,6 +113,9 @@ CASES = {
     "lens_room_frames": ("lens_frames", lambda: R.Scene.from_config(_room_cfg(3, 50, w=48, h=36, spp=4)), FILTERED, 0),
     "lens_coincident_10k": ("lens_one_shot", _with_lens(lambda: _coincident(1), 0.4), FILTERED, 0),
     "lens_adaptive_mixed_2_lights": ("lens_adaptive", _with_lens(ADAPTIVE_SCENES["mixed_2_lights"], 0.3, 12.0), FILTERED, 0),
+    # the full-frame Q_FRAMES and Q_RAYS cases (tests/test_gpu_full_frames.py), whose slots are reclaimed many times over
+    "full_frames_lit": ("full_frames", lambda: FF.full_scene("lit", spp=FF.FRAME_SPP), FILTERED, 0),
+    "full_rays_lit": ("full_rays", lambda: FF.full_scene("lit"), FILTERED, 0),
 }
 
 # Scene staging (RTB200_WF_SMEM) on every build: every mask in both modes that stage bit 0, on scenes whose hierarchy has an
@@ -218,6 +223,19 @@ def render_case(name, kind, sc, opts, out, meta):
         img, lin, cnt, st = R.render_adaptive(sc, ADAPTIVE_PARAMS.get(name, _params)(), opts)
         out[name + ".counts"] = cnt
         meta[name] = _stats(st)
+    elif kind == "full_frames":
+        frames = FF.full_frames(sc)
+        img, st = R.render_frames(sc, frames, opts)
+        lin, st2 = R.render_frames(sc, frames, opts, linear=True)
+        meta[name] = dict(_stats(st), rays_linear=int(st2["rays"]), batches=int(st["batches"]))
+    elif kind == "full_rays":
+        rs = R.ResidentScene(sc, opts)
+        try:
+            got = rs.trace_rays(*FF.full_rays(), FF.RAYS_SPP, rgb8=True, **FF.RAYS_KW)
+        finally:
+            rs.release()
+        lin, img = got["linear"], got["rgb8"]
+        meta[name] = _stats(got["stats"])
     elif kind == "lens_one_shot":
         lin, st = R.render_linear(sc, opts)
         img, st8 = R.render_rgb8(sc, opts)

@@ -1,7 +1,8 @@
 """The trace kernel's frames do not depend on its compile-time capacities (DESIGN.md §4.1): every stress build of the library
 (rust-raytracer_b200/stress, made by `make stress`) renders the same linear f32, RGB8, rays and samples as the CPU oracle, on
 the scenes that reach the hard paths of the closest-hit and shade stages - dense candidate lists, deep node stacks, deep albedo
-stacks, deferred scatters - through every kernel (one frame, many frames, the adaptive list, the rebuild, the refit).
+stacks, deferred scatters - through every kernel (one frame, many frames, the adaptive list, the rebuild, the refit), and
+the full-frame frame group and caller-supplied rays, whose slots are reclaimed many times in one launch.
 
 The library is chosen when rtb200 is imported (RTB200_LIB), so each build renders in a process of its own
 (tests/build_worker.py); this process renders the references once per module. Each build also proves that it is the build
@@ -98,6 +99,13 @@ def reference(name):
         p = BW._params()
         want = A.run(x, rays, M, N, MIN, p.abs_tol, p.rel_tol)
         ref = dict(linear=want["linear"], rgb8=want["rgb8"], counts=want["counts"], rays=want["rays"], samples=want["samples"])
+    elif kind == "full_frames":
+        wants = [FF.frame_want("lit", k) for k in range(2)]
+        ref = dict(linear=np.stack([w["linear"] for w in wants]), rgb8=np.stack([w["rgb8"] for w in wants]),
+                   rays=sum(w["rays"] for w in wants), samples=2 * FF.FRAME_WORK)
+    elif kind == "full_rays":
+        want = FF.rays_want("lit")
+        ref = dict(linear=want["linear"], rgb8=want["rgb8"], rays=want["rays"], samples=FF.RAYS_N * FF.RAYS_SPP)
     elif kind == "lens_one_shot":
         sc = mk()
         want = OL.render(sc, sc.lens)
@@ -127,7 +135,7 @@ def test_the_room_reaches_deep_albedo_levels():
 def compare(name, z, meta):
     ref = reference(name)
     lin, img = z[name + ".linear"], z[name + ".rgb8"]
-    if BW.CASES[name][0] in ("frames", "lens_frames"):
+    if BW.CASES[name][0] in ("frames", "lens_frames", "full_frames"):
         assert lin.shape == ref["linear"].shape, (name, lin.shape)
         for i in range(len(lin)):
             assert_frames_match((lin[i], img[i]), (ref["linear"][i], ref["rgb8"][i]), f"{name} frame {i}")

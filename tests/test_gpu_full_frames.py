@@ -1,11 +1,14 @@
-"""Adaptive rounds, auxiliary buffers and lens frames at frame sizes that fill an H100 (DESIGN.md §3, "At frame sizes that fill
-the GPU"), bit for bit against the oracle: counts equal, linear f32 under assert_frames_match, RGB8 equal, rays and samples
-equal, auxiliary buffers bit-equal.
+"""Adaptive rounds, auxiliary buffers, pinhole and lens frames, their variance, and caller-supplied rays at sizes that fill
+an H100 (DESIGN.md §3, "At frame sizes that fill the GPU"), bit for bit against the oracle: counts equal, linear f32 under
+assert_frames_match, RGB8 equal, rays and samples equal, auxiliary buffers and variances bit-equal; and the launch groups of
+frames at the group bound kGroupMaxFrameWork.
 
-The smaller frames of test_gpu_adaptive.py, test_gpu_aov.py and test_gpu_lens.py fit in the trace kernel's first fill of its
-slots and in one chunk per query warp, so they never run a Q_LIST slot's second claim from the queue, a compaction over many
-tiles, or the auxiliary-buffer kernels' grid-stride step. Every case here asserts that it reaches past them, against the bound
-B = sm_count x max_threads_per_multi_processor of the device it runs on (tests/test_full_frames_cpu.py)."""
+The smaller frames of test_gpu_adaptive.py, test_gpu_aov.py, test_gpu_frames.py, test_gpu_lens.py and test_gpu_trace_rays.py
+fit in the trace kernel's first fill of its slots, or barely leave it, and in one chunk per query warp, so they run few or no
+second claims from the queue, no compaction over many tiles and no grid-stride step of the auxiliary-buffer kernels. Every
+case here asserts that
+it reaches past them, against the bound B = sm_count x max_threads_per_multi_processor of the device it runs on
+(tests/test_full_frames_cpu.py, whose LEDGER names the case of each of the 36 trace kernels)."""
 import time
 
 import numpy as np
@@ -13,10 +16,14 @@ import pytest
 
 import oracle_aov as OA
 import oracle_lens as OL
+import oracle_py as O
 import rtb200 as R
 from rtb200 import scenes
-from test_full_frames_cpu import (COVER_N, MIN, N, ROUNDS, H, W, assert_list_reach, assert_pixel_reach, cover_scene, lit_config,
-                                  lit_scene, params, restated)
+from test_full_frames_cpu import (COVER_N, FRAME_SPP, FRAME_WORK, GROUP_SPP, GROUP_W, LENS_FRAMES, MIN, N, RAYS_KW, RAYS_N, RAYS_SPP,
+                                  ROUNDS, SPLIT_DEPTH, H, W, assert_list_reach, assert_pixel_reach, cover_scene, frame_groups,
+                                  frame_want, full_frames, full_rays, full_scene, lit_config, lit_scene, params, rays_want,
+                                  restated, view_of, with_depth)
+from test_denoise_cpu import assert_bits_equal
 from test_gpu_aov import assert_aov_equal
 from test_gpu_intersect import BRUTE, EXACT, FILTERED, _torch
 from test_gpu_lens import SEED64, lensed
@@ -24,6 +31,7 @@ from test_gpu_shading_edges import assert_frames_match, scene_of, synthetic_text
 
 pytestmark = pytest.mark.gpu
 VARIANTS = {"tree": FILTERED, "brute_force": BRUTE, "exact_f64": EXACT}
+SCENES = ("lit", "unlit")   # the LIGHTS = true and false kernels
 AOV_W, AOV_H = 1920, 1080
 
 
@@ -91,12 +99,22 @@ def test_adaptive_round_by_round_at_scale(m):
         rs.release()
 
 
-def test_adaptive_cover_scene_at_scale(bound):
+def check_cover_scene(variant, bound):
+    """Q_LIST without lights: the cover scene's adaptive rounds in `variant`."""
     sc = cover_scene()
     want = restated("cover", sc, 8)
     assert_list_reach(want, W * H, 8, COVER_N, bound, "cover")
-    img, lin, cnt, st = R.render_adaptive(sc, params(8), R.make_options(variant=FILTERED))
-    assert_adaptive(img, lin, cnt, st, want, "cover")
+    img, lin, cnt, st = R.render_adaptive(sc, params(8), R.make_options(variant=VARIANTS[variant]))
+    assert_adaptive(img, lin, cnt, st, want, f"cover {variant}")
+
+
+def test_adaptive_cover_scene_at_scale(bound):
+    check_cover_scene("tree", bound)
+
+
+@pytest.mark.parametrize("variant", ["brute_force", "exact_f64"])
+def test_adaptive_cover_scene_validation_modes_at_scale(variant, bound):
+    check_cover_scene(variant, bound)
 
 
 def test_adaptive_max_depth_0_at_1080p(bound):
@@ -153,26 +171,34 @@ def test_adaptive_shard_handles_at_scale():
         assert_adaptive(si, sl, scnt, None, want, f"rank {rank}", rows)
 
 
-def lit_lens_scene():
-    return lensed(lit_scene(), 0.4, 0.6)
-
-
-@pytest.mark.parametrize("m", ROUNDS)
-@pytest.mark.parametrize("variant", list(VARIANTS))
-def test_adaptive_lens_rounds_at_scale(variant, m, bound):
-    """Q_LIST_LENS: case 1's scene through a lens, against the restatement on the oracle's lens samples."""
-    sc = lit_lens_scene()
-    want = restated("lit_lens", sc, m, lens=sc.lens)
-    assert_list_reach(want, W * H, m, N, bound, f"lit lens, m = {m}")
+def check_lens_rounds(variant, m, scene, bound):
+    """Q_LIST_LENS: the `scene` through a lens, against the restatement on the oracle's lens samples."""
+    sc = lensed(full_scene(scene), 0.4, 0.6)
+    want = restated(f"{scene}_lens", sc, m, lens=sc.lens)
+    assert_list_reach(want, W * H, m, N, bound, f"{scene} lens, m = {m}")
     rs = R.ResidentScene(sc, R.make_options(variant=VARIANTS[variant]))
     try:
         rs.adaptive_begin(params(m))
         active, st = rs.adaptive_step(100)
         img, lin, cnt = resolve(rs)
         assert active == 0
-        assert_adaptive(img, lin, cnt, st, want, f"lens {variant}, m = {m}")
+        assert_adaptive(img, lin, cnt, st, want, f"{scene} lens {variant}, m = {m}")
     finally:
         rs.release()
+
+
+@pytest.mark.parametrize("m", ROUNDS)
+@pytest.mark.parametrize("variant", list(VARIANTS))
+def test_adaptive_lens_rounds_at_scale(variant, m, bound):
+    """Case 1's scene through a lens."""
+    check_lens_rounds(variant, m, "lit", bound)
+
+
+@pytest.mark.parametrize("m", ROUNDS)
+@pytest.mark.parametrize("variant", list(VARIANTS))
+def test_adaptive_lens_rounds_unlit_at_scale(variant, m, bound):
+    """Case 1's scene without its lights through a lens: the LIGHTS = false kernels of Q_LIST_LENS."""
+    check_lens_rounds(variant, m, "unlit", bound)
 
 
 # ---- auxiliary buffers (rt_aov_kernel, rt_aov_lens_kernel) ----------------------------------------------------------------
@@ -275,27 +301,224 @@ def test_aov_shard_handles_at_1080p():
 
 # ---- lens frames (Q_FRAMES_LENS) -----------------------------------------------------------------------------------------
 
-def test_lens_frames_at_scale(bound):
-    """Four lens frames of 960 x 540 x 4, each with its own camera, lens and 64-bit key, in one launch group."""
-    sc = lit_scene(960, 540, 4)
+_LENS_FRAMES = {}
+
+
+def lens_frames(sc):
+    """Four lens frames of sc, each with its own camera, lens and 64-bit key."""
     specs = [((13.0, 2.0, 3.0), 0.4, None), ((10.0, 3.0, -6.0), 0.2, 8.0), ((-9.0, 2.5, 7.0), 0.6, 5.0), ((4.0, 6.0, 12.0), 0.3, 14.0)]
     frames, lenses = [], []
     for k, (lf, ap, fd) in enumerate(specs):
         f, L = R.make_frame_lens(sc, look_from=list(lf), aperture=ap, focus_dist=fd, seed=SEED64 + k * 0x0000000100000003)
         assert L.radius > 0
         frames.append(f); lenses.append(L)
-    work = len(frames) * 960 * 540 * 4
+    return frames, lenses
+
+
+def lens_frames_want(scene, sc, frames, lenses):
+    """The oracle's lens renders of the frames, once per scene: [(linear, rgb8, rays)]."""
+    if scene not in _LENS_FRAMES:
+        t = time.perf_counter()
+        outs = []
+        for f, L in zip(frames, lenses):
+            w = OL.render(view_of(sc, f), L)
+            outs.append((w["linear"], w["rgb8"], w["rays"]))
+        _LENS_FRAMES[scene] = outs
+        print(f"[oracle] lens frames {scene}: {len(frames) * int(sc.c.width) * int(sc.c.height) * int(sc.c.samples_per_pixel):,} "
+              f"samples in {time.perf_counter() - t:.1f} s")
+    return _LENS_FRAMES[scene]
+
+
+def check_lens_frames(variant, scene, bound):
+    """Four lens frames of 960 x 540 x 4, each with its own camera, lens and 64-bit key, in one launch group."""
+    w, h, spp = LENS_FRAMES
+    sc = full_scene(scene, w, h, spp)
+    frames, lenses = lens_frames(sc)
+    work = len(frames) * w * h * spp
     assert_pixel_reach(work, bound, "lens frames")
-    lin, st = R.render_frames(sc, frames, linear=True, lenses=lenses)
-    img, st8 = R.render_frames(sc, frames, lenses=lenses)
+    opts = R.make_options(variant=VARIANTS[variant])
+    lin, st = R.render_frames(sc, frames, opts, linear=True, lenses=lenses)
+    img, st8 = R.render_frames(sc, frames, opts, lenses=lenses)
     # one group: one trace launch for the four frames and a resolve per frame
     assert st["batches"] == st8["batches"] == 1 and st["kernel_launches"] == st8["kernel_launches"] == 1 + len(frames), st
-    rays, t = 0, time.perf_counter()
-    for k, (f, L) in enumerate(zip(frames, lenses)):
-        one = R.Scene.edited(sc)
-        one.c.camera = f.camera; one.seed = f.seed
-        want = OL.render(one, L)
-        assert_frames_match((lin[k], img[k]), (want["linear"], want["rgb8"]), f"frame {k}")
-        rays += want["rays"]
-    print(f"[oracle] lens frames: {work:,} samples in {time.perf_counter() - t:.1f} s")
+    want = lens_frames_want(scene, sc, frames, lenses)
+    for k, (wl, wi, _) in enumerate(want):
+        assert_frames_match((lin[k], img[k]), (wl, wi), f"{scene} {variant} frame {k}")
+    rays = sum(r for _, _, r in want)
     assert st["rays"] == st8["rays"] == rays and st["samples"] == work, (st["rays"], rays)
+
+
+def test_lens_frames_at_scale(bound):
+    check_lens_frames("tree", "lit", bound)
+
+
+# the other five (mode, scene) pairs of Q_FRAMES_LENS
+@pytest.mark.parametrize("variant, scene", [(v, s) for v in VARIANTS for s in SCENES if (v, s) != ("tree", "lit")])
+def test_lens_frames_every_mode_and_scene_at_scale(variant, scene, bound):
+    check_lens_frames(variant, scene, bound)
+
+
+# ---- pinhole frames (Q_SINGLE, Q_FRAMES) and their variance ----------------------------------------------------------------
+
+def assert_frame(lin, img, want, what):
+    assert_frames_match((lin, img), (want["linear"], want["rgb8"]), what)
+
+
+def frames_opts(variant, **kw):
+    return R.make_options(variant=VARIANTS[variant], **kw)
+
+
+@pytest.mark.parametrize("scene", SCENES)
+@pytest.mark.parametrize("variant", list(VARIANTS))
+def test_single_frame_at_scale(variant, scene, bound):
+    """Q_SINGLE: frame 0 rendered alone, the oracle's samples summed in sample order."""
+    assert_pixel_reach(FRAME_WORK, bound, "one frame")
+    sc = full_scene(scene, spp=FRAME_SPP)
+    view = view_of(sc, full_frames(sc)[0])
+    want = frame_want(scene, 0)
+    lin, st = R.render_linear(view, frames_opts(variant))
+    img, st8 = R.render_rgb8(view, frames_opts(variant))
+    assert_frame(lin, img, want, f"{scene} {variant}")
+    assert st["batches"] == st8["batches"] == 1, st
+    assert st["rays"] == st8["rays"] == want["rays"] and st["samples"] == FRAME_WORK, (st["rays"], want["rays"])
+
+
+@pytest.mark.parametrize("scene", SCENES)
+@pytest.mark.parametrize("variant", list(VARIANTS))
+def test_frame_group_at_scale(variant, scene, bound):
+    """Q_FRAMES: two frames with their own cameras and keys in one launch; with another max_depth for frame 1, two
+    single-frame launches."""
+    assert_pixel_reach(2 * FRAME_WORK, bound, "frame group")
+    sc = full_scene(scene, spp=FRAME_SPP)
+    frames = full_frames(sc)
+    wants = [frame_want(scene, k) for k in range(2)]
+    lin, st = R.render_frames(sc, frames, frames_opts(variant), linear=True)
+    img, st8 = R.render_frames(sc, frames, frames_opts(variant))
+    assert st["batches"] == st8["batches"] == 1 and st["kernel_launches"] == st8["kernel_launches"] == 1 + 2, st
+    for k in range(2):
+        assert_frame(lin[k], img[k], wants[k], f"{scene} {variant} frame {k}")
+    rays = sum(w["rays"] for w in wants)
+    assert st["rays"] == st8["rays"] == rays and st["samples"] == 2 * FRAME_WORK, (st["rays"], rays)
+
+    split = [frames[0], with_depth(frames[1], SPLIT_DEPTH)]
+    assert frame_groups([f.max_depth for f in split], FRAME_WORK) == [1, 1]
+    wants[1] = frame_want(scene, 1, SPLIT_DEPTH)
+    lin, st = R.render_frames(sc, split, frames_opts(variant), linear=True)
+    img, st8 = R.render_frames(sc, split, frames_opts(variant))
+    assert st["batches"] == st8["batches"] == 2 and st["kernel_launches"] == st8["kernel_launches"] == 2 + 2, st
+    for k in range(2):
+        assert_frame(lin[k], img[k], wants[k], f"{scene} {variant} split frame {k}")
+    assert st["rays"] == sum(w["rays"] for w in wants), st["rays"]
+
+
+@pytest.mark.parametrize("scene", SCENES)
+def test_frame_variance_and_batches_at_scale(scene, bound):
+    """The variance of the pixel means of the group and of frame 0 alone, and of frame 0 over three sample batches (3, 3
+    and 2 samples, accum and accum_sq carried over 230,400 pixels), bit for bit against the formula on the oracle's
+    samples; the image is unchanged by the batches."""
+    sc = full_scene(scene, spp=FRAME_SPP)
+    frames = full_frames(sc)
+    wants = [frame_want(scene, k) for k in range(2)]
+    lin, var, st = R.render_frames(sc, frames, linear=True, variance=True)
+    img, _, _ = R.render_frames(sc, frames, variance=True)
+    assert st["batches"] == 1 and st["kernel_launches"] == 1 + 2, st
+    for k in range(2):
+        assert_frame(lin[k], img[k], wants[k], f"{scene} variance group frame {k}")
+        assert_bits_equal(var[k], wants[k]["variance"], f"{scene} variance of group frame {k}")
+    img, var8, _ = R.render_frames(sc, frames[:1], variance=True)
+    lin, var, st = R.render_frames(sc, frames[:1], linear=True, variance=True)
+    assert st["batches"] == 1, st
+    assert_frame(lin[0], img[0], wants[0], f"{scene} variance frame 0")
+    assert_bits_equal(var[0], wants[0]["variance"], f"{scene} variance of frame 0")
+    assert_bits_equal(var8, var, f"{scene} variance of the rgb8 call")
+
+    capped = R.make_options(sample_buffer_bytes=3 * W * H * 16)
+    assert 3 * W * H >= 2 * bound, ("a batch of 3 samples reaches past the first fill", 3 * W * H, bound)
+    img, var8, st8 = R.render_frames(sc, frames[:1], capped, variance=True)
+    lin, var, st = R.render_frames(sc, frames[:1], capped, linear=True, variance=True)
+    assert st["batches"] == st8["batches"] == 3 and st["kernel_launches"] == 3 + 3, st
+    assert_frame(lin[0], img[0], wants[0], f"{scene} frame 0 in three batches")
+    assert_bits_equal(var[0], wants[0]["variance"], f"{scene} variance in three batches")
+    assert_bits_equal(var8, var, f"{scene} variance of the rgb8 call in three batches")
+    assert st["rays"] == wants[0]["rays"] and st["samples"] == FRAME_WORK, st
+
+
+def test_frame_group_shards_at_scale(bound):
+    """Row-band shard handles (world 3, band_rows 7) of the lit frame group in the tree mode: each rank's rows of both
+    frames, one launch group per rank."""
+    sc = full_scene("lit", spp=FRAME_SPP)
+    frames = full_frames(sc)
+    wants = [frame_want("lit", k) for k in range(2)]
+    full, _ = R.render_frames(sc, frames, frames_opts("tree"), linear=True)
+    for rank in range(3):
+        rows = R.shard_row_indices(H, rank, 3, 7)
+        assert_pixel_reach(2 * len(rows) * W * FRAME_SPP, bound, f"rank {rank}")
+        opts = frames_opts("tree", rank=rank, world=3, band_rows=7)
+        lin, st = R.render_frames(sc, frames, opts, linear=True)
+        img, _ = R.render_frames(sc, frames, opts)
+        assert lin.shape[1] == len(rows) > 0 and st["batches"] == 1 and st["kernel_launches"] == 1 + 2, (rank, st)
+        assert_bits_equal(lin, full[:, rows], f"rank {rank} vs the full frames")
+        for k in range(2):
+            assert_frames_match((lin[k], img[k]), (wants[k]["linear"][rows], wants[k]["rgb8"][rows]), f"rank {rank} frame {k}")
+
+
+# ---- caller-supplied rays (Q_RAYS) -----------------------------------------------------------------------------------------
+
+@pytest.mark.parametrize("scene", SCENES)
+@pytest.mark.parametrize("variant", list(VARIANTS))
+def test_trace_rays_at_scale(variant, scene, bound):
+    """300,001 rays x 4 samples in one launch from sample 3 and stream 7, against oracle_trace_rays; then on a handle whose
+    cap holds one sample of every ray, four launches, the same bytes."""
+    assert_pixel_reach(RAYS_N * RAYS_SPP, bound, "trace_rays")
+    sc = full_scene(scene)
+    o, d = full_rays()
+    want = rays_want(scene)
+    rs = R.ResidentScene(sc, frames_opts(variant))
+    small = R.ResidentScene(sc, frames_opts(variant, sample_buffer_bytes=RAYS_N * 16))
+    try:
+        got = rs.trace_rays(o, d, RAYS_SPP, rgb8=True, **RAYS_KW)
+        assert_frames_match((got["linear"], got["rgb8"]), (want["linear"], want["rgb8"]), f"{scene} {variant}")
+        st = got["stats"]
+        assert st["batches"] == 1 and st["kernel_launches"] == 2, st
+        assert st["rays"] == want["rays"] and st["samples"] == RAYS_N * RAYS_SPP, (st["rays"], want["rays"])
+        b = small.trace_rays(o, d, RAYS_SPP, rgb8=True, **RAYS_KW)
+        assert b["stats"]["batches"] == RAYS_SPP and b["stats"]["kernel_launches"] == 2 * RAYS_SPP, b["stats"]
+        assert np.array_equal(b["linear"].view(np.uint32), got["linear"].view(np.uint32)) and np.array_equal(b["rgb8"], got["rgb8"])
+        assert b["stats"]["rays"] == st["rays"]
+    finally:
+        rs.release(); small.release()
+
+
+# ---- the frame-group bound, kGroupMaxFrameWork = 2^24 ----------------------------------------------------------------------
+
+GROUP_VIEWS = [dict(), dict(look_from=[-9.0, 2.5, 7.0], look_at=[0.0, 0.5, 0.0]), dict(look_from=[10.0, 3.0, -6.0]),
+               dict(look_from=[4.0, 6.0, 12.0]), dict(look_from=[-12.0, 1.5, -4.0], look_at=[0.0, 1.0, 0.0])]
+
+
+@pytest.mark.parametrize("rows, n, groups", [(512, 2, [2]), (513, 2, [1, 1]), (512, 5, [4, 1])],
+                         ids=["at_the_bound", "one_row_over", "five_at_the_default_cap"])
+def test_frame_groups_at_the_frame_work_bound(rows, n, groups):
+    """Frames of exactly 2^24 samples (1024 x 512 x 32) group, one row more runs each frame alone, and at the default 1 GiB
+    cap five of them form groups of 4 and 1; every frame equals its own single-frame render bit for bit, and the oracle on
+    its top, middle and bottom rows."""
+    sc = full_scene("lit", GROUP_W, rows, GROUP_SPP)
+    frames = [R.make_frame(sc, seed=SEED64 + 0x100000001 * k, **GROUP_VIEWS[k]) for k in range(n)]
+    assert frame_groups([f.max_depth for f in frames], GROUP_W * rows * GROUP_SPP) == groups
+    lin, st = R.render_frames(sc, frames, linear=True)
+    img, st8 = R.render_frames(sc, frames)
+    assert st["batches"] == st8["batches"] == len(groups) and st["kernel_launches"] == len(groups) + n, st
+    rays, t = 0, 0.0
+    for k, f in enumerate(frames):
+        view = view_of(sc, f)
+        one, st1 = R.render_linear(view)
+        one8, _ = R.render_rgb8(view)
+        assert st1["batches"] == 1
+        assert_frames_match((lin[k], img[k]), (one, one8), f"frame {k} vs its own render")
+        rays += st1["rays"]
+        t0 = time.perf_counter()
+        for y in (0, rows // 2, rows - 1):
+            wl, wi, _ = O.render(view, y0=y, y1=y + 1)
+            assert_frames_match((lin[k, y], img[k, y]), (wl[y], wi[y]), f"frame {k} row {y} vs the oracle")
+        t += time.perf_counter() - t0
+    print(f"[oracle] group bound, {n} frames of {GROUP_W} x {rows}: 3 rows each in {t:.1f} s")
+    assert st["rays"] == st8["rays"] == rays and st["samples"] == n * GROUP_W * rows * GROUP_SPP, (st["rays"], rays)

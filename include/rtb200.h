@@ -448,6 +448,41 @@ int rtb200_scene_intersect(rtb200_scene_handle h, const rt_rays* rays, uint32_t 
 int rtb200_scene_occluded_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, uint8_t* occluded, void* stream);
 int rtb200_scene_occluded(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, uint8_t* occluded, rt_stats* stats);
 
+/* ---- point queries on a resident scene (DESIGN.md §4.19) ------------------------------------------------------------------
+ * Contract: for point p = point[3i..3i+2] (any f64 values) and sphere j of the handle's CURRENT list (centre c, radius R, any
+ * material, lights included), the distance is computed with round-to-nearest and no contraction:
+ *   x = fl(p.x - c.x),  y = fl(p.y - c.y),  z = fl(p.z - c.z)
+ *   s = fl(sqrt(fl(fl(fl(x*x) + fl(y*y)) + fl(z*z))))
+ *   dist_j = fl(s - |R|)
+ * the signed distance to the sphere's surface: negative inside, and |R| because a negative radius has the same surface. numpy
+ * float64 reproduces it bit for bit.
+ * Nearest: point i has the bound b_i = bound[i] (+inf when bound is NULL). The answer is the sphere j with dist_j < b_i and the
+ * least dist_j, the lowest index among equal distances: sphere = j, distance = dist_j. With no such sphere, sphere = 0xffffffff
+ * and distance = +inf. So a NaN distance never qualifies, and neither does +inf; a NaN point, or a NaN or -inf bound, gives
+ * none; a scene with no spheres gives none everywhere.
+ * Overlaps: ball i has centre point i and radius bound[i] (required). overlaps[i] = 1 iff some sphere has dist_j < bound[i],
+ * else 0: bit for bit nearest(point i, bound[i]).sphere != 0xffffffff. Touching (dist_j = r) does not count; r = 0 asks whether
+ * the point lies strictly inside a sphere.
+ * Every variant gives the same answers. */
+typedef struct {
+    const double* point;      /* n x 3 */
+    const double* bound;      /* n, or NULL (nearest only): +inf for every point */
+} rt_points;                  /* 16 bytes */
+typedef struct {              /* either may be NULL, not both */
+    double* distance; uint32_t* sphere;
+} rt_nearest;                 /* 16 bytes */
+/* Device buffers, stream-ordered, with the ordering, memory-kind checks and guard-trip reporting of
+ * rtb200_scene_intersect_device: after the last update, rebuild or edit of h enqueued before, on any stream; later updates,
+ * rebuilds, edits and the release wait for it; no work set. The host forms are blocking, through the same kernels; their stats
+ * (may be NULL): rays = n, candidates (exact distance evaluations), clusters (leaves visited), nodes (nodes visited), the times,
+ * byte counts and kernel_launches; a traversal-guard trip fails the call with RT_ERR_CUDA.
+ * RT_ERR_INVALID, before any device work, for a NULL handle, q, q->point or output, an rt_nearest with both outputs NULL, or an
+ * overlaps call with a NULL q->bound. n == 0 is a no-op. */
+int rtb200_scene_nearest_device(rtb200_scene_handle h, const rt_points* q, uint32_t n, const rt_nearest* out, void* stream);
+int rtb200_scene_nearest(rtb200_scene_handle h, const rt_points* q, uint32_t n, const rt_nearest* out, rt_stats* stats);
+int rtb200_scene_overlaps_device(rtb200_scene_handle h, const rt_points* q, uint32_t n, uint8_t* overlaps, void* stream);
+int rtb200_scene_overlaps(rtb200_scene_handle h, const rt_points* q, uint32_t n, uint8_t* overlaps, rt_stats* stats);
+
 /* ---- radiance of caller-supplied primary rays on a resident scene (DESIGN.md §4.12) --------------------------------------
  * Contract: for ray i (origin, direction as in rt_rays, any f64 values; rays->t_max must be NULL) and sample j < samples, the
  * sample's radiance is ray_color(Ray{o, d}, max_depth, max_depth) (raytracer.rs:71-165) over the handle's CURRENT spheres. It

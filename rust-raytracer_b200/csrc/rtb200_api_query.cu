@@ -1,7 +1,7 @@
-// rtb200_api_query.cu — closest-hit and occlusion queries of caller-supplied rays on a resident scene through the C ABI
-// (DESIGN.md §4.10, §4.11), and the auxiliary buffers of its camera samples (§4.14), in both forms: device buffers on the
-// caller's stream, or host buffers staged through the context's query block (HostStage, which the host form of
-// rtb200_scene_trace_rays uses too).
+// rtb200_api_query.cu — closest-hit and occlusion queries of caller-supplied rays, nearest-sphere and overlap queries of
+// caller-supplied points (DESIGN.md §4.10, §4.11, §4.19) on a resident scene through the C ABI, and the auxiliary buffers of
+// its camera samples (§4.14), in both forms: device buffers on the caller's stream, or host buffers staged through the
+// context's query block (HostStage, which the host form of rtb200_scene_trace_rays uses too).
 
 #include "rtb200_host.cuh"
 
@@ -31,66 +31,101 @@ int HostStage::copy(cudaStream_t st, bool back) {
     return RT_OK;
 }
 
-// What a query writes: the outputs of rt_hits (closest-hit), or the occlusion bits. Output k is ptr[k], bytes[k] per ray.
+// The four kinds of query: closest hits and occlusion of rays (§4.10, §4.11), nearest spheres and overlaps of points (§4.19).
+enum QueryKind { QK_HITS, QK_OCCLUDED, QK_NEAREST, QK_OVERLAPS };
+
+// What a query reads: input k is ptr[k], bytes[k] per ray or point (a null optional input: not read). The rays' origin,
+// direction and t_max, or the points' point and bound; `given` is false when the caller passed no rt_rays or rt_points.
+struct QueryIn {
+    bool given;
+    int count;
+    const void* ptr[3];
+    uint32_t bytes[3];
+    const char* name[3];
+};
+static QueryIn rays_in(const rt_rays* p) {
+    const rt_rays r = p ? *p : rt_rays{};
+    return QueryIn{p != nullptr, 3, {r.origin, r.direction, r.t_max}, {24, 24, 8}, {"rays->origin", "rays->direction", "rays->t_max"}};
+}
+static QueryIn points_in(const rt_points* p) {
+    const rt_points q = p ? *p : rt_points{};
+    return QueryIn{p != nullptr, 2, {q.point, q.bound}, {24, 8}, {"q->point", "q->bound"}};
+}
+
+// What a query writes: the outputs of rt_hits (closest-hit), the occlusion bits, the outputs of rt_nearest, or the overlap bits.
+// Output k is ptr[k], bytes[k] per ray or point; `given` is false when the caller passed no rt_hits or rt_nearest.
 struct QueryOut {
-    bool any;             // occlusion
-    rt_hits hits;         // closest-hit
-    uint8_t* occluded;    // occlusion
+    QueryKind kind;
+    bool given;
     int count;
     void* ptr[6];
     uint32_t bytes[6];
     const char* name[6];
 };
-static QueryOut hits_out(const rt_hits& o) {
-    QueryOut q{false, o, nullptr, 6, {o.t, o.sphere, o.point, o.normal, o.uv, o.front_face}, {8, 4, 24, 24, 16, 1},
-               {"out->t", "out->sphere", "out->point", "out->normal", "out->uv", "out->front_face"}};
-    return q;
+static QueryOut hits_out(const rt_hits* p) {
+    const rt_hits o = p ? *p : rt_hits{};
+    return QueryOut{QK_HITS, p != nullptr, 6, {o.t, o.sphere, o.point, o.normal, o.uv, o.front_face}, {8, 4, 24, 24, 16, 1},
+                    {"out->t", "out->sphere", "out->point", "out->normal", "out->uv", "out->front_face"}};
 }
-static QueryOut occluded_out(uint8_t* o) {
-    QueryOut q{true, rt_hits{}, o, 1, {o}, {1}, {"occluded"}};
-    return q;
+static QueryOut occluded_out(uint8_t* o) { return QueryOut{QK_OCCLUDED, true, 1, {o}, {1}, {"occluded"}}; }
+static QueryOut nearest_out(const rt_nearest* p) {
+    const rt_nearest o = p ? *p : rt_nearest{};
+    return QueryOut{QK_NEAREST, p != nullptr, 2, {o.distance, o.sphere}, {8, 4}, {"out->distance", "out->sphere"}};
 }
-// the same outputs at other addresses (the host form's device image)
-static QueryOut with_ptrs(const QueryOut& o, char* const* p) {
-    if (o.any) return occluded_out((uint8_t*)p[0]);
-    return hits_out(rt_hits{(double*)p[0], (uint32_t*)p[1], (double*)p[2], (double*)p[3], (double*)p[4], (uint8_t*)p[5]});
-}
+static QueryOut overlaps_out(uint8_t* o) { return QueryOut{QK_OVERLAPS, true, 1, {o}, {1}, {"overlaps"}}; }
 
-// The argument checks both forms of both kinds share (no device is touched).
-static int check_query(rtb200_scene_handle h, const rt_rays* rays, const QueryOut* out) {
+// The argument checks all forms of all kinds share (no device is touched).
+static int check_query(rtb200_scene_handle h, const QueryIn* in, const QueryOut* out) {
+    const bool rays = out->kind == QK_HITS || out->kind == QK_OCCLUDED;
     if (!h) return fail(RT_ERR_INVALID, "null scene handle");
-    if (!rays || !out) return fail(RT_ERR_INVALID, "rays or out is null");
-    if (!rays->origin || !rays->direction) return fail(RT_ERR_INVALID, "rays->origin or rays->direction is null");
+    if (!in->given || !out->given) return fail(RT_ERR_INVALID, rays ? "rays or out is null" : "q or out is null");
+    if (rays && (!in->ptr[0] || !in->ptr[1])) return fail(RT_ERR_INVALID, "rays->origin or rays->direction is null");
+    if (!rays && !in->ptr[0]) return fail(RT_ERR_INVALID, "q->point is null");
+    if (out->kind == QK_OVERLAPS && !in->ptr[1]) return fail(RT_ERR_INVALID, "q->bound is null: overlaps needs the balls' radii");
     bool any_out = false;
     for (int k = 0; k < out->count; ++k) any_out = any_out || out->ptr[k];
-    if (!any_out) return fail(RT_ERR_INVALID, out->any ? "occluded is null" : "every output of out is null");
+    if (!any_out) return fail(RT_ERR_INVALID, out->count == 1 ? (out->kind == QK_OCCLUDED ? "occluded is null" : "overlaps is null")
+                                                              : "every output of out is null");
     return RT_OK;
 }
 
-// The one path of both forms: enqueue the query of the n rays `rays` into `out` (device buffers) on `st`, which the caller has
-// ordered after the scene's last writer (scene_stream). Guard trips go to err[1], the counters to stat (null: not counted).
-static int query_enqueue(rtb200_scene_handle h, const rt_rays& rays, uint32_t n, const QueryOut& out, unsigned long long* stat,
+// The one path of both forms: enqueue the query of the n rays or points `in` into `out` (device buffers) on `st`, which the caller
+// has ordered after the scene's last writer (scene_stream). Guard trips go to err[1], the counters to stat (null: not counted).
+static int query_enqueue(rtb200_scene_handle h, const QueryIn& in, uint32_t n, const QueryOut& out, unsigned long long* stat,
                          unsigned long long* err, cudaStream_t st) {
-    int& occ = h->ctx->query_occ[out.any ? 1 : 0][h->mode];
-    if (occ == 0) occ = query_max_ctas_per_sm(h->mode, out.any);
+    static const int kOccRow[4] = {0, 1, 4, 5};   // DeviceCtx::query_occ's row of each kind
+    const bool pts = out.kind == QK_NEAREST || out.kind == QK_OVERLAPS;
+    const bool any = out.kind == QK_OCCLUDED || out.kind == QK_OVERLAPS;
+    int& occ = h->ctx->query_occ[kOccRow[out.kind]][h->mode];
+    if (occ == 0) occ = pts ? distance_max_ctas_per_sm(h->mode, any) : query_max_ctas_per_sm(h->mode, any);
     if (occ <= 0) { occ = 0; return fail(RT_ERR_UNSUPPORTED, "no launch configuration of the query kernel fits shared memory"); }
     const int max_grid = h->ctx->sm_count * occ;
+    if (pts) {
+        DistanceParams q{};
+        q.p = h->tp; q.p.stat = stat; q.p.err = err;
+        q.point = (const double*)in.ptr[0]; q.bound = (const double*)in.ptr[1];
+        q.distance = any ? nullptr : (double*)out.ptr[0]; q.sphere = any ? nullptr : (uint32_t*)out.ptr[1];
+        q.overlaps = any ? (uint8_t*)out.ptr[0] : nullptr;
+        q.n = n;
+        CU(launch_distance(q, h->mode, any, max_grid, st));
+        return RT_OK;
+    }
     auto common = [&](auto& q) {
         q.p = h->tp; q.p.stat = stat; q.p.err = err;
-        q.origin = rays.origin; q.direction = rays.direction; q.t_max = rays.t_max;
+        q.origin = (const double*)in.ptr[0]; q.direction = (const double*)in.ptr[1]; q.t_max = (const double*)in.ptr[2];
         q.n = n;
     };
-    if (out.any) {
+    if (any) {
         OcclusionParams q{};
         common(q);
-        q.occluded = out.occluded;
+        q.occluded = (uint8_t*)out.ptr[0];
         CU(launch_occluded(q, h->mode, max_grid, st));
         return RT_OK;
     }
     QueryParams q{};
     common(q);
-    const rt_hits& o = out.hits;
-    q.t = o.t; q.sphere = o.sphere; q.point = o.point; q.normal = o.normal; q.uv = o.uv; q.front_face = o.front_face;
+    q.t = (double*)out.ptr[0]; q.sphere = (uint32_t*)out.ptr[1]; q.point = (double*)out.ptr[2]; q.normal = (double*)out.ptr[3];
+    q.uv = (double*)out.ptr[4]; q.front_face = (uint8_t*)out.ptr[5];
     CU(launch_query(q, h->mode, max_grid, st));
     return RT_OK;
 }
@@ -113,44 +148,45 @@ static int mark_query(rtb200_scene_handle h, cudaStream_t st) {
     return RT_OK;
 }
 
-// The device form of both kinds.
-static int query_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const QueryOut* out, void* stream_in) {
-    int rc = check_query(h, rays, out);
+// The device form of every kind.
+static int query_device(rtb200_scene_handle h, const QueryIn* in, uint32_t n, const QueryOut* out, void* stream_in) {
+    int rc = check_query(h, in, out);
     if (rc != RT_OK) return rc;
     if (n == 0) return RT_OK;
     HANDLE_PROLOGUE(h);
-    std::vector<std::pair<const void*, const char*>> ptrs = {{rays->origin, "rays->origin"}, {rays->direction, "rays->direction"},
-                                                             {rays->t_max, "rays->t_max"}};
+    std::vector<std::pair<const void*, const char*>> ptrs;
+    for (int k = 0; k < in->count; ++k) ptrs.push_back({in->ptr[k], in->name[k]});
     for (int k = 0; k < out->count; ++k) ptrs.push_back({out->ptr[k], out->name[k]});
     if ((rc = check_device_ptrs(h, ptrs)) != RT_OK) return rc;
     cudaStream_t st;
     CU(scene_stream(h, stream_in, &st));
-    if ((rc = query_enqueue(h, *rays, n, *out, nullptr, h->err, st)) != RT_OK) return rc;
+    if ((rc = query_enqueue(h, *in, n, *out, nullptr, h->err, st)) != RT_OK) return rc;
     return mark_query(h, st);
 }
 
-// The host form of both kinds.
-static int query_host(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const QueryOut* out, rt_stats* stats) {
+// The host form of every kind.
+static int query_host(rtb200_scene_handle h, const QueryIn* in, uint32_t n, const QueryOut* out, rt_stats* stats) {
     if (stats) memset(stats, 0, sizeof *stats);
-    int rc = check_query(h, rays, out);
+    int rc = check_query(h, in, out);
     if (rc != RT_OK) return rc;
     if (n == 0) return RT_OK;
     auto wall0 = std::chrono::steady_clock::now();
     HANDLE_PROLOGUE(h);
-    // device image: counters, then rays and outputs
+    // device image: counters, then the inputs and outputs
     const uint64_t N = n;
     HostStage io;
-    io.add_in(rays->origin, N * 24); io.add_in(rays->direction, N * 24); io.add_in(rays->t_max, rays->t_max ? N * 8 : 0);
+    for (int k = 0; k < in->count; ++k) io.add_in(in->ptr[k], in->ptr[k] ? N * in->bytes[k] : 0);
     for (int k = 0; k < out->count; ++k) io.add_out(out->ptr[k], out->ptr[k] ? N * out->bytes[k] : 0);
     cudaStream_t st;
     CU(scene_stream(h, nullptr, &st));
     unsigned long long hstat[kStatBytes / 8];
     rc = host_call(h->ctx, st, io, hstat, "internal error: the traversal guard tripped; the query results are not valid", wall0, stats,
                    [&](unsigned long long* stat) {
-        char* dout[6] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
-        for (int k = 0; k < out->count; ++k) dout[k] = io.a[3 + k].dev;
-        const rt_rays drays{(const double*)io.a[0].dev, (const double*)io.a[1].dev, (const double*)io.a[2].dev};
-        return query_enqueue(h, drays, n, with_ptrs(*out, dout), stat, stat + 30, st);
+        QueryIn din = *in;
+        QueryOut dout = *out;
+        for (int k = 0; k < in->count; ++k) din.ptr[k] = io.a[k].dev;
+        for (int k = 0; k < out->count; ++k) dout.ptr[k] = io.a[in->count + k].dev;
+        return query_enqueue(h, din, n, dout, stat, stat + 30, st);
     });
     if (rc != RT_OK || !stats) return rc;
     stats->rays = hstat[0]; stats->candidates = hstat[1]; stats->clusters = hstat[4]; stats->nodes = hstat[6];
@@ -160,29 +196,65 @@ static int query_host(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, co
 
 int rtb200_scene_intersect_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_hits* out, void* stream_in) {
   return guarded([&]() -> int {
-    const QueryOut o = hits_out(out ? *out : rt_hits{});
-    return query_device(h, rays, n, out ? &o : nullptr, stream_in);
+    const QueryIn i = rays_in(rays);
+    const QueryOut o = hits_out(out);
+    return query_device(h, &i, n, &o, stream_in);
   });
 }
 
 int rtb200_scene_intersect(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, const rt_hits* out, rt_stats* stats) {
   return guarded([&]() -> int {
-    const QueryOut o = hits_out(out ? *out : rt_hits{});
-    return query_host(h, rays, n, out ? &o : nullptr, stats);
+    const QueryIn i = rays_in(rays);
+    const QueryOut o = hits_out(out);
+    return query_host(h, &i, n, &o, stats);
   });
 }
 
 int rtb200_scene_occluded_device(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, uint8_t* occluded, void* stream_in) {
   return guarded([&]() -> int {
+    const QueryIn i = rays_in(rays);
     const QueryOut o = occluded_out(occluded);
-    return query_device(h, rays, n, &o, stream_in);
+    return query_device(h, &i, n, &o, stream_in);
   });
 }
 
 int rtb200_scene_occluded(rtb200_scene_handle h, const rt_rays* rays, uint32_t n, uint8_t* occluded, rt_stats* stats) {
   return guarded([&]() -> int {
+    const QueryIn i = rays_in(rays);
     const QueryOut o = occluded_out(occluded);
-    return query_host(h, rays, n, &o, stats);
+    return query_host(h, &i, n, &o, stats);
+  });
+}
+
+int rtb200_scene_nearest_device(rtb200_scene_handle h, const rt_points* q, uint32_t n, const rt_nearest* out, void* stream_in) {
+  return guarded([&]() -> int {
+    const QueryIn i = points_in(q);
+    const QueryOut o = nearest_out(out);
+    return query_device(h, &i, n, &o, stream_in);
+  });
+}
+
+int rtb200_scene_nearest(rtb200_scene_handle h, const rt_points* q, uint32_t n, const rt_nearest* out, rt_stats* stats) {
+  return guarded([&]() -> int {
+    const QueryIn i = points_in(q);
+    const QueryOut o = nearest_out(out);
+    return query_host(h, &i, n, &o, stats);
+  });
+}
+
+int rtb200_scene_overlaps_device(rtb200_scene_handle h, const rt_points* q, uint32_t n, uint8_t* overlaps, void* stream_in) {
+  return guarded([&]() -> int {
+    const QueryIn i = points_in(q);
+    const QueryOut o = overlaps_out(overlaps);
+    return query_device(h, &i, n, &o, stream_in);
+  });
+}
+
+int rtb200_scene_overlaps(rtb200_scene_handle h, const rt_points* q, uint32_t n, uint8_t* overlaps, rt_stats* stats) {
+  return guarded([&]() -> int {
+    const QueryIn i = points_in(q);
+    const QueryOut o = overlaps_out(overlaps);
+    return query_host(h, &i, n, &o, stats);
   });
 }
 

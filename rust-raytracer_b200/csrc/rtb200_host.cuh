@@ -103,12 +103,12 @@ struct DeviceCtx {
     std::vector<OccKey> occ_cache;        // cudaOccupancyMaxActiveBlocksPerMultiprocessor answers
     PinnedBuf staging;                    // host image of the arena being uploaded
     cudaEvent_t staging_free = nullptr;   // the last H2D copy out of `staging` has finished
-    // the host forms of rtb200_scene_intersect, _occluded, _trace_rays, _aov, rtb200_denoise and rtb200_temporal: their arrays on the device
-    // (HostStage), host_call's timing events (created at its first call), and the resident CTAs per SM of the query kernel of
-    // each kind and mode (0: not asked yet)
+    // the host forms of rtb200_scene_intersect, _occluded, _nearest, _overlaps, _trace_rays, _aov, rtb200_denoise and rtb200_temporal:
+    // their arrays on the device (HostStage), host_call's timing events (created at its first call), and the resident CTAs per SM of
+    // the query kernel of each kind and mode (0: not asked yet)
     GrowBuf query;
     cudaEvent_t query_ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    int query_occ[4][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}, {0, 0, 0}};   // [closest-hit, occlusion, auxiliary buffers, lens ones][mode]
+    int query_occ[6][3] = {};   // [closest-hit, occlusion, auxiliary buffers, lens ones, nearest, overlaps][mode]
 };
 // the context of a device ordinal below 64, created at its first use
 int get_ctx(int device, DeviceCtx** out);

@@ -296,6 +296,18 @@ struct AovParams {
     uint32_t n;                       // local pixels = npix_local
 };
 
+// Point queries (rtb200_distance.cu, DESIGN.md §4.19): `p` is the handle's TraceParams, of which the kernel reads the scene
+// fields, err (guard trips) and stat (the counters; null: not counted). The nearest kind writes distance and sphere (either may be
+// null), the overlaps kind (bound = the balls' radii, never null) writes overlaps.
+struct DistanceParams {
+    TraceParams p;
+    const double* point;         // [n][3]
+    const double* bound;         // [n] or null: +inf
+    double* distance; uint32_t* sphere;
+    uint8_t* overlaps;
+    uint32_t n;
+};
+
 struct KernelInfo { int registers, max_threads, const_bytes, local_bytes; char name[96]; };
 
 // `queue` (TraceQueue): Q_FRAMES is the multi-frame kernel (work ids span p.ftab's frames), Q_LIST the adaptive round's,
@@ -311,6 +323,10 @@ cudaError_t launch_resolve_var(const ResolveVarParams& p, cudaStream_t st);
 int query_max_ctas_per_sm(uint32_t mode, bool any);
 cudaError_t launch_query(const QueryParams& q, uint32_t mode, int max_grid, cudaStream_t st);
 cudaError_t launch_occluded(const OcclusionParams& q, uint32_t mode, int max_grid, cudaStream_t st);
+// point queries, nearest (any = false) and overlaps (any = true): resident CTAs per SM of the kernel of that kind and `mode` (0
+// when it cannot run on the current device), and a launch of at most `max_grid` CTAs (no more than the points need)
+int distance_max_ctas_per_sm(uint32_t mode, bool any);
+cudaError_t launch_distance(const DistanceParams& q, uint32_t mode, bool any, int max_grid, cudaStream_t st);
 // the auxiliary buffers: resident CTAs per SM of the kernel of `mode` (0 when it cannot run on the current device), and a launch
 // of at most `max_grid` CTAs (through the lens kernel when q.p.lens.radius is not 0)
 int aov_max_ctas_per_sm(uint32_t mode, bool lens);   // lens: the kernel whose camera rays go through p.lens

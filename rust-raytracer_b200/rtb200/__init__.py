@@ -127,6 +127,17 @@ class rt_hits(C.Structure):
                 ("front_face", C.c_void_p)]
 
 
+class rt_points(C.Structure):
+    """Points of a point query (rtb200_scene_nearest[_device], rtb200_scene_overlaps[_device]): point n x 3 f64, bound n f64 or
+    NULL (nearest only: +inf); the balls' radii for overlaps."""
+    _fields_ = [("point", C.c_void_p), ("bound", C.c_void_p)]
+
+
+class rt_nearest(C.Structure):
+    """Outputs of a nearest-sphere query, each NULL or n elements (not both NULL): distance f64, sphere u32."""
+    _fields_ = [("distance", C.c_void_p), ("sphere", C.c_void_p)]
+
+
 class rt_trace_params(C.Structure):
     """Radiance of caller-supplied rays (rtb200_scene_trace_rays[_device]): the Philox key, samples per ray, the first sample
     index, the RNG stream of ray 0 (ray i draws from pixel stream stream0 + i) and the depth of ray_color."""
@@ -187,6 +198,7 @@ assert C.sizeof(rt_rays) == 24 and C.sizeof(rt_hits) == 48 and C.sizeof(rt_trace
 assert C.sizeof(rt_aov_params) == 16 and C.sizeof(rt_aov_out) == 40 and C.sizeof(rt_denoise_params) == 32
 assert C.sizeof(rt_temporal_params) == 224 and C.sizeof(rt_temporal_frame) == 24 and C.sizeof(rt_temporal_history) == 32
 assert C.sizeof(rt_temporal_out) == 16 and C.sizeof(rt_lens) == 64 and C.sizeof(rt_denoise_var_params) == 32
+assert C.sizeof(rt_points) == 16 and C.sizeof(rt_nearest) == 16
 AOV_FIELDS = (("albedo", 3, np.float32), ("normal", 3, np.float32), ("hits", 1, np.uint32), ("sphere", 1, np.int32),
               ("point", 3, np.float64))   # rt_aov_out: name, values per pixel, dtype (sphere -1 = 0xffffffff)
 
@@ -213,6 +225,7 @@ ABI_SYMBOLS = [
     "rtb200_probe_lens_ray",
     "rtb200_denoise_var_scratch_bytes", "rtb200_denoise_var_device", "rtb200_denoise_var",
     "rtb200_render_frames_var_device", "rtb200_render_frames_var", "rtb200_adaptive_resolve_var", "rtb200_render_adaptive_var",
+    "rtb200_scene_nearest_device", "rtb200_scene_nearest", "rtb200_scene_overlaps_device", "rtb200_scene_overlaps",
 ]
 
 _lib = None
@@ -275,6 +288,10 @@ def lib() -> C.CDLL:
     L.rtb200_scene_intersect.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.POINTER(rt_hits), C.POINTER(rt_stats)]
     L.rtb200_scene_occluded_device.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.c_void_p, C.c_void_p]
     L.rtb200_scene_occluded.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.c_void_p, C.POINTER(rt_stats)]
+    L.rtb200_scene_nearest_device.argtypes = [C.c_void_p, C.POINTER(rt_points), C.c_uint32, C.POINTER(rt_nearest), C.c_void_p]
+    L.rtb200_scene_nearest.argtypes = [C.c_void_p, C.POINTER(rt_points), C.c_uint32, C.POINTER(rt_nearest), C.POINTER(rt_stats)]
+    L.rtb200_scene_overlaps_device.argtypes = [C.c_void_p, C.POINTER(rt_points), C.c_uint32, C.c_void_p, C.c_void_p]
+    L.rtb200_scene_overlaps.argtypes = [C.c_void_p, C.POINTER(rt_points), C.c_uint32, C.c_void_p, C.POINTER(rt_stats)]
     L.rtb200_scene_trace_rays_device.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.POINTER(rt_trace_params), C.c_void_p,
                                                  C.c_void_p, C.c_void_p, C.POINTER(rt_stats)]
     L.rtb200_scene_trace_rays.argtypes = [C.c_void_p, C.POINTER(rt_rays), C.c_uint32, C.POINTER(rt_trace_params), C.c_void_p,
@@ -875,6 +892,13 @@ def _rays(A: _Arrays, origin, direction, t_max):
     return rt_rays(A.arg("origin", origin, f64, (n, 3)), A.arg("direction", direction, f64, (n, 3)), A.arg("t_max", t_max, f64, (n,), True)), n
 
 
+def _points(A: _Arrays, point, bound, optional: bool):
+    """rt_points and n of a point query, checked by A: point float64 [n, 3], bound float64 [n] (None when `optional`)."""
+    n = point.shape[0] if getattr(point, "ndim", 0) == 2 else "n"
+    f64 = (np.float64,)
+    return rt_points(A.arg("point", point, f64, (n, 3)), A.arg("bound", bound, f64, (n,), optional)), n
+
+
 class ResidentScene:
     """Scene kept in HBM between frames (rtb200_scene_upload / rtb200_render_device)."""
 
@@ -1044,6 +1068,47 @@ class ResidentScene:
             out["stats"] = st.as_dict()
         elif n:
             _check(lib().rtb200_scene_occluded_device(self.h, C.byref(rays), n, A.ptr(out["occluded"]), self._stream(stream, A.device)))
+        return out
+
+    def nearest(self, points, bound=None, stream=None, outputs=None) -> dict:
+        """The nearest of the handle's current spheres to each point, as include/rtb200.h states it, in every variant: the
+        sphere j with dist_j = fl(|p - c_j|) - |R_j| below bound[i] (+inf without a bound) and the least dist_j, the lowest
+        index among equal distances. Negative inside a sphere.
+
+        CUDA tensors (contiguous float64 [n, 3] and [n], on the handle's device) use the device form
+        (rtb200_scene_nearest_device) on `stream`, numpy arrays the blocking host form (rtb200_scene_nearest), with the
+        arguments, checks and stream ordering of :meth:`intersect`. Returns a dict with one entry per name of `outputs`
+        (default: both): "sphere" int32 [n] (-1: none) and "distance" float64 [n] (+inf: none); numpy arrays add "stats"."""
+        fields = (("distance", np.float64), ("sphere", np.int32))
+        names = [f[0] for f in fields] if outputs is None else list(outputs)
+        if not names or any(k not in dict(fields) for k in names):
+            raise ValueError(f"nearest outputs are a non-empty subset of {[f[0] for f in fields]}, got {names}")
+        A = _Arrays("nearest", device=self.device)
+        q, n = _points(A, points, bound, True)
+        out = A.empty([(k, (n,), ty) for k, ty in fields if k in names], stream)
+        res = rt_nearest(A.ptr(out.get("distance")), A.ptr(out.get("sphere")))
+        if A.host:
+            st = rt_stats()
+            _check(lib().rtb200_scene_nearest(self.h, C.byref(q), n, C.byref(res), C.byref(st)))
+            out["stats"] = st.as_dict()
+        elif n:
+            _check(lib().rtb200_scene_nearest_device(self.h, C.byref(q), n, C.byref(res), self._stream(stream, A.device)))
+        return out
+
+    def overlaps(self, centers, radii, stream=None) -> dict:
+        """Whether each ball (centers[i], radii[i]) overlaps one of the handle's current spheres: 1 iff some dist_j < radii[i]
+        (touching does not count), bit for bit nearest(centers, radii)["sphere"] != -1, but the traversal stops at the first
+        such sphere. Forms, checks and stream ordering as :meth:`nearest`. Returns {"overlaps": uint8 [n]}, and with numpy
+        arrays also "stats"."""
+        A = _Arrays("overlaps", device=self.device)
+        q, n = _points(A, centers, radii, False)
+        out = A.empty([("overlaps", (n,), np.uint8)], stream)
+        if A.host:
+            st = rt_stats()
+            _check(lib().rtb200_scene_overlaps(self.h, C.byref(q), n, A.ptr(out["overlaps"]), C.byref(st)))
+            out["stats"] = st.as_dict()
+        elif n:
+            _check(lib().rtb200_scene_overlaps_device(self.h, C.byref(q), n, A.ptr(out["overlaps"]), self._stream(stream, A.device)))
         return out
 
     def trace_rays(self, origin, direction, samples: int = 1, *, sample0: int = 0, stream0: int = 0, seed: Optional[int] = None,

@@ -64,6 +64,7 @@ struct DenoiseStep {
     const float4* alb; const float4* nrm;   // null when that guide is off
     float* out_linear; uint8_t* out_rgb8;   // the last iteration's outputs (each may be null)
     uint32_t width, height, step;
+    AtrousTiles tiles;               // the step's grid
     float lc, la, ln;                // the weights of this iteration (lc = color_weight * 4^i)
 };
 
@@ -107,17 +108,13 @@ RT_DEV void denoise_store(const DenoiseStep& s, uint64_t p, float4 o) {
 // One iteration on shared-memory tiles of step h's residue classes: the pixels (rx + h i, ry + h j) of residue (rx, ry) form a
 // dense sub-grid on which every tap is a neighbour at distance <= 2, so a CTA stages a (kDenoiseBX + 4) x (kDenoiseBY + 4) block
 // of it (a halo of 2; taps outside the image are staged with w = 0) and reads its 25 taps from shared memory. A 1-D grid of
-// tiles (a grid's y extent is limited to 65535): tile x fastest, then tile y, then the residue.
+// tiles (a grid's y extent is limited to 65535) over the residue classes that hold a pixel (AtrousTiles).
 constexpr int kHX = kDenoiseBX + 4, kHY = kDenoiseBY + 4;
 __global__ void __launch_bounds__(kDenoiseBX * kDenoiseBY) rt_denoise_step_kernel(const DenoiseStep s) {
     __shared__ float4 sc[kHY][kHX], sa[kHY][kHX], sn[kHY][kHX];
     const uint32_t h = s.step;
-    const uint32_t nx = (s.width + h - 1) / h, ny = (s.height + h - 1) / h;
-    const uint32_t tn_x = (nx + kDenoiseBX - 1) / kDenoiseBX, tn_y = (ny + kDenoiseBY - 1) / kDenoiseBY;
-    uint32_t b = blockIdx.x;
-    const uint32_t tix = b % tn_x; b /= tn_x;
-    const uint32_t tiy = b % tn_y; b /= tn_y;
-    const uint32_t rx = b % h, ry = b / h;
+    uint32_t tix, tiy, rx, ry;
+    s.tiles.decode(blockIdx.x, tix, tiy, rx, ry);
     const int64_t gx0 = (int64_t)tix * kDenoiseBX - 2, gy0 = (int64_t)tiy * kDenoiseBY - 2;
     const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int k = threadIdx.y * kDenoiseBX + threadIdx.x; k < kHX * kHY; k += kDenoiseBX * kDenoiseBY) {
@@ -167,9 +164,8 @@ cudaError_t launch_denoise(const DenoiseArgs& a, cudaStream_t st) {
         s.width = a.width; s.height = a.height; s.step = 1u << i;
         s.lc = a.color_weight * (float)(1u << (2 * i));   // exact: the host refused a color_weight whose 4^(L-1) multiple overflows
         s.la = a.albedo_weight; s.ln = a.normal_weight;
-        const uint64_t nx = (a.width + s.step - 1) / s.step, ny = (a.height + s.step - 1) / s.step;
-        const uint64_t grid = (nx + kDenoiseBX - 1) / kDenoiseBX * ((ny + kDenoiseBY - 1) / kDenoiseBY) * s.step * s.step;
-        rt_denoise_step_kernel<<<(unsigned)grid, block, 0, st>>>(s);
+        s.tiles = AtrousTiles(a.width, a.height, s.step, kDenoiseBX, kDenoiseBY);
+        rt_denoise_step_kernel<<<(unsigned)s.tiles.ctas(), block, 0, st>>>(s);   // <= width * height CTAs
         e = cudaGetLastError();
     }
     return e;

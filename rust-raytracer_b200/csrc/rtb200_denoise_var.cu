@@ -96,6 +96,7 @@ struct DenoiseVarStep {
     const float* scale;
     float* out_linear; uint8_t* out_rgb8; float* out_variance;        // the last iteration's outputs (each may be null)
     uint32_t width, height, step;
+    AtrousTiles tiles;               // the step's grid
     float lc, la, ln;
 };
 
@@ -105,12 +106,8 @@ constexpr int kVHX = kVarBX + 4, kVHY = kVarBY + 4;
 __global__ void __launch_bounds__(kVarBX * kVarBY) rt_denoise_var_step_kernel(const DenoiseVarStep s) {
     __shared__ float4 sc[kVHY][kVHX], sv[kVHY][kVHX], sa[kVHY][kVHX], sn[kVHY][kVHX];
     const uint32_t h = s.step;
-    const uint32_t nx = (s.width + h - 1) / h, ny = (s.height + h - 1) / h;
-    const uint32_t tn_x = (nx + kVarBX - 1) / kVarBX, tn_y = (ny + kVarBY - 1) / kVarBY;
-    uint32_t b = blockIdx.x;
-    const uint32_t tix = b % tn_x; b /= tn_x;
-    const uint32_t tiy = b % tn_y; b /= tn_y;
-    const uint32_t rx = b % h, ry = b / h;
+    uint32_t tix, tiy, rx, ry;
+    s.tiles.decode(blockIdx.x, tix, tiy, rx, ry);
     const int64_t gx0 = (int64_t)tix * kVarBX - 2, gy0 = (int64_t)tiy * kVarBY - 2;
     const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
     for (int k = threadIdx.y * kVarBX + threadIdx.x; k < kVHX * kVHY; k += kVarBX * kVarBY) {
@@ -199,9 +196,8 @@ cudaError_t launch_denoise_var(const DenoiseVarArgs& a, cudaStream_t st) {
         s.out_variance = last ? a.out_variance : nullptr;
         s.width = a.width; s.height = a.height; s.step = 1u << i;
         s.lc = a.color_weight; s.la = a.albedo_weight; s.ln = a.normal_weight;
-        const uint64_t nx = (a.width + s.step - 1) / s.step, ny = (a.height + s.step - 1) / s.step;
-        const uint64_t grid = (nx + kVarBX - 1) / kVarBX * ((ny + kVarBY - 1) / kVarBY) * s.step * s.step;
-        rt_denoise_var_step_kernel<<<(unsigned)grid, block, 0, st>>>(s);
+        s.tiles = AtrousTiles(a.width, a.height, s.step, kVarBX, kVarBY);
+        rt_denoise_var_step_kernel<<<(unsigned)s.tiles.ctas(), block, 0, st>>>(s);   // <= width * height CTAs
         e = cudaGetLastError();
     }
     return e;

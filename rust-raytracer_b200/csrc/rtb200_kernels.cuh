@@ -172,6 +172,27 @@ struct DenoiseVarArgs {
     float* out_linear; uint8_t* out_rgb8; float* out_variance;                             // [npix][3]; each may be null, not all
 };
 
+// The 1-D grid of one à-trous step of both filters (rt_denoise_step_kernel, rt_denoise_var_step_kernel; DESIGN.md §4.15). Step h
+// splits a width x height image into the residue classes (rx, ry) = (x mod h, y mod h), each a dense sub-grid of at most
+// ceil(W/h) x ceil(H/h) pixels cut into bx x by tiles. Only the classes that hold a pixel are launched, rx < min(h, W) and
+// ry < min(h, H), so the grid is at most W * H CTAs and stays under gridDim.x's 2^31 - 1 for every image the filters accept.
+// CTA b is tile x fastest, then tile y, then rx, then ry; when h <= min(W, H) that is the grid of all h * h classes. The host
+// computes it once per step and passes it to the kernel, which only decodes.
+struct AtrousTiles {
+    uint32_t tiles_x, tiles_y, res_x, res_y;
+    AtrousTiles() = default;
+    AtrousTiles(uint32_t width, uint32_t height, uint32_t h, uint32_t bx, uint32_t by)
+        : tiles_x(((width + h - 1) / h + bx - 1) / bx), tiles_y(((height + h - 1) / h + by - 1) / by),
+          res_x(h < width ? h : width), res_y(h < height ? h : height) {}
+    uint64_t ctas() const { return (uint64_t)tiles_x * tiles_y * res_x * res_y; }
+    // CTA b's tile (tix, tiy) and residue class (rx, ry)
+    __device__ void decode(uint32_t b, uint32_t& tix, uint32_t& tiy, uint32_t& rx, uint32_t& ry) const {
+        tix = b % tiles_x; b /= tiles_x;
+        tiy = b % tiles_y; b /= tiles_y;
+        rx = b % res_x; ry = b / res_x;
+    }
+};
+
 // The temporal accumulation (rtb200_temporal.cu, DESIGN.md §4.16) of a width x height frame: the caller's buffers.
 struct TemporalArgs {
     uint32_t width, height, max_history, n_motion;

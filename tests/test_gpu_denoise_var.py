@@ -1,6 +1,6 @@
 """The variance-guided denoise on the GPU (rtb200.denoise_var, rtb200_denoise_var[_device], DESIGN.md §4.18), held bit for bit to
 the numpy restatement in tests/denoise_var_restatement.py: edge values on tiny and odd images at L = 1 .. 10, random images
-larger than one tile grid at every iteration count, 800x600 frames, an oracle render with its variance and AOV guides; RGB8
+larger than one tile grid at every iteration count, 800x600 and 1920x1080 frames, an oracle render with its variance and AOV guides; RGB8
 against rtb200_probe_quantise; both forms; the stats of the host form; overlapping calls on two streams; refusals that enqueue
 nothing."""
 import ctypes as C
@@ -85,6 +85,17 @@ def test_800x600(iterations):
     assert st["kernel_launches"] == 2 * iterations + 1
     assert st["h2d_bytes"] == 4 * 800 * 600 * 12 and st["d2h_bytes"] == 800 * 600 * 27
     assert st["trace_ms"] > 0 and st["device_ms"] >= st["trace_ms"] and st["wall_ms"] > 0
+
+
+@pytest.mark.parametrize("iterations", [1, 3, 10])
+def test_full_hd(iterations):
+    color, var, albedo, normal = _random_case(1080, 1920, 200 + iterations)
+    h = both_forms(color, var, albedo, normal, f"1920x1080/L={iterations}", iterations=iterations,
+                   color_weight=R.DENOISE_VAR_COLOR_WEIGHT, albedo_weight=R.DENOISE_VAR_ALBEDO_WEIGHT,
+                   normal_weight=R.DENOISE_VAR_NORMAL_WEIGHT, variance_floor=R.DENOISE_VAR_VARIANCE_FLOOR)
+    st = h["stats"]
+    assert st["kernel_launches"] == 2 * iterations + 1
+    assert st["h2d_bytes"] == 4 * 1920 * 1080 * 12 and st["d2h_bytes"] == 1920 * 1080 * 27
 
 
 def test_the_oracle_cover_render_with_its_variance_and_guides():

@@ -152,12 +152,12 @@ def _to32(x, e, up):
     """x + e (float64 x, a TwoSum error e) rounded down (or up) to float32."""
     with np.errstate(over="ignore"):
         f = f32(x)
-    if up:
-        if float(f) < x or (float(f) == x and e > 0):
-            f = np.nextafter(f, f32(INF))
-    else:
-        if float(f) > x or (float(f) == x and e < 0):
-            f = np.nextafter(f, f32(-INF))
+        if up:
+            if float(f) < x or (float(f) == x and e > 0):
+                f = np.nextafter(f, f32(INF))
+        else:
+            if float(f) > x or (float(f) == x and e < 0):
+                f = np.nextafter(f, f32(-INF))
     return f32(f)
 
 
@@ -181,6 +181,36 @@ def sqrt32(a, up=False):
     elif float(f) * float(f) > float(a):
         f = np.nextafter(f, f32(-INF))
     return f32(f)
+
+
+def rn32(x: Fraction) -> f32:
+    """The exact value x rounded to the nearest float32, ties to even (+-inf past FLT_MAX + half an ulp)."""
+    if x == 0:
+        return f32(0.0)
+    if abs(x) >= Fraction(FMAX) + Fraction(2) ** 103:
+        return f32(INF if x > 0 else -INF)
+    with np.errstate(over="ignore"):
+        f = f32(float(x))                        # within one float32 step of the answer (float() rounds once more)
+    if not np.isfinite(f):
+        f = f32(FMAX if x > 0 else -FMAX)
+    near = [g for g in (np.nextafter(f, f32(-INF)), f, np.nextafter(f, f32(INF))) if np.isfinite(g)]
+    return f32(min(near, key=lambda g: (abs(Fraction(float(g)) - x), int(np.array(g).view(np.uint32)) & 1)))
+
+
+def fma32(a, b, c) -> f32:
+    """fmaf(a, b, c): the exact a*b + c rounded once to the nearest float32."""
+    if not (np.isfinite(a) and np.isfinite(b) and np.isfinite(c)):
+        with np.errstate(over="ignore", invalid="ignore"):
+            return f32(float(a) * float(b) + float(c))
+    return rn32(Fraction(float(a)) * Fraction(float(b)) + Fraction(float(c)))
+
+
+def oo32(pf) -> f32:
+    """The kernel's |pf|^2: fmaf(ofx, ofx, fmaf(ofy, ofy, ofz * ofz)), one rounding per FMA (a float64 sum rounded to float32
+    rounds twice and can land on the other side of a float32 midpoint)."""
+    with np.errstate(over="ignore"):
+        zz = f32(pf[2]) * f32(pf[2])
+    return fma32(pf[0], pf[0], fma32(pf[1], pf[1], zz))
 
 
 def d_up(x: float) -> f32:
@@ -221,9 +251,10 @@ def _subtrees(b):
     return under
 
 
-def emulate(b, c, r, p, bound, any_, stop=True, under=None, d_all=None):
+def emulate(b, c, r, p, bound, any_, stop=True, under=None, d_all=None, info=None):
     """The kernel of one point in emulated float32 and exact float64. Returns (sphere or -1, distance, evaluated spheres, leaves
-    visited). With `under` and `d_all` it also asserts L~ <= dist_j for every sphere under every child it bounds."""
+    visited). With `under` and `d_all` it also asserts L~ <= dist_j for every sphere under every child it bounds; a dict
+    `info` receives "stack", the most entries the traversal stack held, and "tree", whether the point walked the tree."""
     g = b["recentre"]
     best, bj = bound, -1
     evald, leaves = [], 0
@@ -241,8 +272,10 @@ def emulate(b, c, r, p, bound, any_, stop=True, under=None, d_all=None):
     if not bound > -INF:
         return bj, INF, evald, leaves
     pf = np.array([f32(p[a] - g[a]) for a in range(3)])
-    oo = f32(float(pf[0]) * float(pf[0]) + float(f32(float(pf[1]) * float(pf[1]) + float(f32(float(pf[2]) * float(pf[2]))))))
-    if not oo < 1e30:
+    tree = bool(oo32(pf) < f32(1e30))
+    if info is not None:
+        info["stack"], info["tree"] = 0, tree
+    if not tree:
         for j in range(len(r)):
             ev(j)
             if any_ and stop and bj >= 0:
@@ -283,6 +316,9 @@ def emulate(b, c, r, p, bound, any_, stop=True, under=None, d_all=None):
                 kept.append((lv, k, child))
         kept.sort(key=lambda t: (t[0], t[1]), reverse=True)   # the nearest child on top
         stack.extend((child, lv) for lv, _, child in kept)
+        assert len(stack) <= 7 * KMAX_DEPTH + 1
+        if info is not None:
+            info["stack"] = max(info["stack"], len(stack))
     return bj, (best if bj >= 0 else INF), evald, leaves
 
 
@@ -389,6 +425,21 @@ def test_the_directed_roundings_are_exact():
         if np.isfinite(f) and f > -FMAX:
             assert Fraction(float(np.nextafter(f, f32(-INF)))) < Fraction(x)
     assert d_up(INF) == INF and d_up(float(np.finfo(np.float64).max)) == INF and d_up(-INF) == -INF
+
+
+def test_oo_rounds_once_per_fma():
+    """oo32 is the kernel's fmaf chain: on random points it is the exact sum of squares rounded once per FMA, and at a float32
+    midpoint it differs from a float64 sum rounded to float32. pf_y^2 = 2^2k (1 + 2^-11 + 2^-24) lies exactly half way between
+    two float32 values; pf_z^2 = 2^(2k-80) lifts it above, which the float64 sum loses before its rounding to float32."""
+    rng = np.random.default_rng(9)
+    for pf in (rng.normal(size=(300, 3)) * 10.0 ** rng.uniform(-20, 18, size=(300, 3))).astype(f32):
+        zz = pf[2] * pf[2]
+        inner = rn32(Fraction(float(pf[1])) ** 2 + Fraction(float(zz)))
+        assert oo32(pf) == rn32(Fraction(float(pf[0])) ** 2 + Fraction(float(inner)))
+    for k in (0, 49):                                      # 2^49 (1 + 2^-12) is about 5.6e14: |pf|^2 near 1e30
+        pf = np.array([0.0, 2.0 ** k * (1 + 2.0 ** -12), 2.0 ** (k - 40)], f32)
+        twice = f32(float(pf[1]) * float(pf[1]) + float(f32(float(pf[2]) * float(pf[2]))))
+        assert float(oo32(pf)) == 4.0 ** k * (1 + 2.0 ** -11 + 2.0 ** -23) and float(twice) == 4.0 ** k * (1 + 2.0 ** -11)
 
 
 def test_lower_bound_is_a_lower_bound_of_the_box_distance():

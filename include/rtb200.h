@@ -662,7 +662,7 @@ int rtb200_denoise_var(int32_t device, const rt_denoise_var_params* p, const flo
                        const float* albedo, const float* normal, float* out_linear, uint8_t* out_rgb8, float* out_variance,
                        rt_stats* stats);
 
-/* ---- temporal accumulation of animation frames (DESIGN.md §4.16) ----------------------------------------------------------
+/* ---- temporal accumulation of animation frames (DESIGN.md §4.16; the history clamp below, §4.20) --------------------------
  * Blends each pixel of a frame with the history of the previous frame where its first hit was, the reprojection and blend of
  * SVGF's first stage. Every f64 and f32 operation is rounded to nearest and never contracted; sums and products run in the
  * order written. Whole frames only (width x height pixels, row-major, top row first): a shard's compact rows are not image
@@ -720,6 +720,35 @@ int rtb200_temporal_device(int32_t device, const rt_temporal_params* p, const rt
  * kernel_launches (1). Same checks, bar the alignment and the memory kind. */
 int rtb200_temporal(int32_t device, const rt_temporal_params* p, const rt_temporal_frame* cur, const rt_temporal_history* prev,
                     const double* motion, const rt_temporal_out* out, rt_stats* stats);
+
+/* ---- the history clamp of the temporal accumulation (DESIGN.md §4.20) -----------------------------------------------------
+ * rtb200_temporal with one more step between step 6's h and the blend; steps 1-5, the tap rules, L, n and every no-history case
+ * are unchanged. Where n >= 2, for pixel p, window radius r and clamp width gamma:
+ *  7. the window is q = p + (dx, dy), dy = -r..r (outer), dx = -r..r (inner); the q inside the image whose colour color[q] is
+ *     finite in all three channels are kept, m of them (p itself always is: m >= 1). Per channel k, in f32 from 0.0f and in
+ *     window order: S_k += c_q,k and Q_k += c_q,k * c_q,k (the product rounded before the add). mean = S_k / f32(m),
+ *     var = Q_k / f32(m) - mean * mean, sd = sqrt(var < 0 ? 0 : var) (a NaN var stays NaN), lo = mean - gamma * sd,
+ *     hi = mean + gamma * sd, and h'_k = h_k < lo ? lo : (h_k > hi ? hi : h_k), so a NaN lo, hi or h_k leaves h_k as it is.
+ *     The output is h'_k + (1.0f / f32(n)) * (c_k - h'_k) with length n: the clamp does not shorten the history.
+ * Every operation is rounded to nearest and never contracted. The clamp rejects a history whose colour the current frame's
+ * neighbourhood does not show, such as a reflection that moved across the surface the reprojection follows. */
+typedef struct {
+    float    gamma;               /* finite, >= 0: the clamp's width in standard deviations (0: the window mean) */
+    uint32_t radius;              /* r in [1, 3]: a (2r + 1) x (2r + 1) window */
+    uint32_t reserved[2];         /* must be 0 */
+} rt_temporal_clamp;              /* 16 bytes */
+/* Defaults of the Python binding and the CLI's clamp (DESIGN.md §4.20: chosen on 16 frames of C2 at 4 spp and of C2 with its metal
+ * and glass Lambertian, under a one-degree orbit and a still camera, against 1024-spp frames; at N = 2 they beat the denoise
+ * alone on C2's orbit, where the unclamped accumulation loses to it) */
+#define RTB200_TEMPORAL_DEFAULT_CLAMP_GAMMA  0.5f
+#define RTB200_TEMPORAL_DEFAULT_CLAMP_RADIUS 1
+/* rtb200_temporal_device with the history clamp: the same buffers, stream order and checks, and RT_ERR_INVALID, before any
+ * device work, for a NULL clamp, a gamma that is NaN, negative or infinite, a radius outside [1, 3] or a nonzero reserved. */
+int rtb200_temporal_clamped_device(int32_t device, const rt_temporal_params* p, const rt_temporal_clamp* clamp, const rt_temporal_frame* cur,
+                                   const rt_temporal_history* prev, const double* motion, const rt_temporal_out* out, void* stream);
+/* rtb200_temporal with the history clamp: host buffers, blocking, the same stats and checks, and the clamp's checks above. */
+int rtb200_temporal_clamped(int32_t device, const rt_temporal_params* p, const rt_temporal_clamp* clamp, const rt_temporal_frame* cur,
+                            const rt_temporal_history* prev, const double* motion, const rt_temporal_out* out, rt_stats* stats);
 
 /* load_texture_image — materials.rs:213-219, config.rs:36-47: decode a baseline JPEG file to RGB8 (host-side scene staging
  * helper for hosts without their own decoder; the reference uses the jpeg-decoder crate). *out_rgb8 is released with rtb200_free(). */

@@ -1,4 +1,5 @@
-// rtb200_api_temporal.cu — the temporal accumulation of animation frames through the C ABI (DESIGN.md §4.16), in both forms:
+// rtb200_api_temporal.cu — the temporal accumulation of animation frames through the C ABI (DESIGN.md §4.16), unclamped and
+// with the history clamp (§4.20), in both forms:
 // device buffers on the caller's stream, or host buffers staged through the context's query block (HostStage). The kernel is
 // in rtb200_temporal.cu.
 
@@ -41,6 +42,15 @@ int check_temporal(const rt_temporal_params* p, const rt_temporal_frame* cur, co
     return RT_OK;
 }
 
+// The clamp's checks (after check_temporal's, before any device work).
+int check_clamp(const rt_temporal_clamp* c) {
+    if (!c) return fail(RT_ERR_INVALID, "clamp is null");
+    if (!(std::isfinite(c->gamma) && c->gamma >= 0.0f)) return fail(RT_ERR_INVALID, "rt_temporal_clamp.gamma must be finite and >= 0");
+    if (c->radius < 1 || c->radius > 3) return fail(RT_ERR_INVALID, "rt_temporal_clamp.radius must be in [1, 3]");
+    if (c->reserved[0] != 0 || c->reserved[1] != 0) return fail(RT_ERR_INVALID, "rt_temporal_clamp.reserved must be 0");
+    return RT_OK;
+}
+
 TemporalArgs temporal_args(const rt_temporal_params& p, const float* color, const uint32_t* sphere, const double* point, const float* h_color,
                            const uint32_t* h_length, const uint32_t* h_sphere, const double* h_point, const double* motion,
                            float* out_color, uint32_t* out_length) {
@@ -48,34 +58,27 @@ TemporalArgs temporal_args(const rt_temporal_params& p, const float* color, cons
                         h_color, h_length, h_sphere, h_point, p.n_motion ? motion : nullptr, out_color, out_length};
 }
 
-}  // namespace
-
-int rtb200_temporal_device(int32_t device, const rt_temporal_params* p, const rt_temporal_frame* cur, const rt_temporal_history* prev,
-                           const double* motion, const rt_temporal_out* out, void* stream_in) {
-  return guarded([&]() -> int {
-    int rc = check_temporal(p, cur, prev, motion, out, true);
-    if (rc != RT_OK) return rc;
+// Both device forms; clamp null: unclamped (rtb200_temporal_device), else checked by the caller.
+int temporal_device(int32_t device, const rt_temporal_params* p, const TemporalClamp* clamp, const rt_temporal_frame* cur,
+                    const rt_temporal_history* prev, const double* motion, const rt_temporal_out* out, void* stream_in) {
     if ((uint64_t)p->width * p->height == 0) return RT_OK;
     CTX_PROLOGUE(device, ctx);
     const rt_temporal_history none{};
     const rt_temporal_history& h = prev ? *prev : none;
+    int rc;
     if ((rc = check_device_ptrs(ctx->device, {{cur->color, "cur.color"}, {cur->sphere, "cur.sphere"}, {cur->point, "cur.point"},
                                               {h.color, "prev.color"}, {h.length, "prev.length"}, {h.sphere, "prev.sphere"},
                                               {h.point, "prev.point"}, {p->n_motion ? motion : nullptr, "motion"},
                                               {out->color, "out.color"}, {out->length, "out.length"}})) != RT_OK)
         return rc;
     CU(launch_temporal(temporal_args(*p, cur->color, cur->sphere, cur->point, h.color, h.length, h.sphere, h.point, motion, out->color,
-                                     out->length), call_stream(ctx, stream_in)));
+                                     out->length), clamp, call_stream(ctx, stream_in)));
     return RT_OK;
-  });
 }
 
-int rtb200_temporal(int32_t device, const rt_temporal_params* p, const rt_temporal_frame* cur, const rt_temporal_history* prev,
-                    const double* motion, const rt_temporal_out* out, rt_stats* stats) {
-  return guarded([&]() -> int {
-    if (stats) memset(stats, 0, sizeof *stats);
-    int rc = check_temporal(p, cur, prev, motion, out, false);
-    if (rc != RT_OK) return rc;
+// Both host forms, after the checks; clamp as temporal_device.
+int temporal_host(int32_t device, const rt_temporal_params* p, const TemporalClamp* clamp, const rt_temporal_frame* cur,
+                  const rt_temporal_history* prev, const double* motion, const rt_temporal_out* out, rt_stats* stats) {
     const uint64_t N = (uint64_t)p->width * p->height;
     if (N == 0) return RT_OK;
     auto wall0 = std::chrono::steady_clock::now();
@@ -88,15 +91,54 @@ int rtb200_temporal(int32_t device, const rt_temporal_params* p, const rt_tempor
     io.add_in(prev ? prev->sphere : nullptr, hb * 4); io.add_in(prev ? prev->point : nullptr, hb * 24);
     io.add_in(motion, (uint64_t)p->n_motion * 24);
     io.add_out(out->color, N * 12); io.add_out(out->length, N * 4);
-    rc = host_call(ctx, ctx->stream, io, nullptr, nullptr, wall0, stats, [&](unsigned long long*) -> int {
+    int rc = host_call(ctx, ctx->stream, io, nullptr, nullptr, wall0, stats, [&](unsigned long long*) -> int {
         auto dev = [&](int k) { return (const void*)io.a[k].dev; };
         CU(launch_temporal(temporal_args(*p, (const float*)dev(0), (const uint32_t*)dev(1), (const double*)dev(2), (const float*)dev(3),
                                          (const uint32_t*)dev(4), (const uint32_t*)dev(5), (const double*)dev(6), (const double*)dev(7),
-                                         (float*)io.a[8].dev, (uint32_t*)io.a[9].dev), ctx->stream));
+                                         (float*)io.a[8].dev, (uint32_t*)io.a[9].dev), clamp, ctx->stream));
         return RT_OK;
     });
     if (rc != RT_OK || !stats) return rc;
     stats->kernel_launches = 1;
     return RT_OK;
+}
+
+}  // namespace
+
+int rtb200_temporal_device(int32_t device, const rt_temporal_params* p, const rt_temporal_frame* cur, const rt_temporal_history* prev,
+                           const double* motion, const rt_temporal_out* out, void* stream_in) {
+  return guarded([&]() -> int {
+    const int rc = check_temporal(p, cur, prev, motion, out, true);
+    return rc != RT_OK ? rc : temporal_device(device, p, nullptr, cur, prev, motion, out, stream_in);
+  });
+}
+
+int rtb200_temporal_clamped_device(int32_t device, const rt_temporal_params* p, const rt_temporal_clamp* clamp, const rt_temporal_frame* cur,
+                                   const rt_temporal_history* prev, const double* motion, const rt_temporal_out* out, void* stream_in) {
+  return guarded([&]() -> int {
+    int rc = check_temporal(p, cur, prev, motion, out, true);
+    if (rc != RT_OK || (rc = check_clamp(clamp)) != RT_OK) return rc;
+    const TemporalClamp c{clamp->gamma, clamp->radius};
+    return temporal_device(device, p, &c, cur, prev, motion, out, stream_in);
+  });
+}
+
+int rtb200_temporal(int32_t device, const rt_temporal_params* p, const rt_temporal_frame* cur, const rt_temporal_history* prev,
+                    const double* motion, const rt_temporal_out* out, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (stats) memset(stats, 0, sizeof *stats);
+    const int rc = check_temporal(p, cur, prev, motion, out, false);
+    return rc != RT_OK ? rc : temporal_host(device, p, nullptr, cur, prev, motion, out, stats);
+  });
+}
+
+int rtb200_temporal_clamped(int32_t device, const rt_temporal_params* p, const rt_temporal_clamp* clamp, const rt_temporal_frame* cur,
+                            const rt_temporal_history* prev, const double* motion, const rt_temporal_out* out, rt_stats* stats) {
+  return guarded([&]() -> int {
+    if (stats) memset(stats, 0, sizeof *stats);
+    int rc = check_temporal(p, cur, prev, motion, out, false);
+    if (rc != RT_OK || (rc = check_clamp(clamp)) != RT_OK) return rc;
+    const TemporalClamp c{clamp->gamma, clamp->radius};
+    return temporal_host(device, p, &c, cur, prev, motion, out, stats);
   });
 }

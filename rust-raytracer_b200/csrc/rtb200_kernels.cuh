@@ -203,6 +203,8 @@ struct TemporalArgs {
     const double* motion;                                                             // [n_motion][3], null when n_motion is 0
     float* out_color; uint32_t* out_length;
 };
+// The history clamp of rtb200_temporal_clamped (DESIGN.md §4.20): gamma finite and >= 0, radius in [1, 3].
+struct TemporalClamp { float gamma; uint32_t radius; };
 
 struct ResolveParams {
     const float4* samplebuf;
@@ -369,8 +371,8 @@ cudaError_t launch_denoise(const DenoiseArgs& a, cudaStream_t st);
 // prefilter and a step per iteration)
 uint64_t denoise_var_scratch_bytes(uint64_t npix);
 cudaError_t launch_denoise_var(const DenoiseVarArgs& a, cudaStream_t st);
-// the temporal accumulation (rtb200_temporal.cu): one launch, one thread per pixel
-cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t st);
+// the temporal accumulation (rtb200_temporal.cu): one launch, one thread per pixel, with the history clamp when it is given
+cudaError_t launch_temporal(const TemporalArgs& a, const TemporalClamp* clamp, cudaStream_t st);   // clamp null: unclamped
 // geo[idx[k]] = geo_in[k], mat[idx[k]] = mat_in[k] for k < n (idx has no repeats)
 cudaError_t launch_update_scatter(const uint32_t* idx, const double4* geo_in, const DevMat* mat_in, uint32_t n, double4* geo, DevMat* mat,
                                   cudaStream_t st);

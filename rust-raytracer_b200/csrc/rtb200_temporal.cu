@@ -7,6 +7,9 @@
 //                      history colour and length, sphere and point around the reprojected position, in the contract's tap
 //                      order. Memory-bound: about 40 B of the pixel's own inputs, up to 4 x 44 B of neighbours (mostly the
 //                      pixel's own neighbourhood, so L1/L2 hits) and 16 B of output.
+// rt_temporal_clamped_kernel   the same with the history clamp of rtb200_temporal_clamped[_device] (DESIGN.md §4.20): where a
+//                      pixel keeps a history, its colour is clamped to mean +- gamma * sd of the current frame's colours in the
+//                      (2r + 1)^2 window around the pixel, read through the read-only path, before the blend.
 #include "rtb200_kernels.cuh"
 
 using namespace rtd;
@@ -37,9 +40,41 @@ RT_DEV bool project(const rt_camera& c, D3 d, double& u, double& v) {
 
 RT_DEV bool finite3(float a, float b, float c) { return isfinite(a) && isfinite(b) && isfinite(c); }
 
-}  // namespace
+// The history h_k of pixel (x, y) clamped to [mean - gamma * sd, mean + gamma * sd] of the current colours in the window of
+// radius r around the pixel, per channel; a window pixel counts when it is inside the image and its colour is finite.
+RT_DEV void clamp_history(const TemporalArgs& a, uint32_t x, uint32_t y, float gamma, uint32_t r, float& h0, float& h1, float& h2) {
+    const int64_t W = a.width, H = a.height, R = r;
+    float s0 = 0.0f, s1 = 0.0f, s2 = 0.0f, q0 = 0.0f, q1 = 0.0f, q2 = 0.0f;
+    uint32_t m = 0;
+    for (int64_t dy = -R; dy <= R; ++dy) {
+        const int64_t qy = (int64_t)y + dy;
+        if (qy < 0 || qy >= H) continue;
+        for (int64_t dx = -R; dx <= R; ++dx) {
+            const int64_t qx = (int64_t)x + dx;
+            if (qx < 0 || qx >= W) continue;
+            const uint64_t q = (uint64_t)(qy * W + qx);
+            const float c0 = __ldg(a.color + 3 * q), c1 = __ldg(a.color + 3 * q + 1), c2 = __ldg(a.color + 3 * q + 2);
+            if (!finite3(c0, c1, c2)) continue;
+            s0 = __fadd_rn(s0, c0); q0 = __fadd_rn(q0, __fmul_rn(c0, c0));
+            s1 = __fadd_rn(s1, c1); q1 = __fadd_rn(q1, __fmul_rn(c1, c1));
+            s2 = __fadd_rn(s2, c2); q2 = __fadd_rn(q2, __fmul_rn(c2, c2));
+            ++m;
+        }
+    }
+    const float fm = __uint2float_rn(m);
+    auto clamp1 = [&](float s, float q, float& h) {
+        const float mean = __fdiv_rn(s, fm);
+        const float var = __fsub_rn(__fdiv_rn(q, fm), __fmul_rn(mean, mean));
+        const float d = __fmul_rn(gamma, __fsqrt_rn(var < 0.0f ? 0.0f : var));
+        const float lo = __fsub_rn(mean, d), hi = __fadd_rn(mean, d);
+        h = h < lo ? lo : (h > hi ? hi : h);   // a NaN lo, hi or h leaves h as it is
+    };
+    clamp1(s0, q0, h0); clamp1(s1, q1, h1); clamp1(s2, q2, h2);
+}
 
-__global__ void __launch_bounds__(kTemporalBlock) rt_temporal_kernel(const TemporalArgs a) {
+// One pixel of either kernel; CLAMP adds clamp_history between the gathered history and the blend, and nothing else.
+template <bool CLAMP>
+__device__ __forceinline__ void temporal_pixel(const TemporalArgs& a, float gamma, uint32_t radius) {
     const uint64_t W = a.width, H = a.height;
     const uint64_t p = (uint64_t)blockIdx.x * kTemporalBlock + threadIdx.x;
     if (p >= W * H) return;
@@ -98,7 +133,8 @@ __global__ void __launch_bounds__(kTemporalBlock) rt_temporal_kernel(const Tempo
                 if (s != 0.0f) {
                     const uint32_t n = min(L, a.max_history - 1) + 1;
                     if (n >= 2) {
-                        const float g0 = __fdiv_rn(n0, s), g1 = __fdiv_rn(n1, s), g2 = __fdiv_rn(n2, s);
+                        float g0 = __fdiv_rn(n0, s), g1 = __fdiv_rn(n1, s), g2 = __fdiv_rn(n2, s);
+                        if constexpr (CLAMP) clamp_history(a, x, y, gamma, radius, g0, g1, g2);
                         const float alpha = __fdiv_rn(1.0f, __uint2float_rn(n));
                         o0 = __fadd_rn(g0, __fmul_rn(alpha, __fsub_rn(c0, g0)));
                         o1 = __fadd_rn(g1, __fmul_rn(alpha, __fsub_rn(c1, g1)));
@@ -113,9 +149,21 @@ __global__ void __launch_bounds__(kTemporalBlock) rt_temporal_kernel(const Tempo
     a.out_length[p] = len;
 }
 
-cudaError_t launch_temporal(const TemporalArgs& a, cudaStream_t st) {
+}  // namespace
+
+__global__ void __launch_bounds__(kTemporalBlock) rt_temporal_kernel(const TemporalArgs a) { temporal_pixel<false>(a, 0.0f, 0); }
+
+__global__ void __launch_bounds__(kTemporalBlock) rt_temporal_clamped_kernel(const TemporalArgs a, const float gamma, const uint32_t radius) {
+    temporal_pixel<true>(a, gamma, radius);
+}
+
+cudaError_t launch_temporal(const TemporalArgs& a, const TemporalClamp* clamp, cudaStream_t st) {
     const uint64_t npix = (uint64_t)a.width * a.height;
-    rt_temporal_kernel<<<(unsigned)((npix + kTemporalBlock - 1) / kTemporalBlock), kTemporalBlock, 0, st>>>(a);
+    const unsigned grid = (unsigned)((npix + kTemporalBlock - 1) / kTemporalBlock);
+    if (clamp)
+        rt_temporal_clamped_kernel<<<grid, kTemporalBlock, 0, st>>>(a, clamp->gamma, clamp->radius);
+    else
+        rt_temporal_kernel<<<grid, kTemporalBlock, 0, st>>>(a);
     return cudaGetLastError();
 }
 

@@ -18,13 +18,16 @@
 // linear image denoised (rtb200_denoise, DESIGN.md §4.15; omitted weights are the header's RTB200_DENOISE_DEFAULT_*) with the
 // albedo and normal of the frame's own samples (samples_per_pixel samples from sample 0) as guides. The frame is rendered once,
 // in linear f32, and out.png is its quantisation; the AOV pass uploads the scene once more.
-// RTB200_TEMPORAL=<max_history>[,<iterations>[,<color_weight>[,<albedo_weight>[,<normal_weight>]]]], with RTB200_FRAMES only,
+// RTB200_TEMPORAL=<max_history>[,<iterations>[,<color_weight>[,<albedo_weight>[,<normal_weight>[,<clamp_gamma>]]]]], with
+// RTB200_FRAMES only,
 // also writes <prefix>_{i:03}_denoised.png per frame: the AOV pass of the frame's own samples (samples_per_pixel samples from
 // sample 0, the frame's camera and seed), the temporal accumulation of its linear image over the frames before it
 // (rtb200_temporal, DESIGN.md §4.16, without sphere motion: the frames move only the camera; depth_tol is the header's default),
 // then the denoise with the frame's albedo and normal (iterations 0: the accumulated image alone; omitted values are the
 // header's RTB200_DENOISE_DEFAULT_*). The frames are rendered once, in linear f32, and <prefix>_{i:03}.png is each one's
-// quantisation, byte for byte the run's without the variable. Accumulation averages noise only across frames whose seeds
+// quantisation, byte for byte the run's without the variable. With <clamp_gamma> the accumulation clamps each history to the
+// frame's neighbourhood (rtb200_temporal_clamped, DESIGN.md §4.20, at the header's default radius); without it, the
+// accumulation is rtb200_temporal's. Accumulation averages noise only across frames whose seeds
 // differ: a frames file that omits "seed" renders every frame with the scene's seed, and the same noise accumulates.
 // A camera (of the config or of a frame) may carry "aperture" and "focus_dist": the thin lens of DESIGN.md §4.17 (absent or 0
 // aperture: the reference's pinhole camera; absent focus_dist: |look_from - look_at|, or the scene's for a frame). Plain renders
@@ -51,23 +54,28 @@
 
 // RTB200_FRAMES: every frame of frames_path over `s`, written to <prefix>_000.png, <prefix>_001.png, ...
 static int write_temporal(const rt_scene& s, const std::vector<rt_frame>& frames, const rt_options& opts, const float* linear,
-                          const std::vector<std::string>& files, uint32_t max_history, const rt_denoise_params& dp);
+                          const std::vector<std::string>& files, uint32_t max_history, const rt_denoise_params& dp,
+                          const rt_temporal_clamp* clamp);
 
-// RTB200_TEMPORAL: the parameters of `spec` (101 and a message when it is malformed)
-static int parse_temporal(const rt_scene& s, const char* spec, uint32_t* max_history, rt_denoise_params* p) {
-    double v[5] = {0.0, RTB200_DENOISE_DEFAULT_ITERATIONS, RTB200_DENOISE_DEFAULT_COLOR_WEIGHT, RTB200_DENOISE_DEFAULT_ALBEDO_WEIGHT,
-                   RTB200_DENOISE_DEFAULT_NORMAL_WEIGHT};
+// RTB200_TEMPORAL: the parameters of `spec` (101 and a message when it is malformed); *has_clamp tells whether it gives the clamp
+static int parse_temporal(const rt_scene& s, const char* spec, uint32_t* max_history, rt_denoise_params* p, rt_temporal_clamp* clamp,
+                          bool* has_clamp) {
+    double v[6] = {0.0, RTB200_DENOISE_DEFAULT_ITERATIONS, RTB200_DENOISE_DEFAULT_COLOR_WEIGHT, RTB200_DENOISE_DEFAULT_ALBEDO_WEIGHT,
+                   RTB200_DENOISE_DEFAULT_NORMAL_WEIGHT, 0.0};
     int k = 0;
-    for (const char* c = spec; k < 5; ++k) {
+    for (const char* c = spec; k < 6; ++k) {
         char* end = nullptr;
         v[k] = strtod(c, &end);
-        if (end == c || (*end != ',' && *end != 0)) {
-            fprintf(stderr, "RTB200_TEMPORAL: expected <max_history>[,<iterations>[,<color_weight>[,<albedo_weight>[,<normal_weight>]]]], got \"%s\"\n", spec);
+        if (end == c || (*end != ',' && *end != 0) || (k == 5 && *end != 0)) {
+            fprintf(stderr, "RTB200_TEMPORAL: expected <max_history>[,<iterations>[,<color_weight>[,<albedo_weight>[,<normal_weight>[,<clamp_gamma>]]]]], got \"%s\"\n", spec);
             return 101;
         }
         if (*end == 0) break;
         c = end + 1;
     }
+    *has_clamp = k == 5;
+    if (*has_clamp && !(std::isfinite((float)v[5]) && v[5] >= 0)) { fprintf(stderr, "RTB200_TEMPORAL: clamp_gamma must be finite and >= 0\n"); return 101; }
+    *clamp = rt_temporal_clamp{(float)v[5], RTB200_TEMPORAL_DEFAULT_CLAMP_RADIUS, {0u, 0u}};
     if (!(v[0] >= 1 && v[0] <= 4294967295.0 && v[0] == std::floor(v[0]))) { fprintf(stderr, "RTB200_TEMPORAL: max_history must be an integer >= 1\n"); return 101; }
     if (!(v[1] >= 0 && v[1] <= 10 && v[1] == std::floor(v[1]))) { fprintf(stderr, "RTB200_TEMPORAL: iterations must be an integer in [0, 10]\n"); return 101; }
     if ((uint64_t)s.width * s.height >= (1ull << 31)) { fprintf(stderr, "RTB200_TEMPORAL: the frame must have fewer than 2^31 pixels\n"); return 101; }
@@ -114,7 +122,9 @@ static int render_animation(const rthost::SceneHolder& holder, const char* frame
     fflush(stdout);
     uint32_t max_history = 0;
     rt_denoise_params dp{};
-    if (temporal && parse_temporal(s, temporal, &max_history, &dp) != 0) return 101;
+    rt_temporal_clamp clamp{};
+    bool has_clamp = false;
+    if (temporal && parse_temporal(s, temporal, &max_history, &dp, &clamp, &has_clamp) != 0) return 101;
     const size_t frame_bytes = (size_t)s.width * s.height * 3;
     std::vector<uint8_t> pixels(frame_bytes * frames.size());
     std::vector<float> linear(temporal ? frame_bytes * frames.size() : 0);
@@ -139,13 +149,14 @@ static int render_animation(const rthost::SceneHolder& holder, const char* frame
         std::string err;
         if (!rthost::write_png_rgb8(files[i].c_str(), pixels.data() + i * frame_bytes, s.width, s.height, &err)) { fprintf(stderr, "error writing image: %s\n", err.c_str()); return 101; }
     }
-    return temporal ? write_temporal(s, frames, opts, linear.data(), files, max_history, dp) : 0;
+    return temporal ? write_temporal(s, frames, opts, linear.data(), files, max_history, dp, has_clamp ? &clamp : nullptr) : 0;
 }
 
-// RTB200_TEMPORAL: frame i's AOVs, its accumulation over frames 0 .. i (the history ping-pongs between two buffers) and its
-// denoise, written to <prefix>_{i:03}_denoised.png
+// RTB200_TEMPORAL: frame i's AOVs, its accumulation over frames 0 .. i (the history ping-pongs between two buffers; clamped
+// when clamp is given) and its denoise, written to <prefix>_{i:03}_denoised.png
 static int write_temporal(const rt_scene& s, const std::vector<rt_frame>& frames, const rt_options& opts, const float* linear,
-                          const std::vector<std::string>& files, uint32_t max_history, const rt_denoise_params& dp) {
+                          const std::vector<std::string>& files, uint32_t max_history, const rt_denoise_params& dp,
+                          const rt_temporal_clamp* clamp) {
     const size_t npix = (size_t)s.width * s.height;
     std::vector<float> albedo(npix * 3), normal(npix * 3), color[2] = {std::vector<float>(npix * 3), std::vector<float>(npix * 3)};
     std::vector<uint32_t> sphere[2] = {std::vector<uint32_t>(npix), std::vector<uint32_t>(npix)}, length[2] = {std::vector<uint32_t>(npix), std::vector<uint32_t>(npix)};
@@ -165,7 +176,9 @@ static int write_temporal(const rt_scene& s, const std::vector<rt_frame>& frames
         const rt_temporal_frame cur{linear + i * npix * 3, sphere[k].data(), point[k].data()};
         const rt_temporal_history prev{color[k ^ 1].data(), length[k ^ 1].data(), sphere[k ^ 1].data(), point[k ^ 1].data()};
         const rt_temporal_out out{color[k].data(), length[k].data()};
-        if ((rc = rtb200_temporal(opts.device, &tp, &cur, i > 0 ? &prev : nullptr, nullptr, &out, nullptr)) != 0) break;
+        rc = clamp ? rtb200_temporal_clamped(opts.device, &tp, clamp, &cur, i > 0 ? &prev : nullptr, nullptr, &out, nullptr)
+                   : rtb200_temporal(opts.device, &tp, &cur, i > 0 ? &prev : nullptr, nullptr, &out, nullptr);
+        if (rc != 0) break;
         rc = dp.iterations ? rtb200_denoise(opts.device, &dp, color[k].data(), albedo.data(), normal.data(), nullptr, rgb8.data(), nullptr)
                            : rtb200_probe_quantise(color[k].data(), (uint32_t)(npix * 3), rgb8.data());
         if (rc != 0) break;

@@ -190,6 +190,12 @@ class rt_temporal_out(C.Structure):
     _fields_ = [("color", C.c_void_p), ("length", C.c_void_p)]
 
 
+class rt_temporal_clamp(C.Structure):
+    """The history clamp of rtb200_temporal_clamped[_device]: the finite, non-negative width gamma in standard deviations and
+    the window radius in [1, 3]."""
+    _fields_ = [("gamma", C.c_float), ("radius", C.c_uint32), ("reserved", C.c_uint32 * 2)]
+
+
 HIT_FIELDS = (("t", 1, np.float64), ("sphere", 1, np.int32), ("point", 3, np.float64), ("normal", 3, np.float64),
               ("uv", 2, np.float64), ("front_face", 1, np.uint8))   # rt_hits: name, values per ray, dtype (sphere -1 = 0xffffffff)
 
@@ -198,7 +204,7 @@ assert C.sizeof(rt_rays) == 24 and C.sizeof(rt_hits) == 48 and C.sizeof(rt_trace
 assert C.sizeof(rt_aov_params) == 16 and C.sizeof(rt_aov_out) == 40 and C.sizeof(rt_denoise_params) == 32
 assert C.sizeof(rt_temporal_params) == 224 and C.sizeof(rt_temporal_frame) == 24 and C.sizeof(rt_temporal_history) == 32
 assert C.sizeof(rt_temporal_out) == 16 and C.sizeof(rt_lens) == 64 and C.sizeof(rt_denoise_var_params) == 32
-assert C.sizeof(rt_points) == 16 and C.sizeof(rt_nearest) == 16
+assert C.sizeof(rt_points) == 16 and C.sizeof(rt_nearest) == 16 and C.sizeof(rt_temporal_clamp) == 16
 AOV_FIELDS = (("albedo", 3, np.float32), ("normal", 3, np.float32), ("hits", 1, np.uint32), ("sphere", 1, np.int32),
               ("point", 3, np.float64))   # rt_aov_out: name, values per pixel, dtype (sphere -1 = 0xffffffff)
 
@@ -226,6 +232,7 @@ ABI_SYMBOLS = [
     "rtb200_denoise_var_scratch_bytes", "rtb200_denoise_var_device", "rtb200_denoise_var",
     "rtb200_render_frames_var_device", "rtb200_render_frames_var", "rtb200_adaptive_resolve_var", "rtb200_render_adaptive_var",
     "rtb200_scene_nearest_device", "rtb200_scene_nearest", "rtb200_scene_overlaps_device", "rtb200_scene_overlaps",
+    "rtb200_temporal_clamped_device", "rtb200_temporal_clamped",
 ]
 
 _lib = None
@@ -320,6 +327,11 @@ def lib() -> C.CDLL:
                                          C.POINTER(rt_temporal_history), C.c_void_p, C.POINTER(rt_temporal_out), C.c_void_p]
     L.rtb200_temporal.argtypes = [C.c_int32, C.POINTER(rt_temporal_params), C.POINTER(rt_temporal_frame), C.POINTER(rt_temporal_history),
                                   C.c_void_p, C.POINTER(rt_temporal_out), C.POINTER(rt_stats)]
+    L.rtb200_temporal_clamped_device.argtypes = [C.c_int32, C.POINTER(rt_temporal_params), C.POINTER(rt_temporal_clamp),
+                                                 C.POINTER(rt_temporal_frame), C.POINTER(rt_temporal_history), C.c_void_p,
+                                                 C.POINTER(rt_temporal_out), C.c_void_p]
+    L.rtb200_temporal_clamped.argtypes = [C.c_int32, C.POINTER(rt_temporal_params), C.POINTER(rt_temporal_clamp), C.POINTER(rt_temporal_frame),
+                                          C.POINTER(rt_temporal_history), C.c_void_p, C.POINTER(rt_temporal_out), C.POINTER(rt_stats)]
     L.rtb200_camera_from_params_lens.argtypes = [C.POINTER(rt_camera_params), C.c_double, C.c_double, C.POINTER(rt_camera), C.POINTER(rt_lens)]
     L.rtb200_scene_set_lens.argtypes = [C.c_void_p, C.POINTER(rt_lens)]
     L.rtb200_render_frames_lens.argtypes = [C.POINTER(rt_scene), C.POINTER(rt_options), C.POINTER(rt_frame), C.POINTER(rt_lens), C.c_uint32,
@@ -1338,6 +1350,8 @@ def denoise_var(color, variance, albedo=None, normal=None, *, iterations: int = 
 # the temporal accumulation's defaults, include/rtb200.h's RTB200_TEMPORAL_DEFAULT_* (DESIGN.md §4.16: chosen on an orbit of the
 # oracle's 2-spp cover render at 64x48)
 TEMPORAL_MAX_HISTORY, TEMPORAL_DEPTH_TOL = 2, 0.03
+# the history clamp's, RTB200_TEMPORAL_DEFAULT_CLAMP_* (DESIGN.md §4.20): `clamp=TEMPORAL_CLAMP_GAMMA` turns it on
+TEMPORAL_CLAMP_GAMMA, TEMPORAL_CLAMP_RADIUS = 0.5, 1
 
 
 def _camera_of(c) -> rt_camera:
@@ -1349,20 +1363,23 @@ def _camera_of(c) -> rt_camera:
 
 
 def temporal(color, sphere, point, camera, prev: Optional[dict] = None, *, motion=None, max_history: int = TEMPORAL_MAX_HISTORY,
-             depth_tol: float = TEMPORAL_DEPTH_TOL, stream=None) -> dict:
+             depth_tol: float = TEMPORAL_DEPTH_TOL, clamp: Optional[float] = None, clamp_radius: int = TEMPORAL_CLAMP_RADIUS,
+             stream=None) -> dict:
     """Accumulate a frame over time (include/rtb200.h, rtb200_temporal[_device]): each pixel of `color` ([h, w, 3] float32,
     normally a render's linear mean) is reprojected into the previous frame through its first hit (`sphere` [h, w] int32 or
     uint32 with -1 / 0xffffffff for a miss, `point` [h, w, 3] float64: :meth:`ResidentScene.aov`'s, of the same camera) and
     blended with the history there where it shows the same surface. `camera` is this frame's rt_camera (or rt_frame).
     `prev` is None for the first frame, else a dict of the previous call's "color" and "length" and the previous frame's
     "sphere", "point" and "camera". `motion` ([n, 3] float64, may be None) is the displacement of sphere j since the previous
-    frame; spheres j >= n did not move.
+    frame; spheres j >= n did not move. `clamp` (None: off) is the history clamp's gamma: the history is clamped to the mean
+    +- clamp standard deviations of this frame's colours in the window of radius `clamp_radius` around the pixel before the
+    blend (rtb200_temporal_clamped[_device]); :data:`TEMPORAL_CLAMP_GAMMA` is the default width.
 
     numpy arrays use the blocking host form (rtb200_temporal) and the result also holds "stats". CUDA tensors (contiguous, on one
     device) use the device form (rtb200_temporal_device) on `stream` without waiting, with the stream rules of :func:`denoise`:
     the outputs are allocated by torch on the call's stream, and handle 0 is refused. Returns {"color": float32 [h, w, 3],
     "length": uint32 [h, w]}, the new history: pass it back as prev's "color" and "length" with the next frame."""
-    return _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol, stream, None)
+    return _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol, stream, None, _clamp(clamp, clamp_radius))
 
 
 def _max_history(n) -> int:
@@ -1374,8 +1391,20 @@ def _max_history(n) -> int:
     return n
 
 
-def _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol, stream, out):
-    """temporal(), writing into `out` ({"color", "length"} CUDA tensors of the right shapes) when it is given."""
+def _clamp(gamma, radius) -> Optional[rt_temporal_clamp]:
+    """The rt_temporal_clamp of a gamma (None: no clamp) and a radius; a radius outside the u32 field is refused here, the rest by
+    the library."""
+    if gamma is None:
+        return None
+    radius = int(radius)
+    if not 0 <= radius <= 0xFFFFFFFF:
+        raise ValueError(f"clamp_radius must be an integer in [1, 3], got {radius}")
+    return rt_temporal_clamp(float(gamma), radius)
+
+
+def _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol, stream, out, clamp=None):
+    """temporal(), writing into `out` ({"color", "length"} CUDA tensors of the right shapes) when it is given; clamp is an
+    rt_temporal_clamp or None."""
     shape = tuple(color.shape)
     if len(shape) != 3 or shape[2] != 3:
         raise ValueError(f"temporal: color must have shape [h, w, 3], got {shape}")
@@ -1398,8 +1427,9 @@ def _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol
     if A.host:
         out = A.empty(outs)
         st = rt_stats()
-        _check(lib().rtb200_temporal(-1, C.byref(p), C.byref(cur), hp, mp, C.byref(rt_temporal_out(A.ptr(out["color"]), A.ptr(out["length"]))),
-                                     C.byref(st)))
+        o = C.byref(rt_temporal_out(A.ptr(out["color"]), A.ptr(out["length"])))
+        _check(lib().rtb200_temporal(-1, C.byref(p), C.byref(cur), hp, mp, o, C.byref(st)) if clamp is None else
+               lib().rtb200_temporal_clamped(-1, C.byref(p), C.byref(clamp), C.byref(cur), hp, mp, o, C.byref(st)))
         out["stats"] = st.as_dict()
         return out
     stream, handle = _call_stream(stream, A.device, "temporal", "the outputs")
@@ -1407,8 +1437,9 @@ def _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol
         out = A.empty(outs, stream)
     if color.numel() == 0:   # a 0-pixel image (the library's no-op)
         return out
-    _check(lib().rtb200_temporal_device(A.device, C.byref(p), C.byref(cur), hp, mp,
-                                        C.byref(rt_temporal_out(A.ptr(out["color"]), A.ptr(out["length"]))), C.c_void_p(handle)))
+    o = C.byref(rt_temporal_out(A.ptr(out["color"]), A.ptr(out["length"])))
+    _check(lib().rtb200_temporal_device(A.device, C.byref(p), C.byref(cur), hp, mp, o, C.c_void_p(handle)) if clamp is None else
+           lib().rtb200_temporal_clamped_device(A.device, C.byref(p), C.byref(clamp), C.byref(cur), hp, mp, o, C.c_void_p(handle)))
     return out
 
 
@@ -1416,14 +1447,19 @@ class TemporalDenoiser:
     """An animation's low-sample frames made stable and clean on the GPU: each :meth:`push` accumulates the frame over time
     (:func:`temporal`) and denoises the result (:func:`denoise`, guided by the frame's albedo and normal). It owns two history
     buffers, which its pushes ping-pong between, and copies of the previous frame's sphere and point, on the device;
-    :meth:`reset` forgets the history (after an edit that renumbers spheres, or a cut)."""
+    :meth:`reset` forgets the history (after an edit that renumbers spheres, or a cut). `clamp` and `clamp_radius` are
+    :func:`temporal`'s history clamp (None: off)."""
 
     def __init__(self, *, max_history: int = TEMPORAL_MAX_HISTORY, depth_tol: float = TEMPORAL_DEPTH_TOL,
                  iterations: int = DENOISE_ITERATIONS, color_weight: float = DENOISE_COLOR_WEIGHT,
-                 albedo_weight: float = DENOISE_ALBEDO_WEIGHT, normal_weight: float = DENOISE_NORMAL_WEIGHT):
+                 albedo_weight: float = DENOISE_ALBEDO_WEIGHT, normal_weight: float = DENOISE_NORMAL_WEIGHT,
+                 clamp: Optional[float] = None, clamp_radius: int = TEMPORAL_CLAMP_RADIUS):
         self.max_history, self.depth_tol = _max_history(max_history), float(depth_tol)
         if self.max_history < 1:
             raise ValueError("max_history must be >= 1")
+        self.clamp = _clamp(clamp, clamp_radius)
+        if self.clamp is not None and not (math.isfinite(self.clamp.gamma) and self.clamp.gamma >= 0 and 1 <= self.clamp.radius <= 3):
+            raise ValueError("clamp must be finite and >= 0 as a float32, and clamp_radius in [1, 3]")
         self.denoise_kw = dict(iterations=iterations, color_weight=color_weight, albedo_weight=albedo_weight, normal_weight=normal_weight)
         self._hist = None      # two {"color", "length"} buffers; push k writes _hist[k % 2] and reads the other as the history
         self._k = 0
@@ -1458,7 +1494,7 @@ class TemporalDenoiser:
         if self._has_prev:
             h = self._hist[self._k ^ 1]
             prev = {"color": h["color"], "length": h["length"], "sphere": self._sphere, "point": self._point, "camera": self._camera}
-        _temporal(linear, aov["sphere"], aov["point"], camera, prev, motion, self.max_history, self.depth_tol, stream, out)
+        _temporal(linear, aov["sphere"], aov["point"], camera, prev, motion, self.max_history, self.depth_tol, stream, out, self.clamp)
         with torch.cuda.stream(stream):   # the next push's previous frame, after this push has read the current one
             self._sphere.view(aov["sphere"].dtype).copy_(aov["sphere"])
             self._point.copy_(aov["point"])

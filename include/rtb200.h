@@ -750,6 +750,35 @@ int rtb200_temporal_clamped_device(int32_t device, const rt_temporal_params* p, 
 int rtb200_temporal_clamped(int32_t device, const rt_temporal_params* p, const rt_temporal_clamp* clamp, const rt_temporal_frame* cur,
                             const rt_temporal_history* prev, const double* motion, const rt_temporal_out* out, rt_stats* stats);
 
+/* ---- the variance of each pixel's mean through the temporal accumulation (DESIGN.md §4.21) ---------------------------------
+ * rtb200_temporal (clamp NULL) or rtb200_temporal_clamped (clamp given) with one more output; steps 1-7, the tap rules, L, n and
+ * the clamp are unchanged and never read a variance, so out->color and out->length are those calls' outputs bit for bit. New
+ * arrays, 3 x f32 per pixel, row-major like color: variance, this frame's variance of its pixel mean (normally from
+ * rtb200_render_frames_var[_device]); prev_variance, the previous call's out_variance, given exactly when prev is; and
+ * out_variance, the new history's. Per pixel p with this frame's variance v:
+ *  8. with no history (a non-finite c, no previous frame, an invalid projection, s = 0 or n = 1) out_variance = v as given
+ *     (NaN, infinities, negative values and -0 included). For n >= 2: Vh_k = (sum of w * prev_variance_q,k over step 5's valid
+ *     taps, in tap order, from 0.0f) / s, with step 5's weights w and step 6's s (a non-finite tap variance does not make a tap
+ *     invalid: it propagates); a = 1.0f / f32(n), b = 1.0f - a, and out_variance_k = (b * b) * Vh_k + (a * a) * v_k. The clamp
+ *     moves the history's colour only, not Vh.
+ * Every f32 operation is rounded to nearest and never contracted. The blend b h + a c of a history and a frame of another seed has
+ * variance b^2 Var(h) + a^2 v; the linear weights give an upper bound on the variance of the correlated taps' resample. A static
+ * camera with a constant v gives v / k after k <= N frames and a v / (2 - a) past N. */
+/* Device buffers of `device` (-1: the current device) or managed memory, stream-ordered as rtb200_temporal_device. The checks of
+ * rtb200_temporal_device, the clamp's of rtb200_temporal_clamped_device when clamp is given, and RT_ERR_INVALID, before any
+ * device work, for a NULL variance or out_variance, a prev without prev_variance or a prev_variance without prev, a variance
+ * array that is not 4-byte aligned, an out_variance overlapping an input or another output, an out->color or out->length
+ * overlapping variance or prev_variance, or a variance pointer that is not device memory of `device` nor managed memory.
+ * A 0-pixel image is a no-op. */
+int rtb200_temporal_var_device(int32_t device, const rt_temporal_params* p, const rt_temporal_clamp* clamp, const rt_temporal_frame* cur,
+                               const float* variance, const rt_temporal_history* prev, const float* prev_variance, const double* motion,
+                               const rt_temporal_out* out, float* out_variance, void* stream);
+/* Host buffers, blocking: the same through the same kernel on the library's stream, with the inputs copied in and the outputs
+ * copied out; stats as rtb200_temporal's (kernel_launches 1). Same checks, bar the alignment and the memory kind. */
+int rtb200_temporal_var(int32_t device, const rt_temporal_params* p, const rt_temporal_clamp* clamp, const rt_temporal_frame* cur,
+                        const float* variance, const rt_temporal_history* prev, const float* prev_variance, const double* motion,
+                        const rt_temporal_out* out, float* out_variance, rt_stats* stats);
+
 /* load_texture_image — materials.rs:213-219, config.rs:36-47: decode a baseline JPEG file to RGB8 (host-side scene staging
  * helper for hosts without their own decoder; the reference uses the jpeg-decoder crate). *out_rgb8 is released with rtb200_free(). */
 int  rtb200_decode_jpeg_file(const char* path, uint8_t** out_rgb8, uint64_t* width, uint64_t* height);

@@ -281,7 +281,7 @@ int render_collect(rtb200_scene_t* h, rt_stats* stats);
 // h2d and d2h count them.
 struct HostStage {
     struct Array { const void* in; void* out; uint64_t bytes; char* dev; };
-    Array a[10];
+    Array a[13];
     int n = 0;
     uint64_t h2d = 0, d2h = 0;
     void add_in(const void* host, uint64_t bytes) { a[n++] = Array{host, nullptr, bytes, nullptr}; }

@@ -205,6 +205,9 @@ struct TemporalArgs {
 };
 // The history clamp of rtb200_temporal_clamped (DESIGN.md §4.20): gamma finite and >= 0, radius in [1, 3].
 struct TemporalClamp { float gamma; uint32_t radius; };
+// The variance planes of rtb200_temporal_var (DESIGN.md §4.21), 3 x f32 per pixel: this frame's, the history's (null without a
+// history) and the output's. A kernel parameter beside TemporalArgs, which the kernels without them keep as it is.
+struct TemporalVar { const float* var; const float* h_var; float* out_var; };
 
 struct ResolveParams {
     const float4* samplebuf;
@@ -372,7 +375,8 @@ cudaError_t launch_denoise(const DenoiseArgs& a, cudaStream_t st);
 uint64_t denoise_var_scratch_bytes(uint64_t npix);
 cudaError_t launch_denoise_var(const DenoiseVarArgs& a, cudaStream_t st);
 // the temporal accumulation (rtb200_temporal.cu): one launch, one thread per pixel, with the history clamp when it is given
-cudaError_t launch_temporal(const TemporalArgs& a, const TemporalClamp* clamp, cudaStream_t st);   // clamp null: unclamped
+cudaError_t launch_temporal(const TemporalArgs& a, const TemporalClamp* clamp, const TemporalVar* var,   // clamp null: unclamped;
+                            cudaStream_t st);                                                       // var null: no variance
 // geo[idx[k]] = geo_in[k], mat[idx[k]] = mat_in[k] for k < n (idx has no repeats)
 cudaError_t launch_update_scatter(const uint32_t* idx, const double4* geo_in, const DevMat* mat_in, uint32_t n, double4* geo, DevMat* mat,
                                   cudaStream_t st);

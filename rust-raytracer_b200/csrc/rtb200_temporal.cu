@@ -10,6 +10,10 @@
 // rt_temporal_clamped_kernel   the same with the history clamp of rtb200_temporal_clamped[_device] (DESIGN.md §4.20): where a
 //                      pixel keeps a history, its colour is clamped to mean +- gamma * sd of the current frame's colours in the
 //                      (2r + 1)^2 window around the pixel, read through the read-only path, before the blend.
+// rt_temporal_var_kernel, rt_temporal_var_clamped_kernel   either of the above that also carries the variance of each pixel's
+//                      mean through the accumulation (rtb200_temporal_var[_device], DESIGN.md §4.21): the history's variance is
+//                      gathered over the same valid taps with the same weights, and blended with the frame's as b^2 Vh + a^2 v.
+//                      Its three planes are a kernel parameter of their own (TemporalVar), so the kernels above keep theirs.
 #include "rtb200_kernels.cuh"
 
 using namespace rtd;
@@ -72,15 +76,19 @@ RT_DEV void clamp_history(const TemporalArgs& a, uint32_t x, uint32_t y, float g
     clamp1(s0, q0, h0); clamp1(s1, q1, h1); clamp1(s2, q2, h2);
 }
 
-// One pixel of either kernel; CLAMP adds clamp_history between the gathered history and the blend, and nothing else.
-template <bool CLAMP>
-__device__ __forceinline__ void temporal_pixel(const TemporalArgs& a, float gamma, uint32_t radius) {
+// One pixel of any of the kernels; CLAMP adds clamp_history between the gathered history and the blend, and VAR the variance
+// planes of vr beside the colour (a tap's variance is read only when the tap is valid); neither changes anything else.
+template <bool CLAMP, bool VAR>
+__device__ __forceinline__ void temporal_pixel(const TemporalArgs& a, float gamma, uint32_t radius, const TemporalVar& vr) {
     const uint64_t W = a.width, H = a.height;
     const uint64_t p = (uint64_t)blockIdx.x * kTemporalBlock + threadIdx.x;
     if (p >= W * H) return;
     const uint32_t x = (uint32_t)(p % W), y = (uint32_t)(p / W);
     const float c0 = a.color[3 * p], c1 = a.color[3 * p + 1], c2 = a.color[3 * p + 2];
     float o0 = c0, o1 = c1, o2 = c2;
+    float v0 = 0.0f, v1 = 0.0f, v2 = 0.0f;
+    if constexpr (VAR) { v0 = vr.var[3 * p]; v1 = vr.var[3 * p + 1]; v2 = vr.var[3 * p + 2]; }
+    float ov0 = v0, ov1 = v1, ov2 = v2;   // no history: the frame's variance as given
     uint32_t len = 1;
     if (a.h_color && finite3(c0, c1, c2)) {
         const uint32_t j = a.sphere[p];
@@ -110,6 +118,7 @@ __device__ __forceinline__ void temporal_pixel(const TemporalArgs& a, float gamm
                 const double tol2 = __dmul_rn(a.depth_tol, a.depth_tol);
                 const double lim = hit ? __dmul_rn(tol2, dot(dp, dp)) : 0.0;
                 float s = 0.0f, n0 = 0.0f, n1 = 0.0f, n2 = 0.0f;
+                float m0 = 0.0f, m1 = 0.0f, m2 = 0.0f;   // VAR: sum of w * prev_variance
                 uint32_t L = 0xffffffffu;
 #pragma unroll
                 for (int k = 0; k < 4; ++k) {
@@ -128,6 +137,11 @@ __device__ __forceinline__ void temporal_pixel(const TemporalArgs& a, float gamm
                     n0 = __fadd_rn(n0, __fmul_rn(w[k], h0));
                     n1 = __fadd_rn(n1, __fmul_rn(w[k], h1));
                     n2 = __fadd_rn(n2, __fmul_rn(w[k], h2));
+                    if constexpr (VAR) {
+                        m0 = __fadd_rn(m0, __fmul_rn(w[k], vr.h_var[3 * q]));
+                        m1 = __fadd_rn(m1, __fmul_rn(w[k], vr.h_var[3 * q + 1]));
+                        m2 = __fadd_rn(m2, __fmul_rn(w[k], vr.h_var[3 * q + 2]));
+                    }
                     L = min(L, lq);
                 }
                 if (s != 0.0f) {
@@ -139,6 +153,12 @@ __device__ __forceinline__ void temporal_pixel(const TemporalArgs& a, float gamm
                         o0 = __fadd_rn(g0, __fmul_rn(alpha, __fsub_rn(c0, g0)));
                         o1 = __fadd_rn(g1, __fmul_rn(alpha, __fsub_rn(c1, g1)));
                         o2 = __fadd_rn(g2, __fmul_rn(alpha, __fsub_rn(c2, g2)));
+                        if constexpr (VAR) {   // b^2 Vh + a^2 v: the clamp moves the colour only
+                            const float b = __fsub_rn(1.0f, alpha), bb = __fmul_rn(b, b), aa = __fmul_rn(alpha, alpha);
+                            ov0 = __fadd_rn(__fmul_rn(bb, __fdiv_rn(m0, s)), __fmul_rn(aa, v0));
+                            ov1 = __fadd_rn(__fmul_rn(bb, __fdiv_rn(m1, s)), __fmul_rn(aa, v1));
+                            ov2 = __fadd_rn(__fmul_rn(bb, __fdiv_rn(m2, s)), __fmul_rn(aa, v2));
+                        }
                         len = n;
                     }
                 }
@@ -147,20 +167,34 @@ __device__ __forceinline__ void temporal_pixel(const TemporalArgs& a, float gamm
     }
     a.out_color[3 * p] = o0; a.out_color[3 * p + 1] = o1; a.out_color[3 * p + 2] = o2;
     a.out_length[p] = len;
+    if constexpr (VAR) { vr.out_var[3 * p] = ov0; vr.out_var[3 * p + 1] = ov1; vr.out_var[3 * p + 2] = ov2; }
 }
 
 }  // namespace
 
-__global__ void __launch_bounds__(kTemporalBlock) rt_temporal_kernel(const TemporalArgs a) { temporal_pixel<false>(a, 0.0f, 0); }
+__global__ void __launch_bounds__(kTemporalBlock) rt_temporal_kernel(const TemporalArgs a) { temporal_pixel<false, false>(a, 0.0f, 0, TemporalVar{}); }
 
 __global__ void __launch_bounds__(kTemporalBlock) rt_temporal_clamped_kernel(const TemporalArgs a, const float gamma, const uint32_t radius) {
-    temporal_pixel<true>(a, gamma, radius);
+    temporal_pixel<true, false>(a, gamma, radius, TemporalVar{});
 }
 
-cudaError_t launch_temporal(const TemporalArgs& a, const TemporalClamp* clamp, cudaStream_t st) {
+__global__ void __launch_bounds__(kTemporalBlock) rt_temporal_var_kernel(const TemporalArgs a, const TemporalVar v) {
+    temporal_pixel<false, true>(a, 0.0f, 0, v);
+}
+
+__global__ void __launch_bounds__(kTemporalBlock) rt_temporal_var_clamped_kernel(const TemporalArgs a, const float gamma, const uint32_t radius,
+                                                                                 const TemporalVar v) {
+    temporal_pixel<true, true>(a, gamma, radius, v);
+}
+
+cudaError_t launch_temporal(const TemporalArgs& a, const TemporalClamp* clamp, const TemporalVar* var, cudaStream_t st) {
     const uint64_t npix = (uint64_t)a.width * a.height;
     const unsigned grid = (unsigned)((npix + kTemporalBlock - 1) / kTemporalBlock);
-    if (clamp)
+    if (var && clamp)
+        rt_temporal_var_clamped_kernel<<<grid, kTemporalBlock, 0, st>>>(a, clamp->gamma, clamp->radius, *var);
+    else if (var)
+        rt_temporal_var_kernel<<<grid, kTemporalBlock, 0, st>>>(a, *var);
+    else if (clamp)
         rt_temporal_clamped_kernel<<<grid, kTemporalBlock, 0, st>>>(a, clamp->gamma, clamp->radius);
     else
         rt_temporal_kernel<<<grid, kTemporalBlock, 0, st>>>(a);

@@ -37,6 +37,14 @@
 // the variance of its pixel means (rtb200_render_frames_var) and writes <stem>_denoised.png: the variance-guided denoise
 // (rtb200_denoise_var, DESIGN.md §4.18; omitted values are the header's RTB200_DENOISE_VAR_DEFAULT_*) with the AOVs of the
 // frame's own samples. Not with RTB200_DENOISE, RTB200_GPUS, RTB200_FRAMES, RTB200_ADAPTIVE, RTB200_TEMPORAL or a lens camera.
+// RTB200_TEMPORAL_VAR=<max_history>[,<iterations>[,<color_weight>[,<albedo_weight>[,<normal_weight>[,<variance_floor>[,<clamp_gamma>]]]]]],
+// with RTB200_FRAMES only, is RTB200_TEMPORAL with each pixel's variance carried through the accumulation and the variance-guided
+// denoise: the frames are rendered once with the variance of their pixel means (rtb200_render_frames_var), each frame is
+// accumulated with its variance (rtb200_temporal_var, DESIGN.md §4.21; clamped at the header's default radius when <clamp_gamma>
+// is given) and denoised by it (rtb200_denoise_var with the frame's albedo and normal) into <prefix>_{i:03}_denoised.png
+// (iterations 0: the accumulated image alone; omitted values are the header's RTB200_DENOISE_VAR_DEFAULT_*). <prefix>_{i:03}.png
+// is byte for byte the run's without the variable. Not with RTB200_TEMPORAL, RTB200_DENOISE, RTB200_DENOISE_VAR, RTB200_GPUS,
+// RTB200_ADAPTIVE, RTB200_AOV or a lens camera.
 #include <chrono>
 #include <cmath>
 #include <cstring>
@@ -55,7 +63,39 @@
 // RTB200_FRAMES: every frame of frames_path over `s`, written to <prefix>_000.png, <prefix>_001.png, ...
 static int write_temporal(const rt_scene& s, const std::vector<rt_frame>& frames, const rt_options& opts, const float* linear,
                           const std::vector<std::string>& files, uint32_t max_history, const rt_denoise_params& dp,
-                          const rt_temporal_clamp* clamp);
+                          const rt_temporal_clamp* clamp, const float* variance, const rt_denoise_var_params& vp);
+
+// RTB200_TEMPORAL_VAR: the parameters of `spec` (101 and a message when it is malformed or out of range); *has_clamp tells
+// whether it gives the clamp
+static int parse_temporal_var(const rt_scene& s, const char* spec, uint32_t* max_history, rt_denoise_var_params* p,
+                              rt_temporal_clamp* clamp, bool* has_clamp) {
+    double v[7] = {0.0, RTB200_DENOISE_VAR_DEFAULT_ITERATIONS, RTB200_DENOISE_VAR_DEFAULT_COLOR_WEIGHT, RTB200_DENOISE_VAR_DEFAULT_ALBEDO_WEIGHT,
+                   RTB200_DENOISE_VAR_DEFAULT_NORMAL_WEIGHT, RTB200_DENOISE_VAR_DEFAULT_VARIANCE_FLOOR, 0.0};
+    int k = 0;
+    for (const char* c = spec; k < 7; ++k) {
+        char* end = nullptr;
+        v[k] = strtod(c, &end);
+        if (end == c || (*end != ',' && *end != 0) || (k == 6 && *end != 0)) {
+            fprintf(stderr, "RTB200_TEMPORAL_VAR: expected <max_history>[,<iterations>[,<color_weight>[,<albedo_weight>[,<normal_weight>"
+                            "[,<variance_floor>[,<clamp_gamma>]]]]]], got \"%s\"\n", spec);
+            return 101;
+        }
+        if (*end == 0) break;
+        c = end + 1;
+    }
+    *has_clamp = k == 6;
+    if (!(v[0] >= 1 && v[0] <= 4294967295.0 && v[0] == std::floor(v[0]))) { fprintf(stderr, "RTB200_TEMPORAL_VAR: max_history must be an integer >= 1\n"); return 101; }
+    if (!(v[1] >= 0 && v[1] <= 10 && v[1] == std::floor(v[1]))) { fprintf(stderr, "RTB200_TEMPORAL_VAR: iterations must be an integer in [0, 10]\n"); return 101; }
+    for (int i = 2; i < 5; ++i)
+        if (!(std::isfinite((float)v[i]) && v[i] >= 0)) { fprintf(stderr, "RTB200_TEMPORAL_VAR: the weights must be finite and >= 0\n"); return 101; }
+    if (!(std::isfinite((float)v[5]) && (float)v[5] > 0.0f)) { fprintf(stderr, "RTB200_TEMPORAL_VAR: variance_floor must be finite and > 0\n"); return 101; }
+    if (*has_clamp && !(std::isfinite((float)v[6]) && v[6] >= 0)) { fprintf(stderr, "RTB200_TEMPORAL_VAR: clamp_gamma must be finite and >= 0\n"); return 101; }
+    if ((uint64_t)s.width * s.height >= (1ull << 31)) { fprintf(stderr, "RTB200_TEMPORAL_VAR: the frame must have fewer than 2^31 pixels\n"); return 101; }
+    *max_history = (uint32_t)v[0];
+    *p = rt_denoise_var_params{s.width, s.height, (uint32_t)v[1], 0u, (float)v[2], (float)v[3], (float)v[4], (float)v[5]};
+    *clamp = rt_temporal_clamp{(float)v[6], RTB200_TEMPORAL_DEFAULT_CLAMP_RADIUS, {0u, 0u}};
+    return 0;
+}
 
 // RTB200_TEMPORAL: the parameters of `spec` (101 and a message when it is malformed); *has_clamp tells whether it gives the clamp
 static int parse_temporal(const rt_scene& s, const char* spec, uint32_t* max_history, rt_denoise_params* p, rt_temporal_clamp* clamp,
@@ -95,7 +135,8 @@ static int apply_lens(const rthost::LensSpec& spec, rt_camera* cam, rt_lens* len
     return 0;
 }
 
-static int render_animation(const rthost::SceneHolder& holder, const char* frames_path, const std::string& prefix, const char* temporal) {
+static int render_animation(const rthost::SceneHolder& holder, const char* frames_path, const std::string& prefix, const char* temporal,
+                            const char* temporal_var) {
     const rt_scene& s = holder.scene;
     if (getenv("RTB200_GPUS")) { fprintf(stderr, "RTB200_FRAMES with RTB200_GPUS is not supported: animations render on one GPU\n"); return 101; }
     std::ifstream f(frames_path, std::ios::binary);
@@ -112,6 +153,7 @@ static int render_animation(const rthost::SceneHolder& holder, const char* frame
         lensed = lensed || lenses[i].radius != 0.0;
     }
     if (lensed && temporal) { fprintf(stderr, "RTB200_TEMPORAL with a lens camera (aperture > 0) is not supported\n"); return 101; }
+    if (lensed && temporal_var) { fprintf(stderr, "RTB200_TEMPORAL_VAR with a lens camera (aperture > 0) is not supported\n"); return 101; }
     std::vector<std::string> files(frames.size());
     for (size_t i = 0; i < frames.size(); ++i) {
         char num[32];
@@ -125,19 +167,23 @@ static int render_animation(const rthost::SceneHolder& holder, const char* frame
     rt_temporal_clamp clamp{};
     bool has_clamp = false;
     if (temporal && parse_temporal(s, temporal, &max_history, &dp, &clamp, &has_clamp) != 0) return 101;
+    rt_denoise_var_params vp{};
+    if (temporal_var && parse_temporal_var(s, temporal_var, &max_history, &vp, &clamp, &has_clamp) != 0) return 101;
     const size_t frame_bytes = (size_t)s.width * s.height * 3;
     std::vector<uint8_t> pixels(frame_bytes * frames.size());
-    std::vector<float> linear(temporal ? frame_bytes * frames.size() : 0);
+    std::vector<float> linear(temporal || temporal_var ? frame_bytes * frames.size() : 0), variance(temporal_var ? frame_bytes * frames.size() : 0);
     rt_options opts{};
     opts.device = getenv("RTB200_DEVICE") ? atoi(getenv("RTB200_DEVICE")) : -1; opts.rank = 0; opts.world = 1; opts.band_rows = 1;
     rt_stats st{};
     auto t0 = std::chrono::steady_clock::now();
     // the accumulation needs the linear frames: one render gives them, and each PNG is its frame's quantisation by the render's
-    // own routine (rtb200_probe_quantise), byte for byte the RGB8 render's
-    int rc = temporal ? rtb200_render_frames(&s, &opts, frames.data(), (uint32_t)frames.size(), nullptr, linear.data(), &st)
-           : lensed   ? rtb200_render_frames_lens(&s, &opts, frames.data(), lenses.data(), (uint32_t)frames.size(), pixels.data(), nullptr, &st)
-                      : rtb200_render_frames(&s, &opts, frames.data(), (uint32_t)frames.size(), pixels.data(), nullptr, &st);
-    for (size_t i = 0; rc == 0 && temporal && i < frames.size(); ++i)
+    // own routine (rtb200_probe_quantise), byte for byte the RGB8 render's; RTB200_TEMPORAL_VAR's render adds the variance
+    int rc = temporal     ? rtb200_render_frames(&s, &opts, frames.data(), (uint32_t)frames.size(), nullptr, linear.data(), &st)
+           : temporal_var ? rtb200_render_frames_var(&s, &opts, frames.data(), nullptr, (uint32_t)frames.size(), nullptr, linear.data(),
+                                                     variance.data(), &st)
+           : lensed       ? rtb200_render_frames_lens(&s, &opts, frames.data(), lenses.data(), (uint32_t)frames.size(), pixels.data(), nullptr, &st)
+                          : rtb200_render_frames(&s, &opts, frames.data(), (uint32_t)frames.size(), pixels.data(), nullptr, &st);
+    for (size_t i = 0; rc == 0 && (temporal || temporal_var) && i < frames.size(); ++i)
         rc = rtb200_probe_quantise(linear.data() + i * frame_bytes, (uint32_t)frame_bytes, pixels.data() + i * frame_bytes);
     if (rc != 0) { fprintf(stderr, "render failed (%d): %s\n", rc, rtb200_last_error()); return 101; }
     long long ms = std::chrono::duration_cast<std::chrono::milliseconds>(std::chrono::steady_clock::now() - t0).count();
@@ -149,15 +195,19 @@ static int render_animation(const rthost::SceneHolder& holder, const char* frame
         std::string err;
         if (!rthost::write_png_rgb8(files[i].c_str(), pixels.data() + i * frame_bytes, s.width, s.height, &err)) { fprintf(stderr, "error writing image: %s\n", err.c_str()); return 101; }
     }
-    return temporal ? write_temporal(s, frames, opts, linear.data(), files, max_history, dp, has_clamp ? &clamp : nullptr) : 0;
+    if (!temporal && !temporal_var) return 0;
+    return write_temporal(s, frames, opts, linear.data(), files, max_history, dp, has_clamp ? &clamp : nullptr,
+                          temporal_var ? variance.data() : nullptr, vp);
 }
 
 // RTB200_TEMPORAL: frame i's AOVs, its accumulation over frames 0 .. i (the history ping-pongs between two buffers; clamped
-// when clamp is given) and its denoise, written to <prefix>_{i:03}_denoised.png
+// when clamp is given) and its denoise, written to <prefix>_{i:03}_denoised.png. RTB200_TEMPORAL_VAR (variance given: the
+// frames' variances): the same with the variance accumulated beside the colour and the variance-guided denoise of vp.
 static int write_temporal(const rt_scene& s, const std::vector<rt_frame>& frames, const rt_options& opts, const float* linear,
                           const std::vector<std::string>& files, uint32_t max_history, const rt_denoise_params& dp,
-                          const rt_temporal_clamp* clamp) {
+                          const rt_temporal_clamp* clamp, const float* variance, const rt_denoise_var_params& vp) {
     const size_t npix = (size_t)s.width * s.height;
+    std::vector<float> acc_var[2] = {std::vector<float>(variance ? npix * 3 : 0), std::vector<float>(variance ? npix * 3 : 0)};
     std::vector<float> albedo(npix * 3), normal(npix * 3), color[2] = {std::vector<float>(npix * 3), std::vector<float>(npix * 3)};
     std::vector<uint32_t> sphere[2] = {std::vector<uint32_t>(npix), std::vector<uint32_t>(npix)}, length[2] = {std::vector<uint32_t>(npix), std::vector<uint32_t>(npix)};
     std::vector<double> point[2] = {std::vector<double>(npix * 3), std::vector<double>(npix * 3)};
@@ -176,11 +226,18 @@ static int write_temporal(const rt_scene& s, const std::vector<rt_frame>& frames
         const rt_temporal_frame cur{linear + i * npix * 3, sphere[k].data(), point[k].data()};
         const rt_temporal_history prev{color[k ^ 1].data(), length[k ^ 1].data(), sphere[k ^ 1].data(), point[k ^ 1].data()};
         const rt_temporal_out out{color[k].data(), length[k].data()};
-        rc = clamp ? rtb200_temporal_clamped(opts.device, &tp, clamp, &cur, i > 0 ? &prev : nullptr, nullptr, &out, nullptr)
-                   : rtb200_temporal(opts.device, &tp, &cur, i > 0 ? &prev : nullptr, nullptr, &out, nullptr);
+        if (variance)
+            rc = rtb200_temporal_var(opts.device, &tp, clamp, &cur, variance + i * npix * 3, i > 0 ? &prev : nullptr,
+                                     i > 0 ? acc_var[k ^ 1].data() : nullptr, nullptr, &out, acc_var[k].data(), nullptr);
+        else
+            rc = clamp ? rtb200_temporal_clamped(opts.device, &tp, clamp, &cur, i > 0 ? &prev : nullptr, nullptr, &out, nullptr)
+                       : rtb200_temporal(opts.device, &tp, &cur, i > 0 ? &prev : nullptr, nullptr, &out, nullptr);
         if (rc != 0) break;
-        rc = dp.iterations ? rtb200_denoise(opts.device, &dp, color[k].data(), albedo.data(), normal.data(), nullptr, rgb8.data(), nullptr)
-                           : rtb200_probe_quantise(color[k].data(), (uint32_t)(npix * 3), rgb8.data());
+        const uint32_t iterations = variance ? vp.iterations : dp.iterations;
+        rc = !iterations ? rtb200_probe_quantise(color[k].data(), (uint32_t)(npix * 3), rgb8.data())
+           : variance    ? rtb200_denoise_var(opts.device, &vp, color[k].data(), acc_var[k].data(), albedo.data(), normal.data(), nullptr,
+                                              rgb8.data(), nullptr, nullptr)
+                         : rtb200_denoise(opts.device, &dp, color[k].data(), albedo.data(), normal.data(), nullptr, rgb8.data(), nullptr);
         if (rc != 0) break;
         const std::string path = files[i].substr(0, files[i].size() - 4) + "_denoised.png";
         std::string err;
@@ -361,6 +418,14 @@ int main(int argc, char** argv) {
     } catch (const std::exception& e) { fprintf(stderr, "Unable to parse config json: %s\n", e.what()); return 101; }   // main.rs:15
     if (const char* sd = getenv("RTB200_SEED")) holder.scene.seed = strtoull(sd, nullptr, 0);
     const char* temporal = getenv("RTB200_TEMPORAL");
+    const char* temporal_var = getenv("RTB200_TEMPORAL_VAR");
+    if (temporal_var && (!getenv("RTB200_FRAMES") || temporal || getenv("RTB200_DENOISE") || getenv("RTB200_DENOISE_VAR") || getenv("RTB200_GPUS") ||
+                         getenv("RTB200_ADAPTIVE") || getenv("RTB200_AOV"))) {
+        fprintf(stderr, "RTB200_TEMPORAL_VAR needs RTB200_FRAMES, without RTB200_TEMPORAL, RTB200_DENOISE, RTB200_DENOISE_VAR, RTB200_GPUS, "
+                        "RTB200_ADAPTIVE or RTB200_AOV: it accumulates the frames of one animation and their variance on one GPU and "
+                        "denoises them itself\n");
+        return 101;
+    }
     if (temporal && (!getenv("RTB200_FRAMES") || getenv("RTB200_GPUS") || getenv("RTB200_ADAPTIVE") || getenv("RTB200_AOV") || getenv("RTB200_DENOISE"))) {
         fprintf(stderr, "RTB200_TEMPORAL needs RTB200_FRAMES, without RTB200_GPUS, RTB200_ADAPTIVE, RTB200_AOV or RTB200_DENOISE: it accumulates "
                         "the frames of one animation on one GPU and denoises them itself\n");
@@ -390,16 +455,16 @@ int main(int argc, char** argv) {
     rt_lens scene_lens{};
     if (apply_lens(holder.lens_spec, &holder.scene.camera, &scene_lens) != 0) return 101;
     const bool lens = scene_lens.radius != 0.0;
-    if (lens && (getenv("RTB200_GPUS") || adaptive || aov || denoise || denoise_var || temporal)) {
-        fprintf(stderr, "a lens camera (aperture > 0) with RTB200_GPUS, RTB200_ADAPTIVE, RTB200_AOV, RTB200_DENOISE, RTB200_DENOISE_VAR or RTB200_TEMPORAL is not "
-                        "supported: render it without them\n");
+    if (lens && (getenv("RTB200_GPUS") || adaptive || aov || denoise || denoise_var || temporal || temporal_var)) {
+        fprintf(stderr, "a lens camera (aperture > 0) with RTB200_GPUS, RTB200_ADAPTIVE, RTB200_AOV, RTB200_DENOISE, RTB200_DENOISE_VAR, RTB200_TEMPORAL "
+                        "or RTB200_TEMPORAL_VAR is not supported: render it without them\n");
         return 101;
     }
     rt_denoise_params denoise_p{};
     if (denoise && parse_denoise(holder.scene, denoise, &denoise_p) != 0) return 101;
     rt_denoise_var_params denoise_var_p{};
     if (denoise_var && parse_denoise_var(holder.scene, denoise_var, &denoise_var_p) != 0) return 101;
-    if (const char* fp = getenv("RTB200_FRAMES")) return render_animation(holder, fp, argv[2], temporal);
+    if (const char* fp = getenv("RTB200_FRAMES")) return render_animation(holder, fp, argv[2], temporal, temporal_var);
     printf("\nRendering %s\n", argv[2]);                                  // main.rs:18
     fflush(stdout);
     const rt_scene& s = holder.scene;

@@ -233,6 +233,7 @@ ABI_SYMBOLS = [
     "rtb200_render_frames_var_device", "rtb200_render_frames_var", "rtb200_adaptive_resolve_var", "rtb200_render_adaptive_var",
     "rtb200_scene_nearest_device", "rtb200_scene_nearest", "rtb200_scene_overlaps_device", "rtb200_scene_overlaps",
     "rtb200_temporal_clamped_device", "rtb200_temporal_clamped",
+    "rtb200_temporal_var_device", "rtb200_temporal_var",
 ]
 
 _lib = None
@@ -332,6 +333,12 @@ def lib() -> C.CDLL:
                                                  C.POINTER(rt_temporal_out), C.c_void_p]
     L.rtb200_temporal_clamped.argtypes = [C.c_int32, C.POINTER(rt_temporal_params), C.POINTER(rt_temporal_clamp), C.POINTER(rt_temporal_frame),
                                           C.POINTER(rt_temporal_history), C.c_void_p, C.POINTER(rt_temporal_out), C.POINTER(rt_stats)]
+    L.rtb200_temporal_var_device.argtypes = [C.c_int32, C.POINTER(rt_temporal_params), C.POINTER(rt_temporal_clamp),
+                                             C.POINTER(rt_temporal_frame), C.c_void_p, C.POINTER(rt_temporal_history), C.c_void_p,
+                                             C.c_void_p, C.POINTER(rt_temporal_out), C.c_void_p, C.c_void_p]
+    L.rtb200_temporal_var.argtypes = [C.c_int32, C.POINTER(rt_temporal_params), C.POINTER(rt_temporal_clamp), C.POINTER(rt_temporal_frame),
+                                      C.c_void_p, C.POINTER(rt_temporal_history), C.c_void_p, C.c_void_p, C.POINTER(rt_temporal_out),
+                                      C.c_void_p, C.POINTER(rt_stats)]
     L.rtb200_camera_from_params_lens.argtypes = [C.POINTER(rt_camera_params), C.c_double, C.c_double, C.POINTER(rt_camera), C.POINTER(rt_lens)]
     L.rtb200_scene_set_lens.argtypes = [C.c_void_p, C.POINTER(rt_lens)]
     L.rtb200_render_frames_lens.argtypes = [C.POINTER(rt_scene), C.POINTER(rt_options), C.POINTER(rt_frame), C.POINTER(rt_lens), C.c_uint32,
@@ -1364,7 +1371,7 @@ def _camera_of(c) -> rt_camera:
 
 def temporal(color, sphere, point, camera, prev: Optional[dict] = None, *, motion=None, max_history: int = TEMPORAL_MAX_HISTORY,
              depth_tol: float = TEMPORAL_DEPTH_TOL, clamp: Optional[float] = None, clamp_radius: int = TEMPORAL_CLAMP_RADIUS,
-             stream=None) -> dict:
+             variance=None, stream=None) -> dict:
     """Accumulate a frame over time (include/rtb200.h, rtb200_temporal[_device]): each pixel of `color` ([h, w, 3] float32,
     normally a render's linear mean) is reprojected into the previous frame through its first hit (`sphere` [h, w] int32 or
     uint32 with -1 / 0xffffffff for a miss, `point` [h, w, 3] float64: :meth:`ResidentScene.aov`'s, of the same camera) and
@@ -1378,8 +1385,14 @@ def temporal(color, sphere, point, camera, prev: Optional[dict] = None, *, motio
     numpy arrays use the blocking host form (rtb200_temporal) and the result also holds "stats". CUDA tensors (contiguous, on one
     device) use the device form (rtb200_temporal_device) on `stream` without waiting, with the stream rules of :func:`denoise`:
     the outputs are allocated by torch on the call's stream, and handle 0 is refused. Returns {"color": float32 [h, w, 3],
-    "length": uint32 [h, w]}, the new history: pass it back as prev's "color" and "length" with the next frame."""
-    return _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol, stream, None, _clamp(clamp, clamp_radius))
+    "length": uint32 [h, w]}, the new history: pass it back as prev's "color" and "length" with the next frame.
+
+    `variance` ([h, w, 3] float32, the variance of each pixel's mean, normally render_frames(variance=True)'s) carries the
+    variance through the accumulation (rtb200_temporal_var[_device], DESIGN.md §4.21, clamped or not): prev must then hold the
+    previous call's "variance" too, and the result adds "variance", the new history's. "color" and "length" are the same as
+    without it."""
+    return _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol, stream, None, _clamp(clamp, clamp_radius),
+                     variance)
 
 
 def _max_history(n) -> int:
@@ -1402,9 +1415,9 @@ def _clamp(gamma, radius) -> Optional[rt_temporal_clamp]:
     return rt_temporal_clamp(float(gamma), radius)
 
 
-def _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol, stream, out, clamp=None):
-    """temporal(), writing into `out` ({"color", "length"} CUDA tensors of the right shapes) when it is given; clamp is an
-    rt_temporal_clamp or None."""
+def _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol, stream, out, clamp=None, variance=None):
+    """temporal(), writing into `out` ({"color", "length"} CUDA tensors of the right shapes, and "variance" with `variance`) when
+    it is given; clamp is an rt_temporal_clamp or None."""
     shape = tuple(color.shape)
     if len(shape) != 3 or shape[2] != 3:
         raise ValueError(f"temporal: color must have shape [h, w, 3], got {shape}")
@@ -1412,6 +1425,8 @@ def _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol
     prev = dict(prev) if prev is not None else None
     if prev is not None and not {"color", "length", "sphere", "point", "camera"} <= set(prev):
         raise ValueError("temporal: prev holds the previous frame's color, length, sphere, point and camera")
+    if variance is not None and prev is not None and "variance" not in prev:
+        raise ValueError("temporal: with variance, prev holds the previous call's variance too")
     A = _Arrays("temporal")
     f32, f64, u32, ids = (np.float32,), (np.float64,), (np.uint32,), (np.int32, np.uint32)
     cur = rt_temporal_frame(A.arg("color", color, f32, shape), A.arg("sphere", sphere, ids, hw), A.arg("point", point, f64, shape))
@@ -1424,12 +1439,20 @@ def _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol
                            _camera_of(prev["camera"]) if prev is not None else rt_camera(), float(depth_tol))
     hp = C.byref(hist) if hist is not None else None
     outs = [("color", shape, np.float32), ("length", hw, np.uint32)]
+    if variance is not None:
+        vp = A.arg("variance", variance, f32, shape)
+        pvp = A.arg("prev variance", prev["variance"], f32, shape) if prev is not None else None
+        outs.append(("variance", shape, np.float32))
+    cp = C.byref(clamp) if clamp is not None else None
     if A.host:
         out = A.empty(outs)
         st = rt_stats()
         o = C.byref(rt_temporal_out(A.ptr(out["color"]), A.ptr(out["length"])))
-        _check(lib().rtb200_temporal(-1, C.byref(p), C.byref(cur), hp, mp, o, C.byref(st)) if clamp is None else
-               lib().rtb200_temporal_clamped(-1, C.byref(p), C.byref(clamp), C.byref(cur), hp, mp, o, C.byref(st)))
+        if variance is not None:
+            _check(lib().rtb200_temporal_var(-1, C.byref(p), cp, C.byref(cur), vp, hp, pvp, mp, o, A.ptr(out["variance"]), C.byref(st)))
+        else:
+            _check(lib().rtb200_temporal(-1, C.byref(p), C.byref(cur), hp, mp, o, C.byref(st)) if clamp is None else
+                   lib().rtb200_temporal_clamped(-1, C.byref(p), C.byref(clamp), C.byref(cur), hp, mp, o, C.byref(st)))
         out["stats"] = st.as_dict()
         return out
     stream, handle = _call_stream(stream, A.device, "temporal", "the outputs")
@@ -1438,8 +1461,12 @@ def _temporal(color, sphere, point, camera, prev, motion, max_history, depth_tol
     if color.numel() == 0:   # a 0-pixel image (the library's no-op)
         return out
     o = C.byref(rt_temporal_out(A.ptr(out["color"]), A.ptr(out["length"])))
-    _check(lib().rtb200_temporal_device(A.device, C.byref(p), C.byref(cur), hp, mp, o, C.c_void_p(handle)) if clamp is None else
-           lib().rtb200_temporal_clamped_device(A.device, C.byref(p), C.byref(clamp), C.byref(cur), hp, mp, o, C.c_void_p(handle)))
+    if variance is not None:
+        _check(lib().rtb200_temporal_var_device(A.device, C.byref(p), cp, C.byref(cur), vp, hp, pvp, mp, o, A.ptr(out["variance"]),
+                                                C.c_void_p(handle)))
+    else:
+        _check(lib().rtb200_temporal_device(A.device, C.byref(p), C.byref(cur), hp, mp, o, C.c_void_p(handle)) if clamp is None else
+               lib().rtb200_temporal_clamped_device(A.device, C.byref(p), C.byref(clamp), C.byref(cur), hp, mp, o, C.c_void_p(handle)))
     return out
 
 
@@ -1448,20 +1475,30 @@ class TemporalDenoiser:
     (:func:`temporal`) and denoises the result (:func:`denoise`, guided by the frame's albedo and normal). It owns two history
     buffers, which its pushes ping-pong between, and copies of the previous frame's sphere and point, on the device;
     :meth:`reset` forgets the history (after an edit that renumbers spheres, or a cut). `clamp` and `clamp_radius` are
-    :func:`temporal`'s history clamp (None: off)."""
+    :func:`temporal`'s history clamp (None: off).
+
+    With `variance=True` each push also takes the variance of the frame's pixel means, carries it through the accumulation
+    (:func:`temporal` with `variance`) and denoises by it (:func:`denoise_var`, with `variance_floor`). The denoise weights left
+    unset are the chosen filter's defaults: DENOISE_* without the variance, DENOISE_VAR_* with it."""
 
     def __init__(self, *, max_history: int = TEMPORAL_MAX_HISTORY, depth_tol: float = TEMPORAL_DEPTH_TOL,
-                 iterations: int = DENOISE_ITERATIONS, color_weight: float = DENOISE_COLOR_WEIGHT,
-                 albedo_weight: float = DENOISE_ALBEDO_WEIGHT, normal_weight: float = DENOISE_NORMAL_WEIGHT,
-                 clamp: Optional[float] = None, clamp_radius: int = TEMPORAL_CLAMP_RADIUS):
+                 iterations: Optional[int] = None, color_weight: Optional[float] = None, albedo_weight: Optional[float] = None,
+                 normal_weight: Optional[float] = None, clamp: Optional[float] = None, clamp_radius: int = TEMPORAL_CLAMP_RADIUS,
+                 variance: bool = False, variance_floor: float = DENOISE_VAR_VARIANCE_FLOOR):
         self.max_history, self.depth_tol = _max_history(max_history), float(depth_tol)
         if self.max_history < 1:
             raise ValueError("max_history must be >= 1")
         self.clamp = _clamp(clamp, clamp_radius)
         if self.clamp is not None and not (math.isfinite(self.clamp.gamma) and self.clamp.gamma >= 0 and 1 <= self.clamp.radius <= 3):
             raise ValueError("clamp must be finite and >= 0 as a float32, and clamp_radius in [1, 3]")
-        self.denoise_kw = dict(iterations=iterations, color_weight=color_weight, albedo_weight=albedo_weight, normal_weight=normal_weight)
-        self._hist = None      # two {"color", "length"} buffers; push k writes _hist[k % 2] and reads the other as the history
+        self.variance = bool(variance)
+        defaults = ((DENOISE_VAR_ITERATIONS, DENOISE_VAR_COLOR_WEIGHT, DENOISE_VAR_ALBEDO_WEIGHT, DENOISE_VAR_NORMAL_WEIGHT) if self.variance
+                    else (DENOISE_ITERATIONS, DENOISE_COLOR_WEIGHT, DENOISE_ALBEDO_WEIGHT, DENOISE_NORMAL_WEIGHT))
+        given = (iterations, color_weight, albedo_weight, normal_weight)
+        self.denoise_kw = {k: d if v is None else v for k, v, d in zip(("iterations", "color_weight", "albedo_weight", "normal_weight"), given, defaults)}
+        if self.variance:
+            self.denoise_kw["variance_floor"] = variance_floor
+        self._hist = None      # two {"color", "length"[, "variance"]} buffers; push k writes _hist[k % 2] and reads the other as the history
         self._k = 0
         self._sphere = self._point = self._camera = self._stream = None
         self._has_prev = False
@@ -1469,14 +1506,18 @@ class TemporalDenoiser:
     def reset(self):
         self._has_prev = False
 
-    def push(self, linear, aov: dict, camera, motion=None, stream=None) -> dict:
+    def push(self, linear, aov: dict, camera, motion=None, stream=None, variance=None) -> dict:
         """One frame: `linear` [h, w, 3] float32 CUDA tensor, `aov` the frame's :meth:`ResidentScene.aov` on the device with
         albedo, normal, sphere and point, `camera` its rt_camera or rt_frame, `motion` the spheres' displacement since the
-        previous push. Runs on `stream` (by default torch's current stream) after the previous push, on whichever stream it ran.
-        Returns {"color": the accumulated image, "length": its history lengths, "denoised": the accumulated image denoised}.
-        "color" and "length" are the denoiser's own history buffer: the next push reads it as its history and the push after
-        that overwrites it, so do not write to them, and clone them to keep them."""
+        previous push, and with variance=True `variance` the [h, w, 3] float32 variance of the frame's pixel means (required).
+        Runs on `stream` (by default torch's current stream) after the previous push, on whichever stream it ran.
+        Returns {"color": the accumulated image, "length": its history lengths, "denoised": the accumulated image denoised}, and
+        with variance=True "variance": the accumulated image's variance.
+        "color", "length" and "variance" are the denoiser's own history buffer: the next push reads it as its history and the push
+        after that overwrites it, so do not write to them, and clone them to keep them."""
         import torch
+        if self.variance != (variance is not None):
+            raise ValueError("TemporalDenoiser.push: variance is required with variance=True and refused without it")
         stream, _ = _call_stream(stream, linear.device, "TemporalDenoiser.push", "the history")
         shape = tuple(linear.shape)
         hw = shape[:2]
@@ -1486,6 +1527,9 @@ class TemporalDenoiser:
             with torch.cuda.stream(stream):
                 self._hist = [{"color": torch.empty(shape, dtype=torch.float32, device=linear.device),
                                "length": torch.empty(hw, dtype=torch.uint32, device=linear.device)} for _ in range(2)]
+                if self.variance:
+                    for hb in self._hist:
+                        hb["variance"] = torch.empty(shape, dtype=torch.float32, device=linear.device)
                 self._sphere = torch.empty(hw, dtype=torch.int32, device=linear.device)
                 self._point = torch.empty(shape, dtype=torch.float64, device=linear.device)
             self._has_prev = False
@@ -1494,12 +1538,18 @@ class TemporalDenoiser:
         if self._has_prev:
             h = self._hist[self._k ^ 1]
             prev = {"color": h["color"], "length": h["length"], "sphere": self._sphere, "point": self._point, "camera": self._camera}
-        _temporal(linear, aov["sphere"], aov["point"], camera, prev, motion, self.max_history, self.depth_tol, stream, out, self.clamp)
+            if self.variance:
+                prev["variance"] = h["variance"]
+        _temporal(linear, aov["sphere"], aov["point"], camera, prev, motion, self.max_history, self.depth_tol, stream, out, self.clamp,
+                  variance)
         with torch.cuda.stream(stream):   # the next push's previous frame, after this push has read the current one
             self._sphere.view(aov["sphere"].dtype).copy_(aov["sphere"])
             self._point.copy_(aov["point"])
         self._camera = rt_camera.from_buffer_copy(_camera_of(camera))
         self._has_prev, self._k, self._stream = True, self._k ^ 1, stream
+        if self.variance:
+            den = denoise_var(out["color"], out["variance"], aov["albedo"], aov["normal"], stream=stream, **self.denoise_kw)
+            return {"color": out["color"], "length": out["length"], "variance": out["variance"], "denoised": den["linear"]}
         den = denoise(out["color"], aov["albedo"], aov["normal"], stream=stream, **self.denoise_kw)
         return {"color": out["color"], "length": out["length"], "denoised": den["linear"]}
 
